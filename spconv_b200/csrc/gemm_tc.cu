@@ -623,15 +623,16 @@ static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t st
 }
 
 // instantiated (channels x element bytes) combinations: rows of 32..512 bytes, N = 16..256 output
-// channels (tf32: 16..128, int8: 32..256)
+// channels (tf32: 16..128, int8: 32..256).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
+// gathered tile plus a weight slice of 128 or more rows puts two stages over TC_SMEM_BUDGET.
 template <int KIND, int CPR>
 static int launch_tc_cpr(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
     switch (p.n) {
         case 16: if constexpr (KIND != KIND_I8) return launch_tc_n<KIND, CPR, 16>(tm, p, stream); break;
         case 32: return launch_tc_n<KIND, CPR, 32>(tm, p, stream);
         case 64: return launch_tc_n<KIND, CPR, 64>(tm, p, stream);
-        case 128: return launch_tc_n<KIND, CPR, 128>(tm, p, stream);
-        case 256: if constexpr (KIND != KIND_TF32) return launch_tc_n<KIND, CPR, 256>(tm, p, stream); break;
+        case 128: if constexpr (CPR != 32) return launch_tc_n<KIND, CPR, 128>(tm, p, stream); break;
+        case 256: if constexpr (KIND != KIND_TF32 && CPR != 32) return launch_tc_n<KIND, CPR, 256>(tm, p, stream); break;
     }
     set_error("tc_gather_gemm: unsupported output channel count %d", p.n);
     return 2;

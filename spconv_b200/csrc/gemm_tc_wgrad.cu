@@ -202,7 +202,7 @@ tc_wgrad_kernel(const WgParams p) {
 #pragma unroll
         for (int itc = 0; itc < ITERS; ++itc)
             dst_off[itc] = swizzle_offset(((uint32_t)(pw * ROWS_PW + r0 + itc * RPI) << LG_SPAN_X) + chb, SPAN_X);
-        const int lg_apo = p.apo == 1 ? 0 : (p.apo == 2 ? 1 : 2);
+        const int lg_apo = p.apo == 1 ? 0 : (p.apo == 2 ? 1 : (p.apo == 4 ? 2 : 3));   // apo: 1, 2, 4 or 8 (make_plan)
         // per-lane constants of the dout gather: chunk chd of rows rd0 + itc*RPI_D of this warp's rows
         const int rd0 = lane >> LG_CPD;
         const uint32_t chd = (uint32_t)(lane & (CPD - 1)) << 4;
@@ -512,15 +512,19 @@ static bool make_plan(const WgradArgs &a, WgPlan &pl) {
     const bool tf32 = a.dtype == SPX_F32;       // fp32 reaches here only in TF32 mode (api_gemm.cu)
     const int e = tf32 ? 4 : 2;
     if (a.c_in % 16 || a.c_out % 16 || a.c_in > 256 || a.c_out > 256) return false;
-    // tf32: whole 128-byte atoms of 32 channels on both operands, dout rows of at most 512 bytes;
+    // tf32: whole 128-byte atoms of 32 channels on both operands, dout rows of at most 256 bytes (at
+    // c_out = 128 two 64 KB x stages and two dout tiles exceed WG_SMEM_MAX);
     // spx_debug_configure bit 4096 sends it back to the FMA kernel (A/B)
-    if (tf32 && (a.c_in % 32 || a.c_out % 32 || a.c_out > 128 || (runtime_cfg().debug & 4096))) return false;
+    if (tf32 && (a.c_in % 32 || a.c_out % 32 || a.c_out > 64 || (runtime_cfg().debug & 4096))) return false;
     if (!wg_span_ok(a.c_in * e) || !wg_span_ok(a.c_out * e)) return false;
     WgParams &p = pl.p;
     memset(&p, 0, sizeof(p));
     p.xb = a.c_in * e; p.span_x = p.xb < 128 ? p.xb : 128;
     p.lg_span_x = p.span_x == 128 ? 7 : (p.span_x == 64 ? 6 : 5);
     p.apo = p.xb / p.span_x;
+    // the producers split an atom index into (offset slot, chunk) with a shift and a mask: 384- to
+    // 896-byte rows (192 16-bit channels, 96 / 160 / 192 / 224 fp32 channels) run on the FMA kernel
+    if (p.apo & (p.apo - 1)) return false;
     p.atom_elems = p.span_x / e;
     p.apg = 128 / p.atom_elems;
     p.db = a.c_out * e; p.span_d = p.db < 128 ? p.db : 128;
@@ -594,7 +598,6 @@ int tc_wgrad(const WgradArgs &a, cudaStream_t stream) {
     if (a.dtype == SPX_F32) {
         if (cpa == 8 && cpd == 8) fn = tc_wgrad_kernel<8, 8, true>;
         if (cpa == 8 && cpd == 16) fn = tc_wgrad_kernel<8, 16, true>;
-        if (cpa == 8 && cpd == 32) fn = tc_wgrad_kernel<8, 32, true>;
     } else {
 #define WG_PICK(A, D) if (cpa == A && cpd == D) fn = tc_wgrad_kernel<A, D>;
 #define WG_PICK_ROW(A) WG_PICK(A, 2) WG_PICK(A, 4) WG_PICK(A, 8) WG_PICK(A, 16) WG_PICK(A, 32)
