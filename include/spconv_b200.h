@@ -391,17 +391,16 @@ int spx_last_kernel_family(void);
 /* number of kernel launches issued by this library (all host threads) since the last reset */
 int64_t spx_launch_count(int reset);
 /*
- * Test / perf-triage switches (never needed for correct operation; the reference's counterpart is
- * the SPCONV_DEBUG_* environment, spconv/constants.py:100-125).
+ * Test switches (never needed for correct operation; the reference's counterpart is the
+ * SPCONV_DEBUG_* environment, spconv/constants.py:100-125).
  *   force_family: -1 keep, 0 automatic, 1 generic FMA kernels, 2 tensor-core kernels (error if the
  *                 shape does not tile) -- the start-up value comes from SPX_FORCE_SIMT / SPX_FORCE_TC,
  *                 read once when the library is loaded;
  *   tc_ctas:      ignored (kept for ABI compatibility: the tensor-core kernels run one CTA per SM);
- *   debug_bits:   A/B and ablation mask (bits 1..32: ablations of the tensor-core kernels, results are wrong by
- *                 construction; 64 / 512: alternative sorts; 128: legacy regular-conv rulebook; 256: fp32+TF32
- *                 input gradient on the FMA kernel instead of wgmma, 4096: the same for the weight gradient;
- *                 1024: weight-gradient pass split; 2048: regular-conv mask sorts / tile tables one job per launch);
- *   trace_buf:    NULL or a DEVICE buffer of at least 8*2048 int64 that receives clock stamps.
+ *   debug_bits:   any combination of 256 (fp32+TF32 input gradient on the FMA kernel instead of wgmma)
+ *                 and 4096 (the same for the weight gradient); 0 clears both.  Any other bit is refused
+ *                 (returns 2) and leaves every switch unchanged;
+ *   trace_buf:    must be NULL (refused otherwise); trace_bytes is ignored.
  */
 int spx_debug_configure(int force_family, int tc_ctas, int debug_bits, void *trace_buf,
                         size_t trace_bytes);

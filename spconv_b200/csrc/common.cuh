@@ -21,22 +21,25 @@ int sm_count();          // SMs of the current device (cached)
 int current_device();    // cudaGetDevice (0 on failure)
 
 // Process-wide switches.  SPX_FORCE_SIMT / SPX_FORCE_TC are read from the
-// environment ONCE, when the library is loaded; the perf-triage hooks (ablation bits, timeline
-// buffer) are only reachable through spx_debug_configure(), which validates the buffer.
+// environment ONCE, when the library is loaded; spx_debug_configure() can change them and set the
+// two tf32 switches, which send the fp32 input / weight gradient to the FMA kernels.
 struct RuntimeCfg {
     int force_simt = 0, force_tc = 0;
-    int debug = 0;                 // ablation bits, see gemm_tc.cu / gemm_tc_wgrad.cu
-    long long *trace = nullptr;    // [8][2048] int64 device buffer or NULL
+    bool tf32_dgrad_fma = false;   // debug bit 256
+    bool tf32_wgrad_fma = false;   // debug bit 4096
 };
 RuntimeCfg &runtime_cfg();
 
 // cudaFuncSetAttribute is per DEVICE: remember which (function, device) pairs were configured
 bool func_configured(const void *fn, int dev);   // returns the previous state and marks it
 
+// A failed runtime call also leaves its error pending on the thread; it is consumed here so that
+// the next SPX_CHECK_LAUNCH does not report it again (e.g. after a refused stream capture).
 #define SPX_CHECK_CUDA(expr)                                                              \
     do {                                                                                  \
         cudaError_t _e = (expr);                                                          \
         if (_e != cudaSuccess) {                                                          \
+            (void)cudaGetLastError();                                                     \
             spx::set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e),        \
                            __FILE__, __LINE__);                                           \
             return 1;                                                                     \

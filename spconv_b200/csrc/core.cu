@@ -92,19 +92,15 @@ extern "C" int64_t spx_launch_count(int reset) {
 extern "C" int spx_debug_configure(int force_family, int tc_ctas, int debug_bits, void *trace_buf, size_t trace_bytes) {
     RuntimeCfg &c = runtime_cfg();
     SPX_REQUIRE(force_family >= -1 && force_family <= 2, "debug_configure: force_family must be -1 (keep), 0 (auto), 1 (SIMT) or 2 (tensor cores)");
-    SPX_REQUIRE(trace_buf == nullptr || trace_bytes >= (size_t)8 * 2048 * sizeof(long long),
-                "debug_configure: trace buffer must hold [8][2048] int64 (%zu bytes), got %zu",
-                (size_t)8 * 2048 * sizeof(long long), trace_bytes);
-    if (trace_buf) {
-        cudaPointerAttributes attr;
-        SPX_CHECK_CUDA(cudaPointerGetAttributes(&attr, trace_buf));
-        SPX_REQUIRE(attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged,
-                    "debug_configure: trace buffer is not device memory");
-    }
-    if (force_family >= 0) { c.force_simt = force_family == 1; c.force_tc = force_family == 2; }
+    SPX_REQUIRE((debug_bits & ~(256 | 4096)) == 0,
+                "debug_configure: debug_bits %d not supported; accepted bits are 256 (tf32 input gradient on "
+                "the FMA kernel) and 4096 (tf32 weight gradient on the FMA kernel)", debug_bits);
+    SPX_REQUIRE(trace_buf == nullptr, "debug_configure: the trace buffer is not supported; pass NULL");
     (void)tc_ctas;
-    c.debug = debug_bits;
-    c.trace = (long long *)trace_buf;
+    (void)trace_bytes;
+    if (force_family >= 0) { c.force_simt = force_family == 1; c.force_tc = force_family == 2; }
+    c.tf32_dgrad_fma = (debug_bits & 256) != 0;
+    c.tf32_wgrad_fma = (debug_bits & 4096) != 0;
     return 0;
 }
 

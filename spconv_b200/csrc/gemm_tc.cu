@@ -78,8 +78,6 @@ struct TcParams {
     const float *scale, *bias_f32;
     const int8_t *output_add;
     float output_add_scale;
-    long long *dbg_ts;      // optional [8 roles][2048] int64 buffer: rows 6..7 take per-CTA spans (SPX_TC_TRACE, perf triage)
-    int debug;              // SPX_TC_DEBUG ablation bits (perf triage only): 1 no gather, 2 no MMA, 4 no epilogue, 8 no weight TMA
 };
 
 // iterate set bits of a <=128-bit tile mask in ascending order (register-only: no indexed array)
@@ -155,15 +153,6 @@ __device__ __forceinline__ void epilogue_frag(const TcParams &p, const Acc (&acc
     }
 }
 
-// per-CTA wall-clock spans (ns, %globaltimer): rows 6..7 of the trace buffer hold [cta][4] =
-// {kernel entry, prologue done, role loops done, exit}
-__device__ __forceinline__ long long global_ns() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define TC_SPAN(i) do { if (p.dbg_ts && threadIdx.x == 0 && blockIdx.x < 1024) p.dbg_ts[6 * 2048 + blockIdx.x * 4 + (i)] = global_ns(); } while (0)
-
 // one K step of 32 bytes: D[64 x N] += A[64 x 32 B] * B[N x 32 B]^T
 template <int KIND, int N, typename Acc>
 __device__ __forceinline__ void mma_step(Acc (&acc)[N / 2], uint64_t a, uint64_t b, int b_mn, int bf16) {
@@ -199,7 +188,6 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
     static_assert(ROWS_PW * CPR >= 32, "a producer warp must cover at least one full cp.async instruction");
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    TC_SPAN(0);
     // dynamic smem base is only guaranteed 16-byte aligned: align manually to 1024
     const uint32_t raw_addr = smem_u32(smem_raw);
     const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
@@ -252,7 +240,6 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
         tma_prefetch_desc(&tmap_w);
     }
     __syncthreads();
-    TC_SPAN(1);
 
     if (warp >= TC_CONS_WARPS && warp < TC_TMA_WARP) {
         // ================================================= gather producers
@@ -288,12 +275,10 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
             while (k >= 0) {
                 mbar_wait(&empty[stage], phase ^ 1u);
                 const uint32_t a_stage = smem_base + (uint32_t)stage * p.stage_bytes;
-                if (!(p.debug & 1)) {
 #pragma unroll
-                    for (int itc = 0; itc < ITERS; ++itc)
-                        cp_async_16(a_stage + dst_off[itc], x_lane + (int64_t)max(ridx[itc], 0) * XB,
-                                    ridx[itc] >= 0 ? 16u : 0u);
-                }
+                for (int itc = 0; itc < ITERS; ++itc)
+                    cp_async_16(a_stage + dst_off[itc], x_lane + (int64_t)max(ridx[itc], 0) * XB,
+                                ridx[itc] >= 0 ? 16u : 0u);
                 cp_async_mbar_arrive_noinc(&full[stage]);
                 k = it.next();
                 if (k >= 0) {
@@ -339,14 +324,10 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&full[stage]);
                 } else if (lane == 0) {
-                    if (p.debug & 8) {
-                        mbar_arrive(&full[stage]);
-                    } else {
-                        mbar_arrive_expect_tx(&full[stage], (uint32_t)p.b_bytes);
-                        for (int sb = 0; sb < p.b_subtiles; ++sb)
-                            tma_load_2d(b_stage + sb * p.b_sub_bytes, &tmap_w, &full[stage],
-                                        kw * p.w_inner_elems + sb * p.span_b_elems, 0);
-                    }
+                    mbar_arrive_expect_tx(&full[stage], (uint32_t)p.b_bytes);
+                    for (int sb = 0; sb < p.b_subtiles; ++sb)
+                        tma_load_2d(b_stage + sb * p.b_sub_bytes, &tmap_w, &full[stage],
+                                    kw * p.w_inner_elems + sb * p.span_b_elems, 0);
                 }
                 __syncwarp();
                 if (++stage == p.stages) { stage = 0; phase ^= 1u; }
@@ -416,41 +397,38 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                 fence_proxy_async_smem();     // cp.async (generic proxy) writes -> wgmma operand reads
                 const uint32_t a16 = (smem_base + (uint32_t)stage * p.stage_bytes + (uint32_t)(wg * 64 * SPAN_A)) >> 4;
                 const uint32_t b16 = (smem_base + (uint32_t)stage * p.stage_bytes + (uint32_t)p.a_stage_bytes) >> 4;
-                if (!(p.debug & 2)) {
-                    fence_regs(acc);
-                    wgmma_fence();
-                    if (!p.b_mn_major) {
+                fence_regs(acc);
+                wgmma_fence();
+                if (!p.b_mn_major) {
 #pragma unroll
-                        for (int sub = 0; sub < A_SUBTILES; ++sub) {
-                            const uint32_t as = a16 + (uint32_t)sub * (uint32_t)(A_SUB_BYTES >> 4);
-                            const uint32_t bs = b16 + (uint32_t)sub * b_sub16;
+                    for (int sub = 0; sub < A_SUBTILES; ++sub) {
+                        const uint32_t as = a16 + (uint32_t)sub * (uint32_t)(A_SUB_BYTES >> 4);
+                        const uint32_t bs = b16 + (uint32_t)sub * b_sub16;
 #pragma unroll
-                            for (int jr = 0; jr < Q_A; ++jr)
-                                mma_step<KIND, N>(acc, a_hi | (uint64_t)((as + 2u * jr) & 0x3FFFu),
-                                                  b_hi | (uint64_t)((bs + 2u * jr) & 0x3FFFu), 0, p.ab_bf16);
-                        }
-                    } else {
+                        for (int jr = 0; jr < Q_A; ++jr)
+                            mma_step<KIND, N>(acc, a_hi | (uint64_t)((as + 2u * jr) & 0x3FFFu),
+                                              b_hi | (uint64_t)((bs + 2u * jr) & 0x3FFFu), 0, p.ab_bf16);
+                    }
+                } else {
 #pragma unroll
-                        for (int sub = 0; sub < A_SUBTILES; ++sub) {
-                            const uint32_t as = a16 + (uint32_t)sub * (uint32_t)(A_SUB_BYTES >> 4);
+                    for (int sub = 0; sub < A_SUBTILES; ++sub) {
+                        const uint32_t as = a16 + (uint32_t)sub * (uint32_t)(A_SUB_BYTES >> 4);
 #pragma unroll
-                            for (int jr = 0; jr < Q_A; ++jr) {
-                                const uint32_t j = (uint32_t)(sub * Q_A + jr);
-                                mma_step<KIND, N>(acc, a_hi | (uint64_t)((as + 2u * jr) & 0x3FFFu),
-                                                  b_hi | (uint64_t)((b16 + j * (uint32_t)p.b_kstep16_mn) & 0x3FFFu), 1,
-                                                  p.ab_bf16);
-                            }
+                        for (int jr = 0; jr < Q_A; ++jr) {
+                            const uint32_t j = (uint32_t)(sub * Q_A + jr);
+                            mma_step<KIND, N>(acc, a_hi | (uint64_t)((as + 2u * jr) & 0x3FFFu),
+                                              b_hi | (uint64_t)((b16 + j * (uint32_t)p.b_kstep16_mn) & 0x3FFFu), 1,
+                                              p.ab_bf16);
                         }
                     }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    fence_regs(acc);
                 }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(acc);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[stage]);         // this warp is done reading the stage
                 if (++stage == p.stages) { stage = 0; phase ^= 1u; }
             }
-            if (p.debug & 4) continue;             // ablation: accumulator dropped
             const int64_t r_lo = (int64_t)tile * TC_TILE_M + wg * 64 + (warp & 3) * 16 + (lane >> 2);
             const int64_t r_hi = r_lo + 8;
             int64_t d_lo = -1, d_hi = -1;
@@ -470,8 +448,6 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
     }
 
     __syncthreads();
-    TC_SPAN(2);
-    TC_SPAN(3);
 }
 
 // ------------------------------------------------------------------ host side
@@ -540,7 +516,7 @@ bool tc_gather_gemm_supported(const GatherGemmArgs &a) {
     // tf32 input gradient: the weight loader writes the filter slice transposed (tf32 wgmma reads K-major
     // operands only); it is served for whole 128-byte filter rows, otherwise fp32 dgrad runs on the FMA
     // kernel; spx_debug_configure bit 256 switches the tensor-core route off (A/B against the FMA kernel).
-    if (a.dtype == SPX_F32 && a.transpose_w && ((runtime_cfg().debug & 256) || (a.c_in * 4) % 128)) return false;
+    if (a.dtype == SPX_F32 && a.transpose_w && (runtime_cfg().tf32_dgrad_fma || (a.c_in * 4) % 128)) return false;
     if (((size_t)a.kv * a.c_in * dtype_bytes(a.dtype)) % 16) return false;
     return tc_shape_ok(a.dtype, a.kv, a.c_in, a.c_out, a.transpose_w);
 }
@@ -582,7 +558,6 @@ static int fill_params(const GatherGemmArgs &a, TcParams &p) {
     p.a_stage_bytes = (int)align_up((size_t)TC_TILE_M * p.xb, 1024);
     p.stage_bytes = p.a_stage_bytes + (int)align_up((size_t)p.b_bytes, 1024);
     p.idx_bytes = (int)align_up((size_t)(a.kv + 1) * 512, 1024);
-    const RuntimeCfg &cfg = runtime_cfg();
     p.stages = (TC_SMEM_BUDGET - 2 * p.idx_bytes) / p.stage_bytes;
     if (p.stages > TC_MAX_STAGES) p.stages = TC_MAX_STAGES;
     SPX_REQUIRE(p.stages >= 2, "tc_gather_gemm: tile does not fit shared memory (stage %d bytes)", p.stage_bytes);
@@ -600,8 +575,6 @@ static int fill_params(const GatherGemmArgs &a, TcParams &p) {
     }
     p.kv = a.kv; p.words = (a.kv + 31) / 32; p.reverse = a.reverse;
     p.y = a.y; p.out_dtype = a.dtype; p.epi_mode = 0; p.bias = a.bias; p.act = a.act; p.alpha = a.alpha;
-    p.debug = cfg.debug;          // perf-triage hooks, set through spx_debug_configure() only
-    p.dbg_ts = cfg.trace;
     return 0;
 }
 

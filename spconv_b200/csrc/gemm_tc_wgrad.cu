@@ -53,8 +53,6 @@ struct WgParams {
     const int32_t *sched_rec;    // [tiles][TT_REC_INTS] {tile, mask[4]}: tiles by decreasing offset count (gemm.cuh)
     int kv, words, c_in;
     float *partial; int64_t partial_stride;
-    long long *dbg_ts;           // optional [8][2048] int64 buffer: row 2 takes per-CTA spans (SPX_TC_TRACE)
-    int debug;                   // SPX_TC_DEBUG ablation bits (perf triage only): 16 no partial stores
 };
 
 // Offset slots are filled in the order 0, kv-1, 1, kv-2, ...: a group (one M = 128 accumulator)
@@ -93,14 +91,6 @@ __device__ __forceinline__ void wg_load_rec(const int32_t *__restrict__ rec, int
     tile = a.x; m[0] = (uint32_t)a.y; m[1] = (uint32_t)a.z; m[2] = (uint32_t)a.w; m[3] = (uint32_t)b;
 }
 
-__device__ __forceinline__ long long wg_global_ns() {
-    long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-// per-CTA wall-clock spans (ns): row 2 of the trace buffer holds [pass * chunks + chunk][4]
-#define WG_SPAN(i) do { if (p.dbg_ts && threadIdx.x == 0) { const int c_ = blockIdx.y * gridDim.x + blockIdx.x; if (c_ < 512) p.dbg_ts[2 * 2048 + c_ * 4 + (i)] = wg_global_ns(); } } while (0)
-
 __device__ __forceinline__ uint32_t pick_word(const uint32_t (&m)[4], int w) {
     return w == 0 ? m[0] : (w == 1 ? m[1] : (w == 2 ? m[2] : m[3]));     // selects, no local-memory indexing
 }
@@ -138,7 +128,6 @@ tc_wgrad_kernel(const WgParams p) {
     constexpr int ITERS = ROWS_PW / RPI > 0 ? ROWS_PW / RPI : 1;   // copies per thread per atom
     constexpr int ITERS_D = ROWS_PW / RPI_D;                       // copies per thread per dout tile
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    WG_SPAN(0);
     const uint32_t raw_addr = smem_u32(smem_raw);
     const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
     uint8_t *smem = smem_raw + pad;
@@ -187,7 +176,6 @@ tc_wgrad_kernel(const WgParams p) {
         mbar_fence_init();
     }
     __syncthreads();
-    WG_SPAN(1);
 
     if (warp >= WG_CONS_WARPS && warp < WG_SCHED_WARP) {
         // ================================================= producers
@@ -432,39 +420,35 @@ tc_wgrad_kernel(const WgParams p) {
 #pragma unroll
             for (int w = 0; w < 4; ++w) tm[w] = tm_next[w];
         }
-        WG_SPAN(2);
         // ================================================= accumulators -> fp32 partials
         // register i of thread t holds M row 64 wg + 16 (warp % 4) + t / 4 + 8 ((i / 2) % 2),
         // column 8 (i / 4) + 2 (t % 4) + i % 2
-        if (!(p.debug & 16)) {
-            float *part = p.partial + (int64_t)chunk * p.partial_stride;
+        float *part = p.partial + (int64_t)chunk * p.partial_stride;
 #pragma unroll
-            for (int gl = 0; gl < G; ++gl) {
-                if (gl >= ng) break;
-                const int g = g_first + gl * g_step;
+        for (int gl = 0; gl < G; ++gl) {
+            if (gl >= ng) break;
+            const int g = g_first + gl * g_step;
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int L = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // M index inside the group
-                    const int s = L / p.atom_elems;
-                    const int ce = L - s * p.atom_elems;
-                    const int a = g * p.apg + s;
-                    const int ks = a / p.apo;
-                    const int k = slot_offset(ks, p.kv);
-                    const int c = (a - ks * p.apo) * p.atom_elems + ce;
-                    if (k >= p.kv) continue;
-                    float *dst = part + (int64_t)k * p.c_in + c;
+            for (int h = 0; h < 2; ++h) {
+                const int L = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;   // M index inside the group
+                const int s = L / p.atom_elems;
+                const int ce = L - s * p.atom_elems;
+                const int a = g * p.apg + s;
+                const int ks = a / p.apo;
+                const int k = slot_offset(ks, p.kv);
+                const int c = (a - ks * p.apo) * p.atom_elems + ce;
+                if (k >= p.kv) continue;
+                float *dst = part + (int64_t)k * p.c_in + c;
 #pragma unroll
-                    for (int nb8 = 0; nb8 < N / 8; ++nb8)
+                for (int nb8 = 0; nb8 < N / 8; ++nb8)
 #pragma unroll
-                        for (int j = 0; j < 2; ++j)
-                            dst[(int64_t)(nb8 * 8 + 2 * (lane & 3) + j) * p.kv * p.c_in] = acc[gl][nb8 * 4 + 2 * h + j];
-                }
+                    for (int j = 0; j < 2; ++j)
+                        dst[(int64_t)(nb8 * 8 + 2 * (lane & 3) + j) * p.kv * p.c_in] = acc[gl][nb8 * 4 + 2 * h + j];
             }
         }
     }
 
     __syncthreads();
-    WG_SPAN(3);
 }
 
 // 4 outputs per thread (float4 partial reads), the chunk range split over the 8 warps of a block,
@@ -515,7 +499,7 @@ static bool make_plan(const WgradArgs &a, WgPlan &pl) {
     // tf32: whole 128-byte atoms of 32 channels on both operands, dout rows of at most 256 bytes (at
     // c_out = 128 two 64 KB x stages and two dout tiles exceed WG_SMEM_MAX);
     // spx_debug_configure bit 4096 sends it back to the FMA kernel (A/B)
-    if (tf32 && (a.c_in % 32 || a.c_out % 32 || a.c_out > 64 || (runtime_cfg().debug & 4096))) return false;
+    if (tf32 && (a.c_in % 32 || a.c_out % 32 || a.c_out > 64 || runtime_cfg().tf32_wgrad_fma)) return false;
     if (!wg_span_ok(a.c_in * e) || !wg_span_ok(a.c_out * e)) return false;
     WgParams &p = pl.p;
     memset(&p, 0, sizeof(p));
@@ -538,10 +522,6 @@ static bool make_plan(const WgradArgs &a, WgPlan &pl) {
     p.groups_total = (atoms_total + p.apg - 1) / p.apg;
     p.groups_per_pass = WG_ACC_COLS / a.c_out;          // = G of the kernel instance
     if (p.groups_per_pass > 16) p.groups_per_pass = 16;
-    // A/B knob (spx_debug_configure bit 1024): half the accumulators per CTA => twice the passes, half the
-    // chunks.  The fp32 partial volume (chunks x all groups) halves, the dout tile is gathered by twice as
-    // many passes.
-    if ((runtime_cfg().debug & 1024) && p.groups_per_pass >= 2) p.groups_per_pass /= 2;
     pl.passes = (p.groups_total + p.groups_per_pass - 1) / p.groups_per_pass;
     p.a_stage_bytes = p.apg * WG_TILE * p.span_x;
     p.b_buf_bytes = WG_TILE * p.db;
@@ -586,8 +566,6 @@ int tc_wgrad(const WgradArgs &a, cudaStream_t stream) {
     WgPlan pl;
     SPX_REQUIRE(make_plan(a, pl), "tc_wgrad: unsupported shape");
     pl.p.partial = (float *)a.workspace;
-    pl.p.dbg_ts = runtime_cfg().trace;      // perf-triage hooks (spx_debug_configure)
-    pl.p.debug = runtime_cfg().debug;
     SPX_REQUIRE((size_t)pl.chunks * pl.p.partial_stride * sizeof(float) <= a.workspace_bytes,
                 "tc_wgrad: workspace too small");
     SPX_REQUIRE(((uintptr_t)a.workspace & 15u) == 0, "tc_wgrad: workspace must be 16-byte aligned");

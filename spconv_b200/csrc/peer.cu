@@ -44,7 +44,7 @@
 namespace spx {
 
 // ---- exchange buffer layout (bytes from the base of each rank's buffer)
-//   [0, 64)      local state: epoch, finished CTAs of the running finish, CTAs done in the running publish, error
+//   [0, 64)      local state: epoch, finished CTAs of the running finish, one unused word, error
 //   [256, 320)   flags, one per source rank: last epoch (+1) that source has published (written by the peers)
 //   [4096, ...)  data [2 slots][capacity] fp32: this rank's own slices
 constexpr size_t PEER_FLAGS = 256, PEER_DATA = 4096;
@@ -75,7 +75,7 @@ constexpr int PX_THREADS = 256, PX_WARPS = PX_THREADS / 32;
 template <typename T>
 __global__ void __launch_bounds__(PX_THREADS)
 peer_push_kernel(const float *__restrict__ partial, int64_t stride, int chunks, const T *__restrict__ src, int64_t total,
-                 PeerPtrs peers, int world, int rank, int64_t capacity, int publish) {
+                 PeerPtrs peers, int rank, int64_t capacity) {
     __shared__ float4 acc_s[PX_WARPS][32];
     __shared__ unsigned s_epoch;
     PeerState *st = reinterpret_cast<PeerState *>(peers.buf[rank]);
@@ -114,24 +114,6 @@ peer_push_kernel(const float *__restrict__ partial, int64_t stride, int chunks, 
     }
     if (i < total)                                         // the padded tail of the last float4 carries zeros
         *reinterpret_cast<float4 *>(reinterpret_cast<float *>(peers.buf[rank] + PEER_DATA) + (int64_t)(epoch & 1u) * capacity + i) = t;
-    if (!(publish & 1)) return;                            // default: the finish kernel publishes (see there)
-    __threadfence();
-    __syncwarp();
-    unsigned last = 0;
-    if (lane == 0) last = atomicAdd(&st->done, 1u) == gridDim.x - 1 ? 1u : 0u;
-    last = __shfl_sync(0xffffffffu, last, 0);
-    if (!last) return;
-    // every slice of this rank is in its buffer (= visible in this GPU's L2, where the peers' reads arrive): tell everybody
-    if (publish & 2) {                                     // A/B (debug bit 16384): gpu-scope fence + plain system-scope flag store
-        __threadfence();
-        if (lane == 0) st->done = 0;
-        if (lane < world)
-            asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(reinterpret_cast<unsigned *>(peers.buf[lane] + PEER_FLAGS) + rank), "r"(epoch + 1u) : "memory");
-        return;
-    }
-    __threadfence_system();
-    if (lane == 0) st->done = 0;
-    if (lane < world) st_release_sys(reinterpret_cast<unsigned *>(peers.buf[lane] + PEER_FLAGS) + rank, epoch + 1u);
 }
 
 // Receive side.  It runs BESIDE the persistent input-gradient kernel (whose CTAs own most of every SM's register
@@ -146,7 +128,7 @@ constexpr int FIN_MAX_CTAS = 64;               // 0.44 MB per peer = 54 chunks: 
 template <typename T>
 __global__ void __launch_bounds__(PX_THREADS)
 peer_finish_kernel(T *__restrict__ dst, int64_t total, PeerPtrs peers, int world, int rank, int64_t capacity, float scale,
-                   unsigned long long timeout_ns, int publish) {
+                   unsigned long long timeout_ns) {
     extern __shared__ __align__(128) uint8_t fin_smem[];      // [world][FIN_CHUNK_BYTES] + mbarrier
     __shared__ __align__(8) uint64_t bar;
     __shared__ unsigned s_epoch;
@@ -156,11 +138,11 @@ peer_finish_kernel(T *__restrict__ dst, int64_t total, PeerPtrs peers, int world
     if (threadIdx.x == 0) { s_epoch = st->epoch; s_bad = 0; mbar_init(&bar, 1); mbar_fence_init(); }
     __syncthreads();
     const unsigned epoch = s_epoch, target = epoch + 1u;
-    if (publish && blockIdx.x == 0 && threadIdx.x < world) {
+    if (blockIdx.x == 0 && threadIdx.x < world) {
         // This rank's slices were written by an EARLIER kernel of this stream (the weight-gradient reduction): they
         // are complete and visible on this GPU.  One system-scope fence, then the epoch goes to every rank's flag
-        // word.  (Publishing from the reduction kernel itself -- last CTA out, debug bit 8192 -- put a per-CTA fence
-        // + counter and the NVLink store acknowledgement on the critical path: +8 us on the weight gradient.)
+        // word.  (Publishing from the reduction kernel itself -- last CTA out -- put a per-CTA fence + counter and
+        // the NVLink store acknowledgement on the critical path: +8 us on the weight gradient.)
         __threadfence_system();
         st_release_sys(reinterpret_cast<unsigned *>(peers.buf[threadIdx.x] + PEER_FLAGS) + rank, target);
     }
@@ -247,8 +229,7 @@ int peer_push(const float *partial, int64_t stride, int chunks, const void *src,
     const PeerPtrs pp = peer_ptrs(pg);
     const int64_t cap = (int64_t)(pg->capacity_bytes / 4);
     const unsigned grid = push_ctas(total);
-    const int publish = ((runtime_cfg().debug & 8192) ? 1 : 0) | ((runtime_cfg().debug & 16384) ? 2 : 0);
-#define PX_LAUNCH(T) peer_push_kernel<T><<<grid, PX_THREADS, 0, stream>>>(partial, stride, chunks, (const T *)src, total, pp, pg->world, pg->rank, cap, publish)
+#define PX_LAUNCH(T) peer_push_kernel<T><<<grid, PX_THREADS, 0, stream>>>(partial, stride, chunks, (const T *)src, total, pp, pg->rank, cap)
     if (dtype == SPX_F16) PX_LAUNCH(__half);
     else if (dtype == SPX_BF16) PX_LAUNCH(__nv_bfloat16);
     else if (dtype == SPX_F32) PX_LAUNCH(float);
@@ -269,14 +250,13 @@ int peer_finish(void *dst, int64_t total, int dtype, const spx_peer_group *pg, f
     const unsigned grid = (unsigned)(nchunks < max_ctas ? nchunks : max_ctas);
     const size_t smem = (size_t)pg->world * FIN_CHUNK_BYTES;
     const unsigned long long timeout_ns = (unsigned long long)(pg->timeout_ms > 0 ? pg->timeout_ms : 20000) * 1000000ull;
-    const int publish = (runtime_cfg().debug & 8192) ? 0 : 1;          // bit 8192: the reduction kernel has published
 #define PX_LAUNCH(T)                                                                                                  \
     do {                                                                                                              \
         auto fn = peer_finish_kernel<T>;                                                                              \
         if (smem > 48 * 1024 && !func_configured((const void *)fn, current_device()))                                 \
             SPX_CHECK_CUDA(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
                                                 SPX_MAX_PEERS * FIN_CHUNK_BYTES));                                    \
-        fn<<<grid, PX_THREADS, smem, stream>>>((T *)dst, total, pp, pg->world, pg->rank, cap, scale, timeout_ns, publish);      \
+        fn<<<grid, PX_THREADS, smem, stream>>>((T *)dst, total, pp, pg->world, pg->rank, cap, scale, timeout_ns);     \
     } while (0)
     if (dtype == SPX_F16) PX_LAUNCH(__half);
     else if (dtype == SPX_BF16) PX_LAUNCH(__nv_bfloat16);

@@ -19,8 +19,6 @@ namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
 int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
                        int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
-int radix_argsort(uint32_t *mask, int32_t *argsort, int64_t n, int key_bits, void *workspace, size_t workspace_bytes,
-                  cudaStream_t stream);
 }
 
 namespace spx {
@@ -288,67 +286,17 @@ __device__ __forceinline__ bool conv3_out_key(const Geom &g, const int4 c, const
     return true;
 }
 
-// grid (ceil(N/T), kv): hash every hit, payload = k*N + i (first touch in offset-major order)
-template <typename Table, bool FAST3>
-__global__ void conv_insert_kernel(Table table, Geom g, const int32_t *__restrict__ indices, int64_t N) {
-    int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    int k = blockIdx.y;
-    if constexpr (FAST3) {
-        __shared__ Taps3 taps;
-        if (threadIdx.x == 0) taps = block_taps3(g, k);
-        __syncthreads();
-        if (i >= N) return;
-        const int4 c = __ldg(reinterpret_cast<const int4 *>(indices) + i);
-        int64_t key;
-        if (conv3_out_key(g, c, taps, key)) table.insert_min(key, (int32_t)((int64_t)k * N + i));
-    } else {
-        if (i >= N) return;
-        int c[SPX_MAX_NDIM + 1], o[SPX_MAX_NDIM + 1], r[SPX_MAX_NDIM];
-        load_coord(indices, i, g.ndim, c);
-        offset_taps(k, g.ksize, g.ndim, r);
-        if (conv_out_coord(g, c, r, o))
-            table.insert_min(linear_key(o, g.out_dims, g.ndim), (int32_t)((int64_t)k * N + i));
-    }
-}
-
 // 3-D, 3x3x3, non-transposed: one thread per INPUT voxel walks the 27 offsets.  The per-axis output
 // coordinates of the three taps are computed once (9 divisions-by-stride instead of 81), and with a
 // stride > 1 most (axis, tap) pairs fail the divisibility test, so only the surviving combinations
-// (3.4 of 27 on average at stride 2) reach the hash table.  The grid-(N, kv) kernels above re-read
-// the coordinates 27 times and spend a thread per rejected combination.
+// (3.4 of 27 on average at stride 2) reach the hash table.  The grid-(N, kv) kernels re-read the
+// coordinates 27 times and spend a thread per rejected combination.
 struct Axis3 { int o[3]; };
 __device__ __forceinline__ Axis3 axis_taps3(int c, int pad, int dil, int stride, int odim) {
     Axis3 a;
 #pragma unroll
     for (int r = 0; r < 3; ++r) { int o; a.o[r] = axis_out(c, pad, r, dil, stride, odim, o) ? o : -1; }
     return a;
-}
-
-template <typename Table>
-__global__ void conv_insert_k3_kernel(Table table, Geom g, const int32_t *__restrict__ indices, int64_t N) {
-    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (i >= N) return;
-    const int4 c = __ldg(reinterpret_cast<const int4 *>(indices) + i);
-    if (c.x < 0 || c.x >= g.batch) return;
-    const Axis3 az = axis_taps3(c.y, g.padding[0], g.dilation[0], g.stride[0], g.out_dims[0]);
-    const Axis3 ay = axis_taps3(c.z, g.padding[1], g.dilation[1], g.stride[1], g.out_dims[1]);
-    const Axis3 ax = axis_taps3(c.w, g.padding[2], g.dilation[2], g.stride[2], g.out_dims[2]);
-#pragma unroll
-    for (int r0 = 0; r0 < 3; ++r0) {
-        if (az.o[r0] < 0) continue;
-        const int64_t kz = (int64_t)c.x * g.out_dims[0] + az.o[r0];
-#pragma unroll
-        for (int r1 = 0; r1 < 3; ++r1) {
-            if (ay.o[r1] < 0) continue;
-            const int64_t kzy = kz * g.out_dims[1] + ay.o[r1];
-#pragma unroll
-            for (int r2 = 0; r2 < 3; ++r2) {
-                if (ax.o[r2] < 0) continue;
-                const int k = (r0 * 3 + r1) * 3 + r2;
-                table.insert_min(kzy * g.out_dims[2] + ax.o[r2], (int32_t)((int64_t)k * N + i));
-            }
-        }
-    }
 }
 
 // pair_bwd[k][i] = output of (input i, offset k) or -1 (every element written, coalesced over i);
@@ -574,73 +522,6 @@ __global__ void conv_assign_rank_kernel(Table table, Geom g, const uint32_t *__r
     table.set_value(s, r);
     if (mask_zero) mask_zero[r] = 0u;              // the pairs kernel ORs the forward masks into it
     int32_t *dst = out_inds + (int64_t)r * (g.ndim + 1);
-    for (int a = g.ndim - 1; a >= 0; --a) {
-        dst[a + 1] = (int32_t)(key % g.out_dims[a]);
-        key /= g.out_dims[a];
-    }
-    dst[0] = (int32_t)key;
-}
-
-// compact occupied slots -> (first-touch payload, slot); order irrelevant (sorted next).
-// The table is sized for the worst-case output count, so most of it is empty: every thread scans
-// COLLECT_ITEMS slots and a block reserves its output range with ONE atomic (a single global
-// counter serialises same-address atomics; one per warp made this kernel the slowest
-// of the conv rulebook).
-constexpr int COLLECT_THREADS = 256;
-constexpr int COLLECT_ITEMS = 4;
-template <typename Table>
-__global__ void __launch_bounds__(COLLECT_THREADS)
-conv_collect_kernel(Table table, uint32_t capacity, uint32_t *__restrict__ payload,
-                    uint32_t *__restrict__ slot_of, int *__restrict__ counter) {
-    __shared__ int warp_cnt[COLLECT_THREADS / 32];
-    __shared__ int block_base;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t first = blockIdx.x * (uint32_t)(COLLECT_THREADS * COLLECT_ITEMS);
-    bool occ[COLLECT_ITEMS];
-    int32_t val[COLLECT_ITEMS];
-    unsigned ballot[COLLECT_ITEMS];
-    int mine = 0;                                   // occupied slots seen by this warp
-#pragma unroll
-    for (int j = 0; j < COLLECT_ITEMS; ++j) {
-        const uint32_t s = first + j * COLLECT_THREADS + threadIdx.x;
-        int64_t key;
-        val[j] = 0;
-        occ[j] = s < capacity && table.occupied(s, key, val[j]);
-        ballot[j] = __ballot_sync(0xffffffffu, occ[j]);
-        mine += __popc(ballot[j]);
-    }
-    if (lane == 0) warp_cnt[warp] = mine;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int tot = 0;
-        for (int w = 0; w < COLLECT_THREADS / 32; ++w) { const int c = warp_cnt[w]; warp_cnt[w] = tot; tot += c; }
-        block_base = tot ? atomicAdd(counter, tot) : 0;
-    }
-    __syncthreads();
-    int base = block_base + warp_cnt[warp];
-#pragma unroll
-    for (int j = 0; j < COLLECT_ITEMS; ++j) {
-        if (occ[j]) {
-            const int pos = base + __popc(ballot[j] & ((1u << lane) - 1));
-            payload[pos] = (uint32_t)val[j];
-            slot_of[pos] = first + j * COLLECT_THREADS + threadIdx.x;
-        }
-        base += __popc(ballot[j]);
-    }
-}
-
-// rank r (first-touch order) -> write r into its slot, decode the key into out_inds[r]
-template <typename Table>
-__global__ void conv_assign_kernel(Table table, Geom g, const uint32_t *__restrict__ sorted_slot,
-                                   const int32_t *__restrict__ order, int64_t M, int32_t *__restrict__ out_inds) {
-    int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (r >= M) return;
-    // order != NULL: sorted_slot is the UNSORTED slot list and order the argsort of its payloads
-    uint32_t s = order ? sorted_slot[order[r]] : sorted_slot[r];
-    int64_t key; int32_t val;
-    table.occupied(s, key, val);
-    table.set_value(s, (int32_t)r);
-    int32_t *dst = out_inds + r * (g.ndim + 1);
     for (int a = g.ndim - 1; a >= 0; --a) {
         dst[a + 1] = (int32_t)(key % g.out_dims[a]);
         key /= g.out_dims[a];
@@ -1046,26 +927,6 @@ static size_t sort_pairs_temp_bytes(int64_t n) {
     return bytes > floor_bytes ? bytes : floor_bytes;
 }
 
-extern "C" size_t spx_rulebook_workspace_size(const spx_conv_geometry *g, int64_t num_in, int64_t max_out, int is_subm) {
-    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
-    Geom gg = make_geom(g, is_subm != 0);
-    size_t total = 256;
-    if (is_subm) {
-        RbLayout L = rb_layout(gg, num_in, gg.in_dims);
-        total += align_up(L.table_bytes, 256) + align_up(L.table_vals_bytes, 256);
-    } else {
-        max_out = spx_conv_max_out(g, num_in);   // the bound is recomputed by both stages
-        RbLayout L = rb_layout(gg, max_out, gg.out_dims, 2);
-        total += align_up(L.table_bytes, 256) + align_up(L.table_vals_bytes, 256);
-        total += 5 * align_up((size_t)max_out * 4, 256);          // payload, slot (in + out), order
-        total += align_up(sort_pairs_temp_bytes(max_out), 256);
-        total += align_up(radix_argsort_workspace_bytes(max_out), 256);
-        total += align_up(rank_scratch_bytes((int64_t)gg.kv * num_in), 256);
-        total += 256;                                             // counter
-    }
-    return total + 1024;
-}
-
 static bool subm_k3_path(const Geom &gg) {
     return !needs_i64(gg, gg.in_dims) && gg.ndim == 3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
 }
@@ -1124,20 +985,18 @@ extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indi
 namespace {
 struct ConvWs {
     void *tbl; int32_t *tvals;
-    uint32_t *payload, *slot, *payload_sorted, *slot_sorted;
-    void *sort_tmp; size_t sort_tmp_bytes;
-    int32_t *order;                    // argsort of the payloads (default path)
-    void *radix_ws; size_t radix_ws_bytes;
-    uint32_t *rank_bitmap; int *rank_tiles;     // first-touch ranking (default path): bitmap over kv*N + tile counts
+    uint32_t *slot;                             // table slots of the created outputs
+    uint32_t *rank_bitmap; int *rank_tiles;     // first-touch ranking: bitmap over kv*N + tile counts
     size_t rank_bytes; int64_t rank_ntiles;
     int *counter;
+    size_t bytes;                               // end of the carved layout
     RbLayout L;
 };
 
 // which table capacity stage 1 ended up with (the optimistic size, or the full one after an overflow);
 // stage 2 is called right after stage 1 on the same thread with the same workspace
-struct ConvStage1Record { const void *ws; uint32_t capacity; bool legacy; };
-thread_local ConvStage1Record g_stage1 = {nullptr, 0, false};
+struct ConvStage1Record { const void *ws; uint32_t capacity; };
+thread_local ConvStage1Record g_stage1 = {nullptr, 0};
 
 // Optimistic table size: the bound on the outputs (spx_conv_max_out, e.g. 8 N for 3^3 stride 2) is what
 // isolated points would produce; LiDAR-like clouds yield ~0.5 N.  A table for a quarter of the bound
@@ -1147,29 +1006,41 @@ uint32_t optimistic_capacity(int64_t max_out, uint32_t full_capacity) {
     uint32_t cap = table_capacity((max_out + 3) / 4, 2);
     return cap < full_capacity ? cap : full_capacity;
 }
+// The one definition of the regular-conv workspace layout: spx_rulebook_workspace_size carves it
+// dry (workspace NULL, bytes SIZE_MAX) and reads w.bytes.  rank_bitmap .. counter + 64 must stay
+// contiguous: conv_clear_kernel zeroes that range in one pass.
 int carve_conv_ws(const spx_conv_geometry *g, const Geom &gg, int64_t N, void *workspace, size_t bytes, ConvWs &w) {
     int64_t max_out = spx_conv_max_out(g, N);
     w.L = rb_layout(gg, max_out, gg.out_dims, 2);
     WorkspaceCarver ws(workspace, bytes);
     w.tbl = ws.take<char>(w.L.table_bytes);
     w.tvals = w.L.i64 ? ws.take<int32_t>(w.L.capacity) : nullptr;
-    w.payload = ws.take<uint32_t>(max_out);
     w.slot = ws.take<uint32_t>(max_out);
-    w.payload_sorted = ws.take<uint32_t>(max_out);
-    w.slot_sorted = ws.take<uint32_t>(max_out);
-    w.sort_tmp_bytes = sort_pairs_temp_bytes(max_out);
-    w.sort_tmp = ws.take<char>(w.sort_tmp_bytes);
-    w.order = ws.take<int32_t>(max_out);
-    w.radix_ws_bytes = radix_argsort_workspace_bytes(max_out);
-    w.radix_ws = ws.take<char>(w.radix_ws_bytes);
     w.rank_bytes = rank_scratch_bytes((int64_t)gg.kv * N, &w.rank_ntiles);
     w.rank_bitmap = (uint32_t *)ws.take<char>(w.rank_bytes);
     w.rank_tiles = (int *)(w.rank_bitmap + w.rank_ntiles * RANK_TILE_WORDS);
     w.counter = ws.take<int>(64);
+    w.bytes = ws.off;
     SPX_REQUIRE(ws.ok(), "rulebook workspace too small: need %zu, have %zu", ws.off, bytes);
     return 0;
 }
 }  // namespace
+
+extern "C" size_t spx_rulebook_workspace_size(const spx_conv_geometry *g, int64_t num_in, int64_t max_out, int is_subm) {
+    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
+    Geom gg = make_geom(g, is_subm != 0);
+    size_t total = 256;
+    if (is_subm) {
+        RbLayout L = rb_layout(gg, num_in, gg.in_dims);
+        total += align_up(L.table_bytes, 256) + align_up(L.table_vals_bytes, 256);
+    } else {
+        (void)max_out;                           // the bound is recomputed by both stages
+        ConvWs w;
+        carve_conv_ws(g, gg, num_in, nullptr, SIZE_MAX, w);
+        total += align_up(w.bytes, 256);
+    }
+    return total + 1024;
+}
 
 extern "C" int spx_conv_rulebook_stage1(const spx_conv_geometry *g, const int32_t *indices, int64_t N,
                                         int64_t *num_out_host, void *workspace, size_t workspace_bytes,
@@ -1190,87 +1061,50 @@ extern "C" int spx_conv_rulebook_stage1(const spx_conv_geometry *g, const int32_
     dim3 grid((unsigned)div_up64(N, T), gg.kv);
     const bool fast3 = gg.ndim == 3 && !gg.transposed;
     const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
-    const bool legacy = (runtime_cfg().debug & 128) != 0;
-    g_stage1 = {workspace, w.L.capacity, legacy};
-    if (!legacy) {
-        // ---- default path: optimistic table, append-on-create, own radix sort of the first-touch payloads
-        const int64_t max_out = spx_conv_max_out(g, N);
-        int host_state[2] = {0, 0};
-        uint32_t capacity = optimistic_capacity(max_out, w.L.capacity);
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            // ranking scratch and counters are contiguous (carve_conv_ws): one region of zeros
-            const int64_t zero_vec = (int64_t)(((char *)(w.counter + 64) - (char *)w.rank_bitmap) / 16);
-            conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)capacity / 2,
-                                                                  w.L.i64 ? (uint4 *)w.tvals : nullptr,
-                                                                  w.L.i64 ? (int64_t)capacity / 4 : 0,
-                                                                  (uint4 *)w.rank_bitmap, zero_vec);
-            SPX_CHECK_LAUNCH("conv_clear_kernel");
-            if (!w.L.i64) {
-                Table32 t{(unsigned long long *)w.tbl, capacity - 1};
-                if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-                else if (fast3) conv_insert_append_kernel<Table32, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-                else conv_insert_append_kernel<Table32, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            } else {
-                Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-                if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-                else if (fast3) conv_insert_append_kernel<Table64, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-                else conv_insert_append_kernel<Table64, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            }
-            SPX_CHECK_LAUNCH("conv_insert_append_kernel");
-            SPX_CHECK_CUDA(cudaMemcpyAsync(host_state, w.counter, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-            SPX_CHECK_CUDA(cudaStreamSynchronize(stream));
-            if (!host_state[1]) break;
-            SPX_REQUIRE(capacity < w.L.capacity, "conv rulebook: hash table overflow at full capacity (%u slots)", capacity);
-            capacity = w.L.capacity;                     // rare: far more outputs than the optimistic guess
-        }
-        g_stage1.capacity = capacity;
-        const int m_host = host_state[0];
-        *num_out_host = m_host;
-        if (m_host == 0) return 0;
-        const unsigned mblk = (unsigned)div_up64(m_host, MARK_THREADS);
+    g_stage1 = {workspace, w.L.capacity};
+    // optimistic table, append-on-create, outputs ranked by first touch without a sort
+    const int64_t max_out = spx_conv_max_out(g, N);
+    int host_state[2] = {0, 0};
+    uint32_t capacity = optimistic_capacity(max_out, w.L.capacity);
+    for (int attempt = 0; attempt < 2; ++attempt) {
+        // ranking scratch and counters are contiguous (carve_conv_ws): one region of zeros
+        const int64_t zero_vec = (int64_t)(((char *)(w.counter + 64) - (char *)w.rank_bitmap) / 16);
+        conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)capacity / 2,
+                                                              w.L.i64 ? (uint4 *)w.tvals : nullptr,
+                                                              w.L.i64 ? (int64_t)capacity / 4 : 0,
+                                                              (uint4 *)w.rank_bitmap, zero_vec);
+        SPX_CHECK_LAUNCH("conv_clear_kernel");
         if (!w.L.i64) {
             Table32 t{(unsigned long long *)w.tbl, capacity - 1};
-            conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
+            if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+            else if (fast3) conv_insert_append_kernel<Table32, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+            else conv_insert_append_kernel<Table32, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
         } else {
             Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-            conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
+            if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+            else if (fast3) conv_insert_append_kernel<Table64, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+            else conv_insert_append_kernel<Table64, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
         }
-        SPX_CHECK_LAUNCH("conv_mark_kernel");
-        return 0;
+        SPX_CHECK_LAUNCH("conv_insert_append_kernel");
+        SPX_CHECK_CUDA(cudaMemcpyAsync(host_state, w.counter, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+        SPX_CHECK_CUDA(cudaStreamSynchronize(stream));
+        if (!host_state[1]) break;
+        SPX_REQUIRE(capacity < w.L.capacity, "conv rulebook: hash table overflow at full capacity (%u slots)", capacity);
+        capacity = w.L.capacity;                     // rare: far more outputs than the optimistic guess
     }
-    SPX_CHECK_CUDA(cudaMemsetAsync(w.tbl, 0xFF, w.L.table_bytes, stream));
-    SPX_CHECK_CUDA(cudaMemsetAsync(w.counter, 0, sizeof(int), stream));
-    unsigned cblk = (unsigned)div_up64(w.L.capacity, COLLECT_THREADS * COLLECT_ITEMS);
-    if (!w.L.i64) {
-        Table32 t{(unsigned long long *)w.tbl, w.L.capacity - 1};
-        if (k3) conv_insert_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N);
-        else if (fast3) conv_insert_kernel<Table32, true><<<grid, T, 0, stream>>>(t, gg, indices, N);
-        else conv_insert_kernel<Table32, false><<<grid, T, 0, stream>>>(t, gg, indices, N);
-        SPX_CHECK_LAUNCH("conv_insert_kernel");
-        conv_collect_kernel<<<cblk, COLLECT_THREADS, 0, stream>>>(t, w.L.capacity, w.payload, w.slot, w.counter);
-        SPX_CHECK_LAUNCH("conv_collect_kernel");
-    } else {
-        SPX_CHECK_CUDA(cudaMemsetAsync(w.tvals, 0x7F, (size_t)w.L.capacity * 4, stream));
-        Table64 t{(long long *)w.tbl, w.tvals, w.L.capacity - 1};
-        if (k3) conv_insert_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N);
-        else if (fast3) conv_insert_kernel<Table64, true><<<grid, T, 0, stream>>>(t, gg, indices, N);
-        else conv_insert_kernel<Table64, false><<<grid, T, 0, stream>>>(t, gg, indices, N);
-        SPX_CHECK_LAUNCH("conv_insert_kernel");
-        conv_collect_kernel<<<cblk, COLLECT_THREADS, 0, stream>>>(t, w.L.capacity, w.payload, w.slot, w.counter);
-        SPX_CHECK_LAUNCH("conv_collect_kernel");
-    }
-    int m_host = 0;
-    SPX_CHECK_CUDA(cudaMemcpyAsync(&m_host, w.counter, sizeof(int), cudaMemcpyDeviceToHost, stream));
-    SPX_CHECK_CUDA(cudaStreamSynchronize(stream));
+    g_stage1.capacity = capacity;
+    const int m_host = host_state[0];
     *num_out_host = m_host;
     if (m_host == 0) return 0;
-    // rank outputs by first touch: sort (payload, slot) by payload; payload < kv*N
-    int end_bit = 1;
-    while (end_bit < 32 && ((int64_t)1 << end_bit) < (int64_t)gg.kv * N) ++end_bit;
-    size_t tmp_bytes = w.sort_tmp_bytes;
-    SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp_bytes, w.payload, w.payload_sorted, w.slot,
-                                                   w.slot_sorted, m_host, 0, end_bit, stream));
-    count_launch(3);
+    const unsigned mblk = (unsigned)div_up64(m_host, MARK_THREADS);
+    if (!w.L.i64) {
+        Table32 t{(unsigned long long *)w.tbl, capacity - 1};
+        conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
+    } else {
+        Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
+        conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
+    }
+    SPX_CHECK_LAUNCH("conv_mark_kernel");
     return 0;
 }
 
@@ -1292,25 +1126,21 @@ extern "C" int spx_conv_rulebook_stage2(const spx_conv_geometry *g, const int32_
     const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
     SPX_REQUIRE(g_stage1.ws == workspace && g_stage1.capacity != 0,
                 "conv_rulebook_stage2 must follow conv_rulebook_stage1 on the same thread with the same workspace");
-    const bool legacy = g_stage1.legacy;
-    if (legacy) SPX_CHECK_CUDA(cudaMemsetAsync(pair_fwd, 0xFF, (size_t)gg.kv * M * 4, stream));   // default: the assign kernel fills it
     const uint32_t capacity = g_stage1.capacity;
     // 3x3x3, one mask word: the pairs kernel ORs the forward masks too (zeroed by the assign kernel)
-    uint32_t *mask_fwd_or = (k3 && !legacy && mask_fwd && words == 1) ? mask_fwd : nullptr;
+    uint32_t *mask_fwd_or = (k3 && mask_fwd && words == 1) ? mask_fwd : nullptr;
     if (!w.L.i64) {
         Table32 t{(unsigned long long *)w.tbl, capacity - 1};
-        if (legacy) conv_assign_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot_sorted, nullptr, M, out_inds);
-        else conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
-        SPX_CHECK_LAUNCH("conv_assign_kernel");
+        conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
+        SPX_CHECK_LAUNCH("conv_assign_rank_kernel");
         if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
         else if (fast3) conv_pairs_kernel<Table32, true><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
         else conv_pairs_kernel<Table32, false><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
         SPX_CHECK_LAUNCH("conv_pairs_kernel");
     } else {
         Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-        if (legacy) conv_assign_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot_sorted, nullptr, M, out_inds);
-        else conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
-        SPX_CHECK_LAUNCH("conv_assign_kernel");
+        conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
+        SPX_CHECK_LAUNCH("conv_assign_rank_kernel");
         if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
         else if (fast3) conv_pairs_kernel<Table64, true><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
         else conv_pairs_kernel<Table64, false><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
@@ -1404,7 +1234,8 @@ extern "C" int spx_mask_argsort(uint32_t *mask, int32_t *argsort, int64_t N, int
     }
     SPX_REQUIRE(workspace != nullptr, "workspace is NULL");
     if (words == 1)   // hand-written 9-bit-digit stable radix argsort (sort.cu)
-        return radix_argsort(mask, argsort, N, kv > 0 && kv < 32 ? kv : 32, workspace, workspace_bytes, stream);
+        return radix_argsort_pair(mask, argsort, N, nullptr, nullptr, 0, kv > 0 && kv < 32 ? kv : 32, workspace,
+                                  workspace_bytes, nullptr, 0, stream);
     WorkspaceCarver ws(workspace, workspace_bytes);
     uint32_t *keys_in = ws.take<uint32_t>(N);
     uint32_t *keys_out = ws.take<uint32_t>(N);
@@ -1416,14 +1247,6 @@ extern "C" int spx_mask_argsort(uint32_t *mask, int32_t *argsort, int64_t N, int
     SPX_REQUIRE(ws.ok(), "argsort workspace too small: need %zu, have %zu", ws.off, workspace_bytes);
     iota_kernel<<<nblk, 256, 0, stream>>>(perm_a, N);
     SPX_CHECK_LAUNCH("iota_kernel");
-    if (words == 1) {
-        int end_bit = kv > 0 && kv < 32 ? kv : 32;
-        SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, (const uint32_t *)mask, keys_out,
-                                                       (const int32_t *)perm_a, argsort, (int)N, 0, end_bit, stream));
-        count_launch(3);
-        SPX_CHECK_CUDA(cudaMemcpyAsync(mask, keys_out, (size_t)N * 4, cudaMemcpyDeviceToDevice, stream));
-        return 0;
-    }
     // LSD over words: least significant word (last) first; stable sorts compose
     int32_t *cur = perm_a, *nxt = perm_b;
     for (int w = words - 1; w >= 0; --w) {
@@ -1572,8 +1395,8 @@ extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const in
     void *sort_ws = (char *)workspace + align_up(rb, 256);
     const size_t sort_bytes = workspace_bytes - align_up(rb, 256);
     if (int rc = spx_conv_rulebook_stage2(g, indices, N, M, out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, workspace, rb, stream)) return rc;
-    if (words == 1 && do_sort && argsort_bwd && !(runtime_cfg().debug & 2048)) {
-        // both mask sorts, then both tile tables, two jobs per launch (debug bit 2048: one after the other)
+    if (words == 1 && do_sort && argsort_bwd) {
+        // both mask sorts, then both tile tables, two jobs per launch
         const size_t half = (sort_bytes / 2) & ~(size_t)255;
         const int key_bits = kv < 32 ? kv : 32;
         if (int rc = radix_argsort_pair(mask_fwd, argsort_fwd, M, mask_bwd, argsort_bwd, N, key_bits, sort_ws, half,

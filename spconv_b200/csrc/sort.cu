@@ -15,16 +15,6 @@
 //             memory, then one global atomic per distinct (digit, block) cell.
 // The first pass reads the masks with an implicit iota payload, the last pass writes the sorted
 // masks back in place (thrust semantics) and the argsort.
-//
-// Experimental path ("onesweep", debug bit 64 of spx_debug_configure): ONE kernel per pass.  The digit totals of every pass do not depend on
-// the key order, so a single histogram kernel counts all passes up front; a pass kernel then needs
-// only the number of equal digits in the tiles BEFORE its own, which it gets by decoupled
-// look-back over per-tile status words {count | flag} (tile ids are drawn from an atomic ticket, so
-// every predecessor is already running and publishes its aggregate before it waits on anyone).
-// 1 + passes launches instead of 1 + 2 * passes -- but measured slower on an earlier GPU generation at
-// 100 k and 800 k keys (not re-measured on H100): the per-digit look-back is a chain
-// of dependent L2 round trips that costs more than the scan kernel + launch gap it replaces.  Kept
-// for A/B runs only; results are bit-identical.
 #include "common.cuh"
 
 namespace spx {
@@ -224,376 +214,11 @@ rs_scatter_kernel(const RsJobs jobs, int shift) {
     }
 }
 
-
-// ------------------------------------------------------------------ onesweep path
-constexpr uint32_t OS_FLAG_AGG = 1u << 30;      // status word = flag | value (value < 2^30)
-constexpr uint32_t OS_FLAG_PREFIX = 2u << 30;
-constexpr uint32_t OS_VALUE_MASK = (1u << 30) - 1u;
-constexpr int OS_MAX_PASSES = 4;
-
-// digit histograms of ALL passes in one sweep over the keys: hist[pass][digit]
-__global__ void __launch_bounds__(RS_THREADS)
-os_hist_kernel(const uint32_t *__restrict__ keys, int64_t n, int passes, int *__restrict__ hist) {
-    __shared__ int h[OS_MAX_PASSES][RS_BINS];
-    for (int i = threadIdx.x; i < OS_MAX_PASSES * RS_BINS; i += RS_THREADS) (&h[0][0])[i] = 0;
-    __syncthreads();
-    const int64_t base = (int64_t)blockIdx.x * RS_TILE;
-#pragma unroll
-    for (int j = 0; j < RS_ITEMS; ++j) {
-        const int64_t i = base + j * RS_THREADS + threadIdx.x;
-        if (i < n) {
-            const uint32_t k = keys[i];
-            for (int p = 0; p < passes; ++p) atomicAdd(&h[p][(k >> (p * RS_BITS)) & (RS_BINS - 1)], 1);
-        }
-    }
-    __syncthreads();
-    for (int i = threadIdx.x; i < passes * RS_BINS; i += RS_THREADS) {
-        const int v = (&h[0][0])[i];
-        if (v) atomicAdd(hist + i, v);
-    }
-}
-
-__device__ __forceinline__ uint32_t os_load_status(const uint32_t *p) {
-    return *reinterpret_cast<const volatile uint32_t *>(p);          // L2 (never a stale L1 line)
-}
-
-// One radix pass.  status: [tiles][RS_BINS] words, zero before the launch; ticket: one counter.
-template <bool IOTA_IN>
-__global__ void __launch_bounds__(RS_THREADS)
-os_pass_kernel(const uint32_t *__restrict__ keys_in, const int32_t *__restrict__ vals_in, int64_t n, int shift,
-               const int *__restrict__ hist, uint32_t *__restrict__ status, int *__restrict__ ticket,
-               uint32_t *__restrict__ keys_out, int32_t *__restrict__ vals_out) {
-    __shared__ int digit_base[RS_BINS];             // global start of each digit + keys of earlier tiles
-    __shared__ int warp_cnt[RS_WARPS][RS_BINS];
-    __shared__ int scan_tmp[RS_WARPS];
-    __shared__ int tile_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) tile_s = atomicAdd(ticket, 1);
-    for (int i = tid; i < RS_WARPS * RS_BINS; i += RS_THREADS) (&warp_cnt[0][0])[i] = 0;
-    // exclusive scan of the 512 digit totals (digit d = q * 256 + tid)
-    int my_total[RS_BINS / RS_THREADS];
-#pragma unroll
-    for (int q = 0; q < RS_BINS / RS_THREADS; ++q) my_total[q] = __ldg(hist + q * RS_THREADS + tid);
-    __syncthreads();
-    const int tile = tile_s;
-    int run = 0;
-#pragma unroll
-    for (int q = 0; q < RS_BINS / RS_THREADS; ++q) {
-        int v = my_total[q], incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            int t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        if (lane == 31) scan_tmp[warp] = incl;
-        __syncthreads();
-        int wbase = 0, all = 0;
-        for (int w = 0; w < RS_WARPS; ++w) { if (w < warp) wbase += scan_tmp[w]; all += scan_tmp[w]; }
-        digit_base[q * RS_THREADS + tid] = run + wbase + incl - v;
-        run += all;
-        __syncthreads();
-    }
-    // stable rank inside the tile: warp w owns keys [w*128, w*128+128), 4 rounds of 32
-    const int64_t tile_base = (int64_t)tile * RS_TILE + warp * (32 * RS_ITEMS);
-    uint32_t key[RS_ITEMS];
-    int32_t val[RS_ITEMS];
-    int rank[RS_ITEMS];
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const int64_t i = tile_base + r * 32 + lane;
-        const bool ok = i < n;
-        key[r] = ok ? keys_in[i] : 0xffffffffu;
-        val[r] = ok ? (IOTA_IN ? (int32_t)i : vals_in[i]) : -1;
-        const int d = ok ? (int)((key[r] >> shift) & (RS_BINS - 1)) : RS_BINS;
-        const unsigned peers = __match_any_sync(0xffffffffu, d);
-        const int leader = __ffs(peers) - 1;
-        int old = 0;
-        if (ok && lane == leader) { old = warp_cnt[warp][d]; warp_cnt[warp][d] = old + __popc(peers); }
-        old = __shfl_sync(0xffffffffu, old, leader);
-        rank[r] = old + __popc(peers & ((1u << lane) - 1u));
-        __syncwarp();
-    }
-    __syncthreads();
-    // per-digit: warp bases (exclusive over warps) and the tile's count, published at once for both
-    // digits of this thread (nobody must wait for a look-back of ours to see our aggregate) ...
-    int cnt[RS_BINS / RS_THREADS];
-#pragma unroll
-    for (int q = 0; q < RS_BINS / RS_THREADS; ++q) {
-        const int d = q * RS_THREADS + tid;
-        int acc = 0;
-#pragma unroll
-        for (int w = 0; w < RS_WARPS; ++w) { const int c = warp_cnt[w][d]; warp_cnt[w][d] = acc; acc += c; }
-        cnt[q] = acc;
-        atomicExch(status + (int64_t)tile * RS_BINS + d, (tile == 0 ? OS_FLAG_PREFIX : OS_FLAG_AGG) | (uint32_t)acc);
-    }
-    // ... then the look-back: sum the aggregates of the tiles before this one until a tile that
-    // already knows its inclusive prefix, and publish ours
-    if (tile > 0) {
-#pragma unroll
-        for (int q = 0; q < RS_BINS / RS_THREADS; ++q) {
-            const int d = q * RS_THREADS + tid;
-            uint32_t excl = 0;
-            for (int t = tile - 1; t >= 0; --t) {
-                const uint32_t *other = status + (int64_t)t * RS_BINS + d;
-                uint32_t w = os_load_status(other);
-                uint32_t spins = 0;
-                while ((w >> 30) == 0u) {
-                    if (++spins > (1u << 22)) {       // a protocol bug must become an error, not a hung GPU
-                        printf("spconv_b200: radix look-back timed out (tile %d digit %d waits on tile %d)\n", tile, d, t);
-                        __trap();
-                    }
-                    w = os_load_status(other);
-                }
-                excl += w & OS_VALUE_MASK;
-                if (w & OS_FLAG_PREFIX) break;
-            }
-            atomicExch(status + (int64_t)tile * RS_BINS + d, OS_FLAG_PREFIX | (excl + (uint32_t)cnt[q]));
-            digit_base[d] += (int)excl;
-        }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int r = 0; r < RS_ITEMS; ++r) {
-        const int64_t i = tile_base + r * 32 + lane;
-        if (i < n) {
-            const int d = (int)((key[r] >> shift) & (RS_BINS - 1));
-            const int pos = digit_base[d] + warp_cnt[warp][d] + rank[r];
-            keys_out[pos] = key[r];
-            vals_out[pos] = val[r];
-        }
-    }
-}
-
-// ------------------------------------------------------------------ cooperative single-kernel path
-// Experimental (debug bit 512 of spx_debug_configure): all passes in ONE cooperative launch, grid
-// barriers instead of kernel boundaries (6 dependent launches of ~4-6 us each are mostly launch /
-// drain latency at 1e5 keys).  Only when every tile's block is co-resident (n <= CS_MAX_BLOCKS tiles);
-// cudaLaunchCooperativeKernel guarantees the co-residency the barrier relies on.
-template <int IT> struct CsCfg { static constexpr int TILE = RS_THREADS * IT; };
-
-__device__ __forceinline__ void cs_grid_barrier(unsigned *bar, unsigned nblocks, unsigned &gen) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        const unsigned arrived = atomicAdd(&bar[0], 1u);
-        if (arrived == nblocks - 1u) {
-            bar[0] = 0u;
-            __threadfence();
-            atomicAdd(&bar[1], 1u);                            // release the generation
-        } else {
-            unsigned spins = 0;
-            while (*reinterpret_cast<volatile unsigned *>(&bar[1]) == gen) {
-                if (++spins > (1u << 24)) {                    // ~ seconds: a bug must not hang the GPU
-                    printf("spconv_b200: cooperative sort barrier timed out (block %d gen %u)\n", (int)blockIdx.x, gen);
-                    __trap();
-                }
-            }
-        }
-        __threadfence();
-    }
-    ++gen;
-    __syncthreads();
-}
-
-template <int IT>
-__global__ void __launch_bounds__(RS_THREADS)
-cs_sort_kernel(uint32_t *mask, int32_t *argsort, int64_t n, int passes, uint32_t *keys_a, int32_t *vals_a,
-               uint32_t *keys_b, int32_t *vals_b, int *counts, int *totals, unsigned *bar) {
-    constexpr int TILE = RS_THREADS * IT;
-    __shared__ int digit_base[RS_BINS];
-    __shared__ int warp_cnt[RS_WARPS][RS_BINS];
-    __shared__ int scan_tmp[RS_WARPS];
-    __shared__ unsigned gen_s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int blk = blockIdx.x, G = gridDim.x;
-    if (tid == 0) gen_s = *reinterpret_cast<volatile unsigned *>(&bar[1]);
-    __syncthreads();
-    unsigned gen = gen_s;
-    const int64_t tile_base = (int64_t)blk * TILE + warp * (32 * IT);
-    for (int pass = 0; pass < passes; ++pass) {
-        const int shift = pass * RS_BITS;
-        const bool last = pass == passes - 1;
-        const uint32_t *kin = pass == 0 ? mask : ((pass & 1) ? keys_a : keys_b);
-        const int32_t *vin = (pass & 1) ? vals_a : vals_b;
-        uint32_t *kout = last ? mask : ((pass & 1) ? keys_b : keys_a);
-        int32_t *vout = last ? argsort : ((pass & 1) ? vals_b : vals_a);
-        // ---- (1) keys of this tile, per-warp digit counts (= the stable rank bookkeeping), block histogram
-        for (int i = tid; i < RS_WARPS * RS_BINS; i += RS_THREADS) (&warp_cnt[0][0])[i] = 0;
-        __syncthreads();
-        uint32_t key[IT];
-        int32_t val[IT];
-        int rank[IT];
-#pragma unroll
-        for (int r = 0; r < IT; ++r) {
-            const int64_t i = tile_base + r * 32 + lane;
-            const bool ok = i < n;
-            key[r] = ok ? kin[i] : 0xffffffffu;
-            val[r] = ok ? (pass == 0 ? (int32_t)i : vin[i]) : -1;
-            const int d = ok ? (int)((key[r] >> shift) & (RS_BINS - 1)) : RS_BINS;
-            const unsigned peers = __match_any_sync(0xffffffffu, d);
-            const int leader = __ffs(peers) - 1;
-            int old = 0;
-            if (ok && lane == leader) { old = warp_cnt[warp][d]; warp_cnt[warp][d] = old + __popc(peers); }
-            old = __shfl_sync(0xffffffffu, old, leader);
-            rank[r] = old + __popc(peers & ((1u << lane) - 1u));
-            __syncwarp();
-        }
-        __syncthreads();
-        for (int d = tid; d < RS_BINS; d += RS_THREADS) {
-            int acc = 0;
-#pragma unroll
-            for (int w = 0; w < RS_WARPS; ++w) { const int c = warp_cnt[w][d]; warp_cnt[w][d] = acc; acc += c; }
-            counts[(int64_t)d * G + blk] = acc;                 // digit-major
-        }
-        cs_grid_barrier(bar, (unsigned)G, gen);
-        // ---- (2) exclusive prefix over the blocks, one warp per digit; digits dealt to (block, warp)
-        for (int d = blk * RS_WARPS + warp; d < RS_BINS; d += G * RS_WARPS) {
-            int carry = 0;
-            for (int b0 = 0; b0 < G; b0 += 32) {
-                const int b = b0 + lane;
-                const int v = b < G ? counts[(int64_t)d * G + b] : 0;
-                int incl = v;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int t = __shfl_up_sync(0xffffffffu, incl, o);
-                    if (lane >= o) incl += t;
-                }
-                if (b < G) counts[(int64_t)d * G + b] = carry + incl - v;
-                carry += __shfl_sync(0xffffffffu, incl, 31);
-            }
-            if (lane == 0) totals[d] = carry;
-        }
-        cs_grid_barrier(bar, (unsigned)G, gen);
-        // ---- (3) global digit starts (scan of the 512 totals) + this block's share, then scatter
-        int run = 0;
-#pragma unroll
-        for (int q = 0; q < RS_BINS / RS_THREADS; ++q) {
-            const int d = q * RS_THREADS + tid;
-            const int v = *reinterpret_cast<volatile int *>(&totals[d]);
-            int incl = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += t;
-            }
-            if (lane == 31) scan_tmp[warp] = incl;
-            __syncthreads();
-            int wbase = 0, all = 0;
-            for (int w = 0; w < RS_WARPS; ++w) { if (w < warp) wbase += scan_tmp[w]; all += scan_tmp[w]; }
-            digit_base[d] = run + wbase + incl - v + *reinterpret_cast<volatile int *>(&counts[(int64_t)d * G + blk]);
-            run += all;
-            __syncthreads();
-        }
-#pragma unroll
-        for (int r = 0; r < IT; ++r) {
-            const int64_t i = tile_base + r * 32 + lane;
-            if (i < n) {
-                const int d = (int)((key[r] >> shift) & (RS_BINS - 1));
-                const int pos = digit_base[d] + warp_cnt[warp][d] + rank[r];
-                kout[pos] = key[r];
-                vout[pos] = val[r];
-            }
-        }
-        if (!last) cs_grid_barrier(bar, (unsigned)G, gen);
-    }
-}
-
-// blocks of cs_sort_kernel that can be co-resident on the current device (cached per device)
-template <int IT>
-static int cs_max_blocks() {
-    static int cached[64] = {0};
-    const int dev = current_device() & 63;
-    if (!cached[dev]) {
-        int per_sm = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cs_sort_kernel<IT>, RS_THREADS, 0) != cudaSuccess) per_sm = 0;
-        cached[dev] = per_sm > 0 ? sm_count() : -1;            // one block per SM is all the sort needs
-    }
-    return cached[dev] > 0 ? cached[dev] : 0;
-}
-
-template <int IT>
-static int cs_launch(uint32_t *mask, int32_t *argsort, int64_t n, int passes, uint32_t *keys_a, int32_t *vals_a,
-                     uint32_t *keys_b, int32_t *vals_b, int *counts, int *totals, unsigned *bar, cudaStream_t stream) {
-    const int G = (int)div_up64(n, RS_THREADS * IT);
-    void *args[] = {&mask, &argsort, &n, &passes, &keys_a, &vals_a, &keys_b, &vals_b, &counts, &totals, &bar};
-    SPX_CHECK_CUDA(cudaLaunchCooperativeKernel((const void *)cs_sort_kernel<IT>, dim3(G), dim3(RS_THREADS), args, 0, stream));
-    count_launch();
-    return 0;
-}
-
 size_t radix_argsort_workspace_bytes(int64_t n) {
     const int64_t nblk = div_up64(n > 0 ? n : 1, RS_TILE);
-    // legacy path: 2 count matrices + totals; onesweep: hist + tickets + per-pass status words (they share)
-    const size_t legacy = 2 * align_up((size_t)RS_BINS * nblk * 4, 256) + align_up(RS_BINS * 4, 256);
-    const size_t sweep = align_up((size_t)(OS_MAX_PASSES * RS_BINS + 64) * 4, 256) +
-                         align_up((size_t)OS_MAX_PASSES * nblk * RS_BINS * 4, 256);
-    return 4 * align_up((size_t)n * 4, 256) + (legacy > sweep ? legacy : sweep) + 1024;
-}
-
-int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
-                       int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
-
-// keys: mask [n] (sorted in place on return), argsort [n] out.  Returns 0 / error code.
-int radix_argsort(uint32_t *mask, int32_t *argsort, int64_t n, int key_bits, void *workspace, size_t workspace_bytes,
-                  cudaStream_t stream) {
-    if (n == 0) return 0;
-    WorkspaceCarver ws(workspace, workspace_bytes);
-    uint32_t *keys_a = ws.take<uint32_t>(n);
-    int32_t *vals_a = ws.take<int32_t>(n);
-    uint32_t *keys_b = ws.take<uint32_t>(n);
-    int32_t *vals_b = ws.take<int32_t>(n);
-    const int nblk = (int)div_up64(n, RS_TILE);
-    if (key_bits < 1) key_bits = 1;
-    if (key_bits > 32) key_bits = 32;
-    const int passes = (key_bits + RS_BITS - 1) / RS_BITS;
-    const uint32_t *kin = mask;
-    const int32_t *vin = nullptr;
-    if ((runtime_cfg().debug & 512) && passes >= 2) {
-        // ---- cooperative: one launch for all passes when every tile's block can be co-resident
-        const int it = div_up64(n, RS_THREADS * 4) <= cs_max_blocks<4>() ? 4
-                     : (div_up64(n, RS_THREADS * 8) <= cs_max_blocks<8>() ? 8 : 0);
-        if (it) {
-            const int G = (int)div_up64(n, RS_THREADS * it);
-            int *counts = ws.take<int>((size_t)RS_BINS * G);
-            int *totals = ws.take<int>(RS_BINS);
-            unsigned *bar = ws.take<unsigned>(64);
-            SPX_REQUIRE(ws.ok(), "argsort workspace too small: need %zu, have %zu", ws.off, workspace_bytes);
-            SPX_CHECK_CUDA(cudaMemsetAsync(bar, 0, 64 * sizeof(unsigned), stream));
-            return it == 4 ? cs_launch<4>(mask, argsort, n, passes, keys_a, vals_a, keys_b, vals_b, counts, totals, bar, stream)
-                           : cs_launch<8>(mask, argsort, n, passes, keys_a, vals_a, keys_b, vals_b, counts, totals, bar, stream);
-        }
-    }
-    if (runtime_cfg().debug & 64) {
-        // ---- onesweep: memset(scratch) + histogram of all passes + one kernel per pass
-        const size_t head_ints = (size_t)OS_MAX_PASSES * RS_BINS + 64;        // hist[4][512] + tickets
-        int *head = ws.take<int>(head_ints);
-        uint32_t *status = ws.take<uint32_t>((size_t)passes * nblk * RS_BINS);
-        SPX_REQUIRE(ws.ok(), "argsort workspace too small: need %zu, have %zu", ws.off, workspace_bytes);
-        const size_t clear_bytes = (size_t)((char *)(status + (size_t)passes * nblk * RS_BINS) - (char *)head);
-        SPX_CHECK_CUDA(cudaMemsetAsync(head, 0, clear_bytes, stream));
-        int *hist = head, *tickets = head + OS_MAX_PASSES * RS_BINS;
-        os_hist_kernel<<<nblk, RS_THREADS, 0, stream>>>(kin, n, passes, hist);
-        SPX_CHECK_LAUNCH("os_hist_kernel");
-        for (int pass = 0; pass < passes; ++pass) {
-            const bool last = pass == passes - 1;
-            uint32_t *kout = (pass & 1) ? keys_b : keys_a;
-            int32_t *vout = (pass & 1) ? vals_b : vals_a;
-            if (last && pass > 0) { kout = mask; vout = argsort; }
-            uint32_t *st = status + (size_t)pass * nblk * RS_BINS;
-            if (pass == 0)
-                os_pass_kernel<true><<<nblk, RS_THREADS, 0, stream>>>(kin, vin, n, pass * RS_BITS, hist + pass * RS_BINS, st, tickets + pass, kout, vout);
-            else
-                os_pass_kernel<false><<<nblk, RS_THREADS, 0, stream>>>(kin, vin, n, pass * RS_BITS, hist + pass * RS_BINS, st, tickets + pass, kout, vout);
-            SPX_CHECK_LAUNCH("os_pass_kernel");
-            kin = kout; vin = vout;
-        }
-        if (passes == 1) {
-            SPX_CHECK_CUDA(cudaMemcpyAsync(mask, keys_a, (size_t)n * 4, cudaMemcpyDeviceToDevice, stream));
-            SPX_CHECK_CUDA(cudaMemcpyAsync(argsort, vals_a, (size_t)n * 4, cudaMemcpyDeviceToDevice, stream));
-        }
-        return 0;
-    }
-    return radix_argsort_pair(mask, argsort, n, nullptr, nullptr, 0, key_bits, workspace, workspace_bytes, nullptr, 0, stream);
+    // the layout of rs_carve: keys / values double buffers, 2 count matrices, digit totals
+    return 4 * align_up((size_t)n * 4, 256) + 2 * align_up((size_t)RS_BINS * nblk * 4, 256) +
+           align_up(RS_BINS * 4, 256) + 1024;
 }
 
 namespace {

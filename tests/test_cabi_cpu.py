@@ -75,6 +75,24 @@ def test_argument_validation_reports_errors(lib):
         _cabi.check(2, "x")
 
 
+def test_debug_configure_accepts_only_the_tf32_switches(lib):
+    """spx_debug_configure takes debug bits 256 and 4096 only: any other bit, and any trace buffer, is
+    refused before a CUDA call, so an A/B run of a path the library no longer has fails loudly"""
+    import ctypes
+    from spconv_b200 import _cabi
+    try:
+        for bits in (1, 2, 4, 8, 16, 64, 128, 512, 1024, 2048, 8192, 16384, 256 | 64):
+            assert lib.spx_debug_configure(-1, 0, bits, None, 0) == 2, bits
+            msg = _cabi.last_error()
+            assert "debug_bits" in msg and "256" in msg and "4096" in msg, msg
+        for bits in (256, 4096, 256 | 4096, 0):
+            assert lib.spx_debug_configure(-1, 0, bits, None, 0) == 0, bits
+        assert lib.spx_debug_configure(-1, 0, 0, ctypes.c_void_p(1 << 20), 8 * 2048 * 8) == 2
+        assert "trace buffer" in _cabi.last_error()
+    finally:
+        _cabi.check(lib.spx_debug_configure(-1, 0, 0, None, 0), "debug_configure")
+
+
 def test_tile_table_elems_formula_matches_the_library():
     """ops._tile_tables sizes the table buffer without a native call; the formula must stay equal to
     spx_tile_table_elems (layout documented in include/spconv_b200.h)"""
