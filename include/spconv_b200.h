@@ -29,6 +29,8 @@
  *           maxpool_implicit_gemm_backward / avgpool_implicit_gemm_forward / _backward /
  *           global_pool_rearrange                    spconv/csrc/sparse/all.py:664-905
  *           (kernels spconv/csrc/sparse/maxpool.py:41-341)
+ *   spx_sparse_add_group / _fwd / _gather (+ spx_conv_rulebook_stage1+2 for the union)
+ *        <- functional.sparse_add / sparse_add_hash_based spconv/pytorch/functional.py:441-544
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless the name ends in `_host`;
@@ -371,6 +373,39 @@ int spx_indice_pool_bwd(int mode, const void *features, const void *out_features
  */
 int spx_global_pool_rearrange(const int32_t *coords, int64_t n, int row_ints, int batch_size,
                               int32_t *out_indices, int32_t *counts, spx_stream_t stream);
+
+/* ------------------------------------------------------------------ sum over different coordinates */
+
+/*
+ * Replaces spconv.pytorch.functional.sparse_add / sparse_add_hash_based (spconv/pytorch/functional.py:441-544).
+ * The operands are concatenated in VISIT order (the caller's choice; sparse_add visits the largest operand
+ * first); row g of the concatenation is row g - start[t] of operand t.  The union of their coordinates is
+ * the regular-conv rulebook of a 1x..x1 stride-1 convolution over the concatenated coordinates: stage 1/2
+ * give out_inds [M] and dst = pair_bwd[0] [rows] (output row of every visited row, -1 = out of range).
+ *
+ * group:  order [rows] = stable argsort of dst (rows with dst = -1 last), offsets [M + 1]: the visited rows of
+ *         output o are order[offsets[o] .. offsets[o+1]) in ascending visit order.  dst must come from
+ *         the union above (M = its output count).
+ * fwd:    out [M, channels] = per output, the fp32 sum of its rows in visit order, rounded once.
+ * gather: for every visited row g with grads[t] != NULL: grads[t][g - start[t]] = index[g] >= 0 ?
+ *         src[index[g]] : 0 (bit copy), index [rows], src [src_rows, channels].
+ * dtype: f32 / f16 / bf16.  Any channel count >= 1 (16-byte vectors when rows and pointers allow them).
+ */
+#define SPX_SPARSE_ADD_MAX_OPERANDS 64
+typedef struct {
+    int count;                                              /* 1 .. SPX_SPARSE_ADD_MAX_OPERANDS */
+    int64_t rows[SPX_SPARSE_ADD_MAX_OPERANDS];              /* rows of every operand, in visit order */
+    const void *features[SPX_SPARSE_ADD_MAX_OPERANDS];      /* [rows[t], channels], read by fwd */
+    void *grads[SPX_SPARSE_ADD_MAX_OPERANDS];               /* [rows[t], channels], written by gather (NULL = skip) */
+} spx_sparse_add_operands;
+
+size_t spx_sparse_add_group_workspace_size(int64_t rows);
+int spx_sparse_add_group(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets,
+                         void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const int32_t *order, const int32_t *offsets,
+                       int64_t M, int channels, int dtype, void *out, spx_stream_t stream);
+int spx_sparse_add_gather(const int32_t *index, const void *src, int64_t src_rows,
+                          const spx_sparse_add_operands *operands, int channels, int dtype, spx_stream_t stream);
 
 /*
  * int8 inference forward (reference formula: test/test_all_algo.py:272-287,

@@ -53,6 +53,19 @@ class PeerGroup(Structure):
     ]
 
 
+SPX_SPARSE_ADD_MAX_OPERANDS = 64
+
+
+class SparseAddOperands(Structure):
+    """``spx_sparse_add_operands``: the operands of a sparse add in visit order."""
+    _fields_ = [
+        ("count", c_int),
+        ("rows", c_int64 * SPX_SPARSE_ADD_MAX_OPERANDS),
+        ("features", c_void_p * SPX_SPARSE_ADD_MAX_OPERANDS),
+        ("grads", c_void_p * SPX_SPARSE_ADD_MAX_OPERANDS),
+    ]
+
+
 # name -> (restype, argtypes); also the list the CPU test checks against the header
 SIGNATURES = {
     "spx_last_error": (c_char_p, []),
@@ -123,6 +136,12 @@ SIGNATURES = {
     "spx_indice_pool_bwd": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                     c_int64, c_int, c_int, c_void_p, c_void_p]),
     "spx_global_pool_rearrange": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "spx_sparse_add_group_workspace_size": (c_size_t, [c_int64]),
+    "spx_sparse_add_group": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_sparse_add_fwd": (c_int, [POINTER(SparseAddOperands), c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p,
+                                   c_void_p]),
+    "spx_sparse_add_gather": (c_int, [c_void_p, c_void_p, c_int64, POINTER(SparseAddOperands), c_int, c_int,
+                                      c_void_p]),
     "spx_last_kernel_family": (c_int, []),
     "spx_launch_count": (c_int64, [c_int]),
     "spx_debug_configure": (c_int, [c_int, c_int, c_int, c_void_p, c_size_t]),

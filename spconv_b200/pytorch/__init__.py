@@ -6,12 +6,14 @@ from .conv import (SparseConv1d, SparseConv2d, SparseConv3d, SparseConv4d,  # no
                    SparseConvTranspose3d, SparseConvTranspose4d, SparseInverseConv1d,
                    SparseInverseConv2d, SparseInverseConv3d, SparseInverseConv4d, SubMConv1d,
                    SubMConv2d, SubMConv3d, SubMConv4d)
+from .identity import Identity  # noqa: F401
 from .core import (CUDAKernelTimer, ImplicitGemmIndiceData, IndiceData,  # noqa: F401
                    SparseConvTensor, scatter_nd)
 from .modules import (RemoveGrid, SparseBatchNorm, SparseIdentity, SparseModule,  # noqa: F401
                       SparseReLU, SparseSequential, ToDense, assign_name_for_sparse_modules)
 from .pool import (SparseAvgPool1d, SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool,  # noqa: F401
                    SparseGlobalMaxPool, SparseMaxPool1d, SparseMaxPool2d, SparseMaxPool3d, SparseMaxPool4d)
+from .tables import AddTable, ConcatTable, JoinTable  # noqa: F401
 from .utils_fuse import (fuse_act, fuse_bn, fuse_bn_act_sequential, fuse_bn_weights)  # noqa: F401
 from . import quantized  # noqa: F401
 from .graph import GraphedStep, graph_capture  # noqa: F401

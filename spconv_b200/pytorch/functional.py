@@ -8,6 +8,7 @@ reference classes at ``functional.py:59-189,293-357``).
 """
 from __future__ import annotations
 
+import functools
 import sys
 from typing import List, Optional
 
@@ -18,7 +19,7 @@ from torch.autograd.function import once_differentiable
 
 from ..core import Activation
 from . import ops
-from .core import CUDAKernelTimer
+from .core import CUDAKernelTimer, SparseConvTensor
 
 # AMP: inputs are cast to fp16 inside autocast regions, like the reference (functional.py:44-56)
 _amp_fwd = torch.amp.custom_fwd(cast_inputs=torch.float16, device_type="cuda")
@@ -213,3 +214,111 @@ implicit_gemm = SparseImplicitGemmFunction.apply
 indice_maxpool = SparseMaxPoolFunction.apply
 indice_maxpool_implicit_gemm = SparseMaxPoolImplicitGemmFunction.apply
 indice_avgpool_implicit_gemm = SparseAvgPoolImplicitGemmFunction.apply
+
+
+# ---------------------------------------------------------------------------- sparse add
+class SparseAddFunction(Function):
+    """``dst, order, offsets, m, *features`` (operands in visit order) -> their sum over the union of the
+    coordinates (:func:`ops.sparse_add_forward`); the gradient of operand row ``g`` is ``dout[dst[g]]``, or 0
+    for a dropped row, and is computed only for the operands that need it."""
+
+    @staticmethod
+    def forward(ctx, dst, order, offsets, m, *features):
+        ctx.save_for_backward(dst)
+        ctx.rows = [f.shape[0] for f in features]
+        return ops.sparse_add_forward(features, order, offsets, m)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        dst, = ctx.saved_tensors
+        grads = ops.sparse_add_gather(dst, grad_output, ctx.rows, ctx.needs_input_grad[4:])
+        return (None, None, None, None, *grads)
+
+
+def _sparse_add(tens) -> SparseConvTensor:
+    assert len(tens) >= 1, "sparse_add needs at least one operand"
+    first = tens[0]
+    largest = 0
+    for i, ten in enumerate(tens):
+        assert ten.spatial_shape == first.spatial_shape
+        assert ten.batch_size == first.batch_size
+        assert ten.features.shape[1] == first.features.shape[1]
+        ops._sparse_add_dtype(ten.features.dtype)
+        if ten.features.shape[0] > tens[largest].features.shape[0]:     # ties: the earliest operand
+            largest = i
+    dtype = functools.reduce(torch.promote_types, [t.features.dtype for t in tens])
+    visit = [largest] + [i for i in range(len(tens)) if i != largest]
+    out_inds, dst = ops.sparse_add_union([tens[i].indices for i in visit], first.batch_size, first.spatial_shape)
+    m = out_inds.shape[0]
+    order, offsets = ops.sparse_add_group(dst, m)
+    feats = [tens[i].features if tens[i].features.dtype == dtype else tens[i].features.to(dtype) for i in visit]
+    res = SparseConvTensor(SparseAddFunction.apply(dst, order, offsets, m, *feats), out_inds, first.spatial_shape,
+                           first.batch_size, benchmark=first.benchmark)
+    # The largest operand is visited first, so its rows are output rows 0, 1, .. in order exactly when they
+    # are all distinct and in range, i.e. when its last row is output row N - 1.  Only then do the output
+    # coordinates equal its coordinates row for row and its rulebooks stay valid (a second host sync).
+    n_l = tens[largest].features.shape[0]
+    if m == n_l and (n_l == 0 or int(dst[n_l - 1]) == n_l - 1):
+        res.indice_dict = tens[largest].indice_dict
+    res.benchmark_record = first.benchmark_record
+    res._timer = first._timer
+    res.thrust_allocator = first.thrust_allocator
+    return res
+
+
+def sparse_add(*tens: SparseConvTensor) -> SparseConvTensor:
+    """Sum of sparse tensors with the same shape, batch size and channels but different coordinates
+    (``spconv/pytorch/functional.py:517-544``).
+
+    Every distinct in-range coordinate appears once in the result.  Rows are in first-touch order: the
+    largest operand (ties: the earliest) is visited first, then the others in argument order, each row by
+    row, and an output row's rank is that of the first visited row carrying its coordinate.  Each output
+    row is the sum of every row with its coordinate, duplicates within one operand included, accumulated in
+    fp32 in visit order and rounded once: the result is bit-reproducible.  Rows whose batch index or
+    coordinate is out of range are dropped and get a zero gradient.  Operands of different dtypes are
+    promoted as ``+`` would.  The largest operand's ``indice_dict`` is kept exactly when the result's
+    coordinates equal its coordinates row for row, so a following ``SparseInverseConv`` on one of its keys
+    gathers the right rows.
+
+    Differences from the reference: the reference orders rows by ``torch.sparse`` coalesce (sorted linear
+    index), which is not the row order of the operand whose ``indice_dict`` it keeps; here the order above
+    makes that documented usage correct.  Host syncs: one for the output count, plus one 4-byte read when
+    the output count equals the largest operand's row count (to decide on ``indice_dict``)."""
+    return _sparse_add(tens)
+
+
+def sparse_add_hash_based(*tens: SparseConvTensor) -> SparseConvTensor:
+    """The same result as :func:`sparse_add` (``spconv/pytorch/functional.py:441-514``).  Unlike the
+    reference, whose ``index_put`` keeps one arbitrary row of duplicate coordinates within one operand, every
+    such row is summed, and rows come in first-touch order rather than hash-slot order."""
+    return _sparse_add(tens)
+
+
+class _RowGather(Function):
+    """``out[o] = features[heads[o]]``; gradient ``din[i] = dout[inverse[i]]`` (0 where ``inverse[i] < 0``)."""
+
+    @staticmethod
+    def forward(ctx, features, heads, inverse):
+        ctx.save_for_backward(inverse)
+        return ops.sparse_add_gather(heads, features, [heads.shape[0]])[0]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        inverse, = ctx.saved_tensors
+        return ops.sparse_add_gather(inverse, grad_output, [inverse.shape[0]])[0], None, None
+
+
+def remove_duplicate(x: SparseConvTensor) -> SparseConvTensor:
+    """Keep the first row of every coordinate (rows in first-touch order) and drop rows whose batch index or
+    coordinate is out of range; see :class:`spconv_b200.pytorch.spatial.RemoveDuplicate`."""
+    ops._sparse_add_dtype(x.features.dtype)
+    out_inds, dst = ops.sparse_add_union([x.indices], x.batch_size, x.spatial_shape)
+    m = out_inds.shape[0]
+    order, offsets = ops.sparse_add_group(dst, m)
+    heads = order[offsets[:m].long()]
+    inverse = torch.full_like(dst, -1)
+    inverse[heads.long()] = torch.arange(m, dtype=torch.int32, device=dst.device)
+    feats = _RowGather.apply(x.features, heads, inverse)
+    return SparseConvTensor(feats, out_inds, x.spatial_shape, x.batch_size, x.grid)

@@ -73,7 +73,8 @@ class SparseSequential(SparseModule):
         x = input
         for layer in self._modules.values():
             if isinstance(layer, SparseModule):
-                assert isinstance(x, SparseConvTensor)
+                # a list comes out of ConcatTable and goes into AddTable / JoinTable (modules.py:133-134)
+                assert isinstance(x, (SparseConvTensor, list))
                 x = layer(x)
             elif isinstance(x, SparseConvTensor):
                 # dense layers (BatchNorm1d, ReLU, ...) act on the feature matrix

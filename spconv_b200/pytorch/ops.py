@@ -941,6 +941,115 @@ def global_pool_rearrange(coords: torch.Tensor, batch_size: int):
     return out_indices, counts
 
 
+# ---------------------------------------------------------------------------- sparse add
+_SPARSE_ADD_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def sparse_add_union(indices: Sequence[torch.Tensor], batch_size: int, spatial_shape: List[int]):
+    """Union of coordinate sets visited in the given order -> ``(out_inds [M, ndim+1], dst [sum N])``.
+
+    ``out_inds`` holds every distinct in-range coordinate once, ranked by the first visited row that carries
+    it; ``dst[g]`` is the output row of visited row ``g`` (-1: batch index or coordinate out of range).  This is
+    the regular-conv rulebook of a 1x..x1, stride-1, padding-0 convolution over the concatenated coordinates
+    (``dst`` is its ``pair_bwd[0]``).  One host sync (the output count).  An empty union returns 0 rows."""
+    for ind in indices:
+        _require_cuda(ind, "indices")
+    dev = indices[0].device
+    ndim = len(spatial_shape)
+    cat = torch.cat([i.to(torch.int32).reshape(-1, ndim + 1) for i in indices], 0).contiguous()
+    n = cat.shape[0]
+    if n == 0:
+        return torch.empty((0, ndim + 1), dtype=torch.int32, device=dev), torch.empty((0,), dtype=torch.int32, device=dev)
+    ones, zeros = [1] * ndim, [0] * ndim
+    geo = _geometry(cat, batch_size, spatial_shape, spatial_shape, ones, ones, zeros, ones, False)
+    lib = _lib()
+    ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n, 0, 0), dev)
+    m_host = ctypes.c_int64(0)
+    _cabi.check(lib.spx_conv_rulebook_stage1(ctypes.byref(geo), cat.data_ptr(), n, ctypes.byref(m_host),
+                                             ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_stage1(sparse_add)")
+    m = int(m_host.value)
+    out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
+    dst = torch.empty((n,), dtype=torch.int32, device=dev)
+    if m == 0:
+        return out_inds, dst.fill_(-1)
+    pair_fwd = torch.empty((1, m), dtype=torch.int32, device=dev)        # written by stage 2, not read
+    _cabi.check(lib.spx_conv_rulebook_stage2(ctypes.byref(geo), cat.data_ptr(), n, m, out_inds.data_ptr(),
+                                             pair_fwd.data_ptr(), dst.data_ptr(), None, None, ws.data_ptr(),
+                                             ws.numel(), _stream()), "conv_rulebook_stage2(sparse_add)")
+    return out_inds, dst
+
+
+def sparse_add_group(dst: torch.Tensor, m: int):
+    """``(order [N], offsets [M+1])``: the visited rows of output ``o`` are ``order[offsets[o]:offsets[o+1]]``,
+    ascending; ``order[offsets[o]]`` is the row that created ``o``.  Dropped rows sort last."""
+    lib = _lib()
+    n = dst.shape[0]
+    order = torch.empty((n,), dtype=torch.int32, device=dst.device)
+    offsets = torch.empty((int(m) + 1,), dtype=torch.int32, device=dst.device)
+    ws = _bytes(lib.spx_sparse_add_group_workspace_size(n), dst.device)
+    _cabi.check(lib.spx_sparse_add_group(_ptr(dst), n, int(m), _ptr(order), offsets.data_ptr(), ws.data_ptr(),
+                                         ws.numel(), _stream()), "sparse_add_group")
+    return order, offsets
+
+
+def _sparse_add_operands(rows: Sequence[int], features=None, grads=None) -> "_cabi.SparseAddOperands":
+    if len(rows) > _cabi.SPX_SPARSE_ADD_MAX_OPERANDS:
+        raise ValueError(f"sparse_add supports at most {_cabi.SPX_SPARSE_ADD_MAX_OPERANDS} operands, got {len(rows)}")
+    ops = _cabi.SparseAddOperands()
+    ops.count = len(rows)
+    for t, r in enumerate(rows):
+        ops.rows[t] = int(r)
+        ops.features[t] = _ptr(features[t]) if features is not None else None
+        ops.grads[t] = _ptr(grads[t]) if grads is not None else None
+    return ops
+
+
+def _sparse_add_dtype(dtype: torch.dtype) -> int:
+    if dtype not in _SPARSE_ADD_DTYPES:
+        raise RuntimeError(f"sparse_add supports float32, float16 and bfloat16 features, got {dtype}")
+    return _DTYPE_CODE[dtype]
+
+
+def sparse_add_forward(features: Sequence[torch.Tensor], order: torch.Tensor, offsets: torch.Tensor,
+                       m: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out [M, C]``: per output row the fp32 sum of its visited rows in visit order, rounded once.
+    ``features`` are the operands in visit order, all of one dtype; ``out`` (optional) is written in place."""
+    for f in features:
+        _require_cuda(f, "features")
+    features = [f.contiguous() for f in features]
+    c = features[0].shape[1]
+    code = _sparse_add_dtype(features[0].dtype)
+    if out is None:
+        out = torch.empty((int(m), c), dtype=features[0].dtype, device=features[0].device)
+    assert out.shape == (int(m), c) and out.dtype == features[0].dtype and out.is_contiguous()
+    ops = _sparse_add_operands([f.shape[0] for f in features], features=features)
+    _cabi.check(_lib().spx_sparse_add_fwd(ctypes.byref(ops), _ptr(order), _ptr(offsets), int(m), int(c), code,
+                                          _ptr(out), _stream()), "sparse_add_fwd")
+    return out
+
+
+def sparse_add_gather(index: torch.Tensor, src: torch.Tensor, rows: Sequence[int],
+                      needed: Optional[Sequence[bool]] = None,
+                      outs: Optional[Sequence[torch.Tensor]] = None) -> List[Optional[torch.Tensor]]:
+    """Row ``g`` of the concatenation of the returned blocks is ``src[index[g]]``, or zero where ``index[g] < 0``
+    (the backward pass of :func:`sparse_add_forward` with ``index = dst``).  Blocks with ``needed[t]`` false
+    are not computed and come back as None; ``outs`` (optional) are written in place."""
+    _require_cuda(src, "src")
+    src = src.contiguous()
+    code = _sparse_add_dtype(src.dtype)
+    c = src.shape[1]
+    needed = [True] * len(rows) if needed is None else list(needed)
+    if outs is None:
+        outs = [torch.empty((int(r), c), dtype=src.dtype, device=src.device) if need else None
+                for r, need in zip(rows, needed)]
+    for o, r in zip(outs, rows):
+        assert o is None or (o.shape == (int(r), c) and o.dtype == src.dtype and o.is_contiguous())
+    ops = _sparse_add_operands(rows, grads=outs)
+    _cabi.check(_lib().spx_sparse_add_gather(_ptr(index), _ptr(src), int(src.shape[0]), ctypes.byref(ops), int(c),
+                                             code, _stream()), "sparse_add_gather")
+    return outs
+
+
 # ---------------------------------------------------------------------------- misc
 def bias_add_act_inplace(x: torch.Tensor, bias: Optional[torch.Tensor], act_type=Activation.None_,
                          act_alpha: float = 0.0, act_beta: float = 0.0) -> torch.Tensor:
