@@ -24,14 +24,19 @@ struct P2VGeom {
     int grid[SPX_MAX_NDIM];
 };
 
-// grid coordinate of a point on internal axis j: floor((p - lo) / vsize) in fp32, as the reference
+// grid coordinate of a point on internal axis j: floor((p - lo) / vsize) in fp32, as the reference.
+// The cell is range-checked as a float, before any conversion: NaN fails every comparison and inf /
+// huge values fail the upper bound, so a point with a non-finite coordinate makes no voxel (a float ->
+// int conversion of NaN is undefined and gives 0 on the GPU, which used to put such points in cell 0).
 __device__ __forceinline__ bool p2v_coord(const P2VGeom &g, const float *__restrict__ pt, int (&c)[SPX_MAX_NDIM]) {
 #pragma unroll
     for (int j = 0; j < SPX_MAX_NDIM; ++j) {
         if (j < g.ndim) {
             const float p = pt[g.zyx ? g.ndim - 1 - j : j];
-            const int v = (int)floorf(__fdiv_rn(p - g.lo[j], g.vsize[j]));
-            if (v < 0 || v >= g.grid[j]) return false;
+            const float f = floorf(__fdiv_rn(p - g.lo[j], g.vsize[j]));
+            if (!(f >= 0.f && f < 2147483648.f)) return false;
+            const int v = (int)f;
+            if (v >= g.grid[j]) return false;
             c[j] = v;
         }
     }

@@ -38,6 +38,8 @@ template <> __device__ __forceinline__ float lowest_of<__half>() { return -65504
 template <> __device__ __forceinline__ float lowest_of<__nv_bfloat16>() { return -3.3895313892515355e+38f; }
 template <> __device__ __forceinline__ float lowest_of<int8_t>() { return -128.f; }
 
+// Max: a candidate replaces the running max only when it is greater, as in the reference -- NaN never
+// wins, and of two equal values (-0 and +0) the first stays.
 // MODE 0: max, accumulator starts at lowest()   (maxpool.py:76-117)
 // MODE 1: max, accumulator starts at 0          (Native: the output buffer is zero-initialised and
 //                                                only raised, spconv/pytorch/ops.py:1910 + maxpool.py:63-66)
@@ -62,12 +64,13 @@ __global__ void pool_fwd_kernel(const T *__restrict__ x, T *__restrict__ out, co
         float f[N];
         load_vec(x + (int64_t)i * channels + ch * N, f);
 #pragma unroll
-        for (int j = 0; j < N; ++j) acc[j] = MODE == 2 ? acc[j] + f[j] : fmaxf(acc[j], f[j]);
+        for (int j = 0; j < N; ++j) acc[j] = MODE == 2 ? acc[j] + f[j] : (f[j] > acc[j] ? f[j] : acc[j]);
     }
     if (MODE == 2) {
-        const float inv = count > 0 ? 1.f / (float)count : 0.f;
+        // a division, as the reference (maxpool.py:255): acc * (1 / count) differs from it in the last
+        // bit for about a third of the sums at count 3
 #pragma unroll
-        for (int j = 0; j < N; ++j) acc[j] = count > 0 ? acc[j] * inv : 0.f;
+        for (int j = 0; j < N; ++j) acc[j] = count > 0 ? acc[j] / (float)count : 0.f;
         if (count_out && ch == 0) count_out[o] = count;
     }
     store_vec(out + o * channels + ch * N, acc);

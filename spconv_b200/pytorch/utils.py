@@ -4,7 +4,9 @@
 Unlike the reference's GPU generator (atomic appends: voxel order and the points kept per voxel
 depend on scheduling) the result is deterministic and equal to the reference's CPU generator
 (``Point2VoxelCPU``, ``spconv/csrc/sparse/pointops.py:589-695``): voxels are numbered by their first
-point, a voxel keeps its first ``max_num_points_per_voxel`` points, both in input order.
+point, a voxel keeps its first ``max_num_points_per_voxel`` points, both in input order.  A point is
+in a voxel when ``floor((p - lo) / vsize)`` (fp32) is a finite value in ``[0, grid)`` on every axis; a
+point with a NaN or infinite coordinate gets ``pc_voxel_id`` -1 and makes no voxel.
 """
 from __future__ import annotations
 
