@@ -99,17 +99,8 @@ int64_t spx_conv_max_out(const spx_conv_geometry *g, int64_t num_in);
  * `words` = ceil(kv/32).
  */
 int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N,
-                      int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask, int32_t *row_table,
-                      void *workspace, size_t workspace_bytes, spx_stream_t stream);
-
-/*
- * Optional by-product of spx_subm_rulebook: row_table [N][32] int32 (16-byte aligned), row o =
- * pair_fwd[0..kv-1][o] padded with -1 -- the forward table transposed to one 128-byte line per
- * voxel.  spx_build_tile_table re-reads the rulebook in mask_argsort order; from this copy that
- * costs 4 sectors per row instead of one per (row, offset).  Produced only for geometries where
- * this returns 1 (3-D 3x3x3 with 32-bit keys); pass NULL otherwise.
- */
-int spx_subm_row_table_supported(const spx_conv_geometry *g);
+                      int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask, void *workspace,
+                      size_t workspace_bytes, spx_stream_t stream);
 
 /*
  * Regular / transposed conv rulebook, two-phase because the output count M is
@@ -132,8 +123,11 @@ int spx_conv_rulebook_stage2(const spx_conv_geometry *g, const int32_t *indices,
  * spx_build_tile_table (resp. spx_conv_rulebook_stage2 + both argsorts + both tile tables), all
  * scratch carved from ONE workspace.  They exist because an eager Python caller pays ~10 us of
  * interpreter / ctypes / allocator time per separate call; results are identical.
- * `mask` is left sorted; tile_table / tile_mask (spx_tile_table_elems, tiles * words) may be NULL to
- * skip the tile table.  argsort_bwd / table_bwd may be NULL (inference: no backward direction).
+ * `mask` is left sorted; tile_table / tile_mask (spx_tile_table_elems, tiles * words) are required.
+ * argsort_bwd, table_bwd and tmask_bwd are all NULL (inference: no backward direction) or all given.
+ * For a 3-D 3x3x3 SubM with 32-bit keys spx_subm_rulebook_all also keeps a row-major copy of
+ * pair_fwd in its workspace (one 128-byte line per voxel), from which the tile table is built with
+ * 4 sectors per row instead of one per (row, offset).
  * spx_conv_rulebook_stage2_all continues a spx_conv_rulebook_stage1 that was given a workspace of
  * spx_conv_rulebook_all_workspace_size bytes.
  */
@@ -221,23 +215,17 @@ typedef struct {
  *             so up to 32 launches may be in flight on one table (other streams, graph branches).
  */
 size_t spx_tile_table_elems(int64_t rows, int kv);
-/*
- * row_table (optional, kv <= 32): the [rows][32] by-product of spx_subm_rulebook for the same
- * `pair`; when given, `pair` is not read.
- */
 int spx_build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, const int32_t *argsort,
-                         const uint32_t *mask, int64_t rows, const int32_t *row_table,
-                         int32_t *table, uint32_t *tile_mask, spx_stream_t stream);
+                         const uint32_t *mask, int64_t rows, int32_t *table, uint32_t *tile_mask,
+                         spx_stream_t stream);
 
 /*
  * out[o, :] = act( sum_k x[pair[k][o], :] @ W[:, k, :]^T  + bias )      rows = n_out
  * filters: KRSC [c_out, kv, c_in].  bias (same dtype as features) may be NULL.
- * mask_out [ceil(n_out/128), words] (may be NULL) receives the per-128-row-tile OR of `mask`
- * (the reference's mask_output_fwd, mask_width = 128).
  */
 int spx_implicit_gemm_fwd(const spx_gemm_desc *d, const void *features, const void *filters,
                           void *out, const void *bias, int act, float act_alpha,
-                          uint32_t *mask_out, spx_stream_t stream);
+                          spx_stream_t stream);
 
 /*
  * din[i, :] = sum_k dout[pair[k][i], :] @ W[:, k', :]        rows = n_in, k' = k or kv-1-k

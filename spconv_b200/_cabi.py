@@ -74,8 +74,7 @@ SIGNATURES = {
     "spx_rulebook_workspace_size": (c_size_t, [POINTER(ConvGeometry), c_int64, c_int64, c_int]),
     "spx_conv_max_out": (c_int64, [POINTER(ConvGeometry), c_int64]),
     "spx_subm_rulebook": (c_int, [POINTER(ConvGeometry), c_void_p, c_int64, c_void_p, c_void_p,
-                                  c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "spx_subm_row_table_supported": (c_int, [POINTER(ConvGeometry)]),
+                                  c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_conv_rulebook_stage1": (c_int, [POINTER(ConvGeometry), c_void_p, c_int64,
                                          POINTER(c_int64), c_void_p, c_size_t, c_void_p]),
     "spx_conv_rulebook_stage2": (c_int, [POINTER(ConvGeometry), c_void_p, c_int64, c_int64,
@@ -97,10 +96,10 @@ SIGNATURES = {
     "spx_mask_argsort": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_void_p,
                                  c_size_t, c_void_p]),
     "spx_tile_table_elems": (c_size_t, [c_int64, c_int]),
-    "spx_build_tile_table": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p,
+    "spx_build_tile_table": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int64,
                                      c_void_p, c_void_p, c_void_p]),
     "spx_implicit_gemm_fwd": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_int, c_float, c_void_p, c_void_p]),
+                                      c_int, c_float, c_void_p]),
     "spx_implicit_gemm_dgrad": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p,
                                         c_void_p]),
     "spx_implicit_gemm_wgrad_workspace_size": (c_size_t, [POINTER(GemmDesc)]),

@@ -30,6 +30,3 @@ class AllocKeys:
     OutFeatures = "OutFeatures"
     DIn = "DIn"
     DFilters = "DFilters"
-
-# one native call per rulebook (hash + probe + mask sort + tile table); 0 = the separate calls
-SPCONV_B200_FUSED_RULEBOOK = os.getenv("SPCONV_B200_FUSED_RULEBOOK", "1") == "1"

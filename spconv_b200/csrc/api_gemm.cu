@@ -6,10 +6,6 @@
 
 using namespace spx;
 
-namespace spx {
-int write_tile_masks(const uint32_t *mask, int64_t rows, int kv, uint32_t *out, cudaStream_t stream);
-}
-
 // SPX_FORCE_SIMT=1 pins the generic kernels (debug / A-B comparisons in tests); read once at load
 static bool force_simt() { return runtime_cfg().force_simt != 0; }
 static bool force_tc() { return runtime_cfg().force_tc != 0; }
@@ -54,8 +50,7 @@ static int run_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
 }
 
 extern "C" int spx_implicit_gemm_fwd(const spx_gemm_desc *d, const void *features, const void *filters, void *out,
-                                     const void *bias, int act, float act_alpha, uint32_t *mask_out,
-                                     spx_stream_t stream) {
+                                     const void *bias, int act, float act_alpha, spx_stream_t stream) {
     if (check_desc(d, "implicit_gemm_fwd")) return 2;
     SPX_REQUIRE(d->dtype == SPX_F32 || d->dtype == SPX_F16 || d->dtype == SPX_BF16,
                 "implicit_gemm_fwd: dtype %d not supported (int8 has its own entry point)", d->dtype);
@@ -63,7 +58,6 @@ extern "C" int spx_implicit_gemm_fwd(const spx_gemm_desc *d, const void *feature
     SPX_REQUIRE(features && filters && out, "implicit_gemm_fwd: NULL tensor");
     GatherGemmArgs a = make_args(d, false);
     a.x = features; a.w = filters; a.y = out; a.bias = bias; a.act = act; a.alpha = act_alpha;
-    a.mask_out = mask_out;
     return run_gather_gemm(a, (cudaStream_t)stream);
 }
 

@@ -21,7 +21,6 @@ struct GatherGemmArgs {
     int64_t pair_stride;
     const uint32_t *mask;      // [rows, words] in visiting order, or NULL
     const int32_t *argsort;    // [rows] or NULL
-    uint32_t *mask_out;        // [ceil(rows/128), words] or NULL
     const int32_t *tile_table; // [tiles][kv+1][128] or NULL (spx_build_tile_table)
     const uint32_t *tile_mask; // [tiles][words] or NULL
     __host__ __device__ int cx() const { return transpose_w ? c_out : c_in; }

@@ -145,43 +145,14 @@ simt_gather_gemm_kernel(GatherGemmArgs a, SimtEpilogue ep) {
             }
         }
     }
-    if (a.mask_out && tid < words) a.mask_out[(int64_t)blockIdx.x * words + tid] = tile_mask[tid];
 }
 
 template <typename T>
 static int launch_simt(const GatherGemmArgs &a, const SimtEpilogue &ep, cudaStream_t stream) {
     if (a.rows == 0) return 0;
     unsigned nblk = (unsigned)div_up64(a.rows, S_TM);
-    GatherGemmArgs b = a;
-    b.mask_out = nullptr;     // written by the dedicated kernel below (128-row granularity)
-    simt_gather_gemm_kernel<T><<<nblk, S_THREADS, 0, stream>>>(b, ep);
+    simt_gather_gemm_kernel<T><<<nblk, S_THREADS, 0, stream>>>(a, ep);
     SPX_CHECK_LAUNCH("simt_gather_gemm_kernel");
-    return 0;
-}
-
-// per-128-row OR of the visiting-order masks (reference mask_output_fwd, convops.py:2180-2189)
-__global__ void tile_mask_or_kernel(const uint32_t *__restrict__ mask, int64_t rows, int words, int kv,
-                                    uint32_t *__restrict__ out) {
-    int64_t tile = blockIdx.x;
-    int w = threadIdx.y;
-    uint32_t m = 0;
-    for (int r = threadIdx.x; r < 128; r += 32) {
-        int64_t row = tile * 128 + r;
-        if (row < rows) {
-            if (mask) m |= mask[row * words + w];
-            else { int hi = kv - 32 * w; m |= hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u); }
-        }
-    }
-    m = __reduce_or_sync(0xffffffffu, m);
-    if (threadIdx.x == 0) out[tile * words + w] = m;
-}
-
-int write_tile_masks(const uint32_t *mask, int64_t rows, int kv, uint32_t *out, cudaStream_t stream) {
-    if (!out || rows == 0) return 0;
-    int words = (kv + 31) / 32;
-    dim3 block(32, words);
-    tile_mask_or_kernel<<<(unsigned)div_up64(rows, 128), block, 0, stream>>>(mask, rows, words, kv, out);
-    SPX_CHECK_LAUNCH("tile_mask_or_kernel");
     return 0;
 }
 
@@ -189,15 +160,12 @@ int simt_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
     SimtEpilogue ep;
     memset(&ep, 0, sizeof(ep));
     ep.mode = 0; ep.bias = a.bias; ep.act = a.act; ep.alpha = a.alpha;
-    int rc;
     switch (a.dtype) {
-        case SPX_F32: rc = launch_simt<float>(a, ep, stream); break;
-        case SPX_F16: rc = launch_simt<__half>(a, ep, stream); break;
-        case SPX_BF16: rc = launch_simt<__nv_bfloat16>(a, ep, stream); break;
+        case SPX_F32: return launch_simt<float>(a, ep, stream);
+        case SPX_F16: return launch_simt<__half>(a, ep, stream);
+        case SPX_BF16: return launch_simt<__nv_bfloat16>(a, ep, stream);
         default: set_error("simt_gather_gemm: unsupported dtype %d", a.dtype); return 2;
     }
-    if (rc) return rc;
-    return write_tile_masks(a.mask, a.rows, a.kv, a.mask_out, stream);
 }
 
 int simt_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
@@ -206,9 +174,7 @@ int simt_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
     ep.mode = 1; ep.act = q.g.act; ep.alpha = q.g.alpha;
     ep.scale = q.scale; ep.bias_f32 = q.bias_f32; ep.output_add = q.output_add;
     ep.output_add_scale = q.output_add_scale; ep.out_dtype = q.out_dtype;
-    int rc = launch_simt<int8_t>(q.g, ep, stream);
-    if (rc) return rc;
-    return write_tile_masks(q.g.mask, q.g.rows, q.g.kv, q.g.mask_out, stream);
+    return launch_simt<int8_t>(q.g, ep, stream);
 }
 
 // ------------------------------------------------------------------ weight gradient

@@ -624,17 +624,9 @@ static int launch_tc(const CUtensorMap &tm, const TcParams &p, cudaStream_t stre
     return 2;
 }
 
-static int copy_mask_out(const GatherGemmArgs &a, cudaStream_t stream) {
-    if (!a.mask_out) return 0;      // mask_output_fwd == the per-tile OR masks of the tile table
-    const size_t bytes = (size_t)div_up64(a.rows, TC_TILE_M) * ((a.kv + 31) / 32) * sizeof(uint32_t);
-    SPX_CHECK_CUDA(cudaMemcpyAsync(a.mask_out, a.tile_mask, bytes, cudaMemcpyDeviceToDevice, stream));
-    return 0;
-}
-
 int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
     TcParams p;
     if (fill_params(a, p)) return 2;
-    if (copy_mask_out(a, stream)) return 1;
     CUtensorMap tm;
     if (make_weight_tmap(&tm, a.w, a.dtype, a.kv, a.c_in, a.c_out, p.b_transposed ? 128 : p.span_b)) return 2;
     if (a.dtype == SPX_F32) return launch_tc<KIND_TF32>(tm, p, stream);
@@ -644,7 +636,6 @@ int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
 int tc_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
     TcParams p;
     if (fill_params(q.g, p)) return 2;
-    if (copy_mask_out(q.g, stream)) return 1;
     p.out_dtype = q.out_dtype;
     p.epi_mode = 1;
     p.scale = q.scale; p.bias_f32 = q.bias_f32; p.output_add = q.output_add;

@@ -226,7 +226,7 @@ subm_probe_k3_kernel(Table32 table, Geom g, const int32_t *__restrict__ indices,
         mask[vbase + v] = m;
     }
     if (row_table) {
-        // row-major copy [N][32] (one 128-byte line per voxel, -1 padded) for spx_build_tile_table:
+        // row-major copy [N][32] (one 128-byte line per voxel, -1 padded) for build_tile_table_rows_kernel:
         // the permuted re-read then costs 4 sectors per row instead of one per (row, offset)
         for (int e = threadIdx.x; e < K3_VOX * 32; e += 27 * 32) {
             const int v = e >> 5, kk = e & 31;
@@ -931,14 +931,10 @@ static bool subm_k3_path(const Geom &gg) {
     return !needs_i64(gg, gg.in_dims) && gg.ndim == 3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
 }
 
-extern "C" int spx_subm_row_table_supported(const spx_conv_geometry *g) {
-    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
-    return subm_k3_path(make_geom(g, true)) ? 1 : 0;
-}
-
-extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int32_t *pair_fwd,
-                                 int32_t *pair_bwd, uint32_t *mask, int32_t *row_table, void *workspace,
-                                 size_t workspace_bytes, spx_stream_t stream_) {
+// row_table: NULL, or (subm_k3_path only) [N][32] that the probe kernel fills with the rows of pair_fwd
+static int subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int32_t *pair_fwd,
+                         int32_t *pair_bwd, uint32_t *mask, int32_t *row_table, void *workspace,
+                         size_t workspace_bytes, spx_stream_t stream_) {
     if (validate_geom(g)) return 2;
     for (int a = 0; a < g->ndim; ++a)
         SPX_REQUIRE(g->ksize[a] % 2 == 1, "subm only support odd ksize");
@@ -965,7 +961,6 @@ extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indi
             subm_probe_k3_kernel<<<(unsigned)div_up64(N, K3_VOX), 27 * 32, 0, stream>>>(t, gg, indices, N, pair_fwd,
                                                                                         pair_bwd, mask, row_table);
         } else {
-            SPX_REQUIRE(row_table == nullptr, "row_table is only produced when spx_subm_row_table_supported()");
             subm_probe_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N, pair_fwd, pair_bwd, mask, words);
         }
         SPX_CHECK_LAUNCH("subm_probe_kernel");
@@ -974,11 +969,16 @@ extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indi
         Table64 t{(long long *)tbl, tvals, L.capacity - 1};
         subm_insert_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N);
         SPX_CHECK_LAUNCH("subm_insert_kernel");
-        SPX_REQUIRE(row_table == nullptr, "row_table is only produced when spx_subm_row_table_supported()");
         subm_probe_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N, pair_fwd, pair_bwd, mask, words);
         SPX_CHECK_LAUNCH("subm_probe_kernel");
     }
     return 0;
+}
+
+extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int32_t *pair_fwd,
+                                 int32_t *pair_bwd, uint32_t *mask, void *workspace, size_t workspace_bytes,
+                                 spx_stream_t stream) {
+    return subm_rulebook(g, indices, N, pair_fwd, pair_bwd, mask, nullptr, workspace, workspace_bytes, stream);
 }
 
 
@@ -1268,9 +1268,10 @@ extern "C" size_t spx_tile_table_elems(int64_t rows, int kv) {
     return (size_t)tt_total_elems(div_up64(rows > 0 ? rows : 1, 128), kv);
 }
 
-extern "C" int spx_build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, const int32_t *argsort,
-                                    const uint32_t *mask, int64_t rows, const int32_t *row_table, int32_t *table,
-                                    uint32_t *tile_mask, spx_stream_t stream_) {
+// row_table: NULL, or the [rows][32] copy of `pair` (kv <= 32) written by subm_rulebook; then `pair` is not read
+static int build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, const int32_t *argsort,
+                            const uint32_t *mask, int64_t rows, const int32_t *row_table, int32_t *table,
+                            uint32_t *tile_mask, spx_stream_t stream_) {
     SPX_REQUIRE(kv >= 1 && kv <= 128, "build_tile_table: kernel volume %d not in [1,128]", kv);
     if (rows == 0) return 0;
     SPX_REQUIRE((pair || row_table) && table && tile_mask, "build_tile_table: NULL pointer argument");
@@ -1299,6 +1300,12 @@ extern "C" int spx_build_tile_table(const int32_t *pair, int64_t pair_stride, in
     tile_order_kernel<<<1, TO_THREADS, 0, stream>>>(oj, words);
     SPX_CHECK_LAUNCH("tile_order_kernel");
     return 0;
+}
+
+extern "C" int spx_build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, const int32_t *argsort,
+                                    const uint32_t *mask, int64_t rows, int32_t *table, uint32_t *tile_mask,
+                                    spx_stream_t stream) {
+    return build_tile_table(pair, pair_stride, kv, argsort, mask, rows, nullptr, table, tile_mask, stream);
 }
 
 // forward + backward tile tables of a regular conv in one launch each (gather kernel, schedule records)
@@ -1330,12 +1337,13 @@ static int build_tile_tables_pair(int kv, const int32_t *pair0, const int32_t *a
 
 // ====================================================================== fused host entry points
 // One C-ABI call per rulebook (the eager Python path was paying ~10 us of interpreter + ctypes +
-// allocator time for every separate call, workspace query and scratch tensor).  Pure orchestration:
-// the launches are exactly those of the separate entry points, scratch regions are carved from ONE
-// caller-provided workspace.
+// allocator time for every separate call, workspace query and scratch tensor).  Pure orchestration of
+// the kernels behind the separate entry points; scratch regions are carved from ONE caller-provided
+// workspace.
 
+// the row-major copy of pair_fwd that subm_probe_k3_kernel writes for the tile-table build
 static size_t subm_row_table_bytes(const spx_conv_geometry *g, int64_t N) {
-    return spx_subm_row_table_supported(g) ? align_up((size_t)N * 32 * sizeof(int32_t), 256) : 0;
+    return subm_k3_path(make_geom(g, true)) ? align_up((size_t)N * 32 * sizeof(int32_t), 256) : 0;
 }
 
 extern "C" size_t spx_subm_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N) {
@@ -1353,7 +1361,7 @@ extern "C" int spx_subm_rulebook_all(const spx_conv_geometry *g, const int32_t *
                                      spx_stream_t stream) {
     if (validate_geom(g)) return 2;
     if (N == 0) return 0;
-    SPX_REQUIRE(mask && argsort && workspace, "subm_rulebook_all: NULL pointer argument");
+    SPX_REQUIRE(mask && argsort && tile_table && tile_mask && workspace, "subm_rulebook_all: NULL pointer argument");
     SPX_REQUIRE(workspace_bytes >= spx_subm_rulebook_all_workspace_size(g, N), "subm_rulebook_all: workspace too small");
     int kv = 1;
     for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
@@ -1361,11 +1369,9 @@ extern "C" int spx_subm_rulebook_all(const spx_conv_geometry *g, const int32_t *
     const size_t rb = spx_rulebook_workspace_size(g, N, 0, 1), as = spx_mask_argsort_workspace_size(N, words);
     const size_t shared = align_up(rb > as ? rb : as, 256);          // rulebook and sort scratch are used one after the other
     int32_t *row_table = subm_row_table_bytes(g, N) ? (int32_t *)((char *)workspace + shared) : nullptr;
-    if (int rc = spx_subm_rulebook(g, indices, N, pair_fwd, pair_bwd, mask, row_table, workspace, rb, stream)) return rc;
+    if (int rc = subm_rulebook(g, indices, N, pair_fwd, pair_bwd, mask, row_table, workspace, rb, stream)) return rc;
     if (int rc = spx_mask_argsort(mask, argsort, N, words, kv, do_sort, workspace, as, stream)) return rc;
-    if (tile_table)
-        return spx_build_tile_table(pair_fwd, N, kv, argsort, mask, N, row_table, tile_table, tile_mask, stream);
-    return 0;
+    return build_tile_table(pair_fwd, N, kv, argsort, mask, N, row_table, tile_table, tile_mask, stream);
 }
 
 extern "C" size_t spx_conv_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N) {
@@ -1377,7 +1383,7 @@ extern "C" size_t spx_conv_rulebook_all_workspace_size(const spx_conv_geometry *
            2 * align_up(spx_mask_argsort_workspace_size(max_rows, (kv + 31) / 32), 256) + 256;   // two sorts side by side
 }
 
-// stage 2 + both mask argsorts + both tile tables (argsort_bwd / table_bwd may be NULL: inference)
+// stage 2 + both mask argsorts + both tile tables (the backward ones are skipped for inference)
 extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int64_t M,
                                             int32_t *out_inds, int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd,
                                             uint32_t *mask_bwd, int32_t *argsort_fwd, int32_t *argsort_bwd, int do_sort,
@@ -1386,7 +1392,12 @@ extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const in
                                             spx_stream_t stream) {
     if (validate_geom(g)) return 2;
     if (N == 0 || M == 0) return 0;
-    SPX_REQUIRE(mask_fwd && mask_bwd && argsort_fwd && workspace, "conv_rulebook_stage2_all: NULL pointer argument");
+    SPX_REQUIRE(mask_fwd && mask_bwd && argsort_fwd && table_fwd && tmask_fwd && workspace,
+                "conv_rulebook_stage2_all: NULL pointer argument");
+    const bool train = argsort_bwd != nullptr;
+    SPX_REQUIRE((table_bwd != nullptr) == train && (tmask_bwd != nullptr) == train,
+                "conv_rulebook_stage2_all: argsort_bwd, table_bwd and tmask_bwd must all be given (training) or all be "
+                "NULL (inference)");
     SPX_REQUIRE(workspace_bytes >= spx_conv_rulebook_all_workspace_size(g, N), "conv_rulebook_stage2_all: workspace too small");
     int kv = 1;
     for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
@@ -1395,28 +1406,18 @@ extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const in
     void *sort_ws = (char *)workspace + align_up(rb, 256);
     const size_t sort_bytes = workspace_bytes - align_up(rb, 256);
     if (int rc = spx_conv_rulebook_stage2(g, indices, N, M, out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, workspace, rb, stream)) return rc;
-    if (words == 1 && do_sort && argsort_bwd) {
+    if (words == 1 && do_sort && train) {
         // both mask sorts, then both tile tables, two jobs per launch
         const size_t half = (sort_bytes / 2) & ~(size_t)255;
         const int key_bits = kv < 32 ? kv : 32;
         if (int rc = radix_argsort_pair(mask_fwd, argsort_fwd, M, mask_bwd, argsort_bwd, N, key_bits, sort_ws, half,
                                         (char *)sort_ws + half, half, (cudaStream_t)stream)) return rc;
-        if (table_fwd && table_bwd)
-            return build_tile_tables_pair(kv, pair_fwd, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, pair_bwd, argsort_bwd,
-                                          mask_bwd, N, table_bwd, tmask_bwd, (cudaStream_t)stream);
-        if (table_fwd)
-            if (int rc = spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, nullptr, table_fwd, tmask_fwd, stream)) return rc;
-        if (table_bwd)
-            if (int rc = spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, nullptr, table_bwd, tmask_bwd, stream)) return rc;
-        return 0;
+        return build_tile_tables_pair(kv, pair_fwd, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, pair_bwd, argsort_bwd,
+                                      mask_bwd, N, table_bwd, tmask_bwd, (cudaStream_t)stream);
     }
     if (int rc = spx_mask_argsort(mask_fwd, argsort_fwd, M, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
-    if (table_fwd)
-        if (int rc = spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, nullptr, table_fwd, tmask_fwd, stream)) return rc;
-    if (argsort_bwd) {
-        if (int rc = spx_mask_argsort(mask_bwd, argsort_bwd, N, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
-        if (table_bwd)
-            if (int rc = spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, nullptr, table_bwd, tmask_bwd, stream)) return rc;
-    }
-    return 0;
+    if (int rc = spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, stream)) return rc;
+    if (!train) return 0;
+    if (int rc = spx_mask_argsort(mask_bwd, argsort_bwd, N, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
+    return spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, table_bwd, tmask_bwd, stream);
 }

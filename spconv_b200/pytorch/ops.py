@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from .. import _cabi
-from ..constants import SPCONV_ALLOW_TF32, SPCONV_B200_FUSED_RULEBOOK, SPCONV_DO_SORT
+from ..constants import SPCONV_ALLOW_TF32, SPCONV_DO_SORT
 from ..core import Activation, ConvAlgo
 from .core import CUDAKernelTimer, ThrustSortAllocator
 
@@ -165,17 +165,21 @@ def _zero_counts(kv: int, device) -> torch.Tensor:
     return t
 
 
+def _conv_stage1(geo, indices, n_in, ws) -> int:
+    """Stage 1 of the regular-conv rulebook on workspace ``ws``: returns the output count M (one host sync)."""
+    m_host = ctypes.c_int64(0)
+    _cabi.check(_lib().spx_conv_rulebook_stage1(ctypes.byref(geo), _ptr(indices), n_in, ctypes.byref(m_host),
+                                                ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_stage1")
+    return int(m_host.value)
+
+
 def _conv_rulebook(geo, indices, n_in, kv, words, want_masks, alloc):
     """Two-phase regular-conv rulebook; returns (out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd)."""
     lib = _lib()
     dev = indices.device
     ws_bytes = lib.spx_rulebook_workspace_size(ctypes.byref(geo), n_in, 0, 0)
     ws = _bytes(ws_bytes, dev, alloc)
-    m_host = ctypes.c_int64(0)
-    _cabi.check(lib.spx_conv_rulebook_stage1(ctypes.byref(geo), _ptr(indices), n_in,
-                                             ctypes.byref(m_host), ws.data_ptr(), ws.numel(),
-                                             _stream()), "conv_rulebook_stage1")
-    m = int(m_host.value)
+    m = _conv_stage1(geo, indices, n_in, ws)
     if m == 0:
         raise ValueError(_VANISHED)
     ndim = indices.shape[1] - 1
@@ -198,10 +202,7 @@ def _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, 
     lib = _lib()
     dev = indices.device
     ws = _bytes(lib.spx_conv_rulebook_all_workspace_size(ctypes.byref(geo), n_in), dev, alloc)
-    m_host = ctypes.c_int64(0)
-    _cabi.check(lib.spx_conv_rulebook_stage1(ctypes.byref(geo), _ptr(indices), n_in, ctypes.byref(m_host),
-                                             ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_stage1")
-    m = int(m_host.value)
+    m = _conv_stage1(geo, indices, n_in, ws)
     if m == 0:
         raise ValueError(_VANISHED)
     ndim = indices.shape[1] - 1
@@ -284,7 +285,7 @@ def get_indice_pairs(indices: torch.Tensor, batch_size: int, spatial_shape: List
         pair_bwd = torch.empty((kv, n_in), dtype=torch.int32, device=dev)
         ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n_in, 0, 1), dev)
         _cabi.check(lib.spx_subm_rulebook(ctypes.byref(geo), _ptr(indices), n_in,
-                                          pair_fwd.data_ptr(), pair_bwd.data_ptr(), None, None,
+                                          pair_fwd.data_ptr(), pair_bwd.data_ptr(), None,
                                           ws.data_ptr(), ws.numel(), _stream()), "subm_rulebook")
         out_inds = indices
     else:
@@ -340,62 +341,41 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
                 raise RuntimeError("subm only support odd ksize")
         pair = torch.empty((2 if is_train else 1, kv, n_in), dtype=torch.int32, device=dev)
         pair_mask = torch.empty((1, n_in, words), dtype=torch.int32, device=dev)
-        if SPCONV_B200_FUSED_RULEBOOK and not timer.enable and not is_split and n_in:
-            # one native call: hash + probe + mask sort + tile table (the separate calls below are kept
-            # for profiling regions and the mask-split algo)
-            mask_argsort = torch.empty((1, n_in), dtype=torch.int32, device=dev)
-            table, tile_mask = _alloc_tile_tables(n_in, kv, dev)
-            ws = _bytes(lib.spx_subm_rulebook_all_workspace_size(ctypes.byref(geo), n_in), dev, alloc)
-            _cabi.check(lib.spx_subm_rulebook_all(ctypes.byref(geo), _ptr(indices), n_in, pair[0].data_ptr(),
-                                                  pair[1].data_ptr() if is_train else None, _ptr(pair_mask),
-                                                  _ptr(mask_argsort), int(bool(do_sort)), _ptr(table), _ptr(tile_mask),
-                                                  ws.data_ptr(), ws.numel(), _stream()), "subm_rulebook_all")
-            pair_fwd, argsort_view = pair[0], mask_argsort[0]
-            argsort_view._spx_tile_cache = (_tile_key(pair_fwd, argsort_view, n_in), table, tile_mask)
-            return (indices, indice_num_per_loc, pair_fwd, pair[1] if is_train else torch.Tensor(),
-                    [pair_mask[0]], [], [argsort_view], [], masks)
-        # row-major by-product of the probe kernel; consumed (and dropped) by the first tile-table build
-        rows = None
-        if n_in and lib.spx_subm_row_table_supported(ctypes.byref(geo)):
-            rows = torch.empty((n_in, 32), dtype=torch.int32, device=dev)
-        with timer.record("gen_subm_inds", _stream()):
-            ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n_in, 0, 1), dev, alloc)
-            _cabi.check(lib.spx_subm_rulebook(ctypes.byref(geo), _ptr(indices), n_in,
-                                              pair[0].data_ptr(),
-                                              pair[1].data_ptr() if is_train and n_in else None,
-                                              _ptr(pair_mask), _ptr(rows), ws.data_ptr(), ws.numel(),
-                                              _stream()), "subm_rulebook")
         pair_bwd = pair[1] if is_train else torch.Tensor()
         if is_split:
+            # the splits AND the unsorted mask with their constants: separate rulebook and sort calls
+            with timer.record("gen_subm_inds", _stream()):
+                ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n_in, 0, 1), dev, alloc)
+                _cabi.check(lib.spx_subm_rulebook(ctypes.byref(geo), _ptr(indices), n_in, pair[0].data_ptr(),
+                                                  pair[1].data_ptr() if is_train and n_in else None,
+                                                  _ptr(pair_mask), ws.data_ptr(), ws.numel(), _stream()),
+                            "subm_rulebook")
             with timer.record("gen_subm_inds_sort", _stream()):
                 mask_s, sort_s = _split_and_sort(pair_mask, masks, kv, do_sort, alloc)
             return (indices, indice_num_per_loc, pair[0], pair_bwd, mask_s, [], sort_s, [], masks)
-        with timer.record("gen_subm_inds_sort", _stream()):
-            mask_argsort = _argsort_masks(pair_mask, kv, do_sort, alloc)
+        # one native call: hash + probe + mask sort + tile table
+        mask_argsort = torch.empty((1, n_in), dtype=torch.int32, device=dev)
+        table, tile_mask = _alloc_tile_tables(n_in, kv, dev)
+        with timer.record("gen_subm_inds", _stream()):
+            ws = _bytes(lib.spx_subm_rulebook_all_workspace_size(ctypes.byref(geo), n_in), dev, alloc)
+            _cabi.check(lib.spx_subm_rulebook_all(
+                ctypes.byref(geo), _ptr(indices), n_in, pair[0].data_ptr(), pair[1].data_ptr() if is_train else None,
+                _ptr(pair_mask), _ptr(mask_argsort), int(bool(do_sort)), _ptr(table), _ptr(tile_mask),
+                ws.data_ptr(), ws.numel(), _stream()), "subm_rulebook_all")
         argsort_view = mask_argsort[0]
-        if rows is not None:
-            argsort_view._spx_row_table = (pair[0].data_ptr(), rows)
-        return (indices, indice_num_per_loc, pair[0], pair_bwd, [pair_mask[0]], [],
-                [argsort_view], [], masks)
-    if SPCONV_B200_FUSED_RULEBOOK and not timer.enable and not is_split and n_in:
-        return _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks)
-    with timer.record("gen_conv_inds", _stream()):
-        out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd = _conv_rulebook(
-            geo, indices, n_in, kv, words, True, alloc)
+        argsort_view._spx_tile_cache = (_tile_key(pair[0], argsort_view, n_in), table, tile_mask)
+        return (indices, indice_num_per_loc, pair[0], pair_bwd, [pair_mask[0]], [], [argsort_view], [], masks)
     if is_split:
+        # the splits AND the unsorted masks with their constants: separate rulebook and sort calls
+        with timer.record("gen_conv_inds", _stream()):
+            out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd = _conv_rulebook(
+                geo, indices, n_in, kv, words, True, alloc)
         with timer.record("gen_conv_inds_sort", _stream()):
             mf, sf = _split_and_sort(mask_fwd, masks, kv, do_sort, alloc)
             mb, sb = _split_and_sort(mask_bwd, masks, kv, do_sort, alloc) if is_train else ([], [])
         return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, mf, mb, sf, sb, masks)
-    with timer.record("gen_conv_inds_sort", _stream()):
-        argsort_fwd = _argsort_masks(mask_fwd, kv, do_sort, alloc)
-        if is_train:
-            argsort_bwd = _argsort_masks(mask_bwd, kv, do_sort, alloc)
-    if is_train:
-        return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [mask_bwd[0]],
-                [argsort_fwd[0]], [argsort_bwd[0]], masks)
-    return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [], [argsort_fwd[0]],
-            [], masks)
+    with timer.record("gen_conv_inds", _stream()):
+        return _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks)
 
 
 # ---------------------------------------------------------------------------- GEMM descriptor
@@ -429,15 +409,9 @@ def _tile_tables(pair: torch.Tensor, mask: Optional[torch.Tensor], argsort: Opti
             return hit[1], hit[2]
     lib = _lib()
     table, tile_mask = _alloc_tile_tables(rows, kv, pair.device)
-    row_table = None
-    hint = getattr(owner, "_spx_row_table", None) if owner is not None else None
-    if hint is not None and hint[0] == pair.data_ptr() and hint[1].shape[0] == int(rows):
-        row_table = hint[1]
     _cabi.check(lib.spx_build_tile_table(_ptr(pair), int(pair.stride(0)), kv, _ptr(argsort), _ptr(mask),
-                                         int(rows), _ptr(row_table), _ptr(table), _ptr(tile_mask), _stream()),
+                                         int(rows), _ptr(table), _ptr(tile_mask), _stream()),
                 "build_tile_table")
-    if hint is not None:
-        owner._spx_row_table = None                # one-shot: 128 B per voxel are not kept alive
     if owner is not None:
         owner._spx_tile_cache = (key, table, tile_mask)
     return table, tile_mask
@@ -532,7 +506,7 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     with timer.record("implicit_gemm", _stream()):
         _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
                                               _ptr(out), _ptr(bias), _act_code(act_type),
-                                              float(act_alpha), None, _stream()), "implicit_gemm_fwd")
+                                              float(act_alpha), _stream()), "implicit_gemm_fwd")
     if output_add is not None:
         out = out + output_add
     if output_dtype != out.dtype:
@@ -559,7 +533,7 @@ def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_spli
         part = torch.empty((n_out, c_out), dtype=features.dtype, device=features.device)
         with timer.record("implicit_gemm", _stream()):
             _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters), _ptr(part),
-                                                  None, _cabi.SPX_ACT_NONE, 0.0, None, _stream()),
+                                                  None, _cabi.SPX_ACT_NONE, 0.0, _stream()),
                         "implicit_gemm_fwd(split)")
         out = part if out is None else out.add_(part)
         if tiles is not None:
@@ -798,7 +772,7 @@ def indice_conv(features: torch.Tensor, filters: torch.Tensor, indice_pairs: tor
     with timer.record("indice_conv", _stream()):
         _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
                                               _ptr(out), _ptr(bias), _act_code(act_type),
-                                              float(act_alpha), None, _stream()),
+                                              float(act_alpha), _stream()),
                     "implicit_gemm_fwd(native)")
     return out
 
@@ -964,10 +938,7 @@ def sparse_add_union(indices: Sequence[torch.Tensor], batch_size: int, spatial_s
     geo = _geometry(cat, batch_size, spatial_shape, spatial_shape, ones, ones, zeros, ones, False)
     lib = _lib()
     ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n, 0, 0), dev)
-    m_host = ctypes.c_int64(0)
-    _cabi.check(lib.spx_conv_rulebook_stage1(ctypes.byref(geo), cat.data_ptr(), n, ctypes.byref(m_host),
-                                             ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_stage1(sparse_add)")
-    m = int(m_host.value)
+    m = _conv_stage1(geo, cat, n, ws)
     out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
     dst = torch.empty((n,), dtype=torch.int32, device=dev)
     if m == 0:

@@ -62,14 +62,14 @@ def test_argument_validation_reports_errors(lib):
     import ctypes
     from spconv_b200 import _cabi
     bad = _cabi.make_geometry(3, 1, [8] * 3, [8] * 3, [2] * 3, [1] * 3, [0] * 3, [1] * 3)
-    rc = lib.spx_subm_rulebook(ctypes.byref(bad), 1, 10, 1, None, None, None, 1, 1, None)
+    rc = lib.spx_subm_rulebook(ctypes.byref(bad), 1, 10, 1, None, None, 1, 1, None)
     assert rc != 0 and "odd ksize" in _cabi.last_error()
     bad.ndim = 7
-    rc = lib.spx_subm_rulebook(ctypes.byref(bad), 1, 10, 1, None, None, None, 1, 1, None)
+    rc = lib.spx_subm_rulebook(ctypes.byref(bad), 1, 10, 1, None, None, 1, 1, None)
     assert rc != 0 and "ndim" in _cabi.last_error()
     d = _cabi.GemmDesc()
     d.kv, d.c_in, d.c_out, d.dtype = 0, 16, 16, _cabi.SPX_F16
-    assert lib.spx_implicit_gemm_fwd(ctypes.byref(d), None, None, None, None, 0, 0.0, None, None) != 0
+    assert lib.spx_implicit_gemm_fwd(ctypes.byref(d), None, None, None, None, 0, 0.0, None) != 0
     assert "kernel volume" in _cabi.last_error()
     with pytest.raises(RuntimeError, match="kernel volume"):
         _cabi.check(2, "x")

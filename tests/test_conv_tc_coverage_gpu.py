@@ -269,7 +269,7 @@ class Conv:
         def launch():
             out = _nan((self.n_out, K), x.dtype, x.device)
             _cabi.check(_lib().spx_implicit_gemm_fwd(ctypes.byref(d), x.data_ptr(), w.data_ptr(), out.data_ptr(),
-                                                     None if bias is None else bias.data_ptr(), act, alpha, None,
+                                                     None if bias is None else bias.data_ptr(), act, alpha,
                                                      ops._stream()), "implicit_gemm_fwd")
             return out
         return _launch("fwd", inst, launch)

@@ -184,45 +184,30 @@ def test_vanished_points_error(cuda_dev):
                              [1] * 3, [0] * 3, True)
 
 
-def test_tile_table_from_row_table_matches_column_path(cuda_dev):
-    """spx_build_tile_table has two sources for the same table: the column-major pair table and
-    the row-major by-product of the 3x3x3 probe kernel.  Both must give identical blocks and
-    tile masks (== per-tile OR of the sorted masks, the reference's mask_output_fwd with
-    mask_width 128, spconv/csrc/sparse/convops.py:2180-2189)."""
+def test_fused_subm_tile_table_matches_column_path(cuda_dev):
+    """A tile table has two sources: spx_subm_rulebook_all builds it for a 3x3x3 SubM from the row-major
+    copy of the pair table that the probe kernel keeps in its workspace, spx_build_tile_table from the
+    column-major pair table.  Both must give identical blocks and tile masks (== per-tile OR of the
+    sorted masks, the reference's mask_output_fwd with mask_width 128,
+    spconv/csrc/sparse/convops.py:2180-2189)."""
     from spconv_b200.core import ConvAlgo
     from spconv_b200.pytorch import ops
     rng = np.random.default_rng(5)
     shape = [24, 200, 176]
     inds = torch.from_numpy(surface_cloud(rng, shape, 9000 + 77)).to(cuda_dev)
     n = inds.shape[0]
-    # the fused native call (default) builds the table from the row-major by-product inside C; its cached
-    # result must equal what the separate calls produce from either source
-    fused = ops.get_indice_pairs_implicit_gemm(inds, 1, shape, ConvAlgo.MaskImplicitGemm, [3] * 3, [1] * 3,
-                                               [1] * 3, [1] * 3, [0] * 3, True, False, is_train=True)
-    fused_cache = getattr(fused[6][0], "_spx_tile_cache", None)
-    assert fused_cache is not None, "the fused rulebook call must leave the tile table cached on the argsort"
-    old = ops.SPCONV_B200_FUSED_RULEBOOK
-    ops.SPCONV_B200_FUSED_RULEBOOK = False
-    try:
-        res = ops.get_indice_pairs_implicit_gemm(inds, 1, shape, ConvAlgo.MaskImplicitGemm, [3] * 3, [1] * 3,
-                                                 [1] * 3, [1] * 3, [0] * 3, True, False, is_train=True)
-    finally:
-        ops.SPCONV_B200_FUSED_RULEBOOK = old
-    for a, b in ((fused[2], res[2]), (fused[3], res[3]), (fused[4][0], res[4][0]), (fused[6][0], res[6][0])):
-        assert torch.equal(a, b)
+    res = ops.get_indice_pairs_implicit_gemm(inds, 1, shape, ConvAlgo.MaskImplicitGemm, [3] * 3, [1] * 3,
+                                             [1] * 3, [1] * 3, [0] * 3, True, False, is_train=True)
     pair_fwd, mask, argsort = res[2], res[4][0], res[6][0]
-    hint = getattr(argsort, "_spx_row_table", None)
-    assert hint is not None, "3x3x3 SubM rulebook must hand the row-major table to the tile builder"
-    rows = hint[1].cpu().numpy()
-    pf = pair_fwd.cpu().numpy()
-    assert np.array_equal(rows[:, :27], pf.T) and (rows[:, 27:] == -1).all()
-    t_rows, m_rows = ops._tile_tables(pair_fwd, mask, argsort, n, 27, owner=argsort)
-    assert argsort._spx_row_table is None                       # consumed
+    cache = getattr(argsort, "_spx_tile_cache", None)
+    assert cache is not None, "the fused rulebook call must leave the tile table cached on the argsort"
+    assert cache[0] == ops._tile_key(pair_fwd, argsort, n)
+    t_rows, m_rows = cache[1], cache[2]
     t_cols, m_cols = ops._tile_tables(pair_fwd, mask, argsort, n, 27, owner=None)
     assert torch.equal(t_rows, t_cols) and torch.equal(m_rows, m_cols)
-    assert torch.equal(fused_cache[1], t_cols) and torch.equal(fused_cache[2], m_cols)
+    pf = pair_fwd.cpu().numpy()
     tiles = (n + 127) // 128
-    flat = t_cols.cpu().numpy()
+    flat = t_rows.cpu().numpy()
     tab = flat[:tiles * 28 * 128].reshape(tiles, 28, 128)
     order = argsort.cpu().numpy()
     padded = np.full(tiles * 128, -1, np.int64)
@@ -232,15 +217,80 @@ def test_tile_table_from_row_table_matches_column_path(cuda_dev):
     assert np.array_equal(tab[:, :27, :].transpose(1, 0, 2).reshape(27, -1), want)
     sm = np.zeros(tiles * 128, np.uint32)
     sm[:n] = mask.cpu().numpy().reshape(-1).view(np.uint32)
-    assert np.array_equal(m_cols.cpu().numpy().reshape(-1).view(np.uint32),
+    assert np.array_equal(m_rows.cpu().numpy().reshape(-1).view(np.uint32),
                           np.bitwise_or.reduce(sm.reshape(tiles, 128), axis=1))
     # schedule records behind the blocks: every tile once, heaviest (most offsets) first, ties in
     # ascending tile order; scheduler scratch zeroed
     rec = flat[tiles * 28 * 128: tiles * 28 * 128 + tiles * 8].reshape(tiles, 8)
-    tmask = m_cols.cpu().numpy().reshape(-1).view(np.uint32)
+    tmask = m_rows.cpu().numpy().reshape(-1).view(np.uint32)
     cost = np.array([bin(int(v)).count("1") for v in np.where(tmask == 0, 1, tmask)])
     want_order = np.argsort(-cost, kind="stable")
     assert np.array_equal(rec[:, 0], want_order)
     assert np.array_equal(rec[:, 1].view(np.uint32), np.where(tmask == 0, 1, tmask)[want_order])
     assert (rec[:, 2:] == 0).all()
     assert (flat[tiles * 28 * 128 + tiles * 8:] == 0).all() and flat.shape[0] == tiles * 28 * 128 + tiles * 8 + 64
+
+
+TIMER_CASES = [CASES[0], CASES[7], CASES[2],
+               ([9, 10, 11, 12], [2000], [3] * 4, [2] * 4, [1] * 4, [1] * 4, False, False)]   # kv = 81: 3 mask words
+
+
+@pytest.mark.parametrize("case", TIMER_CASES, ids=lambda c: f"{'subm' if c[6] else 'conv'}-{len(c[0])}d-k{c[2][0]}s{c[3][0]}")
+@pytest.mark.parametrize("is_train", [True, False])
+def test_timer_does_not_change_rulebook_path(case, is_train, cuda_dev):
+    """With a CUDAKernelTimer enabled the MaskImplicitGemm rulebook runs the same fused native calls: the
+    9-tuple and the tile tables cached on the argsorts equal those of the call without a timer, and the
+    whole rulebook is one gen_*_inds region."""
+    from spconv_b200.core import ConvAlgo
+    from spconv_b200.pytorch import ops
+    from spconv_b200.pytorch.core import CUDAKernelTimer
+    shape, pts, ksize, stride, padding, dilation, subm, transpose = case
+    rng = np.random.default_rng(31)
+    _, inds = random_cloud(rng, shape, pts, 1)
+    args = (torch.from_numpy(inds).to(cuda_dev), len(pts), shape, ConvAlgo.MaskImplicitGemm, ksize, stride,
+            padding, dilation, [0] * len(shape), subm, transpose)
+    ref = ops.get_indice_pairs_implicit_gemm(*args, is_train=is_train)
+    timer = CUDAKernelTimer(True)
+    got = ops.get_indice_pairs_implicit_gemm(*args, is_train=is_train, timer=timer)
+    for i in (0, 1, 2, 3):
+        assert got[i].dtype == ref[i].dtype and torch.equal(got[i], ref[i]), i
+    for i in (4, 5, 6, 7):
+        assert len(got[i]) == len(ref[i]), i
+        assert all(torch.equal(a, b) for a, b in zip(got[i], ref[i])), i
+    assert len(got[8]) == len(ref[8]) and all(np.array_equal(a, b) for a, b in zip(got[8], ref[8]))
+    owners = list(zip(got[6] + got[7], ref[6] + ref[7]))
+    assert len(owners) == (1 if subm or not is_train else 2)
+    for g, r in owners:
+        gc, rc = getattr(g, "_spx_tile_cache", None), getattr(r, "_spx_tile_cache", None)
+        assert gc is not None and rc is not None, "the rulebook call must leave the tile table cached on the argsort"
+        assert torch.equal(gc[1], rc[1]) and torch.equal(gc[2], rc[2])
+    assert list(timer.get_all_pair_time()) == ["gen_subm_inds" if subm else "gen_conv_inds"]
+
+
+ZERO_CASES = [([20, 20, 20], [3] * 3), ([40, 50], [3, 3]), ([9, 10, 11, 12], [3] * 4)]
+
+
+@pytest.mark.parametrize("case", ZERO_CASES, ids=lambda c: f"{len(c[0])}d-kv{int(np.prod(c[1]))}")
+@pytest.mark.parametrize("is_train", [True, False])
+def test_zero_row_subm_implicit_gemm_rulebook(case, is_train, cuda_dev):
+    """A SubM MaskImplicitGemm rulebook of no voxels is the 9-tuple of empty tables"""
+    from spconv_b200.core import ConvAlgo
+    from spconv_b200.pytorch import ops
+    shape, ksize = case
+    ndim, kv = len(shape), int(np.prod(ksize))
+    words = (kv + 31) // 32
+    inds = torch.empty((0, ndim + 1), dtype=torch.int32, device=cuda_dev)
+    res = ops.get_indice_pairs_implicit_gemm(inds, 1, shape, ConvAlgo.MaskImplicitGemm, ksize, [1] * ndim,
+                                             [1] * ndim, [1] * ndim, [0] * ndim, True, False, is_train=is_train)
+    out_inds, num, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
+    assert out_inds.shape == (0, ndim + 1) and out_inds.dtype == torch.int32
+    assert num.shape == (kv,) and num.dtype == torch.int32 and not num.any()
+    assert pair_fwd.shape == (kv, 0) and pair_fwd.dtype == torch.int32
+    if is_train:
+        assert pair_bwd.shape == (kv, 0) and pair_bwd.dtype == torch.int32
+    else:
+        assert pair_bwd.shape == (0,) and pair_bwd.dtype == torch.float32
+    assert len(mask_fwd) == 1 and mask_fwd[0].shape == (0, words) and mask_fwd[0].dtype == torch.int32
+    assert len(sort_fwd) == 1 and sort_fwd[0].shape == (0,) and sort_fwd[0].dtype == torch.int32
+    assert mask_bwd == [] and sort_bwd == []
+    assert len(masks) == 1 and masks[0].dtype == np.uint32 and masks[0].tolist() == [0xffffffff]
