@@ -734,9 +734,23 @@ build_tile_table_kernel(const TtJobs jobs, int kv, int words) {
     // 3N x 4 threads with <= 8 independent scattered 4-byte loads each: the kernel is a pure
     // L2-latency problem, so it is sized for memory-level parallelism, not for work per thread
     const int32_t *col = pair + (src >= 0 ? src : 0);
+    // An offset whose bit is clear in the row's mask stores -1.  A mask split clears the offsets of the
+    // other split while pair still holds them, and the GEMM kernels gather every entry >= 0 of a stage
+    // they run (an all-zero tile still runs one stage at offset 0).  Without a split a bit is clear
+    // exactly where the pair is -1.
+    uint32_t rm0 = ~0u, rm1 = ~0u, rm2 = ~0u, rm3 = ~0u;
+    if (mask && j < rows) {
+        const uint32_t *mr = mask + j * words;
+        rm0 = __ldg(mr);
+        if (words > 1) rm1 = __ldg(mr + 1);
+        if (words > 2) rm2 = __ldg(mr + 2);
+        if (words > 3) rm3 = __ldg(mr + 3);
+    }
 #pragma unroll 8
-    for (int k = q; k < kv; k += TT_SPLIT)
-        blk[k * 128 + r] = src >= 0 ? __ldg(col + (int64_t)k * pair_stride) : -1;
+    for (int k = q; k < kv; k += TT_SPLIT) {
+        const uint32_t w = k < 32 ? rm0 : k < 64 ? rm1 : k < 96 ? rm2 : rm3;
+        blk[k * 128 + r] = src >= 0 && ((w >> (k & 31)) & 1u) ? __ldg(col + (int64_t)k * pair_stride) : -1;
+    }
     if (q == 0) blk[kv * 128 + r] = src;
     __shared__ uint32_t red[4][4];
     if (q == 0) {
