@@ -156,6 +156,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         }
     }
 }
+// mbar_wait without the printf, for kernels that keep a wgmma group in flight across a wait: a
+// function call anywhere in such a kernel (ptxas does not tell the warp roles' paths apart) makes
+// ptxas serialise all its wgmma.  The timeout still traps.
+__device__ __forceinline__ void mbar_wait_silent(uint64_t *bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return;
+    const long long t0 = clock64();
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, parity)) {
+        if ((++spins & 0x3FFFu) == 0u && clock64() - t0 > 4000000000ll) __trap();
+    }
+}
 // arrive (no pending-count increment) once all prior cp.async of this thread have landed
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t *bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");

@@ -13,7 +13,8 @@
 //   * the TMA warp loads that offset's KRSC weight slice W[:, k, :] (a strided 2-D box);
 //   * two consumer warpgroups (rows 0-63 and 64-127) issue wgmma.mma_async (M = 64 each,
 //     N = out channels, K = 32 bytes per instruction) accumulating the whole offset sum in
-//     registers, and store their rows (bias / activation / int8 requantisation) once the tile's
+//     registers (one group stays in flight: a stage is released once the next stage's group is
+//     issued), and store their rows (bias / activation / int8 requantisation) once the tile's
 //     last offset is in; the producers meanwhile fill the stages of the next tile.
 // 384 threads leave 168 registers per thread: room for the accumulator fragment (128 fp32 per
 // consumer thread at N = 256) and for the hoisted per-lane gather addressing of the producers.
@@ -214,7 +215,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
     // ring slot n % TC_INFO_DEPTH and index buffer n % 2; tile < 0 ends the stream.
     auto read_info = [&](int n, uint32_t (&tm)[4]) -> int {
         const int e = n & (TC_INFO_DEPTH - 1);
-        mbar_wait(&info_full[e], (uint32_t)((n / TC_INFO_DEPTH) & 1));
+        mbar_wait_silent(&info_full[e], (uint32_t)((n / TC_INFO_DEPTH) & 1));
         const volatile int32_t *r = info + e * 8;
         const int tile = r[0];
         tm[0] = (uint32_t)r[1]; tm[1] = (uint32_t)r[2]; tm[2] = (uint32_t)r[3]; tm[3] = (uint32_t)r[4];
@@ -261,7 +262,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
             uint32_t tm[4];
             if (read_info(n, tm) < 0) break;
             const int buf = n & 1;
-            mbar_wait(&idx_full[buf], (uint32_t)((n >> 1) & 1));
+            mbar_wait_silent(&idx_full[buf], (uint32_t)((n >> 1) & 1));
             const int32_t *idx_lane = reinterpret_cast<const int32_t *>(smem + idx_off + (size_t)buf * p.idx_bytes) +
                                       pw * ROWS_PW + r0;
             BitIter it(tm);
@@ -273,7 +274,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                 for (int itc = 0; itc < ITERS; ++itc) ridx[itc] = idx_lane[k * 128 + itc * RPI];
             }
             while (k >= 0) {
-                mbar_wait(&empty[stage], phase ^ 1u);
+                mbar_wait_silent(&empty[stage], phase ^ 1u);
                 const uint32_t a_stage = smem_base + (uint32_t)stage * p.stage_bytes;
 #pragma unroll
                 for (int itc = 0; itc < ITERS; ++itc)
@@ -300,7 +301,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
             if (read_info(n, tm) < 0) break;
             BitIter it(tm);
             for (int k = it.next(); k >= 0; k = it.next()) {
-                mbar_wait(&empty[stage], phase ^ 1u);
+                mbar_wait_silent(&empty[stage], phase ^ 1u);
                 const int kw = p.reverse ? p.kv - 1 - k : k;
                 const uint32_t b_stage = smem_base + (uint32_t)stage * p.stage_bytes + p.a_stage_bytes;
                 if (p.b_transposed) {
@@ -341,8 +342,8 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
         const uint32_t blk_bytes = (uint32_t)(p.kv + 1) * 512u;
         for (int n = 0;; ++n) {
             const int b = n & 1, e = n & (TC_INFO_DEPTH - 1);
-            mbar_wait(&idx_empty[b], (uint32_t)(((n >> 1) & 1) ^ 1));
-            mbar_wait(&info_empty[e], (uint32_t)(((n / TC_INFO_DEPTH) & 1) ^ 1));
+            mbar_wait_silent(&idx_empty[b], (uint32_t)(((n >> 1) & 1) ^ 1));
+            mbar_wait_silent(&info_empty[e], (uint32_t)(((n / TC_INFO_DEPTH) & 1) ^ 1));
             int tile = -1;
             if (lane == 0) {
                 const int ticket = atomicAdd(p.sched_state, 1);
@@ -392,8 +393,13 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) acc[i] = (Acc)0;
             BitIter it(tm);
+            // One wgmma group stays in flight across stages: stage s is released once the group of
+            // stage s+1 is issued (wait_group 1), so the next stage's full-barrier wait and MMA issue
+            // overlap the current MMAs.  Groups of one warpgroup retire in issue order, so every row
+            // still sums its offsets in ascending order.
+            int held = -1;                    // stage whose wgmma group may still be reading it
             for (int k = it.next(); k >= 0; k = it.next()) {
-                mbar_wait(&full[stage], phase);
+                mbar_wait_silent(&full[stage], phase);
                 fence_proxy_async_smem();     // cp.async (generic proxy) writes -> wgmma operand reads
                 const uint32_t a16 = (smem_base + (uint32_t)stage * p.stage_bytes + (uint32_t)(wg * 64 * SPAN_A)) >> 4;
                 const uint32_t b16 = (smem_base + (uint32_t)stage * p.stage_bytes + (uint32_t)p.a_stage_bytes) >> 4;
@@ -423,11 +429,20 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                     }
                 }
                 wgmma_commit();
-                wgmma_wait<0>();
+                wgmma_wait<1>();
                 fence_regs(acc);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[stage]);         // this warp is done reading the stage
+                if (held >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty[held]);      // this warp is done reading that stage
+                }
+                held = stage;
                 if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (held >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[held]);
             }
             const int64_t r_lo = (int64_t)tile * TC_TILE_M + wg * 64 + (warp & 3) * 16 + (lane >> 2);
             const int64_t r_hi = r_lo + 8;
