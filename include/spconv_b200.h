@@ -31,6 +31,8 @@
  *           (kernels spconv/csrc/sparse/maxpool.py:41-341)
  *   spx_sparse_add_group / _fwd / _gather (+ spx_conv_rulebook_stage1+2 for the union)
  *        <- functional.sparse_add / sparse_add_hash_based spconv/pytorch/functional.py:441-544
+ *   spx_hash_clear / _insert / _query / _insert_exist / _rank
+ *        <- HashTable (spconv/pytorch/hash.py)        spconv/csrc/hash/core.py
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless the name ends in `_host`;
@@ -394,6 +396,46 @@ int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const int32_t *o
                        int64_t M, int channels, int dtype, void *out, spx_stream_t stream);
 int spx_sparse_add_gather(const int32_t *index, const void *src, int64_t src_rows,
                           const spx_sparse_add_operands *operands, int channels, int dtype, spx_stream_t stream);
+
+/* ------------------------------------------------------------------ hash table */
+
+/*
+ * Replaces the CUDA branch of spconv.pytorch.hash.HashTable (spconv/pytorch/hash.py, spconv/csrc/hash/core.py)
+ * with the semantics of its CPU branch (tsl::robin_map) plus a defined order.  One table is:
+ *   table_keys [max_size] (key_size bytes each), table_values [max_size] (value_size bytes, moved as raw bits),
+ *   first [max_size] int32 (insertion ordinal of the stored key, INT32_MAX = empty slot),
+ *   tag [max_size] (epoch << 32 | position of the last insert_exist write).
+ * key_size and value_size are 4 or 8; 1 <= max_size <= 2^31 - 1 (slots = max_size exactly).  The largest
+ * value of the signed key type marks an empty slot: that key is never stored and is never found.
+ *
+ * clear:        every slot empty, values 0, first INT32_MAX, tag 0.
+ * insert:       keys [n], values [n] or NULL (value 0); key i gets ordinal ordinal_base + i.  The first
+ *               insertion of a key wins; later duplicates and re-inserts leave its value unchanged.  Requires
+ *               ordinal_base + n < max_size (the reference's capacity rule), so a probe always ends.
+ * query:        values [n] (written for found keys only), is_empty [n] = 1 for a missing key.
+ * insert_exist: found keys take the value of their LAST occurrence in the call; missing keys are not inserted
+ *               (is_empty [n] = 1).  epoch in [1, 2^32 - 1] must grow from call to call of one table.
+ * rank:         numbers the stored keys 0 .. count-1 in first-insertion order; ordinal_count = the sum of n
+ *               over all inserts.  assign != 0: each stored value becomes its number (integer values);
+ *               otherwise row r < out_rows of out_keys / out_values gets the key numbered r and its value.
+ *               count [1] (key_size bytes, unsigned) = the number of stored keys, written on the device.
+ * workspace:    spx_hash_workspace_size(n, 0) bytes for insert / insert_exist,
+ *               spx_hash_workspace_size(0, ordinal_count) for rank.  Nothing reads back to the host.
+ */
+size_t spx_hash_workspace_size(int64_t num_keys, int64_t ordinal_count);
+int spx_hash_clear(void *table_keys, void *table_values, int32_t *first, uint64_t *tag, int64_t max_size,
+                   int key_size, int value_size, spx_stream_t stream);
+int spx_hash_insert(void *table_keys, void *table_values, int32_t *first, int64_t max_size, int key_size,
+                    int value_size, const void *keys, const void *values, int64_t n, int64_t ordinal_base,
+                    void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_hash_query(const void *table_keys, const void *table_values, int64_t max_size, int key_size, int value_size,
+                   const void *keys, void *values, uint8_t *is_empty, int64_t n, spx_stream_t stream);
+int spx_hash_insert_exist(const void *table_keys, void *table_values, uint64_t *tag, int64_t max_size, int key_size,
+                          int value_size, const void *keys, const void *values, uint8_t *is_empty, int64_t n,
+                          int64_t epoch, void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_hash_rank(const void *table_keys, void *table_values, const int32_t *first, int64_t max_size, int key_size,
+                  int value_size, int64_t ordinal_count, int assign, void *out_keys, void *out_values,
+                  int64_t out_rows, void *count, void *workspace, size_t workspace_bytes, spx_stream_t stream);
 
 /*
  * int8 inference forward (reference formula: test/test_all_algo.py:272-287,

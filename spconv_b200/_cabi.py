@@ -141,6 +141,16 @@ SIGNATURES = {
                                    c_void_p]),
     "spx_sparse_add_gather": (c_int, [c_void_p, c_void_p, c_int64, POINTER(SparseAddOperands), c_int, c_int,
                                       c_void_p]),
+    "spx_hash_workspace_size": (c_size_t, [c_int64, c_int64]),
+    "spx_hash_clear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
+    "spx_hash_insert": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,
+                                c_int64, c_void_p, c_size_t, c_void_p]),
+    "spx_hash_query": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int64,
+                               c_void_p]),
+    "spx_hash_insert_exist": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p, c_int64, c_int64, c_void_p, c_size_t, c_void_p]),
+    "spx_hash_rank": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_int64, c_int, c_void_p,
+                              c_void_p, c_int64, c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_last_kernel_family": (c_int, []),
     "spx_launch_count": (c_int64, [c_int]),
     "spx_debug_configure": (c_int, [c_int, c_int, c_int, c_void_p, c_size_t]),

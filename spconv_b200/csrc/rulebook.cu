@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "gemm.cuh"
 #include "hash.cuh"
+#include "rank.cuh"
 #include <cub/cub.cuh>
 
 namespace spx {
@@ -439,16 +440,9 @@ conv_insert_append_kernel(Table table, Geom g, const int32_t *__restrict__ indic
 
 // ---- ranking the outputs by first touch WITHOUT a sort.  Every output's final payload p = k*N + i
 // (the smallest (offset, input) pair that produces it) is distinct, so the rank of an output is the
-// number of outputs with a smaller payload = the number of set bits below p in a bitmap over
-// [0, kv*N).  mark: one atomicOr per output (+ a count per 1024-bit tile); scan: exclusive prefix over
-// the tile counts (one block); assign: tile prefix + popcount of at most 32 words.  Replaces the
-// radix sort of the payloads (1 + 2 x 3 launches at 22 key bits) by one single-block kernel.
-constexpr int RANK_TILE_WORDS = 32;              // bitmap words per counted tile (1024 payloads)
-static size_t rank_scratch_bytes(int64_t kvn, int64_t *ntiles = nullptr) {
-    const int64_t words = div_up64(kvn > 0 ? kvn : 1, 32), tiles = div_up64(words, RANK_TILE_WORDS);
-    if (ntiles) *ntiles = tiles;
-    return align_up((size_t)(tiles * RANK_TILE_WORDS + tiles + 1) * 4, 256);
-}
+// number of outputs with a smaller payload: the bitmap / tile-prefix / popcount ranking of rank.cuh
+// over [0, kv*N).  conv_mark_kernel marks and its last block builds the tile prefix;
+// conv_assign_rank_kernel ranks.  Replaces a radix sort of the payloads (1 + 2 x 3 launches at 22 key bits).
 
 // one launch clears everything stage 1 needs: hash table (0xFF), 64-bit-key value array (0x7F), ranking scratch and counters (0)
 __global__ void conv_clear_kernel(uint4 *__restrict__ table, int64_t table_vec, uint4 *__restrict__ tvals, int64_t tvals_vec,
@@ -468,39 +462,10 @@ __global__ void __launch_bounds__(MARK_THREADS)
 conv_mark_kernel(Table table, const uint32_t *__restrict__ slot_list, int64_t M, uint32_t *__restrict__ bitmap,
                  int *__restrict__ tile_cnt, int64_t tiles, int *__restrict__ done) {
     const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (j < M) {
-        const uint32_t p = (uint32_t)table.value_at(slot_list[j]);   // final: all inserts finished in an earlier kernel
-        atomicOr(&bitmap[p >> 5], 1u << (p & 31));
-        atomicAdd(&tile_cnt[p >> 10], 1);
-    }
-    __shared__ int warp_sums[MARK_THREADS / 32];
-    __shared__ int carry_s, last_s;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) { last_s = atomicAdd(done, 1) == (int)gridDim.x - 1; carry_s = 0; }
-    __syncthreads();
-    if (!last_s) return;
-    __threadfence();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int64_t t0 = 0; t0 < tiles; t0 += MARK_THREADS) {
-        const int64_t t = t0 + threadIdx.x;
-        const int v = t < tiles ? __ldcg(tile_cnt + t) : 0;
-        int incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int up = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += up;
-        }
-        if (lane == 31) warp_sums[warp] = incl;
-        __syncthreads();
-        int wbase = 0;
-        for (int w = 0; w < warp; ++w) wbase += warp_sums[w];
-        const int carry = carry_s;
-        if (t < tiles) tile_cnt[t] = carry + wbase + incl - v;
-        __syncthreads();
-        if (threadIdx.x == MARK_THREADS - 1) carry_s = carry + wbase + incl;
-        __syncthreads();
-    }
+    if (j < M)      // final payload: all inserts finished in an earlier kernel
+        rank_mark((uint32_t)table.value_at(slot_list[j]), bitmap, tile_cnt);
+    int total;
+    rank_prefix_last_block<MARK_THREADS>(tile_cnt, tiles, done, &total);
 }
 
 // created slot j -> rank r of its payload: write r into the slot, decode the key into out_inds[r]
@@ -516,9 +481,7 @@ __global__ void conv_assign_rank_kernel(Table table, Geom g, const uint32_t *__r
     const uint32_t s = slot_list[j];
     int64_t key; int32_t val;
     table.occupied(s, key, val);
-    const uint32_t p = (uint32_t)val, word = p >> 5, first = word & ~(uint32_t)(RANK_TILE_WORDS - 1);
-    int r = __ldg(tile_prefix + (p >> 10)) + __popc(__ldg(bitmap + word) & ((1u << (p & 31)) - 1u));
-    for (uint32_t wd = first; wd < word; ++wd) r += __popc(__ldg(bitmap + wd));
+    const int r = rank_of((uint32_t)val, bitmap, tile_prefix);
     table.set_value(s, r);
     if (mask_zero) mask_zero[r] = 0u;              // the pairs kernel ORs the forward masks into it
     int32_t *dst = out_inds + (int64_t)r * (g.ndim + 1);
