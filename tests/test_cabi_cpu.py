@@ -53,8 +53,27 @@ def test_host_only_entry_points(lib):
     assert lib.spx_rulebook_workspace_size(ctypes.byref(g), 100000, 0, 1) >= 2 * 100000 * 8
     assert lib.spx_mask_argsort_workspace_size(100000, 1) > 100000 * 4 * 4
     assert lib.spx_native_pairs_workspace_size(100000, 27) > 0
-    assert lib.spx_launch_count(1) == 0
-    assert lib.spx_last_kernel_family() == 0
+    # The launch counter and the last kernel family are process-wide, and GPU tests may have run in this
+    # process before: check in a fresh process that the host entry points launch nothing.
+    import subprocess
+    import sys
+    script = "\n".join([
+        "import ctypes, sys",
+        f"sys.path.insert(0, {ROOT!r})",
+        "from spconv_b200 import _cabi",
+        "lib = _cabi.load()",
+        "g = _cabi.make_geometry(3, 1, [41, 1600, 1408], [21, 800, 704], [3] * 3, [2] * 3, [1] * 3, [1] * 3)",
+        "lib.spx_version()",
+        "lib.spx_conv_max_out(ctypes.byref(g), 1000)",
+        "lib.spx_rulebook_workspace_size(ctypes.byref(g), 100000, 0, 0)",
+        "lib.spx_rulebook_workspace_size(ctypes.byref(g), 100000, 0, 1)",
+        "lib.spx_mask_argsort_workspace_size(100000, 1)",
+        "lib.spx_native_pairs_workspace_size(100000, 27)",
+        "print(lib.spx_launch_count(1), lib.spx_last_kernel_family())",
+    ])
+    res = subprocess.run([sys.executable, "-c", script], capture_output=True, text=True)
+    assert res.returncode == 0, res.stderr
+    assert res.stdout.split() == ["0", "0"], res.stdout
 
 
 def test_argument_validation_reports_errors(lib):

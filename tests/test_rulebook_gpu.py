@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.util import random_cloud, surface_cloud
+from tests.util import check_tile_table, random_cloud, surface_cloud
 
 pytestmark = pytest.mark.gpu
 
@@ -205,30 +205,10 @@ def test_fused_subm_tile_table_matches_column_path(cuda_dev):
     t_rows, m_rows = cache[1], cache[2]
     t_cols, m_cols = ops._tile_tables(pair_fwd, mask, argsort, n, 27, owner=None)
     assert torch.equal(t_rows, t_cols) and torch.equal(m_rows, m_cols)
-    pf = pair_fwd.cpu().numpy()
-    tiles = (n + 127) // 128
-    flat = t_rows.cpu().numpy()
-    tab = flat[:tiles * 28 * 128].reshape(tiles, 28, 128)
-    order = argsort.cpu().numpy()
-    padded = np.full(tiles * 128, -1, np.int64)
-    padded[:n] = order
-    assert np.array_equal(tab[:, 27, :].reshape(-1), padded)
-    want = np.where(padded[None, :] >= 0, pf[:, np.maximum(padded, 0)], -1)            # [27, tiles*128]
-    assert np.array_equal(tab[:, :27, :].transpose(1, 0, 2).reshape(27, -1), want)
-    sm = np.zeros(tiles * 128, np.uint32)
-    sm[:n] = mask.cpu().numpy().reshape(-1).view(np.uint32)
-    assert np.array_equal(m_rows.cpu().numpy().reshape(-1).view(np.uint32),
-                          np.bitwise_or.reduce(sm.reshape(tiles, 128), axis=1))
-    # schedule records behind the blocks: every tile once, heaviest (most offsets) first, ties in
-    # ascending tile order; scheduler scratch zeroed
-    rec = flat[tiles * 28 * 128: tiles * 28 * 128 + tiles * 8].reshape(tiles, 8)
-    tmask = m_rows.cpu().numpy().reshape(-1).view(np.uint32)
-    cost = np.array([bin(int(v)).count("1") for v in np.where(tmask == 0, 1, tmask)])
-    want_order = np.argsort(-cost, kind="stable")
-    assert np.array_equal(rec[:, 0], want_order)
-    assert np.array_equal(rec[:, 1].view(np.uint32), np.where(tmask == 0, 1, tmask)[want_order])
-    assert (rec[:, 2:] == 0).all()
-    assert (flat[tiles * 28 * 128 + tiles * 8:] == 0).all() and flat.shape[0] == tiles * 28 * 128 + tiles * 8 + 64
+    # blocks, tile masks, schedule records (every tile once, heaviest first, ties in ascending tile
+    # order) and the zeroed scheduler scratch
+    check_tile_table(t_rows.cpu().numpy(), m_rows.cpu().numpy(), pair_fwd.cpu().numpy(), mask.cpu().numpy(),
+                     argsort.cpu().numpy(), n, 27, 1)
 
 
 TIMER_CASES = [CASES[0], CASES[7], CASES[2],

@@ -62,6 +62,48 @@ def assert_equals_reference(key, got, compute_ref, oracle):
     assert digest(got) == stored[key], f"{key}: output differs from the reference's (digest mismatch)"
 
 
+def check_tile_table(table, tile_mask, pair, mask, argsort, rows, kv, words, name="tile table"):
+    """Restates spx_build_tile_table's output from the rulebook it was built from (numpy arrays).
+
+    table [tiles*(kv+1)*128 + tiles*8 + 64]: per 128-row tile one block of kv rows of gather indices
+    (pair[k, argsort[j]] where bit k of the sorted mask row j is set, else -1) and one row of argsort
+    (-1 past the end); then one 8-int schedule record per tile: the tiles heaviest first (most set bits
+    of the tile mask, an empty tile counted as one stage with mask word 0 = 1), ties in ascending tile
+    order, as (tile, mask words 0-3, 0, 0, 0); then 64 ints of scheduler scratch, zero between launches.
+    tile_mask [tiles, words]: per-tile OR of the sorted masks."""
+    tiles = (rows + 127) // 128
+    blocks_len = tiles * (kv + 1) * 128
+    assert table.shape == (blocks_len + tiles * 8 + 64,), f"{name}: {table.shape[0]} ints for {tiles} tiles"
+    blocks = table[:blocks_len].reshape(tiles, kv + 1, 128)
+    src = np.full(tiles * 128, -1, np.int64)
+    src[:rows] = argsort
+    assert np.array_equal(blocks[:, kv, :].reshape(-1), src), f"{name}: argsort row of the blocks"
+    sm = np.zeros((tiles * 128, 4), np.uint32)
+    sm[:rows, :words] = np.asarray(mask).view(np.uint32).reshape(rows, words)
+    col = np.maximum(src, 0)
+    for k in range(kv):
+        hit = (((sm[:, k // 32] >> np.uint32(k % 32)) & 1) == 1) & (src >= 0)
+        got = blocks[:, k, :].reshape(-1)
+        want = np.where(hit, pair[k][col], -1)
+        bad = np.nonzero(got != want)[0]
+        assert not len(bad), (f"{name}: offset {k}: {len(bad)} gather entries differ, first at row {bad[0]} "
+                              f"(tile {bad[0] // 128}): got {got[bad[0]]} want {want[bad[0]]}")
+    tm = np.bitwise_or.reduce(sm.reshape(tiles, 128, 4), axis=1)
+    assert np.array_equal(np.asarray(tile_mask).view(np.uint32).reshape(tiles, words), tm[:, :words]), \
+        f"{name}: tile masks"
+    eff = tm.copy()
+    eff[~eff.any(axis=1), 0] = 1
+    cost = np.bitwise_count(eff).sum(axis=1)
+    order = np.argsort(-cost, kind="stable")
+    rec = table[blocks_len:blocks_len + tiles * 8].reshape(tiles, 8)
+    bad = np.nonzero(rec[:, 0] != order)[0]
+    assert not len(bad), (f"{name}: schedule order differs at record {bad[0]} of {tiles}: tile {rec[bad[0], 0]}, "
+                          f"want {order[bad[0]]}")
+    assert np.array_equal(rec[:, 1:5].view(np.uint32), eff[order]), f"{name}: record masks"
+    assert (rec[:, 5:] == 0).all(), f"{name}: record padding"
+    assert (table[blocks_len + tiles * 8:] == 0).all(), f"{name}: scheduler scratch is not zero"
+
+
 def rel_l2(a, b):
     a = np.asarray(a, dtype=np.float64)
     b = np.asarray(b, dtype=np.float64)
