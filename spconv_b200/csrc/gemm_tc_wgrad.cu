@@ -40,13 +40,14 @@ constexpr int WG_MAX_STAGES = 6;
 constexpr int WG_SMEM_BUDGET = 200 * 1024;    // operand stages are sized inside this ...
 constexpr int WG_SMEM_MAX = 224 * 1024;       // ... what is left up to here buys deeper index prefetch
 constexpr int WG_MAX_IDX = 4;                 // index-block ring depth (prefetch distance = depth - 1 tiles)
+constexpr int WG_MAX_B = 3;                   // dout tile buffers
 
 struct WgParams {
     const uint8_t *x; int xb, span_x, lg_span_x, apo, apg, atom_elems;
     const uint8_t *d; int db, span_d, lg_span_d, lg_cpr_d;
     int n, ab_bf16;
     int groups_total, groups_per_pass;
-    int stages, a_stage_bytes, b_buf_bytes, idx_bytes, idx_bufs;
+    int stages, a_stage_bytes, b_buf_bytes, b_bufs, idx_bytes, idx_bufs;
     int64_t rows;
     const int32_t *tile_table;   // [tiles][kv+1][128]
     const uint32_t *tile_mask;   // [tiles][words]
@@ -55,30 +56,38 @@ struct WgParams {
     float *partial; int64_t partial_stride;
 };
 
-// Offset slots are filled in the order 0, kv-1, 1, kv-2, ...: a group (one M = 128 accumulator)
-// then stacks an offset with its point mirror.  On surface-like clouds a voxel that has the
-// neighbour +d usually has -d too, so the two halves of a group are active together and almost no
-// all-zero atom is gathered (with the natural order k, k+1 about half of the gathered atoms of
-// config 2 were zero fill).  Any permutation is valid; this one only changes which accumulator
-// rows an offset owns.
-__device__ __forceinline__ int slot_offset(int slot, int kv) {
-    if (slot >= kv) return kv;                       // padding slot of the last group
-    return (slot & 1) ? kv - 1 - (slot >> 1) : (slot >> 1);
-}
+// Atoms are stacked in natural offset order: atom a holds channels (a % apo) of offset a / apo, and a
+// group (one M = 128 accumulator) covers atoms [g apg, (g + 1) apg) -- offsets k, k + 1 for 64
+// 16-bit channels; atoms past kv apo in the last group are padding.  Pairing k with its point
+// mirror kv-1-k was tried: on tilted surface patches the two are rarely active together (the
+// dz = +-1 groups of config 2 had both halves active in 1-23 of their 48-270 active tiles), and 37 %
+// of its warpgroup-atom wgmma multiplied zero fill; natural pairs cut the stages from 5543 to 4761
+// (tools/wgrad_schedule_model.py).
 
-// bit gl set iff group gl of this pass has an active offset in the tile
-__device__ __forceinline__ uint32_t active_groups(const uint32_t (&tm)[4], const uint32_t *gmask, int ng, int words) {
+// bit gl: the atoms of local group gl that warpgroup 0 reads (M rows 0-63) hold an offset active in
+// the tile; bit 16 + gl: the same for warpgroup 1 (rows 64-127).  gmask = [16][2 halves][4 words].
+__device__ __forceinline__ uint32_t active_halves(const uint32_t (&tm)[4], const uint32_t *gmask, int ng, int words) {
     uint32_t act = 0;
     if (words == 1) {                                   // kv <= 32: the common 3x3x3 case
-        for (int gl = 0; gl < ng; ++gl) act |= (tm[0] & gmask[gl * 4]) ? 1u << gl : 0u;
+        for (int gl = 0; gl < ng; ++gl) {
+            act |= (tm[0] & gmask[gl * 8]) ? 1u << gl : 0u;
+            act |= (tm[0] & gmask[gl * 8 + 4]) ? 0x10000u << gl : 0u;
+        }
         return act;
     }
-    for (int gl = 0; gl < ng; ++gl) {
-        const uint32_t hit = (tm[0] & gmask[gl * 4]) | (tm[1] & gmask[gl * 4 + 1]) | (tm[2] & gmask[gl * 4 + 2]) |
-                             (tm[3] & gmask[gl * 4 + 3]);
-        if (hit) act |= 1u << gl;
-    }
+    for (int gl = 0; gl < ng; ++gl)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t *m = gmask + gl * 8 + h * 4;
+            if ((tm[0] & m[0]) | (tm[1] & m[1]) | (tm[2] & m[2]) | (tm[3] & m[3])) act |= 1u << (16 * h + gl);
+        }
     return act;
+}
+
+// mask bits of offsets k_lo..k_hi.  The offsets of half a group are an aligned run of 1, 2 or 4
+// offsets (apg / apo is a power of two), so they never straddle a mask word.
+__device__ __forceinline__ uint32_t offset_run_bits(int k_lo, int k_hi) {
+    return (2u << (k_hi & 31)) - (1u << (k_lo & 31));
 }
 
 // record visited by CTA `chunk` at step i (snake order over the cost-sorted schedule records)
@@ -132,46 +141,45 @@ tc_wgrad_kernel(const WgParams p) {
     const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
     uint8_t *smem = smem_raw + pad;
     const uint32_t smem_base = raw_addr + pad;
-    // layout: [2 x B buffer][stages x A stage][idx_bufs x index block][barriers]
+    // layout: [b_bufs x B buffer][stages x A stage][idx_bufs x index block][barriers]
     const uint32_t b_base = smem_base;
-    const uint32_t a_base = smem_base + 2u * p.b_buf_bytes;
-    const uint32_t idx_off = 2u * p.b_buf_bytes + (uint32_t)p.stages * p.a_stage_bytes;
+    const uint32_t a_base = smem_base + (uint32_t)p.b_bufs * p.b_buf_bytes;
+    const uint32_t idx_off = (uint32_t)p.b_bufs * p.b_buf_bytes + (uint32_t)p.stages * p.a_stage_bytes;
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + idx_off + (uint32_t)p.idx_bufs * p.idx_bytes);
     uint64_t *full_a = bars;                          // [stages]
     uint64_t *empty_a = bars + WG_MAX_STAGES;         // [stages]
-    uint64_t *full_b = bars + 2 * WG_MAX_STAGES;      // [2]
-    uint64_t *empty_b = bars + 2 * WG_MAX_STAGES + 2; // [2]
-    uint64_t *idx_full = bars + 2 * WG_MAX_STAGES + 4;                // [WG_MAX_IDX]
-    uint64_t *idx_empty = bars + 2 * WG_MAX_STAGES + 4 + WG_MAX_IDX;  // [WG_MAX_IDX]
-    uint32_t *gmask = reinterpret_cast<uint32_t *>(bars + 2 * WG_MAX_STAGES + 4 + 2 * WG_MAX_IDX);  // [32][4] offsets covered by each group of this pass
-    uint32_t *slot_info = gmask + 32 * 4;             // [WG_MAX_IDX][8]: {active groups, tile mask[4]} per ring slot
+    uint64_t *full_b = bars + 2 * WG_MAX_STAGES;                // [WG_MAX_B]
+    uint64_t *empty_b = bars + 2 * WG_MAX_STAGES + WG_MAX_B;     // [WG_MAX_B]
+    uint64_t *idx_full = bars + 2 * WG_MAX_STAGES + 2 * WG_MAX_B;                // [WG_MAX_IDX]
+    uint64_t *idx_empty = bars + 2 * WG_MAX_STAGES + 2 * WG_MAX_B + WG_MAX_IDX;  // [WG_MAX_IDX]
+    uint32_t *gmask = reinterpret_cast<uint32_t *>(bars + 2 * WG_MAX_STAGES + 2 * WG_MAX_B + 2 * WG_MAX_IDX);  // [16][2][4] offsets of each warpgroup's half of each group of this pass
+    uint32_t *slot_info = gmask + 16 * 8;             // [WG_MAX_IDX][8]: {active halves, tile mask[4]} per ring slot
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int64_t num_tiles = (p.rows + WG_TILE - 1) / WG_TILE;
     const int chunk = blockIdx.x, chunks = gridDim.x;
-    // Groups are dealt to the passes round-robin (pass y owns groups y, y + passes, ...): with the
-    // mirror-paired slot order the frequently active in-plane offsets sit in neighbouring groups,
-    // and a contiguous split gave one pass 70 % of the stages of the 100 k-voxel cloud.
+
+    // Groups are dealt to the passes round-robin (pass y owns groups y, y + passes, ...).  Balancing the
+    // passes by their active-tile counts (LPT, computed in every CTA's prologue) cut the busiest CTA of
+    // config 2 from 54 to 41 stages, but not the training step: the input-gradient kernel runs beside
+    // this one and fills the SMs that lighter passes leave early, so the step pays for total SM time,
+    // which the prologue only adds to (DESIGN.md section 7).
     const int g_first = blockIdx.y, g_step = gridDim.y;
     const int ng = g_first < p.groups_total ? (p.groups_total - g_first + g_step - 1) / g_step : 0;
-
     if (threadIdx.x < 32) {
-        // group gl covers atoms [g*apg, (g+1)*apg) -> offset slots a / apo; one thread per group
-        const int g = g_first + (int)threadIdx.x * g_step;
-        uint32_t m[4] = {0, 0, 0, 0};
-        if ((int)threadIdx.x < ng) {
-            for (int a = g * p.apg; a < (g + 1) * p.apg; ++a) {
-                const int k = slot_offset(a / p.apo, p.kv);
-                if (k < p.kv) m[k >> 5] |= 1u << (k & 31);
-            }
-        }
+        // local group gl = thread / 2, warpgroup half h = thread % 2: atoms [g apg + h apg / 2, ...)
+        const int gl = (int)threadIdx.x >> 1, h = (int)threadIdx.x & 1;
+        const int g = g_first + gl * g_step, hp = p.apg >> 1;
+        const int k_lo = (g * p.apg + h * hp) / p.apo;
+        const int k_hi = min((g * p.apg + (h + 1) * hp - 1) / p.apo, p.kv - 1);
+        const uint32_t bits = gl < ng && k_lo <= k_hi ? offset_run_bits(k_lo, k_hi) : 0u;
 #pragma unroll
-        for (int w = 0; w < 4; ++w) gmask[threadIdx.x * 4 + w] = m[w];
+        for (int w = 0; w < 4; ++w) gmask[threadIdx.x * 4 + w] = w == (k_lo >> 5) ? bits : 0u;
     }
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) { mbar_init(&full_a[s], WG_PROD_THREADS); mbar_init(&empty_a[s], WG_CONS_WARPS); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&full_b[b], WG_PROD_THREADS); mbar_init(&empty_b[b], WG_CONS_WARPS); }
+        for (int b = 0; b < p.b_bufs; ++b) { mbar_init(&full_b[b], WG_PROD_THREADS); mbar_init(&empty_b[b], WG_CONS_WARPS); }
         for (int b = 0; b < p.idx_bufs; ++b) { mbar_init(&idx_full[b], 1); mbar_init(&idx_empty[b], WG_PROD_WARPS); }
         mbar_fence_init();
     }
@@ -181,7 +189,7 @@ tc_wgrad_kernel(const WgParams p) {
         // ================================================= producers
         const int pw = warp - WG_CONS_WARPS;
         int stage = 0; uint32_t phase = 0;
-        int64_t nb = 0;                                  // B buffers filled so far
+        int bbuf = 0; uint32_t bphase = 0;               // next B buffer to fill, its phase
         // per-lane constants of the atom gather: chunk chb of rows r0 + itc*RPI of this warp's rows
         const int r0 = lane >> LG_CPA;
         const uint32_t chb = (uint32_t)(lane & (CPA - 1)) << 4;
@@ -199,21 +207,19 @@ tc_wgrad_kernel(const WgParams p) {
         const int nring = p.idx_bufs;
         // dout tile (B operand) of the tile whose index block is idx_s; source rows = block row kv
         auto issue_b = [&](const int32_t *idx_s) {
-            const int bb = (int)(nb & 1);
-            mbar_wait(&empty_b[bb], (uint32_t)(((nb >> 1) & 1) ^ 1));
+            const int bb = bbuf;
+            mbar_wait_silent(&empty_b[bb], bphase ^ 1u);
             const uint32_t dstb = b_base + (uint32_t)bb * p.b_buf_bytes;
             const int32_t *rows_s = idx_s + p.kv * 128 + pw * ROWS_PW + rd0;
-            int32_t rsrc[ITERS_D];
-#pragma unroll
-            for (int itc = 0; itc < ITERS_D; ++itc) rsrc[itc] = rows_s[itc * RPI_D];
             if constexpr (TF32) {
-                // batches of 8 rows keep the float4 loads in flight without spilling
+                // batches of 8 rows keep the float4 loads in flight without spilling; the row indices
+                // are read per batch, as a whole-tile register array would be indexed dynamically
 #pragma unroll 1
                 for (int i0 = 0; i0 < ITERS_D; i0 += 8) {
                     float4 v[8];
 #pragma unroll
                     for (int i = 0; i < 8; ++i) {
-                        const int32_t r = i0 + i < ITERS_D ? rsrc[i0 + i] : -1;
+                        const int32_t r = i0 + i < ITERS_D ? rows_s[(i0 + i) * RPI_D] : -1;
                         v[i] = r >= 0 ? __ldg(reinterpret_cast<const float4 *>(d_lane + (int64_t)r * DB)) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
 #pragma unroll
@@ -224,6 +230,9 @@ tc_wgrad_kernel(const WgParams p) {
                 fence_proxy_async_smem();
                 mbar_arrive(&full_b[bb]);
             } else {
+                int32_t rsrc[ITERS_D];                    // all index loads first, then the copies
+#pragma unroll
+                for (int itc = 0; itc < ITERS_D; ++itc) rsrc[itc] = rows_s[itc * RPI_D];
 #pragma unroll
                 for (int itc = 0; itc < ITERS_D; ++itc) {
                     const uint32_t row_in_tile = (uint32_t)(pw * ROWS_PW + rd0 + itc * RPI_D);
@@ -233,7 +242,7 @@ tc_wgrad_kernel(const WgParams p) {
                 }
                 cp_async_mbar_arrive_noinc(&full_b[bb]);
             }
-            ++nb;
+            if (++bbuf == p.b_bufs) { bbuf = 0; bphase ^= 1u; }
         };
         auto idx_block = [&](int b) {
             return reinterpret_cast<const int32_t *>(smem + idx_off + (size_t)b * p.idx_bytes);
@@ -242,7 +251,7 @@ tc_wgrad_kernel(const WgParams p) {
         // tile's group set) filled nring-1 tiles ahead; right after the first x stage of tile t
         // the dout tile of t+1 is issued -- nothing but the first x stage sits on the boundary.
         auto read_slot = [&](int slot, uint32_t use, uint32_t (&m)[4]) -> uint32_t {
-            mbar_wait(&idx_full[slot], use & 1u);
+            mbar_wait_silent(&idx_full[slot], use & 1u);
             const volatile uint32_t *r = slot_info + slot * 8;
             m[0] = r[1]; m[1] = r[2]; m[2] = r[3]; m[3] = r[4];
             return r[0];
@@ -266,14 +275,17 @@ tc_wgrad_kernel(const WgParams p) {
                 next_ready = true;
             };
             const int32_t *idx_s = idx_block(cur_slot);
-            // ---- gathered x atoms, one stage per active group
-            for (uint32_t rem = act; rem; rem &= rem - 1) {
-                const int g = g_first + (__ffs(rem) - 1) * g_step;
-                mbar_wait(&empty_a[stage], phase ^ 1u);
+            // ---- gathered x atoms, one stage per active group.  A warpgroup's half without an active
+            // offset is not copied at all: its consumer warpgroup skips the stage's wgmma.
+            for (uint32_t rem = (act | act >> 16) & 0xFFFFu; rem; rem &= rem - 1) {
+                const int gl = __ffs(rem) - 1;
+                const int g = g_first + gl * g_step;
+                mbar_wait_silent(&empty_a[stage], phase ^ 1u);
                 const uint32_t a_stage = a_base + (uint32_t)stage * p.a_stage_bytes;
                 for (int s = 0; s < p.apg; ++s) {
+                    if (!((act >> (gl + (s >= (p.apg >> 1) ? 16 : 0))) & 1u)) continue;
                     const int a = g * p.apg + s;
-                    const int k = slot_offset(a >> lg_apo, p.kv);
+                    const int k = a >> lg_apo;
                     const int cb = a & (p.apo - 1);
                     const bool active = k < p.kv && ((pick_word(tm, k >> 5) >> (k & 31)) & 1u);
                     const int32_t *idx_k = idx_s + (active ? k : 0) * 128 + pw * ROWS_PW + r0;
@@ -318,7 +330,7 @@ tc_wgrad_kernel(const WgParams p) {
     } else if (warp == WG_SCHED_WARP) {
         // ================================================= tile feeder
         // Per tile of this CTA (static snake order, so the summation order of dW is fixed): compute
-        // the active groups of this pass from the tile mask, publish them with the mask through
+        // the active group halves of this pass from the tile mask, publish them with the mask through
         // the ring slot, and bulk-copy the tile's index block -- only when the pass has work for
         // the tile.  Schedule records are fetched 32 at a time, one per lane.
         const uint32_t blk_bytes = (uint32_t)(p.kv + 1) * 512u;
@@ -335,8 +347,8 @@ tc_wgrad_kernel(const WgParams p) {
 #pragma unroll
             for (int w = 0; w < 4; ++w) tm[w] = __shfl_sync(0xffffffffu, mw[w], (int)(i & 31));
             const int64_t tile = __shfl_sync(0xffffffffu, mtile, (int)(i & 31));
-            const uint32_t act = active_groups(tm, gmask, ng, p.words);
-            mbar_wait(&idx_empty[slot], (use & 1u) ^ 1u);
+            const uint32_t act = active_halves(tm, gmask, ng, p.words);
+            mbar_wait_silent(&idx_empty[slot], (use & 1u) ^ 1u);
             if (lane == 0) {
                 uint32_t *r = slot_info + slot * 8;
                 r[0] = act; r[1] = tm[0]; r[2] = tm[1]; r[3] = tm[2]; r[4] = tm[3];
@@ -355,7 +367,7 @@ tc_wgrad_kernel(const WgParams p) {
         // ================================================= consumers: warpgroup wg owns M rows 64 wg .. 64 wg + 63 of every group
         const int wg = warp >> 2;
         int stage = 0; uint32_t phase = 0;
-        int64_t nb = 0;
+        int bbuf = 0; uint32_t bphase = 0;               // next B buffer to read, its phase
         uint32_t tm[4] = {0, 0, 0, 0};
         int64_t tile_unused = 0;
         if (wg_rec_index(0, chunk, chunks) < num_tiles)
@@ -373,19 +385,39 @@ tc_wgrad_kernel(const WgParams p) {
         for (int gl = 0; gl < G; ++gl)
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) acc[gl][i] = 0.f;
+        // One wgmma group stays in flight: it reads A stage `held` and, when it was the last group of its
+        // tile, dout buffer `held_b`; both are released once it has retired (wait_group 1 after the next
+        // group is issued).  A stage this warpgroup has no active atoms in is not multiplied (its rows
+        // are zero): the group in flight is retired and both stages are released at once, so the
+        // producers never wait on a stage held across stages this warpgroup skips.
+        int held = -1, held_b = -1;
         for (int64_t step = 0; wg_rec_index(step, chunk, chunks) < num_tiles; ++step) {
             const int64_t next = wg_rec_index(step + 1, chunk, chunks);
             uint32_t tm_next[4] = {0, 0, 0, 0};
             if (next < num_tiles) wg_load_rec(p.sched_rec, next, tile_unused, tm_next);
-            const uint32_t act = active_groups(tm, gmask, ng, p.words);
+            const uint32_t halves = active_halves(tm, gmask, ng, p.words);
+            const uint32_t act = (halves | halves >> 16) & 0xFFFFu;
+            const uint32_t mine = (halves >> (16 * wg)) & 0xFFFFu;
             if (act) {
-                const int bb = (int)(nb & 1);
-                mbar_wait(&full_b[bb], (uint32_t)((nb >> 1) & 1));
+                const int bb = bbuf;
+                mbar_wait_silent(&full_b[bb], bphase);
                 const uint32_t b16 = (b_base + (uint32_t)bb * p.b_buf_bytes) >> 4;
 #pragma unroll
                 for (int gl = 0; gl < G; ++gl) {
                     if (!((act >> gl) & 1u)) continue;
-                    mbar_wait(&full_a[stage], phase);
+                    mbar_wait_silent(&full_a[stage], phase);
+                    if (!((mine >> gl) & 1u)) {
+                        wgmma_wait<0>();
+                        __syncwarp();
+                        if (lane == 0) {
+                            if (held >= 0) mbar_arrive(&empty_a[held]);
+                            if (held_b >= 0) mbar_arrive(&empty_b[held_b]);
+                            mbar_arrive(&empty_a[stage]);
+                        }
+                        held = -1; held_b = -1;
+                        if (++stage == p.stages) { stage = 0; phase ^= 1u; }
+                        continue;
+                    }
                     fence_proxy_async_smem();     // generic-proxy writes (cp.async / st.shared) -> wgmma operand reads
                     const uint32_t a16 = (a_base + (uint32_t)stage * p.a_stage_bytes + a_wg) >> 4;
                     fence_regs(acc[gl]);
@@ -407,19 +439,30 @@ tc_wgrad_kernel(const WgParams p) {
                         }
                     }
                     wgmma_commit();
-                    wgmma_wait<0>();
+                    wgmma_wait<1>();
                     fence_regs(acc[gl]);
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_a[stage]);
+                    if (lane == 0) {
+                        if (held >= 0) mbar_arrive(&empty_a[held]);
+                        if (held_b >= 0) mbar_arrive(&empty_b[held_b]);
+                    }
+                    held = stage; held_b = -1;
                     if (++stage == p.stages) { stage = 0; phase ^= 1u; }
                 }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_b[bb]);
-                ++nb;
+                if (held >= 0) {
+                    held_b = bb;                  // released with the tile's last group
+                } else {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_b[bb]);
+                }
+                if (++bbuf == p.b_bufs) { bbuf = 0; bphase ^= 1u; }
             }
 #pragma unroll
             for (int w = 0; w < 4; ++w) tm[w] = tm_next[w];
         }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int gl = 0; gl < G; ++gl) fence_regs(acc[gl]);
         // ================================================= accumulators -> fp32 partials
         // register i of thread t holds M row 64 wg + 16 (warp % 4) + t / 4 + 8 ((i / 2) % 2),
         // column 8 (i / 4) + 2 (t % 4) + i % 2
@@ -434,9 +477,8 @@ tc_wgrad_kernel(const WgParams p) {
                 const int s = L / p.atom_elems;
                 const int ce = L - s * p.atom_elems;
                 const int a = g * p.apg + s;
-                const int ks = a / p.apo;
-                const int k = slot_offset(ks, p.kv);
-                const int c = (a - ks * p.apo) * p.atom_elems + ce;
+                const int k = a / p.apo;
+                const int c = (a - k * p.apo) * p.atom_elems + ce;
                 if (k >= p.kv) continue;
                 float *dst = part + (int64_t)k * p.c_in + c;
 #pragma unroll
@@ -532,7 +574,12 @@ static bool make_plan(const WgradArgs &a, WgPlan &pl) {
     if (avail < 2 * p.a_stage_bytes) return false;
     p.stages = avail / p.a_stage_bytes;
     if (p.stages > WG_MAX_STAGES) p.stages = WG_MAX_STAGES;
+    // A third dout buffer where it fits: the producers issue the dout tile of tile t+1 right after the
+    // first x stage of tile t, and with two buffers that waits until the consumers have retired the
+    // last group of tile t-1 -- a gather latency on every tile.  Stage count and index ring come first.
+    p.b_bufs = 2;
     size_t fixed = 2 * (size_t)p.b_buf_bytes + (size_t)p.stages * p.a_stage_bytes + 1024 + 1024;
+    if (fixed + p.b_buf_bytes + 2 * (size_t)p.idx_bytes <= (size_t)WG_SMEM_MAX) { p.b_bufs = 3; fixed += p.b_buf_bytes; }
     p.idx_bufs = 2;
     while (p.idx_bufs < WG_MAX_IDX && fixed + (size_t)(p.idx_bufs + 1) * p.idx_bytes <= (size_t)WG_SMEM_MAX) ++p.idx_bufs;
     pl.smem = fixed + (size_t)p.idx_bufs * p.idx_bytes;
