@@ -147,6 +147,40 @@ int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const int32_t *indi
                                  void *workspace, size_t workspace_bytes, spx_stream_t stream);
 
 /*
+ * Regular / transposed conv rulebook with the output count kept on the device: the bounded twin of
+ * spx_conv_rulebook_stage1 + spx_conv_rulebook_stage2_all in ONE call with no host read-back, so the
+ * launch sequence is fixed and CUDA-graph capturable.  The caller gives `bound`, an upper limit on the
+ * number of outputs (the role of the reference's num_out_act_bound, spconv/csrc/sparse/all.py:1915);
+ * every output-side tensor has exactly `bound` rows: out_inds [bound, ndim+1], pair_fwd [kv, bound],
+ * mask_fwd [bound, words], argsort_fwd [bound], table_fwd / tmask_fwd for `bound` rows.  With M the true
+ * count (M <= bound):
+ *   - rows [0, M) of out_inds, pair_fwd, mask_fwd (before the sort) and all of pair_bwd / mask_bwd are
+ *     bit-identical to the unbounded rulebook of the same input (same first-touch ranking);
+ *   - rows [M, bound) are padding: out_inds = -1 in every column, pair_fwd = -1, mask 0; pair_bwd never
+ *     refers to a padding row.  A padded out_inds fed to the next rulebook contributes nothing: rows
+ *     whose batch index is outside [0, batch) are dropped by every insert / probe kernel;
+ *   - *num_out = M;  *status |= 1 when more than `bound` outputs existed: those ranked >= bound were
+ *     dropped and every pair that pointed at them is -1 (deterministic truncation, *num_out = bound);
+ *     *status |= 2 when a hash probe chain overflowed (far more outputs than `bound`): then *num_out = 0
+ *     and every pair is -1.  `status` is only ever ORed into: the caller zeroes it once.
+ * The hash table is sized from `bound` (load <= 0.5 at M = bound).  1-D to 4-D, 32- and 64-bit keys,
+ * 1 to 4 mask words.  argsort_bwd, table_bwd and tmask_bwd are all NULL (inference) or all given.
+ */
+size_t spx_conv_rulebook_bounded_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t bound);
+int spx_conv_rulebook_bounded_all(const spx_conv_geometry *g, const int32_t *indices, int64_t N,
+                                  int64_t bound, int32_t *out_inds, int32_t *pair_fwd, int32_t *pair_bwd,
+                                  uint32_t *mask_fwd, uint32_t *mask_bwd, int32_t *argsort_fwd,
+                                  int32_t *argsort_bwd, int do_sort, int32_t *table_fwd,
+                                  uint32_t *tmask_fwd, int32_t *table_bwd, uint32_t *tmask_bwd,
+                                  int32_t *num_out, int32_t *status, void *workspace,
+                                  size_t workspace_bytes, spx_stream_t stream);
+
+/* Zero rows [*count, rows) of a row-major matrix with `row_bytes` (even) bytes per row; `count` is a
+ * device int32 (the num_out of a bounded rulebook).  Used on gradients that arrive for padded tensors. */
+int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_bytes, const int32_t *count,
+                             spx_stream_t stream);
+
+/*
  * Compact "Native" rulebook  pairs [2, kv, N] (-1 padded) + indice_pair_num [kv]  in the
  * reference CPU order (ascending input index per offset), derived from pair_bwd [kv, N] by a
  * stable scan.  For SubM only offsets < kv/2 are counted and their mirrors written, the centre

@@ -124,6 +124,7 @@ struct Table64 {
         return true;
     }
     __device__ __forceinline__ void set_value(uint32_t s, int32_t val) const { vals[s] = val; }
+    __device__ __forceinline__ void clear_slot(uint32_t s) const { keys[s] = -1ll; }
 };
 
 // load factor <= 0.25: with linear probing the expected miss chain is ~1.4 slots and -- what

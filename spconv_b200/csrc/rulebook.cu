@@ -534,6 +534,142 @@ __global__ void table_mask_kernel(const int32_t *__restrict__ table, int64_t row
     }
 }
 
+// ------------------------------------------------------------------ bounded regular conv (no host read-back)
+// The caller gives an upper limit `bound` on the outputs; the table holds at most 4 x bound slots, so the
+// distinct outputs are found by scanning it instead of keeping a list of created slots, and the count
+// never leaves the device.  Every output is ranked (same bitmap ranking, so rows below the count equal
+// the unbounded rulebook bit for bit); outputs ranked >= bound get the value -1, which the pairs kernels
+// above already treat as "no output": the deterministic truncation.  `state`: [0] number of outputs
+// (written by the marking kernel), [1] probe-chain overflow, [2] completion counter of the marking kernel.
+template <typename Table>
+__global__ void conv_insert_k3_bounded_kernel(Table table, Geom g, const int32_t *__restrict__ indices, int64_t N,
+                              int *__restrict__ state) {
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int4 c = __ldg(reinterpret_cast<const int4 *>(indices) + i);
+    if (c.x < 0 || c.x >= g.batch) return;
+    const Axis3 az = axis_taps3(c.y, g.padding[0], g.dilation[0], g.stride[0], g.out_dims[0]);
+    const Axis3 ay = axis_taps3(c.z, g.padding[1], g.dilation[1], g.stride[1], g.out_dims[1]);
+    const Axis3 ax = axis_taps3(c.w, g.padding[2], g.dilation[2], g.stride[2], g.out_dims[2]);
+#pragma unroll
+    for (int r0 = 0; r0 < 3; ++r0) {
+        if (az.o[r0] < 0) continue;
+        const int64_t kz = (int64_t)c.x * g.out_dims[0] + az.o[r0];
+#pragma unroll
+        for (int r1 = 0; r1 < 3; ++r1) {
+            if (ay.o[r1] < 0) continue;
+            const int64_t kzy = kz * g.out_dims[1] + ay.o[r1];
+#pragma unroll
+            for (int r2 = 0; r2 < 3; ++r2) {
+                if (ax.o[r2] < 0) continue;
+                const int k = (r0 * 3 + r1) * 3 + r2;
+                bool created;
+                if (table.insert_min_slot(kzy * g.out_dims[2] + ax.o[r2], (int32_t)((int64_t)k * N + i), created,
+                                          CONV_MAX_PROBES) < 0)
+                    state[1] = 1;
+            }
+        }
+    }
+}
+
+// grid (ceil(N/T), kv): one (input, offset) per thread
+template <typename Table, bool FAST3>
+__global__ void __launch_bounds__(APPEND_THREADS)
+conv_insert_bounded_kernel(Table table, Geom g, const int32_t *__restrict__ indices, int64_t N, int *__restrict__ state) {
+    __shared__ Taps3 taps;
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const int k = blockIdx.y;
+    if (FAST3 && threadIdx.x == 0) taps = block_taps3(g, k);
+    __syncthreads();
+    if (i >= N) return;
+    int64_t key = 0;
+    bool valid;
+    if constexpr (FAST3) {
+        const int4 c = __ldg(reinterpret_cast<const int4 *>(indices) + i);
+        valid = conv3_out_key(g, c, taps, key);
+    } else {
+        int c[SPX_MAX_NDIM + 1], o[SPX_MAX_NDIM + 1], r[SPX_MAX_NDIM];
+        load_coord(indices, i, g.ndim, c);
+        offset_taps(k, g.ksize, g.ndim, r);
+        valid = conv_out_coord(g, c, r, o);
+        if (valid) key = linear_key(o, g.out_dims, g.ndim);
+    }
+    bool created;
+    if (valid && table.insert_min_slot(key, (int32_t)((int64_t)k * N + i), created, CONV_MAX_PROBES) < 0) state[1] = 1;
+}
+
+// one thread per table slot: mark the final payload of every output; the last block builds the tile
+// prefix and leaves the number of outputs in state[0]
+template <typename Table>
+__global__ void __launch_bounds__(MARK_THREADS)
+conv_mark_table_kernel(Table table, int64_t capacity, uint32_t *__restrict__ bitmap, int *__restrict__ tile_cnt,
+                       int64_t tiles, int *__restrict__ state) {
+    const int64_t s = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    int64_t key; int32_t val;
+    if (s < capacity && table.occupied((uint32_t)s, key, val)) rank_mark((uint32_t)val, bitmap, tile_cnt);
+    int total;
+    if (rank_prefix_last_block<MARK_THREADS>(tile_cnt, tiles, state + 2, &total) && threadIdx.x == 0) state[0] = total;
+}
+
+// one thread per table slot and per output row (grid covers max(capacity, bound)):
+//   slot s:  payload -> rank r; r < bound: the slot's value becomes r and out_inds[r] its coordinate,
+//            else the value becomes -1 (dropped).  After a probe-chain overflow every slot is emptied
+//            instead, so the pairs kernel finds nothing and cannot walk a full table for ever.
+//   row j:   column j of pair_fwd = -1 (the pairs kernel fills it), mask 0 where the pairs kernel ORs into
+//            it, and for j >= M (padding) out_inds[j] = -1.
+// Thread 0 publishes num_out and ORs the status bits.
+template <typename Table>
+__global__ void conv_assign_table_kernel(Table table, Geom g, int64_t capacity, int64_t bound,
+                                         const uint32_t *__restrict__ bitmap, const int *__restrict__ tile_prefix,
+                                         const int *__restrict__ state, int32_t *__restrict__ out_inds,
+                                         uint32_t *__restrict__ mask_zero, int32_t *__restrict__ pair_fill, int kv,
+                                         int32_t *__restrict__ num_out, int32_t *__restrict__ status) {
+    const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const bool overflow = state[1] != 0;
+    const int64_t total = overflow ? 0 : state[0];
+    const int64_t M = total < bound ? total : bound;
+    if (j == 0) {
+        *num_out = (int32_t)M;
+        const int bits = (total > bound ? 1 : 0) | (overflow ? 2 : 0);
+        if (bits) atomicOr(status, bits);
+    }
+    if (j < bound) {
+        for (int k = 0; k < kv; ++k) pair_fill[(int64_t)k * bound + j] = -1;
+        if (mask_zero) mask_zero[j] = 0u;
+        if (j >= M) {
+            int32_t *dst = out_inds + j * (g.ndim + 1);
+            for (int a = 0; a <= g.ndim; ++a) dst[a] = -1;
+        }
+    }
+    if (j >= capacity) return;
+    const uint32_t s = (uint32_t)j;
+    if (overflow) { table.clear_slot(s); return; }
+    int64_t key; int32_t val;
+    if (!table.occupied(s, key, val)) return;
+    const int r = rank_of((uint32_t)val, bitmap, tile_prefix);
+    if (r >= bound) { table.set_value(s, -1); return; }
+    table.set_value(s, r);
+    int32_t *dst = out_inds + (int64_t)r * (g.ndim + 1);
+    for (int a = g.ndim - 1; a >= 0; --a) {
+        dst[a + 1] = (int32_t)(key % g.out_dims[a]);
+        key /= g.out_dims[a];
+    }
+    dst[0] = (int32_t)key;
+}
+
+// zero rows [*count, rows) of a row-major matrix; V = uint4 (16-byte stores) or uint16_t
+template <typename V>
+__global__ void zero_rows_from_count_kernel(V *__restrict__ p, int64_t rows, int64_t row_vec,
+                                            const int32_t *__restrict__ count) {
+    int64_t m = *count;
+    m = m < 0 ? 0 : (m > rows ? rows : m);
+    const int64_t n = (rows - m) * row_vec, stride = (int64_t)gridDim.x * blockDim.x;
+    V *q = p + m * row_vec;
+    V z;
+    memset(&z, 0, sizeof(V));
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) q[i] = z;
+}
+
 // ------------------------------------------------------------------ Native compact pairs (stable scan)
 constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_ITEMS = 4;
@@ -1351,6 +1487,30 @@ extern "C" int spx_subm_rulebook_all(const spx_conv_geometry *g, const int32_t *
     return build_tile_table(pair_fwd, N, kv, argsort, mask, N, row_table, tile_table, tile_mask, stream);
 }
 
+// both mask argsorts + both tile tables of a regular conv whose pair tables and masks are in place
+// (M rows forward, N rows backward; the backward direction is skipped for inference)
+static int conv_sort_and_tiles(int kv, int64_t N, int64_t M, int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd,
+                               uint32_t *mask_bwd, int32_t *argsort_fwd, int32_t *argsort_bwd, int do_sort,
+                               int32_t *table_fwd, uint32_t *tmask_fwd, int32_t *table_bwd, uint32_t *tmask_bwd,
+                               void *sort_ws, size_t sort_bytes, spx_stream_t stream) {
+    const int words = (kv + 31) / 32;
+    const bool train = argsort_bwd != nullptr;
+    if (words == 1 && do_sort && train) {
+        // both mask sorts, then both tile tables, two jobs per launch
+        const size_t half = (sort_bytes / 2) & ~(size_t)255;
+        const int key_bits = kv < 32 ? kv : 32;
+        if (int rc = radix_argsort_pair(mask_fwd, argsort_fwd, M, mask_bwd, argsort_bwd, N, key_bits, sort_ws, half,
+                                        (char *)sort_ws + half, half, (cudaStream_t)stream)) return rc;
+        return build_tile_tables_pair(kv, pair_fwd, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, pair_bwd, argsort_bwd,
+                                      mask_bwd, N, table_bwd, tmask_bwd, (cudaStream_t)stream);
+    }
+    if (int rc = spx_mask_argsort(mask_fwd, argsort_fwd, M, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
+    if (int rc = spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, stream)) return rc;
+    if (!train) return 0;
+    if (int rc = spx_mask_argsort(mask_bwd, argsort_bwd, N, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
+    return spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, table_bwd, tmask_bwd, stream);
+}
+
 extern "C" size_t spx_conv_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N) {
     if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
     int kv = 1;
@@ -1378,23 +1538,154 @@ extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const in
     SPX_REQUIRE(workspace_bytes >= spx_conv_rulebook_all_workspace_size(g, N), "conv_rulebook_stage2_all: workspace too small");
     int kv = 1;
     for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
-    const int words = (kv + 31) / 32;
     const size_t rb = spx_rulebook_workspace_size(g, N, 0, 0);
     void *sort_ws = (char *)workspace + align_up(rb, 256);
     const size_t sort_bytes = workspace_bytes - align_up(rb, 256);
     if (int rc = spx_conv_rulebook_stage2(g, indices, N, M, out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, workspace, rb, stream)) return rc;
-    if (words == 1 && do_sort && train) {
-        // both mask sorts, then both tile tables, two jobs per launch
-        const size_t half = (sort_bytes / 2) & ~(size_t)255;
-        const int key_bits = kv < 32 ? kv : 32;
-        if (int rc = radix_argsort_pair(mask_fwd, argsort_fwd, M, mask_bwd, argsort_bwd, N, key_bits, sort_ws, half,
-                                        (char *)sort_ws + half, half, (cudaStream_t)stream)) return rc;
-        return build_tile_tables_pair(kv, pair_fwd, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, pair_bwd, argsort_bwd,
-                                      mask_bwd, N, table_bwd, tmask_bwd, (cudaStream_t)stream);
+    return conv_sort_and_tiles(kv, N, M, pair_fwd, pair_bwd, mask_fwd, mask_bwd, argsort_fwd, argsort_bwd, do_sort,
+                               table_fwd, tmask_fwd, table_bwd, tmask_bwd, sort_ws, sort_bytes, stream);
+}
+
+// ====================================================================== bounded regular-conv rulebook
+namespace {
+struct BoundedWs {
+    void *tbl; int32_t *tvals;
+    uint32_t *rank_bitmap; int *rank_tiles; int64_t rank_ntiles;
+    int *state;
+    void *sort_ws; size_t sort_bytes;
+    size_t bytes;
+    RbLayout L;
+};
+
+// rank_bitmap .. state + 64 stay contiguous: conv_clear_kernel zeroes that range in one pass.
+// The table is sized from the bound alone (load <= 0.5 with `bound` outputs): there is no second attempt.
+void carve_bounded_ws(const Geom &gg, int64_t N, int64_t bound, void *workspace, size_t bytes, BoundedWs &w) {
+    w.L = rb_layout(gg, bound, gg.out_dims, 2);
+    WorkspaceCarver ws(workspace, bytes);
+    w.tbl = ws.take<char>(w.L.table_bytes);
+    w.tvals = w.L.i64 ? ws.take<int32_t>(w.L.capacity) : nullptr;
+    const size_t rank_bytes = rank_scratch_bytes((int64_t)gg.kv * N, &w.rank_ntiles);
+    w.rank_bitmap = (uint32_t *)ws.take<char>(rank_bytes);
+    w.rank_tiles = (int *)(w.rank_bitmap + w.rank_ntiles * RANK_TILE_WORDS);
+    w.state = ws.take<int>(64);
+    const int64_t max_rows = bound > N ? bound : N;
+    w.sort_bytes = 2 * align_up(spx_mask_argsort_workspace_size(max_rows, (gg.kv + 31) / 32), 256);   // two sorts side by side
+    w.sort_ws = ws.take<char>(w.sort_bytes);
+    w.bytes = ws.off;
+}
+
+template <typename Table>
+int bounded_rulebook_kernels(Table t, const Geom &gg, const BoundedWs &w, const int32_t *indices, int64_t N, int64_t bound,
+                             int32_t *out_inds, int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd,
+                             uint32_t *mask_bwd, int32_t *num_out, int32_t *status, cudaStream_t stream) {
+    const int T = 128, words = (gg.kv + 31) / 32;
+    const dim3 grid((unsigned)div_up64(N > 0 ? N : 1, T), gg.kv);
+    const bool fast3 = gg.ndim == 3 && !gg.transposed;
+    const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
+    const int64_t capacity = w.L.capacity;
+    if (N > 0) {
+        if (k3) conv_insert_k3_bounded_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+        else if (fast3) conv_insert_bounded_kernel<Table, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+        else conv_insert_bounded_kernel<Table, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+        SPX_CHECK_LAUNCH("conv_insert_bounded_kernel");
     }
-    if (int rc = spx_mask_argsort(mask_fwd, argsort_fwd, M, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
-    if (int rc = spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, stream)) return rc;
-    if (!train) return 0;
-    if (int rc = spx_mask_argsort(mask_bwd, argsort_bwd, N, words, kv, do_sort, sort_ws, sort_bytes, stream)) return rc;
-    return spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, table_bwd, tmask_bwd, stream);
+    conv_mark_table_kernel<<<(unsigned)div_up64(capacity, MARK_THREADS), MARK_THREADS, 0, stream>>>(
+        t, capacity, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.state);
+    SPX_CHECK_LAUNCH("conv_mark_table_kernel");
+    // 3x3x3, one mask word: the pairs kernel ORs the forward masks too (zeroed by the assign kernel)
+    uint32_t *mask_fwd_or = (k3 && words == 1) ? mask_fwd : nullptr;
+    const int64_t span = capacity > bound ? capacity : bound;
+    conv_assign_table_kernel<<<(unsigned)div_up64(span, 256), 256, 0, stream>>>(
+        t, gg, capacity, bound, w.rank_bitmap, w.rank_tiles, w.state, out_inds, mask_fwd_or, pair_fwd, gg.kv, num_out, status);
+    SPX_CHECK_LAUNCH("conv_assign_table_kernel");
+    if (N > 0) {
+        if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
+        else if (fast3) conv_pairs_kernel<Table, true><<<grid, T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd);
+        else conv_pairs_kernel<Table, false><<<grid, T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd);
+        SPX_CHECK_LAUNCH("conv_pairs_kernel");
+    }
+    if (!mask_fwd_or) {
+        table_mask_kernel<<<(unsigned)div_up64(bound, 256), 256, 0, stream>>>(pair_fwd, bound, gg.kv, words, mask_fwd);
+        SPX_CHECK_LAUNCH("table_mask_kernel");
+    }
+    if (!k3 && N > 0) {                          // the 3x3x3 pairs kernel has already written it
+        table_mask_kernel<<<(unsigned)div_up64(N, 256), 256, 0, stream>>>(pair_bwd, N, gg.kv, words, mask_bwd);
+        SPX_CHECK_LAUNCH("table_mask_kernel");
+    }
+    return 0;
+}
+
+int validate_bounded(const spx_conv_geometry *g, int64_t N, int64_t bound) {
+    if (validate_geom(g)) return 2;
+    for (int a = 0; a < g->ndim; ++a)
+        SPX_REQUIRE(g->stride[a] > 0 && g->out_dims[a] > 0, "bad stride/out_dims on axis %d", a);
+    SPX_REQUIRE(bound > 0 && bound < (1ll << 30), "bound must be in [1, 2^30), got %lld", (long long)bound);
+    SPX_REQUIRE(N >= 0, "bad N");
+    int64_t kv = 1;
+    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    SPX_REQUIRE(kv <= 128, "conv_rulebook_bounded: kernel volume %lld not in [1,128]", (long long)kv);
+    SPX_REQUIRE(kv * N < 2000000000ll, "kv*N must stay below 2e9 (kv=%lld, N=%lld)", (long long)kv, (long long)N);
+    return 0;
+}
+}  // namespace
+
+extern "C" size_t spx_conv_rulebook_bounded_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t bound) {
+    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM || N < 0 || bound <= 0 || bound >= (1ll << 30)) return 0;
+    BoundedWs w;
+    carve_bounded_ws(make_geom(g, false), N, bound, nullptr, SIZE_MAX, w);
+    return align_up(w.bytes, 256) + 256;
+}
+
+extern "C" int spx_conv_rulebook_bounded_all(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int64_t bound,
+                                             int32_t *out_inds, int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd,
+                                             uint32_t *mask_bwd, int32_t *argsort_fwd, int32_t *argsort_bwd, int do_sort,
+                                             int32_t *table_fwd, uint32_t *tmask_fwd, int32_t *table_bwd,
+                                             uint32_t *tmask_bwd, int32_t *num_out, int32_t *status, void *workspace,
+                                             size_t workspace_bytes, spx_stream_t stream_) {
+    if (validate_bounded(g, N, bound)) return 2;
+    SPX_REQUIRE(out_inds && pair_fwd && mask_fwd && argsort_fwd && table_fwd && tmask_fwd && num_out && status && workspace,
+                "conv_rulebook_bounded_all: NULL pointer argument");
+    SPX_REQUIRE(N == 0 || (indices && pair_bwd && mask_bwd), "conv_rulebook_bounded_all: NULL pointer argument");
+    const bool train = argsort_bwd != nullptr;
+    SPX_REQUIRE((table_bwd != nullptr) == train && (tmask_bwd != nullptr) == train,
+                "conv_rulebook_bounded_all: argsort_bwd, table_bwd and tmask_bwd must all be given (training) or all be "
+                "NULL (inference)");
+    const size_t need = spx_conv_rulebook_bounded_workspace_size(g, N, bound);
+    SPX_REQUIRE(workspace_bytes >= need, "conv_rulebook_bounded_all: workspace too small: need %zu, have %zu", need,
+                workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const Geom gg = make_geom(g, false);
+    BoundedWs w;
+    carve_bounded_ws(gg, N, bound, workspace, workspace_bytes, w);
+    const int64_t zero_vec = (int64_t)(((char *)(w.state + 64) - (char *)w.rank_bitmap) / 16);
+    conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)w.L.capacity / 2,
+                                                          w.L.i64 ? (uint4 *)w.tvals : nullptr,
+                                                          w.L.i64 ? (int64_t)w.L.capacity / 4 : 0,
+                                                          (uint4 *)w.rank_bitmap, zero_vec);
+    SPX_CHECK_LAUNCH("conv_clear_kernel");
+    int rc;
+    if (!w.L.i64)
+        rc = bounded_rulebook_kernels(Table32{(unsigned long long *)w.tbl, w.L.capacity - 1}, gg, w, indices, N, bound,
+                                      out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
+    else
+        rc = bounded_rulebook_kernels(Table64{(long long *)w.tbl, w.tvals, w.L.capacity - 1}, gg, w, indices, N, bound,
+                                      out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
+    if (rc) return rc;
+    return conv_sort_and_tiles(gg.kv, N, bound, pair_fwd, pair_bwd, mask_fwd, mask_bwd, argsort_fwd, argsort_bwd, do_sort,
+                               table_fwd, tmask_fwd, table_bwd, tmask_bwd, w.sort_ws, w.sort_bytes, stream_);
+}
+
+extern "C" int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_bytes, const int32_t *count,
+                                        spx_stream_t stream_) {
+    SPX_REQUIRE(rows >= 0 && row_bytes > 0 && row_bytes % 2 == 0, "zero_rows_from_count: bad rows / row_bytes");
+    if (rows == 0) return 0;
+    SPX_REQUIRE(ptr && count, "zero_rows_from_count: NULL pointer argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const unsigned blocks = (unsigned)sm_count() * 4;
+    if (row_bytes % 16 == 0 && ((uintptr_t)ptr & 15u) == 0)
+        zero_rows_from_count_kernel<<<blocks, 256, 0, stream>>>((uint4 *)ptr, rows, row_bytes / 16, count);
+    else
+        zero_rows_from_count_kernel<<<blocks, 256, 0, stream>>>((uint16_t *)ptr, rows, row_bytes / 2, count);
+    SPX_CHECK_LAUNCH("zero_rows_from_count_kernel");
+    return 0;
 }

@@ -72,6 +72,11 @@ class SparseConvolution(SparseModule):
         self.inverse = inverse
         self.indice_key = indice_key
         self.record_voxel_count = record_voxel_count
+        # strided / transposed layers with the masked implicit-GEMM algo: an upper limit on the output count.
+        # When set the rulebook runs without a host read-back, the output has exactly this many rows and
+        # carries ``num_valid`` (spconv.set_output_bounds finds the value).  None: exact shapes, one sync.
+        self.num_out_act_bound: Optional[int] = None
+        self._bound_status: Optional[torch.Tensor] = None
         self.fp32_accum = fp32_accum
         self.act_type, self.act_alpha, self.act_beta = act_type, act_alpha, act_beta
         kv = int(np.prod(self.kernel_size))
@@ -160,6 +165,17 @@ class SparseConvolution(SparseModule):
     def is_inverseable(self):
         return self.indice_key is not None and not self.subm
 
+    def _bounded(self, algo: ConvAlgo) -> bool:
+        return (self.num_out_act_bound is not None and self.num_out_act_bound > 0 and not self.subm
+                and not self.inverse and algo == ConvAlgo.MaskImplicitGemm)
+
+    def _status_word(self, device) -> torch.Tensor:
+        """This layer's bounded-rulebook status word.  It lives on the module, outside any captured step, so
+        the bits stay set across graph replays until spconv.check_bounds reads them."""
+        if self._bound_status is None or self._bound_status.device != device:
+            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=device)
+        return self._bound_status
+
     # ------------------------------------------------------------------ cache validity
     def _check_subm_reuse_valid(self, inp: SparseConvTensor, spatial_shape: List[int], datas):
         assert datas.is_subm, "only support reuse subm indices"
@@ -219,6 +235,9 @@ class SparseConvolution(SparseModule):
         return ops.get_conv_output_size(spatial_shape, self.kernel_size, self.stride,
                                         self.padding, self.dilation)
 
+    def _layer_name(self) -> str:
+        return self._sparse_unique_name or self.name or self.indice_key or type(self).__name__
+
     def _rulebook_error(self, tag, indices, batch_size, spatial_shape, algo):
         print(f"[Exception|{tag}]indices={indices.shape},bs={batch_size},ss={spatial_shape},"
               f"algo={algo},ksize={self.kernel_size},stride={self.stride},padding={self.padding},"
@@ -246,6 +265,8 @@ class SparseConvolution(SparseModule):
         bias_infer = None if training else bias
         out_spatial_shape = self._out_spatial_shape(spatial_shape)
         out_tensor = input.shadow_copy()
+        # SubM inherits the padding of its input; strided and inverse layers set it below
+        num_valid = input.num_valid
 
         if self.conv1x1:
             w2d = weight.view(self.out_channels, self.in_channels)
@@ -314,6 +335,7 @@ class SparseConvolution(SparseModule):
                     "inverse conv can only be used with standard conv and pool ops."
                 # the inverse conv walks the paired conv's rulebook backwards
                 outids = datas.indices
+                num_valid = datas.in_voxel_num
                 pair_fwd, pair_bwd = datas.pair_bwd, datas.pair_fwd
                 mask_fwd, mask_bwd = datas.pair_mask_bwd_splits, datas.pair_mask_fwd_splits
                 sort_fwd, sort_bwd = datas.mask_argsort_bwd_splits, datas.mask_argsort_fwd_splits
@@ -330,6 +352,7 @@ class SparseConvolution(SparseModule):
                     self._check_subm_reuse_valid(input, spatial_shape, datas)
                 else:
                     self._check_prefetched_valid(input, datas)
+                    num_valid = datas.out_voxel_num
             else:
                 with timer.namespace("gen_pairs"):
                     try:
@@ -340,13 +363,22 @@ class SparseConvolution(SparseModule):
                             stride=self.stride, padding=self.padding, dilation=self.dilation,
                             out_padding=self.output_padding, subm=self.subm,
                             transpose=self.transposed, is_train=(not self.subm) or training,
-                            alloc=input.thrust_allocator, timer=timer)
+                            alloc=input.thrust_allocator, timer=timer,
+                            num_out_act_bound=self.num_out_act_bound if self._bounded(algo) else -1,
+                            bound_status=self._status_word(indices.device) if self._bounded(algo) else None)
                     except Exception:
                         self._rulebook_error("implicit_gemm_pair", indices, batch_size,
                                              spatial_shape, algo)
                         raise
                 (outids, _num_per_loc, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd,
                  masks) = res
+                in_valid = input.num_valid
+                if not self.subm:
+                    # a bounded rulebook leaves the count on the device; an unbounded one has exact rows
+                    num_valid = getattr(outids, "_spx_num_valid", None)
+                    if num_valid is not None:
+                        out_tensor.bound_status = {**(input.bound_status or {}),
+                                                   self._layer_name(): outids._spx_bound_status}
                 if self.indice_key is not None:
                     assert self.indice_key not in indice_dict, \
                         f"your indice key {self.indice_key} already exists in this sparse tensor."
@@ -356,7 +388,8 @@ class SparseConvolution(SparseModule):
                         mask_argsort_bwd_splits=sort_bwd, masks=masks, is_subm=self.subm,
                         spatial_shape=spatial_shape, out_spatial_shape=out_spatial_shape,
                         algo=algo, ksize=self.kernel_size, stride=self.stride,
-                        dilation=self.dilation, padding=self.padding)
+                        dilation=self.dilation, padding=self.padding, in_voxel_num=in_valid,
+                        out_voxel_num=num_valid)
             num_activate_out = outids.shape[0]
             if training:
                 out_features = Fsp.implicit_gemm(features, weight, pair_fwd, pair_bwd, mask_fwd,
@@ -377,8 +410,11 @@ class SparseConvolution(SparseModule):
         if not self.subm and not self.inverse and self.record_voxel_count:
             if hasattr(self, _MAX_NUM_VOXELS_DURING_TRAINING):
                 ops.maximum_value_int_(getattr(self, _MAX_NUM_VOXELS_DURING_TRAINING),
-                                       outids.shape[0])
+                                       outids.shape[0] if num_valid is None else num_valid)
+        if num_valid is not None and out_features.requires_grad:
+            out_features = Fsp.zero_padding_grad(out_features, num_valid)
         out_tensor = out_tensor.replace_feature(out_features)
+        out_tensor.num_valid = num_valid
         out_tensor.indices = outids
         out_tensor.indice_dict = indice_dict
         out_tensor.spatial_shape = out_spatial_shape

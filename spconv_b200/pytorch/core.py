@@ -201,6 +201,11 @@ class SparseConvTensor:
         self._timer = CUDAKernelTimer(enable_timer)
         self.force_algo = force_algo
         self.int8_scale: Optional[np.ndarray] = None
+        # padded tensors (bounded rulebooks, pad_to): device int32 [1] = number of valid rows, rows beyond it
+        # are padding (indices -1); None = every row is valid.  bound_status: {layer name: status word} of the
+        # bounded layers the tensor went through (spconv.check_bounds)
+        self.num_valid: Optional[torch.Tensor] = None
+        self.bound_status: Optional[Dict[str, torch.Tensor]] = None
 
     # ------------------------------------------------------------------ cloning
     def _derive(self, features: torch.Tensor) -> "SparseConvTensor":
@@ -223,7 +228,40 @@ class SparseConvTensor:
         picked = self._derive(self._features[valid_indices])
         picked.indices = self.indices[valid_indices]
         picked.indice_dict = {}          # cached rulebooks describe the old coordinate set
+        picked.num_valid = None          # the caller picked the rows: padding among them stays inert (indices -1)
         return picked
+
+    # ------------------------------------------------------------------ padding
+    def valid_mask(self) -> torch.Tensor:
+        """Device bool ``[rows]``: True for valid rows, False for padding (no host sync)."""
+        rows = self._features.shape[0]
+        dev = self._features.device
+        if self.num_valid is None:
+            return torch.ones((rows,), dtype=torch.bool, device=dev)
+        return torch.arange(rows, dtype=torch.int32, device=dev) < self.num_valid.to(dev)
+
+    def pad_to(self, rows: int) -> "SparseConvTensor":
+        """The same tensor with ``rows`` rows: index rows of -1 and zero features are appended and
+        ``num_valid`` is set, so inputs of different sizes share one static shape (CUDA-graph replay).
+        Sizes are host-known here: no sync.  Cached rulebooks are dropped."""
+        n = self._features.shape[0]
+        if rows < n:
+            raise ValueError(f"pad_to({rows}): the tensor already has {n} rows")
+        dev = self._features.device
+        feats = torch.cat([self._features, self._features.new_zeros((rows - n, self._features.shape[1]))], 0)
+        inds = torch.cat([self.indices, self.indices.new_full((rows - n, self.indices.shape[1]), -1)], 0)
+        out = self._derive(feats)
+        out.indices = inds
+        out.indice_dict = {}
+        if self.num_valid is None:
+            out.num_valid = torch.full((1,), n, dtype=torch.int32, device=dev)
+        return out
+
+    def require_unpadded(self, what: str) -> None:
+        if self.num_valid is not None:
+            raise NotImplementedError(
+                f"padded SparseConvTensor: {what} reduces over rows and is not padding-aware; run it on an "
+                "unpadded tensor (no num_out_act_bound / pad_to before it)")
 
     def minus(self) -> "SparseConvTensor":
         return self._derive(-self._features)
@@ -261,7 +299,15 @@ class SparseConvTensor:
     def dense(self, channels_first: bool = True) -> torch.Tensor:
         nd = len(self.spatial_shape)
         full = [self.batch_size, *self.spatial_shape, self._features.shape[1]]
-        grid = scatter_nd(self.indices.to(self._features.device), self._features, full)
+        if self.num_valid is not None:
+            # padding rows go to one spare sample that is cut off again: no sync, valid cells untouched
+            spare = torch.zeros_like(self.indices[:1])
+            spare[0, 0] = self.batch_size
+            inds = torch.where(self.valid_mask().unsqueeze(1), self.indices, spare)
+            full[0] += 1
+            grid = scatter_nd(inds, self._features, full)[:self.batch_size]
+        else:
+            grid = scatter_nd(self.indices.to(self._features.device), self._features, full)
         if not channels_first:
             return grid
         return grid.permute(0, nd + 1, *range(1, nd + 1)).contiguous()

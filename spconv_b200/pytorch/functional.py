@@ -124,6 +124,25 @@ class SparseImplicitGemmFunction(Function):
         return (din, dw) + (None,) * 16
 
 
+class ZeroPaddingGrad(Function):
+    """Identity on the features of a padded tensor whose backward zeroes the gradient rows at and beyond
+    ``num_valid``.  The conv modules put it behind every layer that produces a padded tensor (after the bias
+    add), so the bias gradient ``dout.sum(0)`` and the weight gradient of a SubM layer (whose centre tap
+    pairs a padding row with itself) are exact whatever the loss did with the padding rows."""
+
+    @staticmethod
+    def forward(ctx, features, num_valid):
+        ctx.save_for_backward(num_valid)
+        return features.view_as(features)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        num_valid, = ctx.saved_tensors
+        grad = grad_output.contiguous().clone()      # the incoming gradient may be shared: never zero it in place
+        return ops.zero_rows_from_count_(grad, num_valid), None
+
+
 class SparseMaxPoolFunction(Function):
     """ConvAlgo.Native max pooling (reference ``functional.py:360-378``)."""
 
@@ -148,8 +167,10 @@ class SparseMaxPoolImplicitGemmFunction(Function):
 
     @staticmethod
     @_amp_fwd
-    def forward(ctx, features, indice_pairs_fwd, indice_pairs_bwd, num_activate_out):
+    def forward(ctx, features, indice_pairs_fwd, indice_pairs_bwd, num_activate_out, num_valid=None):
         out = ops.indice_maxpool_implicit_gemm(features, indice_pairs_fwd, num_activate_out)
+        if num_valid is not None:                 # padding rows of a bounded rulebook: 0, not the lowest value
+            ops.zero_rows_from_count_(out, num_valid)
         ctx.save_for_backward(indice_pairs_bwd, features, out)
         return out
 
@@ -159,7 +180,7 @@ class SparseMaxPoolImplicitGemmFunction(Function):
     def backward(ctx, grad_output):
         indice_pairs_bwd, features, out = ctx.saved_tensors
         return ops.indice_maxpool_implicit_gemm_backward(features, out, grad_output,
-                                                         indice_pairs_bwd), None, None, None
+                                                         indice_pairs_bwd), None, None, None, None
 
 
 class SparseAvgPoolImplicitGemmFunction(Function):
@@ -211,6 +232,7 @@ def indice_subm_conv(features, filters, indice_pairs, indice_pair_num, num_activ
 
 
 implicit_gemm = SparseImplicitGemmFunction.apply
+zero_padding_grad = ZeroPaddingGrad.apply
 indice_maxpool = SparseMaxPoolFunction.apply
 indice_maxpool_implicit_gemm = SparseMaxPoolImplicitGemmFunction.apply
 indice_avgpool_implicit_gemm = SparseAvgPoolImplicitGemmFunction.apply
@@ -238,6 +260,8 @@ class SparseAddFunction(Function):
 
 def _sparse_add(tens) -> SparseConvTensor:
     assert len(tens) >= 1, "sparse_add needs at least one operand"
+    for ten in tens:
+        ten.require_unpadded("sparse_add")
     first = tens[0]
     largest = 0
     for i, ten in enumerate(tens):
@@ -313,6 +337,7 @@ class _RowGather(Function):
 def remove_duplicate(x: SparseConvTensor) -> SparseConvTensor:
     """Keep the first row of every coordinate (rows in first-touch order) and drop rows whose batch index or
     coordinate is out of range; see :class:`spconv_b200.pytorch.spatial.RemoveDuplicate`."""
+    x.require_unpadded("remove_duplicate")
     ops._sparse_add_dtype(x.features.dtype)
     out_inds, dst = ops.sparse_add_union([x.indices], x.batch_size, x.spatial_shape)
     m = out_inds.shape[0]

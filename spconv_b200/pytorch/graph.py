@@ -4,11 +4,12 @@ The device time of a SubM layer-step at LiDAR sizes (~0.15 ms) is several times 
 host time torch + Python need to issue its ~25 launches eagerly, so a step whose SHAPES repeat
 (the same cloud evaluated many times, a static calibration batch, a benchmark) is best replayed as
 one graph.  ``graph_capture`` wraps the boilerplate: warm-up on a side stream, capture, static
-input buffers that later calls copy into.  Every kernel of this library is capturable except the
-regular-conv rulebook, whose data-dependent output count is read back by the host
-(``spx_conv_rulebook_stage1``; the reference syncs at the same point,
-``spconv/csrc/sparse/indices.py:1454-1455``) -- SubM stacks, pooling on cached rulebooks and the
-int8 path capture fine.
+input buffers that later calls copy into.  Every kernel of this library is capturable; the one host
+read-back is the output count of an UNBOUNDED regular-conv rulebook (``spx_conv_rulebook_stage1``; the
+reference syncs at the same point, ``spconv/csrc/sparse/indices.py:1454-1455``).  Give the strided layers
+an output bound (``spconv.set_output_bounds``) and pad the inputs to one size
+(``SparseConvTensor.pad_to``): then the rulebooks keep the count on the device and a whole encoder
+step, forward and backward, captures; ``spconv.check_bounds`` tells when a bound was exceeded.
 """
 from __future__ import annotations
 
@@ -40,9 +41,10 @@ class GraphedStep:
         except Exception as e:
             torch.cuda.synchronize()
             raise RuntimeError(
-                "graph_capture failed. A regular SparseConv / SparseMaxPool builds its rulebook with one host "
-                "read-back (the output count) and cannot be captured; capture SubM-only stacks, or run the strided "
-                f"layers eagerly around the captured part. Original error: {type(e).__name__}: {e}") from e
+                "graph_capture failed. A regular SparseConv / SparseMaxPool without an output bound builds its "
+                "rulebook with one host read-back (the output count) and cannot be captured: call "
+                "spconv.set_output_bounds(net, example) first and pad the inputs with SparseConvTensor.pad_to, or "
+                f"capture SubM-only stacks. Original error: {type(e).__name__}: {e}") from e
 
     def __call__(self, *inputs: torch.Tensor):
         assert len(inputs) == len(self.static_inputs), "same number of inputs as at capture time"

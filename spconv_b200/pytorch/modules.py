@@ -79,6 +79,8 @@ class SparseSequential(SparseModule):
             elif isinstance(x, SparseConvTensor):
                 # dense layers (BatchNorm1d, ReLU, ...) act on the feature matrix
                 if x.indices.shape[0] != 0:
+                    if isinstance(layer, nn.modules.batchnorm._BatchNorm) and layer.training:
+                        x.require_unpadded("BatchNorm in training mode")
                     x = x.replace_feature(layer(x.features))
             else:
                 x = layer(x)
@@ -118,6 +120,11 @@ class SparseBatchNorm(_FeatureWise):
     def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True,
                  track_running_stats=True):
         super().__init__(nn.BatchNorm1d(num_features, eps, momentum, affine, track_running_stats))
+
+    def forward(self, x: SparseConvTensor):
+        if self.inner.training:
+            x.require_unpadded("SparseBatchNorm in training mode")
+        return super().forward(x)
 
 
 class SparseIdentity(SparseModule):

@@ -229,6 +229,46 @@ def _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, 
     return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [mask_bwd[0]], [sf], [sb], masks)
 
 
+def _conv_rulebook_bounded(geo, indices, n_in, kv, words, bound, is_train, do_sort, alloc, indice_num_per_loc, masks,
+                           status):
+    """Bounded regular-conv implicit-GEMM rulebook (``spx_conv_rulebook_bounded_all``): one native call, no host
+    read-back.  Every output-side tensor has ``bound`` rows; the true count (device int32 ``[1]``) and the status
+    word ride on ``out_inds`` as ``_spx_num_valid`` / ``_spx_bound_status``."""
+    lib = _lib()
+    dev = indices.device
+    m = int(bound)
+    if n_in == 0:                        # host-known: the unbounded path raises the same error for M == 0
+        raise ValueError(_VANISHED)
+    ws = _bytes(lib.spx_conv_rulebook_bounded_workspace_size(ctypes.byref(geo), n_in, m), dev, alloc)
+    ndim = indices.shape[1] - 1
+    out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
+    pair_fwd = torch.empty((kv, m), dtype=torch.int32, device=dev)
+    pair_bwd = torch.empty((kv, n_in), dtype=torch.int32, device=dev)
+    mask_fwd = torch.empty((1, m, words), dtype=torch.int32, device=dev)
+    mask_bwd = torch.empty((1, n_in, words), dtype=torch.int32, device=dev)
+    sort_fwd = torch.empty((1, m), dtype=torch.int32, device=dev)
+    sort_bwd = torch.empty((1, n_in), dtype=torch.int32, device=dev) if is_train else None
+    t_fwd, tm_fwd = _alloc_tile_tables(m, kv, dev)
+    t_bwd, tm_bwd = _alloc_tile_tables(n_in, kv, dev) if is_train else (None, None)
+    num_out = torch.empty((1,), dtype=torch.int32, device=dev)
+    if status is None:
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+    _cabi.check(lib.spx_conv_rulebook_bounded_all(
+        ctypes.byref(geo), _ptr(indices), n_in, m, out_inds.data_ptr(), pair_fwd.data_ptr(), _ptr(pair_bwd),
+        mask_fwd.data_ptr(), _ptr(mask_bwd), sort_fwd.data_ptr(), _ptr(sort_bwd), int(bool(do_sort)),
+        _ptr(t_fwd), _ptr(tm_fwd), _ptr(t_bwd), _ptr(tm_bwd), num_out.data_ptr(), status.data_ptr(),
+        ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_bounded_all")
+    out_inds._spx_num_valid = num_out
+    out_inds._spx_bound_status = status
+    sf = sort_fwd[0]
+    sf._spx_tile_cache = (_tile_key(pair_fwd, sf, m), t_fwd, tm_fwd)
+    if not is_train:
+        return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [], [sf], [], masks)
+    sb = sort_bwd[0]
+    sb._spx_tile_cache = (_tile_key(pair_bwd, sb, n_in), t_bwd, tm_bwd)
+    return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [mask_bwd[0]], [sf], [sb], masks)
+
+
 def _argsort_masks(mask: torch.Tensor, kv: int, do_sort: bool, alloc) -> torch.Tensor:
     """mask [1, n, words] -> argsort [1, n]; mask is left sorted (thrust::sort_by_key semantics,
     ``spconv/csrc/sparse/all.py:935-1000``)."""
@@ -264,7 +304,9 @@ def get_indice_pairs(indices: torch.Tensor, batch_size: int, spatial_shape: List
                      transpose: bool = False, num_out_act_bound: int = -1):
     """ConvAlgo.Native rulebook: ``(out_inds [M, ndim+1], pairs [2, kv, N], indice_pair_num [kv])``
     with pair ORDER equal to the reference CPU implementation
-    (``spconv/csrc/sparse/indices.py:1640-1778``)."""
+    (``spconv/csrc/sparse/indices.py:1640-1778``).  ``num_out_act_bound`` is accepted and ignored: the
+    Native rulebook always reads the output count back (only the masked implicit-GEMM rulebook has a
+    bounded mode)."""
     _require_cuda(indices, "indices")
     lib = _lib()
     dev = indices.device
@@ -307,10 +349,19 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
                                    timer: CUDAKernelTimer = CUDAKernelTimer(False),
                                    num_out_act_bound: int = -1,
                                    direct_table: bool = True,
-                                   do_sort=SPCONV_DO_SORT):
+                                   do_sort=SPCONV_DO_SORT,
+                                   bound_status: Optional[torch.Tensor] = None):
     """Masked implicit-GEMM rulebook.  Returns the reference's 9-tuple
     ``(out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd], [mask_bwd],
-    [argsort_fwd], [argsort_bwd], masks)`` (``ops.py:329-359``)."""
+    [argsort_fwd], [argsort_bwd], masks)`` (``ops.py:329-359``).
+
+    ``num_out_act_bound = b > 0`` with ``subm=False`` and ``ConvAlgo.MaskImplicitGemm`` selects the bounded
+    rulebook: no host read-back (CUDA-graph capturable), every output-side tensor has exactly ``b`` rows, the
+    true count M stays on the device (``out_inds._spx_num_valid``, int32 ``[1]``) and rows ``[M, b)`` are
+    padding (``out_inds`` -1, pairs -1, mask 0).  Rows below M are bit-identical to the unbounded rulebook.
+    ``out_inds._spx_bound_status`` (``bound_status`` if given, which is only ever ORed into) has bit 0 set when
+    more than ``b`` outputs existed (those ranked >= b were dropped) and bit 1 when the hash table sized from
+    ``b`` overflowed.  SubM and ``MaskSplitImplicitGemm`` ignore the bound."""
     _require_cuda(indices, "indices")
     assert algo in (ConvAlgo.MaskImplicitGemm, ConvAlgo.MaskSplitImplicitGemm), "TODO"
     lib = _lib()
@@ -374,6 +425,10 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
             mf, sf = _split_and_sort(mask_fwd, masks, kv, do_sort, alloc)
             mb, sb = _split_and_sort(mask_bwd, masks, kv, do_sort, alloc) if is_train else ([], [])
         return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, mf, mb, sf, sb, masks)
+    if num_out_act_bound is not None and int(num_out_act_bound) > 0:
+        with timer.record("gen_conv_inds", _stream()):
+            return _conv_rulebook_bounded(geo, indices, n_in, kv, words, int(num_out_act_bound), is_train, do_sort,
+                                          alloc, indice_num_per_loc, masks, bound_status)
     with timer.record("gen_conv_inds", _stream()):
         return _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks)
 
@@ -1035,10 +1090,23 @@ def bias_add_act_inplace(x: torch.Tensor, bias: Optional[torch.Tensor], act_type
     return x
 
 
-def maximum_value_int_(ten: torch.Tensor, value: int):
-    """running max of the active-voxel count (``ops.py`` maximum_value_int_)."""
-    ten.clamp_(min=int(value))
+def maximum_value_int_(ten: torch.Tensor, value):
+    """running max of the active-voxel count (``ops.py`` maximum_value_int_).  ``value`` is a host integer or
+    a device int32 scalar (the count of a bounded rulebook: no read-back)."""
+    if isinstance(value, torch.Tensor):
+        torch.maximum(ten, value.to(ten.dtype).view(1), out=ten)
+    else:
+        ten.clamp_(min=int(value))
     return ten
+
+
+def zero_rows_from_count_(x: torch.Tensor, num_valid: torch.Tensor) -> torch.Tensor:
+    """Zero rows ``[num_valid, rows)`` of the contiguous matrix ``x`` in place (``num_valid``: device int32)."""
+    _require_cuda(x, "x")
+    assert x.is_contiguous() and x.dim() == 2 and num_valid.dtype == torch.int32
+    _cabi.check(_lib().spx_zero_rows_from_count(_ptr(x), x.shape[0], x.shape[1] * x.element_size(),
+                                                num_valid.data_ptr(), _stream()), "zero_rows_from_count")
+    return x
 
 
 def last_kernel_family() -> int:

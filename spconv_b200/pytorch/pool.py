@@ -39,6 +39,9 @@ class _SparsePool(SparseModule):
         self.subm = subm
         self.indice_key = indice_key
         self.record_voxel_count = record_voxel_count
+        # as SparseConvolution.num_out_act_bound: bounded implicit-GEMM rulebook, padded output, no host sync
+        self.num_out_act_bound: Optional[int] = None
+        self._bound_status: Optional[torch.Tensor] = None
         if record_voxel_count and not subm:
             self.register_buffer(_MAX_NUM_VOXELS_DURING_TRAINING, torch.zeros(1, dtype=torch.int32))
         self.algo = algo
@@ -60,12 +63,18 @@ class _SparsePool(SparseModule):
         return ops.get_conv_output_size(spatial_shape, self.kernel_size, self.stride, self.padding, self.dilation)
 
     def _implicit_rulebook(self, input: SparseConvTensor, out_spatial_shape, indice_dict):
+        bounded = (self.num_out_act_bound is not None and self.num_out_act_bound > 0 and not self.subm
+                   and self.algo == ConvAlgo.MaskImplicitGemm)
+        if bounded and (self._bound_status is None or self._bound_status.device != input.indices.device):
+            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=input.indices.device)
         with input._timer.namespace("gen_pairs"):
             res = ops.get_indice_pairs_implicit_gemm(
                 input.indices, input.batch_size, input.spatial_shape, self.algo, ksize=self.kernel_size,
                 stride=self.stride, padding=self.padding, dilation=self.dilation,
                 out_padding=[0] * self.ndim, subm=self.subm, is_train=(not self.subm) or self.training,
-                alloc=input.thrust_allocator, timer=input._timer)
+                alloc=input.thrust_allocator, timer=input._timer,
+                num_out_act_bound=self.num_out_act_bound if bounded else -1,
+                bound_status=self._bound_status if bounded else None)
         outids, _, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
         if self.indice_key is not None:
             assert self.indice_key not in indice_dict, \
@@ -75,13 +84,21 @@ class _SparsePool(SparseModule):
                 pair_mask_bwd_splits=mask_bwd, mask_argsort_fwd_splits=sort_fwd,
                 mask_argsort_bwd_splits=sort_bwd, masks=masks, is_subm=self.subm,
                 spatial_shape=input.spatial_shape, out_spatial_shape=out_spatial_shape, algo=self.algo,
-                ksize=self.kernel_size, stride=self.stride, dilation=self.dilation, padding=self.padding)
+                ksize=self.kernel_size, stride=self.stride, dilation=self.dilation, padding=self.padding,
+                in_voxel_num=input.num_valid,
+                out_voxel_num=input.num_valid if self.subm else getattr(outids, "_spx_num_valid", None))
         return outids, pair_fwd, pair_bwd
 
     def _finish(self, input: SparseConvTensor, out_features, outids, indice_dict, out_spatial_shape):
+        num_valid = input.num_valid if self.subm else getattr(outids, "_spx_num_valid", None)
         if not self.subm and self.record_voxel_count and hasattr(self, _MAX_NUM_VOXELS_DURING_TRAINING):
-            ops.maximum_value_int_(getattr(self, _MAX_NUM_VOXELS_DURING_TRAINING), outids.shape[0])
+            ops.maximum_value_int_(getattr(self, _MAX_NUM_VOXELS_DURING_TRAINING),
+                                   outids.shape[0] if num_valid is None else num_valid)
         out = input.shadow_copy().replace_feature(out_features)
+        out.num_valid = num_valid
+        if num_valid is not None and not self.subm:
+            name = self._sparse_unique_name or self.name or self.indice_key or type(self).__name__
+            out.bound_status = {**(input.bound_status or {}), name: outids._spx_bound_status}
         out.indices = outids
         out.indice_dict = indice_dict
         out.spatial_shape = out_spatial_shape
@@ -119,7 +136,8 @@ class SparseMaxPool(_SparsePool):
             out_features = Fsp.indice_maxpool(input.features, indice_pairs, indice_pairs_num, outids.shape[0])
         else:
             outids, pair_fwd, pair_bwd = self._implicit_rulebook(input, out_spatial_shape, indice_dict)
-            out_features = Fsp.indice_maxpool_implicit_gemm(input.features, pair_fwd, pair_bwd, outids.shape[0])
+            out_features = Fsp.indice_maxpool_implicit_gemm(input.features, pair_fwd, pair_bwd, outids.shape[0],
+                                                            getattr(outids, "_spx_num_valid", None))
         return self._finish(input, out_features, outids, indice_dict, out_spatial_shape)
 
 
@@ -154,6 +172,7 @@ class SparseGlobalMaxOrAvgPool(SparseModule):
 
     def forward(self, input: SparseConvTensor):
         assert isinstance(input, SparseConvTensor)
+        input.require_unpadded("global pooling")
         out_indices, counts = ops.global_pool_rearrange(input.indices, input.batch_size)
         counts_cpu = counts.cpu().tolist()
         rows = []

@@ -17,6 +17,7 @@ from .modules import SparseModule
 
 def _check_aligned(input: List[SparseConvTensor], msg: str) -> None:
     for ten in input:
+        ten.require_unpadded("the table modules")
         assert ten.spatial_shape == input[0].spatial_shape, msg
         assert ten.batch_size == input[0].batch_size, msg
         assert ten.features.shape[1] == input[0].features.shape[1], msg
