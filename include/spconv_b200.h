@@ -431,6 +431,36 @@ int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const int32_t *o
 int spx_sparse_add_gather(const int32_t *index, const void *src, int64_t src_rows,
                           const spx_sparse_add_operands *operands, int channels, int dtype, spx_stream_t stream);
 
+/* ------------------------------------------------------------------ padding-aware BatchNorm */
+
+/*
+ * Training-mode BatchNorm1d over the valid rows of x [rows, channels] (MaskedBatchNorm1d).  M = *num_valid
+ * (device int32, clamped to [0, rows]; NULL = every row).  Rows [M, rows) are never read; y and dx are 0 there.
+ * dtype: f32 / f16 / bf16 features; param_dtype (weight, bias, running stats, dweight, dbias): f32 or dtype.
+ * Statistics and every sum are fp32, reduced in fixed chunks of rows merged in chunk order, so all results
+ * are bit-reproducible and independent of `rows` (padding).  Nothing is read back to the host.
+ * fwd_train: y = (x - mean) * weight * invstd + bias with the batch mean and biased variance; save_mean /
+ *            save_invstd [channels] fp32 receive them for the backward.  weight / bias may be NULL (1 / 0).
+ *            running_mean / running_var (both or neither) are updated when M > 1:
+ *            r = (1 - f) r + f s with s the mean / unbiased variance and f = momentum, or, when cumulative != 0,
+ *            f = 1 / *num_batches_tracked (device int64, already incremented by the caller).
+ *            M = 0: y = 0; M = 1: y = bias; running stats unchanged in both cases.
+ * bwd:       dx = weight * invstd * (dy - sum(dy) / M - xhat * sum(dy * xhat) / M) on valid rows,
+ *            dbias = sum(dy), dweight = sum(dy * xhat) over valid rows (either may be NULL).
+ * workspace: the matching _workspace_size(rows, channels) bytes.
+ */
+size_t spx_masked_bn_fwd_train_workspace_size(int64_t rows, int channels);
+int spx_masked_bn_fwd_train(const void *x, void *y, int64_t rows, int channels, int dtype, const int32_t *num_valid,
+                            const void *weight, const void *bias, void *running_mean, void *running_var,
+                            const int64_t *num_batches_tracked, int param_dtype, float momentum, int cumulative,
+                            float eps, float *save_mean, float *save_invstd, void *workspace, size_t workspace_bytes,
+                            spx_stream_t stream);
+size_t spx_masked_bn_bwd_workspace_size(int64_t rows, int channels);
+int spx_masked_bn_bwd(const void *x, const void *dy, void *dx, int64_t rows, int channels, int dtype,
+                      const int32_t *num_valid, const void *weight, int param_dtype, const float *save_mean,
+                      const float *save_invstd, void *dweight, void *dbias, void *workspace, size_t workspace_bytes,
+                      spx_stream_t stream);
+
 /* ------------------------------------------------------------------ hash table */
 
 /*

@@ -147,6 +147,13 @@ SIGNATURES = {
                                    c_void_p]),
     "spx_sparse_add_gather": (c_int, [c_void_p, c_void_p, c_int64, POINTER(SparseAddOperands), c_int, c_int,
                                       c_void_p]),
+    "spx_masked_bn_fwd_train_workspace_size": (c_size_t, [c_int64, c_int]),
+    "spx_masked_bn_fwd_train": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_float, c_void_p,
+                                        c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_masked_bn_bwd_workspace_size": (c_size_t, [c_int64, c_int]),
+    "spx_masked_bn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_hash_workspace_size": (c_size_t, [c_int64, c_int64]),
     "spx_hash_clear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     "spx_hash_insert": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,

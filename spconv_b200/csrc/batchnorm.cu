@@ -1,0 +1,579 @@
+// Training-mode BatchNorm over the valid rows of a (possibly padded) feature matrix [rows, C]
+// (MaskedBatchNorm1d, pytorch/modules.py).  M = *num_valid (NULL: every row); rows [M, rows) are never read
+// and come out as exact zeros in y and dx.
+//
+// Every row reduction uses the same fixed structure, so results depend only on rows [0, M) and their
+// values, never on `rows` or on the grid size (no float atomics):
+//   chunk    : BN_CHUNK consecutive rows, one block per (chunk, channel slice).  Row lane l of the block
+//              folds rows r0 + l, r0 + l + lanes, ... in ascending order, then the lanes merge in a fixed
+//              binary tree; the chunk's partial goes to workspace [chunks][C].  Chunks at or beyond M exit.
+//   finalize : lane p of 32 sums the partials p, p + 32, ... below ceil(M / BN_CHUNK) in order, then a fixed
+//              tree over the 32 lanes.  Partials of empty chunks are never read, so padding is a no-op.
+// Forward: stats (per-chunk Welford mean / M2, merged by Chan's rule) -> finalize (mean, biased variance,
+// invstd, running-stat update) -> apply y = (x - mean) * (gamma * invstd) + beta.
+// Backward: reduce (per-chunk sums of dy and dy * xhat) -> finalize (dbeta, dgamma, coefficients) ->
+// apply dx = gamma * invstd * (dy - sum(dy) / M - xhat * sum(dy * xhat) / M).
+// Feature rows move as 16-byte vectors when the row length and the pointers allow it, else per element.
+#include "common.cuh"
+
+namespace spx {
+
+constexpr int BN_THREADS = 256;
+constexpr int BN_CHUNK = 512;        // rows per partial
+constexpr int BN_FIN_CH = 8;         // finalize: channels per block
+constexpr int BN_FIN_LANES = 32;     // finalize: partial lanes per channel
+
+__device__ __forceinline__ int64_t bn_valid_rows(const int32_t *num_valid, int64_t rows) {
+    if (num_valid == nullptr) return rows;
+    const int64_t m = __ldg(num_valid);
+    return m < 0 ? 0 : (m > rows ? rows : m);
+}
+
+// rows of chunk k that are valid
+__device__ __forceinline__ float bn_chunk_count(int64_t k, int64_t M) {
+    const int64_t n = M - k * BN_CHUNK;
+    return (float)(n < 0 ? 0 : (n > BN_CHUNK ? BN_CHUNK : n));
+}
+
+template <typename T, int W> __device__ __forceinline__ void bn_load(const T *p, float (&f)[W]) {
+    if constexpr (W * sizeof(T) == 16) {
+        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
+        const T *e = reinterpret_cast<const T *>(&v);
+#pragma unroll
+        for (int j = 0; j < W; ++j) f[j] = to_float(e[j]);
+    } else {
+#pragma unroll
+        for (int j = 0; j < W; ++j) f[j] = to_float(__ldg(p + j));
+    }
+}
+template <typename T, int W> __device__ __forceinline__ void bn_store(T *p, const float (&f)[W]) {
+    if constexpr (W * sizeof(T) == 16) {
+        uint4 v;
+        T *e = reinterpret_cast<T *>(&v);
+#pragma unroll
+        for (int j = 0; j < W; ++j) e[j] = from_float<T>(f[j]);
+        *reinterpret_cast<uint4 *>(p) = v;
+    } else {
+#pragma unroll
+        for (int j = 0; j < W; ++j) p[j] = from_float<T>(f[j]);
+    }
+}
+
+// Chan et al.: fold (nb, mb, qb) into (na, ma, qa).  An empty side changes nothing, bit for bit.
+__device__ __forceinline__ void chan_merge(float &na, float &ma, float &qa, float nb, float mb, float qb) {
+    if (nb == 0.f) return;
+    if (na == 0.f) { na = nb; ma = mb; qa = qb; return; }
+    const float n = na + nb, d = mb - ma, f = __fdiv_rn(nb, n);
+    ma = fmaf(d, f, ma);
+    qa = qa + qb + d * d * na * f;
+    na = n;
+}
+
+// Block layout of the row kernels: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
+// `lanes` = BN_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
+struct BnRowThread {
+    int lane, v;
+    bool active;
+};
+__device__ __forceinline__ BnRowThread bn_row_thread(int vecs, int tpr) {
+    BnRowThread t;
+    t.lane = threadIdx.x / tpr;
+    t.v = blockIdx.y * tpr + (threadIdx.x % tpr);
+    t.active = t.v < vecs;
+    return t;
+}
+
+// ---------------------------------------------------------------- forward
+template <typename T, int W>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_stats_kernel(const T *__restrict__ x, int64_t rows, int channels, int vecs, int tpr,
+                const int32_t *__restrict__ num_valid, float2 *__restrict__ partials) {
+    __shared__ float s_mean[BN_THREADS * W], s_q[BN_THREADS * W], s_n[BN_THREADS];
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t r0 = (int64_t)blockIdx.x * BN_CHUNK;
+    if (r0 >= M) return;                                   // the whole block: nothing valid here
+    const int lanes = BN_THREADS / tpr;
+    const BnRowThread t = bn_row_thread(vecs, tpr);
+    const int64_t end = M < r0 + BN_CHUNK ? M : r0 + BN_CHUNK;
+    float n = 0.f, mean[W], q[W];
+#pragma unroll
+    for (int j = 0; j < W; ++j) mean[j] = q[j] = 0.f;
+    if (t.active) {
+        const T *base = x + (int64_t)t.v * W;
+        auto fold = [&](const float (&f)[W]) {             // Welford, rows in ascending order
+            n += 1.f;
+            const float inv = __frcp_rn(n);
+#pragma unroll
+            for (int j = 0; j < W; ++j) {
+                const float d = f[j] - mean[j];
+                mean[j] = fmaf(d, inv, mean[j]);
+                q[j] = fmaf(d, f[j] - mean[j], q[j]);
+            }
+        };
+        int64_t r = r0 + t.lane;
+        for (; r + 3 * lanes < end; r += 4 * lanes) {     // four loads in flight, folded in row order
+            float f[4][W];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) bn_load<T, W>(base + (r + (int64_t)u * lanes) * channels, f[u]);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) fold(f[u]);
+        }
+        for (; r < end; r += lanes) {
+            float f[W];
+            bn_load<T, W>(base + r * channels, f);
+            fold(f);
+        }
+    }
+    // fixed tree over the row lanes: at step s, lanes [0, s) fold lanes [s, 2s) into their own slots
+    const int slot = threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < W; ++j) { s_mean[slot * W + j] = mean[j]; s_q[slot * W + j] = q[j]; }
+    s_n[slot] = n;
+    for (int s = lanes >> 1; s >= 1; s >>= 1) {
+        __syncthreads();
+        if (t.lane < s) {
+            const int o = slot + s * tpr;
+            const float nb = s_n[o];
+#pragma unroll
+            for (int j = 0; j < W; ++j) {
+                float na = n;
+                chan_merge(na, mean[j], q[j], nb, s_mean[o * W + j], s_q[o * W + j]);
+                s_mean[slot * W + j] = mean[j];
+                s_q[slot * W + j] = q[j];
+            }
+            s_n[slot] = n = n + nb;
+        }
+    }
+    if (t.lane == 0 && t.active) {
+        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
+#pragma unroll
+        for (int j = 0; j < W; ++j) dst[j] = make_float2(mean[j], q[j]);
+    }
+}
+
+// Sum over the 32 partial lanes of one channel in a fixed tree; every thread of the channel gets the total.
+__device__ __forceinline__ float bn_lane_sum(float v, float (*buf)[BN_FIN_CH], int pl, int cl) {
+    buf[pl][cl] = v;
+    for (int s = BN_FIN_LANES / 2; s >= 1; s >>= 1) {
+        __syncthreads();
+        if (pl < s) buf[pl][cl] += buf[pl + s][cl];
+    }
+    __syncthreads();
+    const float total = buf[0][cl];
+    __syncthreads();
+    return total;
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
+bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
+                       const int32_t *__restrict__ num_valid, const P *__restrict__ weight, const P *__restrict__ bias,
+                       P *__restrict__ running_mean, P *__restrict__ running_var,
+                       const int64_t *__restrict__ num_batches_tracked, float momentum, int cumulative, float eps,
+                       float *__restrict__ save_mean, float *__restrict__ save_invstd, float *__restrict__ coef) {
+    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
+    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
+    const int c = blockIdx.x * BN_FIN_CH + cl;
+    const bool active = c < channels;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t K = (M + BN_CHUNK - 1) / BN_CHUNK;
+    float s = 0.f;
+    if (active)
+        for (int64_t k = pl; k < K; k += BN_FIN_LANES) s = fmaf(bn_chunk_count(k, M), partials[k * channels + c].x, s);
+    const float Mf = (float)M;
+    const float sum = bn_lane_sum(s, buf, pl, cl);
+    const float mean = M > 0 ? __fdiv_rn(sum, Mf) : 0.f;
+    float q = 0.f;
+    if (active)
+        for (int64_t k = pl; k < K; k += BN_FIN_LANES) {
+            const float2 p = partials[k * channels + c];
+            const float d = p.x - mean;
+            q += fmaf(bn_chunk_count(k, M) * d, d, p.y);
+        }
+    const float m2 = bn_lane_sum(q, buf, pl, cl);
+    if (pl != 0 || !active) return;
+    const float var = M > 0 ? __fdiv_rn(m2, Mf) : 0.f;
+    const float invstd = __frsqrt_rn(var + eps);
+    const float gamma = weight ? to_float(weight[c]) : 1.f;
+    const float beta = bias ? to_float(bias[c]) : 0.f;
+    save_mean[c] = mean;
+    save_invstd[c] = invstd;
+    coef[c] = mean;
+    coef[channels + c] = gamma * invstd;
+    coef[2 * channels + c] = beta;
+    if (running_mean != nullptr && M > 1) {                // one value per channel has no unbiased variance
+        // divisors >= 1: the 2-ulp fast division is accurate here, and a third IEEE division would make ptxas
+        // keep a value on the stack across its slow-path call
+        const float f = cumulative ? __fdividef(1.f, (float)__ldg(num_batches_tracked)) : momentum;
+        const float unbiased = __fdividef(m2, (float)(M - 1));
+        running_mean[c] = from_float<P>((1.f - f) * to_float(running_mean[c]) + f * mean);
+        running_var[c] = from_float<P>((1.f - f) * to_float(running_var[c]) + f * unbiased);
+    }
+}
+
+template <typename T, int W>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, int channels, int vecs,
+                    const int32_t *__restrict__ num_valid, const float *__restrict__ coef) {
+    const int64_t idx = blockIdx.x * (int64_t)BN_THREADS + threadIdx.x;
+    const int64_t r = idx / vecs;
+    const int v = (int)(idx - r * vecs);
+    if (r >= rows) return;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    float f[W];
+    if (r < M) {
+        bn_load<T, W>(x + r * channels + v * W, f);
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+            const int c = v * W + j;
+            f[j] = fmaf(f[j] - __ldg(coef + c), __ldg(coef + channels + c), __ldg(coef + 2 * channels + c));
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < W; ++j) f[j] = 0.f;
+    }
+    bn_store<T, W>(y + r * channels + v * W, f);
+}
+
+// ---------------------------------------------------------------- backward
+template <typename T, int W>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t rows, int channels, int vecs, int tpr,
+                     const int32_t *__restrict__ num_valid, const float *__restrict__ save_mean,
+                     const float *__restrict__ save_invstd, float2 *__restrict__ partials) {
+    __shared__ float s_a[BN_THREADS * W], s_b[BN_THREADS * W];
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t r0 = (int64_t)blockIdx.x * BN_CHUNK;
+    if (r0 >= M) return;
+    const int lanes = BN_THREADS / tpr;
+    const BnRowThread t = bn_row_thread(vecs, tpr);
+    const int64_t end = M < r0 + BN_CHUNK ? M : r0 + BN_CHUNK;
+    float sdy[W], sdyx[W];
+#pragma unroll
+    for (int j = 0; j < W; ++j) sdy[j] = sdyx[j] = 0.f;
+    if (t.active) {
+        float mean[W], invstd[W];
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+            mean[j] = __ldg(save_mean + t.v * W + j);
+            invstd[j] = __ldg(save_invstd + t.v * W + j);
+        }
+        const int64_t off = (int64_t)t.v * W;
+        auto fold = [&](const float (&fx)[W], const float (&fd)[W]) {
+#pragma unroll
+            for (int j = 0; j < W; ++j) {
+                sdy[j] += fd[j];
+                sdyx[j] = fmaf(fd[j], (fx[j] - mean[j]) * invstd[j], sdyx[j]);
+            }
+        };
+        int64_t r = r0 + t.lane;
+        for (; r + lanes < end; r += 2 * lanes) {          // two rows of x and dy in flight
+            float fx[2][W], fd[2][W];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                const int64_t o = (r + (int64_t)u * lanes) * channels + off;
+                bn_load<T, W>(x + o, fx[u]);
+                bn_load<T, W>(dy + o, fd[u]);
+            }
+#pragma unroll
+            for (int u = 0; u < 2; ++u) fold(fx[u], fd[u]);
+        }
+        for (; r < end; r += lanes) {
+            float fx[W], fd[W];
+            bn_load<T, W>(x + r * channels + off, fx);
+            bn_load<T, W>(dy + r * channels + off, fd);
+            fold(fx, fd);
+        }
+    }
+    const int slot = threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < W; ++j) { s_a[slot * W + j] = sdy[j]; s_b[slot * W + j] = sdyx[j]; }
+    for (int s = lanes >> 1; s >= 1; s >>= 1) {
+        __syncthreads();
+        if (t.lane < s) {
+            const int o = slot + s * tpr;
+#pragma unroll
+            for (int j = 0; j < W; ++j) {
+                s_a[slot * W + j] = sdy[j] = sdy[j] + s_a[o * W + j];
+                s_b[slot * W + j] = sdyx[j] = sdyx[j] + s_b[o * W + j];
+            }
+        }
+    }
+    if (t.lane == 0 && t.active) {
+        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
+#pragma unroll
+        for (int j = 0; j < W; ++j) dst[j] = make_float2(sdy[j], sdyx[j]);
+    }
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
+bn_bwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
+                       const int32_t *__restrict__ num_valid, const P *__restrict__ weight,
+                       const float *__restrict__ save_invstd, P *__restrict__ dweight, P *__restrict__ dbias,
+                       float *__restrict__ coef) {
+    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
+    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
+    const int c = blockIdx.x * BN_FIN_CH + cl;
+    const bool active = c < channels;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t K = (M + BN_CHUNK - 1) / BN_CHUNK;
+    float a = 0.f, b = 0.f;
+    if (active)
+        for (int64_t k = pl; k < K; k += BN_FIN_LANES) {
+            const float2 p = partials[k * channels + c];
+            a += p.x;
+            b += p.y;
+        }
+    const float sdy = bn_lane_sum(a, buf, pl, cl);
+    const float sdyx = bn_lane_sum(b, buf, pl, cl);
+    if (pl != 0 || !active) return;
+    if (dbias) dbias[c] = from_float<P>(sdy);
+    if (dweight) dweight[c] = from_float<P>(sdyx);
+    const float Mf = (float)M;
+    const float gamma = weight ? to_float(weight[c]) : 1.f;
+    coef[c] = gamma * save_invstd[c];
+    coef[channels + c] = M > 0 ? __fdiv_rn(sdy, Mf) : 0.f;
+    coef[2 * channels + c] = M > 0 ? __fdiv_rn(sdyx, Mf) : 0.f;
+}
+
+template <typename T, int W>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__restrict__ dx, int64_t rows, int channels,
+                    int vecs, const int32_t *__restrict__ num_valid, const float *__restrict__ save_mean,
+                    const float *__restrict__ save_invstd, const float *__restrict__ coef) {
+    const int64_t idx = blockIdx.x * (int64_t)BN_THREADS + threadIdx.x;
+    const int64_t r = idx / vecs;
+    const int v = (int)(idx - r * vecs);
+    if (r >= rows) return;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    float f[W];
+    if (r < M) {
+        float fx[W];
+        bn_load<T, W>(x + r * channels + v * W, fx);
+        bn_load<T, W>(dy + r * channels + v * W, f);
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+            const int c = v * W + j;
+            const float xhat = (fx[j] - __ldg(save_mean + c)) * __ldg(save_invstd + c);
+            f[j] = __ldg(coef + c) * (f[j] - __ldg(coef + channels + c) - xhat * __ldg(coef + 2 * channels + c));
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < W; ++j) f[j] = 0.f;
+    }
+    bn_store<T, W>(dx + r * channels + v * W, f);
+}
+
+// ---------------------------------------------------------------- host side
+static int64_t bn_chunks(int64_t rows) { return (rows + BN_CHUNK - 1) / BN_CHUNK; }
+
+static size_t bn_workspace(int64_t rows, int channels, int coefs) {
+    if (rows < 0 || channels < 1) return 0;
+    return align_up((size_t)bn_chunks(rows) * channels * sizeof(float2), 256) + align_up((size_t)coefs * channels * 4, 256);
+}
+
+static bool bn_float_dtype(int dt) { return dt == SPX_F32 || dt == SPX_F16 || dt == SPX_BF16; }
+
+static int bn_check(const char *who, int64_t rows, int channels, int dtype, int param_dtype) {
+    SPX_REQUIRE(rows >= 0 && rows < 2147483647ll, "%s: bad row count %lld", who, (long long)rows);
+    SPX_REQUIRE(channels >= 1 && channels <= (1 << 20), "%s: channels must be in [1, 2^20], got %d", who, channels);
+    SPX_REQUIRE(bn_float_dtype(dtype), "%s: unsupported dtype %d (float32, float16 and bfloat16 only)", who, dtype);
+    SPX_REQUIRE(param_dtype == SPX_F32 || param_dtype == dtype,
+                "%s: parameter dtype %d must be float32 or the feature dtype %d", who, param_dtype, dtype);
+    return 0;
+}
+
+static bool bn_aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
+
+static int bn_tpr(int vecs) {
+    int tpr = 1;
+    while (tpr < vecs && tpr < 32) tpr <<= 1;
+    return tpr;
+}
+
+struct BnFwdArgs {
+    const void *x;
+    void *y;
+    int64_t rows;
+    int channels;
+    const int32_t *num_valid;
+    const void *weight, *bias;
+    void *running_mean, *running_var;
+    const int64_t *nbt;
+    float momentum;
+    int cumulative;
+    float eps;
+    float *save_mean, *save_invstd;
+    float2 *partials;
+    float *coef;
+};
+
+template <typename T, int W> static int bn_fwd_rows(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
+    const int vecs = a.channels / W;
+    if (stats) {
+        const int tpr = bn_tpr(vecs);
+        const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
+        bn_stats_kernel<T, W><<<grid, BN_THREADS, 0, stream>>>(static_cast<const T *>(a.x), a.rows, a.channels, vecs,
+                                                               tpr, a.num_valid, a.partials);
+        SPX_CHECK_LAUNCH("bn_stats_kernel");
+    } else {
+        bn_fwd_apply_kernel<T, W><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
+            static_cast<const T *>(a.x), static_cast<T *>(a.y), a.rows, a.channels, vecs, a.num_valid, a.coef);
+        SPX_CHECK_LAUNCH("bn_fwd_apply_kernel");
+    }
+    return 0;
+}
+
+template <typename T> static int bn_fwd_rows_dispatch(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
+    constexpr int W = 16 / sizeof(T);
+    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && bn_aligned16(a.x) && bn_aligned16(a.y);
+    return vec ? bn_fwd_rows<T, W>(a, stats, stream) : bn_fwd_rows<T, 1>(a, stats, stream);
+}
+
+static int bn_fwd_rows_typed(int dtype, const BnFwdArgs &a, bool stats, cudaStream_t stream) {
+    switch (dtype) {
+        case SPX_F32: return bn_fwd_rows_dispatch<float>(a, stats, stream);
+        case SPX_F16: return bn_fwd_rows_dispatch<__half>(a, stats, stream);
+        default: return bn_fwd_rows_dispatch<__nv_bfloat16>(a, stats, stream);
+    }
+}
+
+template <typename P> static int bn_fwd_finalize(const BnFwdArgs &a, cudaStream_t stream) {
+    bn_fwd_finalize_kernel<P><<<(unsigned)div_up64(a.channels, BN_FIN_CH), BN_FIN_CH * BN_FIN_LANES, 0, stream>>>(
+        a.partials, a.rows, a.channels, a.num_valid, static_cast<const P *>(a.weight), static_cast<const P *>(a.bias),
+        static_cast<P *>(a.running_mean), static_cast<P *>(a.running_var), a.nbt, a.momentum, a.cumulative, a.eps,
+        a.save_mean, a.save_invstd, a.coef);
+    SPX_CHECK_LAUNCH("bn_fwd_finalize_kernel");
+    return 0;
+}
+
+struct BnBwdArgs {
+    const void *x, *dy;
+    void *dx;
+    int64_t rows;
+    int channels;
+    const int32_t *num_valid;
+    const void *weight;
+    const float *save_mean, *save_invstd;
+    void *dweight, *dbias;
+    float2 *partials;
+    float *coef;
+};
+
+template <typename T, int W> static int bn_bwd_rows(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
+    const int vecs = a.channels / W;
+    if (reduce) {
+        const int tpr = bn_tpr(vecs);
+        const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
+        bn_bwd_reduce_kernel<T, W><<<grid, BN_THREADS, 0, stream>>>(
+            static_cast<const T *>(a.x), static_cast<const T *>(a.dy), a.rows, a.channels, vecs, tpr, a.num_valid,
+            a.save_mean, a.save_invstd, a.partials);
+        SPX_CHECK_LAUNCH("bn_bwd_reduce_kernel");
+    } else {
+        bn_bwd_apply_kernel<T, W><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
+            static_cast<const T *>(a.x), static_cast<const T *>(a.dy), static_cast<T *>(a.dx), a.rows, a.channels, vecs,
+            a.num_valid, a.save_mean, a.save_invstd, a.coef);
+        SPX_CHECK_LAUNCH("bn_bwd_apply_kernel");
+    }
+    return 0;
+}
+
+template <typename T> static int bn_bwd_rows_dispatch(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
+    constexpr int W = 16 / sizeof(T);
+    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && bn_aligned16(a.x) && bn_aligned16(a.dy) &&
+                     bn_aligned16(a.dx);
+    return vec ? bn_bwd_rows<T, W>(a, reduce, stream) : bn_bwd_rows<T, 1>(a, reduce, stream);
+}
+
+static int bn_bwd_rows_typed(int dtype, const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
+    switch (dtype) {
+        case SPX_F32: return bn_bwd_rows_dispatch<float>(a, reduce, stream);
+        case SPX_F16: return bn_bwd_rows_dispatch<__half>(a, reduce, stream);
+        default: return bn_bwd_rows_dispatch<__nv_bfloat16>(a, reduce, stream);
+    }
+}
+
+template <typename P> static int bn_bwd_finalize(const BnBwdArgs &a, cudaStream_t stream) {
+    bn_bwd_finalize_kernel<P><<<(unsigned)div_up64(a.channels, BN_FIN_CH), BN_FIN_CH * BN_FIN_LANES, 0, stream>>>(
+        a.partials, a.rows, a.channels, a.num_valid, static_cast<const P *>(a.weight), a.save_invstd,
+        static_cast<P *>(a.dweight), static_cast<P *>(a.dbias), a.coef);
+    SPX_CHECK_LAUNCH("bn_bwd_finalize_kernel");
+    return 0;
+}
+
+}  // namespace spx
+
+using namespace spx;
+
+extern "C" size_t spx_masked_bn_fwd_train_workspace_size(int64_t rows, int channels) {
+    return bn_workspace(rows, channels, 3);
+}
+
+extern "C" size_t spx_masked_bn_bwd_workspace_size(int64_t rows, int channels) {
+    return bn_workspace(rows, channels, 3);
+}
+
+extern "C" int spx_masked_bn_fwd_train(const void *x, void *y, int64_t rows, int channels, int dtype,
+                                       const int32_t *num_valid, const void *weight, const void *bias,
+                                       void *running_mean, void *running_var, const int64_t *num_batches_tracked,
+                                       int param_dtype, float momentum, int cumulative, float eps, float *save_mean,
+                                       float *save_invstd, void *workspace, size_t workspace_bytes,
+                                       spx_stream_t stream_) {
+    const char *who = "masked_bn_fwd_train";
+    if (int rc = bn_check(who, rows, channels, dtype, param_dtype)) return rc;
+    SPX_REQUIRE(save_mean && save_invstd && workspace, "%s: NULL pointer argument (save_mean, save_invstd, workspace)",
+                who);
+    SPX_REQUIRE(rows == 0 || (x && y), "%s: NULL pointer argument (x, y)", who);
+    SPX_REQUIRE((running_mean == nullptr) == (running_var == nullptr),
+                "%s: running_mean and running_var must both be given or both be NULL", who);
+    SPX_REQUIRE(!(running_mean && cumulative && num_batches_tracked == nullptr),
+                "%s: a cumulative average (momentum None) needs num_batches_tracked", who);
+    SPX_REQUIRE(eps > 0.f, "%s: eps must be positive", who);
+    const size_t need = spx_masked_bn_fwd_train_workspace_size(rows, channels);
+    SPX_REQUIRE(workspace_bytes >= need, "%s: workspace too small: need %zu, have %zu", who, need, workspace_bytes);
+    WorkspaceCarver ws(workspace, workspace_bytes);
+    BnFwdArgs a{x, y, rows, channels, num_valid, weight, bias, running_mean, running_var, num_batches_tracked,
+                momentum, cumulative, eps, save_mean, save_invstd, nullptr, nullptr};
+    a.partials = ws.take<float2>((size_t)bn_chunks(rows) * channels);
+    a.coef = ws.take<float>((size_t)3 * channels);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (rows > 0)
+        if (int rc = bn_fwd_rows_typed(dtype, a, true, stream)) return rc;
+    int rc = 0;
+    switch (param_dtype) {
+        case SPX_F32: rc = bn_fwd_finalize<float>(a, stream); break;
+        case SPX_F16: rc = bn_fwd_finalize<__half>(a, stream); break;
+        default: rc = bn_fwd_finalize<__nv_bfloat16>(a, stream); break;
+    }
+    if (rc || rows == 0) return rc;
+    return bn_fwd_rows_typed(dtype, a, false, stream);
+}
+
+extern "C" int spx_masked_bn_bwd(const void *x, const void *dy, void *dx, int64_t rows, int channels, int dtype,
+                                 const int32_t *num_valid, const void *weight, int param_dtype, const float *save_mean,
+                                 const float *save_invstd, void *dweight, void *dbias, void *workspace,
+                                 size_t workspace_bytes, spx_stream_t stream_) {
+    const char *who = "masked_bn_bwd";
+    if (int rc = bn_check(who, rows, channels, dtype, param_dtype)) return rc;
+    SPX_REQUIRE(save_mean && save_invstd && workspace, "%s: NULL pointer argument (save_mean, save_invstd, workspace)",
+                who);
+    SPX_REQUIRE(rows == 0 || (x && dy && dx), "%s: NULL pointer argument (x, dy, dx)", who);
+    const size_t need = spx_masked_bn_bwd_workspace_size(rows, channels);
+    SPX_REQUIRE(workspace_bytes >= need, "%s: workspace too small: need %zu, have %zu", who, need, workspace_bytes);
+    WorkspaceCarver ws(workspace, workspace_bytes);
+    BnBwdArgs a{x, dy, dx, rows, channels, num_valid, weight, save_mean, save_invstd, dweight, dbias, nullptr, nullptr};
+    a.partials = ws.take<float2>((size_t)bn_chunks(rows) * channels);
+    a.coef = ws.take<float>((size_t)3 * channels);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (rows > 0)
+        if (int rc = bn_bwd_rows_typed(dtype, a, true, stream)) return rc;
+    int rc = 0;
+    switch (param_dtype) {
+        case SPX_F32: rc = bn_bwd_finalize<float>(a, stream); break;
+        case SPX_F16: rc = bn_bwd_finalize<__half>(a, stream); break;
+        default: rc = bn_bwd_finalize<__nv_bfloat16>(a, stream); break;
+    }
+    if (rc || rows == 0) return rc;
+    return bn_bwd_rows_typed(dtype, a, false, stream);
+}

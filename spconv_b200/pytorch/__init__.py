@@ -9,8 +9,8 @@ from .conv import (SparseConv1d, SparseConv2d, SparseConv3d, SparseConv4d,  # no
 from .identity import Identity  # noqa: F401
 from .core import (CUDAKernelTimer, ImplicitGemmIndiceData, IndiceData,  # noqa: F401
                    SparseConvTensor, scatter_nd)
-from .modules import (RemoveGrid, SparseBatchNorm, SparseIdentity, SparseModule,  # noqa: F401
-                      SparseReLU, SparseSequential, ToDense, assign_name_for_sparse_modules)
+from .modules import (MaskedBatchNorm1d, RemoveGrid, SparseBatchNorm, SparseIdentity,  # noqa: F401
+                      SparseModule, SparseReLU, SparseSequential, ToDense, assign_name_for_sparse_modules)
 from .pool import (SparseAvgPool1d, SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool,  # noqa: F401
                    SparseGlobalMaxPool, SparseMaxPool1d, SparseMaxPool2d, SparseMaxPool3d, SparseMaxPool4d)
 from .tables import AddTable, ConcatTable, JoinTable  # noqa: F401

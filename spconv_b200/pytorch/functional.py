@@ -347,3 +347,28 @@ def remove_duplicate(x: SparseConvTensor) -> SparseConvTensor:
     inverse[heads.long()] = torch.arange(m, dtype=torch.int32, device=dst.device)
     feats = _RowGather.apply(x.features, heads, inverse)
     return SparseConvTensor(feats, out_inds, x.spatial_shape, x.batch_size, x.grid)
+
+
+# ---------------------------------------------------------------------------- padding-aware BatchNorm
+class MaskedBatchNormFunction(Function):
+    """``x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps`` -> training-mode
+    BatchNorm over rows ``[0, num_valid)`` (:func:`ops.masked_batch_norm_forward`); the running stats are updated
+    in place.  The backward gives dx (0 on padding rows), dweight and dbias."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps):
+        y, mean, invstd = ops.masked_batch_norm_forward(x, num_valid, weight, bias, running_mean, running_var,
+                                                        num_batches_tracked, momentum, eps)
+        ctx.save_for_backward(x, weight, mean, invstd, num_valid)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        x, weight, mean, invstd, num_valid = ctx.saved_tensors
+        dx, dw, db = ops.masked_batch_norm_backward(x, grad_output, num_valid, weight, mean, invstd,
+                                                    ctx.needs_input_grad[1], ctx.needs_input_grad[2])
+        return dx, dw, db, None, None, None, None, None, None
+
+
+masked_batch_norm = MaskedBatchNormFunction.apply

@@ -9,6 +9,7 @@ from typing import Any, Optional
 import torch
 from torch import nn
 
+from . import functional
 from .core import SparseConvTensor
 
 
@@ -122,9 +123,86 @@ class SparseBatchNorm(_FeatureWise):
         super().__init__(nn.BatchNorm1d(num_features, eps, momentum, affine, track_running_stats))
 
     def forward(self, x: SparseConvTensor):
+        if isinstance(self.inner, MaskedBatchNorm1d):
+            return self.inner(x)
         if self.inner.training:
             x.require_unpadded("SparseBatchNorm in training mode")
         return super().forward(x)
+
+
+class MaskedBatchNorm1d(SparseModule, nn.BatchNorm1d):
+    """``nn.BatchNorm1d`` on the features of a :class:`SparseConvTensor` whose batch statistics cover only the
+    valid rows (``x.num_valid``; every row of an unpadded tensor), so a padded net trains at static shapes and
+    captures as one CUDA graph.  Same constructor, parameters, buffers and ``state_dict`` keys as
+    ``nn.BatchNorm1d``; convert an existing net with :meth:`convert_masked_batchnorm`.
+
+    Training mode (and eval mode without running stats) runs the CUDA kernels of ``csrc/batchnorm.cu``: the
+    results are those of ``nn.BatchNorm1d`` on the valid rows alone, computed in fp32 in a fixed order, so they
+    are bit-reproducible and independent of how far the tensor is padded.  Padding rows are never read; they
+    are 0 in the output and in the input gradient.  The running stats update on the device (``momentum=None``
+    reads ``num_batches_tracked`` there), so nothing is read back to the host.  Eval mode with running stats
+    is torch's row-wise ``F.batch_norm``, bit-identical to the unconverted module.
+
+    Differences from ``nn.BatchNorm1d``, which raises for one value per channel where this cannot:
+      * no valid row: the output is 0, every gradient is 0 and the running stats are unchanged;
+      * one valid row: the normalised value is 0, so the output is ``bias``; dx = 0, dbias = dy, dweight = 0,
+        and the running stats are unchanged.
+    ``num_batches_tracked`` counts every training call on a non-empty tensor, as torch increments it before its
+    check; a tensor without rows passes through untouched."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True,
+                 device=None, dtype=None):
+        nn.BatchNorm1d.__init__(self, num_features, eps, momentum, affine, track_running_stats, device, dtype)
+        self.name = None
+        self._sparse_unique_name = ""
+
+    def forward(self, x: SparseConvTensor):
+        feats = x.features
+        if feats.shape[0] == 0:
+            return x
+        if feats.dim() != 2 or feats.shape[1] != self.num_features:
+            raise ValueError(f"MaskedBatchNorm1d({self.num_features}): features of shape {tuple(feats.shape)}")
+        momentum = self.momentum
+        if self.training and self.track_running_stats and self.num_batches_tracked is not None:
+            self.num_batches_tracked.add_(1)
+        use_batch = self.training or (self.running_mean is None and self.running_var is None)
+        if not use_batch:
+            return x.replace_feature(nn.functional.batch_norm(
+                feats, self.running_mean, self.running_var, self.weight, self.bias, False, 0.0, self.eps))
+        track = not self.training or self.track_running_stats
+        rm = self.running_mean if track else None
+        rv = self.running_var if track else None
+        return x.replace_feature(functional.masked_batch_norm(
+            feats, self.weight, self.bias, rm, rv, self.num_batches_tracked if rm is not None else None,
+            x.num_valid, momentum, self.eps))
+
+    @classmethod
+    def convert_masked_batchnorm(cls, module: nn.Module) -> nn.Module:
+        """Replace, in place, every ``nn.BatchNorm1d`` (that exact type) that is a direct child of a
+        :class:`SparseSequential`, and the ``inner`` BatchNorm of every :class:`SparseBatchNorm`, by a
+        ``MaskedBatchNorm1d`` that takes over its parameters and buffers; returns ``module``.  ``SyncBatchNorm``,
+        other subclasses and BatchNorm layers outside sparse containers (dense heads) are left alone."""
+        if isinstance(module, SparseSequential):
+            for key, child in list(module._modules.items()):
+                if type(child) is nn.BatchNorm1d:
+                    module._modules[key] = cls._from_batchnorm(child)
+        elif isinstance(module, SparseBatchNorm) and type(module.inner) is nn.BatchNorm1d:
+            module.inner = cls._from_batchnorm(module.inner)
+        for child in module.children():
+            cls.convert_masked_batchnorm(child)
+        return module
+
+    @classmethod
+    def _from_batchnorm(cls, bn: nn.BatchNorm1d) -> "MaskedBatchNorm1d":
+        out = cls(bn.num_features, bn.eps, bn.momentum, bn.affine, bn.track_running_stats, device="meta")
+        if bn.affine:
+            out.weight = bn.weight
+            out.bias = bn.bias
+        out.running_mean = bn.running_mean
+        out.running_var = bn.running_var
+        out.num_batches_tracked = bn.num_batches_tracked
+        out.training = bn.training
+        return out
 
 
 class SparseIdentity(SparseModule):

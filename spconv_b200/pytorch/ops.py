@@ -1109,6 +1109,84 @@ def zero_rows_from_count_(x: torch.Tensor, num_valid: torch.Tensor) -> torch.Ten
     return x
 
 
+_BN_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _bn_param_code(x: torch.Tensor, params: Sequence[Optional[torch.Tensor]]) -> int:
+    """dtype code of the BatchNorm parameters / buffers: all float32, or all the feature dtype."""
+    given = [p for p in params if p is not None]
+    dt = given[0].dtype if given else torch.float32
+    for p in given:
+        _require_cuda(p, "BatchNorm parameters and buffers")
+        if p.dtype != dt or p.dim() != 1 or p.shape[0] != x.shape[1] or not p.is_contiguous():
+            raise RuntimeError(f"masked_batch_norm: parameters and buffers must be contiguous [{x.shape[1]}] tensors "
+                               "of one dtype")
+    if dt not in (torch.float32, x.dtype):
+        raise RuntimeError(f"masked_batch_norm: parameter dtype {dt} must be float32 or the feature dtype {x.dtype}")
+    return _DTYPE_CODE[dt]
+
+
+def _bn_features(x: torch.Tensor, num_valid: Optional[torch.Tensor]) -> torch.Tensor:
+    _require_cuda(x, "features")
+    if x.dim() != 2 or x.dtype not in _BN_DTYPES:
+        raise RuntimeError(f"masked_batch_norm: features must be a [rows, C] float32 / float16 / bfloat16 matrix, got "
+                           f"{tuple(x.shape)} {x.dtype}")
+    if num_valid is not None and (num_valid.dtype != torch.int32 or num_valid.device != x.device):
+        raise RuntimeError("masked_batch_norm: num_valid must be an int32 tensor on the features' device")
+    return x.contiguous()
+
+
+def masked_batch_norm_forward(x: torch.Tensor, num_valid: Optional[torch.Tensor], weight: Optional[torch.Tensor],
+                              bias: Optional[torch.Tensor], running_mean: Optional[torch.Tensor],
+                              running_var: Optional[torch.Tensor], num_batches_tracked: Optional[torch.Tensor],
+                              momentum: Optional[float], eps: float):
+    """Training-mode BatchNorm over rows ``[0, num_valid)`` of ``x`` (all rows when ``num_valid`` is None):
+    ``(y, mean, invstd)``; rows at and beyond ``num_valid`` of ``y`` are 0.  ``running_mean`` / ``running_var``
+    are updated in place; ``momentum=None`` takes ``1 / num_batches_tracked`` on the device (the caller
+    increments it first, as torch does)."""
+    x = _bn_features(x, num_valid)
+    code = _bn_param_code(x, [weight, bias, running_mean, running_var])
+    rows, c = x.shape
+    cumulative = momentum is None
+    if cumulative and running_mean is not None and num_batches_tracked is None:
+        raise RuntimeError("masked_batch_norm: momentum=None needs num_batches_tracked")
+    y = torch.empty_like(x)
+    mean = torch.empty((c,), dtype=torch.float32, device=x.device)
+    invstd = torch.empty((c,), dtype=torch.float32, device=x.device)
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_bn_fwd_train_workspace_size(rows, c), x.device)
+    _cabi.check(lib.spx_masked_bn_fwd_train(
+        _ptr(x), _ptr(y), rows, c, _DTYPE_CODE[x.dtype], _ptr(num_valid), _ptr(weight), _ptr(bias),
+        _ptr(running_mean), _ptr(running_var), _ptr(num_batches_tracked), code,
+        0.0 if cumulative else float(momentum), int(cumulative), float(eps), mean.data_ptr(), invstd.data_ptr(),
+        ws.data_ptr(), ws.numel(), _stream()), "masked_bn_fwd_train")
+    return y, mean, invstd
+
+
+def masked_batch_norm_backward(x: torch.Tensor, dy: torch.Tensor, num_valid: Optional[torch.Tensor],
+                               weight: Optional[torch.Tensor], mean: torch.Tensor, invstd: torch.Tensor,
+                               need_weight_grad: bool = True, need_bias_grad: bool = True):
+    """``(dx, dweight, dbias)`` of :func:`masked_batch_norm_forward`; padding rows of ``dx`` are 0, the
+    parameter gradients (None when not needed) have the parameters' dtype (float32 without ``weight``)."""
+    x = _bn_features(x, num_valid)
+    dy = dy.contiguous()
+    if dy.shape != x.shape or dy.dtype != x.dtype:
+        raise RuntimeError("masked_batch_norm: the output gradient must match the features' shape and dtype")
+    code = _bn_param_code(x, [weight])
+    pdt = weight.dtype if weight is not None else torch.float32
+    rows, c = x.shape
+    dx = torch.empty_like(x)
+    dw = torch.empty((c,), dtype=pdt, device=x.device) if need_weight_grad else None
+    db = torch.empty((c,), dtype=pdt, device=x.device) if need_bias_grad else None
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_bn_bwd_workspace_size(rows, c), x.device)
+    _cabi.check(lib.spx_masked_bn_bwd(
+        _ptr(x), _ptr(dy), _ptr(dx), rows, c, _DTYPE_CODE[x.dtype], _ptr(num_valid), _ptr(weight), code,
+        mean.data_ptr(), invstd.data_ptr(), _ptr(dw), _ptr(db), ws.data_ptr(), ws.numel(), _stream()),
+        "masked_bn_bwd")
+    return dx, dw, db
+
+
 def last_kernel_family() -> int:
     """0 none, 1 generic FMA kernels, 2 wgmma tensor-core kernels (what served the last GEMM call)."""
     return int(_lib().spx_last_kernel_family())
