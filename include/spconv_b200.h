@@ -29,6 +29,8 @@
  *           maxpool_implicit_gemm_backward / avgpool_implicit_gemm_forward / _backward /
  *           global_pool_rearrange                    spconv/csrc/sparse/all.py:664-905
  *           (kernels spconv/csrc/sparse/maxpool.py:41-341)
+ *   spx_global_pool_fwd / spx_global_pool_bwd
+ *        <- no kernel: the per-sample torch loop of SparseGlobalMaxPool / AvgPool, spconv/pytorch/pool.py:251-278
  *   spx_sparse_add_group / _fwd / _gather (+ spx_conv_rulebook_stage1+2 for the union)
  *        <- functional.sparse_add / sparse_add_hash_based spconv/pytorch/functional.py:441-544
  *   spx_hash_clear / _insert / _query / _insert_exist / _rank
@@ -397,6 +399,29 @@ int spx_indice_pool_bwd(int mode, const void *features, const void *out_features
  */
 int spx_global_pool_rearrange(const int32_t *coords, int64_t n, int row_ints, int batch_size,
                               int32_t *out_indices, int32_t *counts, spx_stream_t stream);
+/*
+ * Padding-aware global pooling (MaskedGlobalMaxPool / MaskedGlobalAvgPool): out [batch_size, channels] per
+ * sample, with no host read-back.  M = *num_valid (device int32, clamped to [0, rows]; NULL = every row).
+ * Row r counts for sample b when r < M and coords[r * row_ints] == b with 0 <= b < batch_size; rows [M, rows)
+ * are never read (features nor coords), rows with another batch index are dropped.
+ *   mode 0  max: out[b, c] = x[a, c] bit for bit, a = argmax[b, c] [batch_size, channels] the first row in
+ *           ascending order that attains the maximum; a NaN counts as the maximum, -0 and +0 tie
+ *   mode 1  mean: out[b, c] = (fp32 sum of the sample's rows) / count[b], rounded once; count [batch_size]
+ * An empty sample gives out = 0, argmax = -1, count = 0.  The rows of a sample are reduced in a fixed order
+ * that depends on them alone (chunks of rows merged in chunk order, no float atomics), so every result is
+ * bit-reproducible and independent of `rows` (padding).
+ * bwd: din [rows, channels], every element written once: mode 0 din[a, c] = dy[b, c] at a = argmax[b, c],
+ *      mode 1 din[r, c] = dy[b, c] / count[b] in fp32, rounded once; 0 on padding and dropped rows.
+ * dtype: f32 / f16 / bf16.  batch_size in [1, 2^20], channels in [1, 65536], rows < 2^31 - 1.
+ * workspace (fwd only): spx_global_pool_workspace_size(rows, batch_size, channels) bytes.
+ */
+size_t spx_global_pool_workspace_size(int64_t rows, int batch_size, int channels);
+int spx_global_pool_fwd(int mode, const void *features, const int32_t *coords, int64_t rows, int row_ints,
+                        int batch_size, int channels, int dtype, const int32_t *num_valid, void *out, int32_t *argmax,
+                        int32_t *count, void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_global_pool_bwd(int mode, const void *dy, const int32_t *coords, int64_t rows, int row_ints, int batch_size,
+                        int channels, int dtype, const int32_t *num_valid, const int32_t *argmax, const int32_t *count,
+                        void *din, spx_stream_t stream);
 
 /* ------------------------------------------------------------------ sum over different coordinates */
 

@@ -141,6 +141,11 @@ SIGNATURES = {
     "spx_indice_pool_bwd": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                     c_int64, c_int, c_int, c_void_p, c_void_p]),
     "spx_global_pool_rearrange": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "spx_global_pool_workspace_size": (c_size_t, [c_int64, c_int, c_int]),
+    "spx_global_pool_fwd": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_global_pool_bwd": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p]),
     "spx_sparse_add_group_workspace_size": (c_size_t, [c_int64]),
     "spx_sparse_add_group": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_sparse_add_fwd": (c_int, [POINTER(SparseAddOperands), c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p,

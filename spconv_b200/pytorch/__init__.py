@@ -11,8 +11,9 @@ from .core import (CUDAKernelTimer, ImplicitGemmIndiceData, IndiceData,  # noqa:
                    SparseConvTensor, scatter_nd)
 from .modules import (MaskedBatchNorm1d, RemoveGrid, SparseBatchNorm, SparseIdentity,  # noqa: F401
                       SparseModule, SparseReLU, SparseSequential, ToDense, assign_name_for_sparse_modules)
-from .pool import (SparseAvgPool1d, SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool,  # noqa: F401
-                   SparseGlobalMaxPool, SparseMaxPool1d, SparseMaxPool2d, SparseMaxPool3d, SparseMaxPool4d)
+from .pool import (MaskedGlobalAvgPool, MaskedGlobalMaxPool, SparseAvgPool1d,  # noqa: F401
+                   SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool, SparseGlobalMaxPool, SparseMaxPool1d,
+                   SparseMaxPool2d, SparseMaxPool3d, SparseMaxPool4d)
 from .tables import AddTable, ConcatTable, JoinTable  # noqa: F401
 from .utils_fuse import (fuse_act, fuse_bn, fuse_bn_act_sequential, fuse_bn_weights)  # noqa: F401
 from . import quantized  # noqa: F401

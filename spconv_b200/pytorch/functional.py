@@ -372,3 +372,28 @@ class MaskedBatchNormFunction(Function):
 
 
 masked_batch_norm = MaskedBatchNormFunction.apply
+
+
+# ---------------------------------------------------------------------------- padding-aware global pooling
+class MaskedGlobalPoolFunction(Function):
+    """``features, indices, batch_size, num_valid, is_mean`` -> ``[batch_size, C]``: per-sample max or mean over
+    the rows ``[0, num_valid)`` whose batch index is in range (:func:`ops.masked_global_pool_fwd`).  The backward
+    gives the features' gradient: ``dy`` at the argmax row (max) or ``dy / count`` (mean), 0 on the other rows."""
+
+    @staticmethod
+    def forward(ctx, features, indices, batch_size, num_valid, is_mean):
+        out, aux = ops.masked_global_pool_fwd(features, indices, batch_size, num_valid, is_mean)
+        ctx.save_for_backward(indices, num_valid, aux)
+        ctx.batch_size = batch_size
+        ctx.is_mean = is_mean
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        indices, num_valid, aux = ctx.saved_tensors
+        din = ops.masked_global_pool_bwd(grad_output, indices, ctx.batch_size, num_valid, aux, ctx.is_mean)
+        return din, None, None, None, None
+
+
+masked_global_pool = MaskedGlobalPoolFunction.apply

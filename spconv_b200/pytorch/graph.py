@@ -9,7 +9,9 @@ read-back is the output count of an UNBOUNDED regular-conv rulebook (``spx_conv_
 reference syncs at the same point, ``spconv/csrc/sparse/indices.py:1454-1455``).  Give the strided layers
 an output bound (``spconv.set_output_bounds``) and pad the inputs to one size
 (``SparseConvTensor.pad_to``): then the rulebooks keep the count on the device and a whole encoder
-step, forward and backward, captures; ``spconv.check_bounds`` tells when a bound was exceeded.
+step, forward and backward, captures; ``spconv.check_bounds`` tells when a bound was exceeded.  Of the
+modules, ``SparseGlobalMaxPool`` / ``SparseGlobalAvgPool`` read the per-sample counts back to the host:
+``MaskedGlobalMaxPool`` / ``MaskedGlobalAvgPool`` reduce on the device and capture.
 """
 from __future__ import annotations
 

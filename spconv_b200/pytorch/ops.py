@@ -970,6 +970,70 @@ def global_pool_rearrange(coords: torch.Tensor, batch_size: int):
     return out_indices, counts
 
 
+_GLOBAL_POOL_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
+
+
+def _global_pool_check(features: torch.Tensor, indices: torch.Tensor, batch_size: int,
+                       num_valid: Optional[torch.Tensor]):
+    if features.dtype not in _GLOBAL_POOL_DTYPES:
+        raise RuntimeError(f"masked global pooling supports float32, float16 and bfloat16 features, got "
+                           f"{features.dtype}")
+    _require_cuda(features, "features")
+    _require_cuda(indices, "indices")
+    if features.dim() != 2 or indices.dim() != 2 or indices.dtype != torch.int32 \
+            or indices.shape[0] != features.shape[0]:
+        raise RuntimeError(f"masked global pooling: features [rows, C] and int32 indices [rows, ndim + 1] expected, "
+                           f"got {tuple(features.shape)} and {tuple(indices.shape)} {indices.dtype}")
+    if num_valid is not None and (num_valid.dtype != torch.int32 or num_valid.device != features.device):
+        raise RuntimeError("masked global pooling: num_valid must be an int32 tensor on the features' device")
+    if int(batch_size) < 1:
+        raise RuntimeError(f"masked global pooling: batch_size must be positive, got {batch_size}")
+
+
+def masked_global_pool_fwd(features: torch.Tensor, indices: torch.Tensor, batch_size: int,
+                           num_valid: Optional[torch.Tensor], is_mean: bool):
+    """Per-sample max or mean over rows ``[0, num_valid)`` (all rows when ``num_valid`` is None) whose batch index
+    ``indices[:, 0]`` is in ``[0, batch_size)``: ``(out [batch_size, C], aux)``.  ``aux`` is what the backward
+    needs: ``argmax [batch_size, C]`` int32 (max; the first row that attains the maximum, NaN counting as the
+    maximum) or ``count [batch_size]`` int32 (mean).  An empty sample gives 0 (argmax -1, count 0).  No host
+    synchronisation; bit-reproducible whatever the padding."""
+    _global_pool_check(features, indices, batch_size, num_valid)
+    features, indices = features.contiguous(), indices.contiguous()
+    rows, c = features.shape
+    b = int(batch_size)
+    out = torch.empty((b, c), dtype=features.dtype, device=features.device)
+    if is_mean:
+        aux = torch.empty((b,), dtype=torch.int32, device=features.device)
+    else:
+        aux = torch.empty((b, c), dtype=torch.int32, device=features.device)
+    lib = _lib()
+    ws = _bytes(lib.spx_global_pool_workspace_size(rows, b, c), features.device)
+    _cabi.check(lib.spx_global_pool_fwd(
+        int(is_mean), _ptr(features), _ptr(indices), rows, int(indices.shape[1]), b, c, _DTYPE_CODE[features.dtype],
+        _ptr(num_valid), out.data_ptr(), None if is_mean else aux.data_ptr(), aux.data_ptr() if is_mean else None,
+        ws.data_ptr(), ws.numel(), _stream()), "global_pool_fwd")
+    return out, aux
+
+
+def masked_global_pool_bwd(dy: torch.Tensor, indices: torch.Tensor, batch_size: int,
+                           num_valid: Optional[torch.Tensor], aux: torch.Tensor, is_mean: bool) -> torch.Tensor:
+    """``din [rows, C]`` of :func:`masked_global_pool_fwd`: ``dy[b]`` at the argmax rows (max) or
+    ``dy[b] / count[b]`` on every row of sample ``b`` (mean), 0 on padding and dropped rows."""
+    dy = dy.contiguous()
+    b = int(batch_size)
+    rows = indices.shape[0]
+    din = torch.empty((rows, dy.shape[1]), dtype=dy.dtype, device=dy.device)
+    _global_pool_check(din, indices, b, num_valid)
+    if dy.shape != (b, din.shape[1]):
+        raise RuntimeError(f"masked global pooling: the output gradient must be [{b}, C], got {tuple(dy.shape)}")
+    indices = indices.contiguous()
+    _cabi.check(_lib().spx_global_pool_bwd(
+        int(is_mean), dy.data_ptr(), _ptr(indices), rows, int(indices.shape[1]), b, int(dy.shape[1]),
+        _DTYPE_CODE[dy.dtype], _ptr(num_valid), None if is_mean else aux.data_ptr(),
+        aux.data_ptr() if is_mean else None, _ptr(din), _stream()), "global_pool_bwd")
+    return din
+
+
 # ---------------------------------------------------------------------------- sparse add
 _SPARSE_ADD_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 

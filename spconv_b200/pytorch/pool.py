@@ -1,5 +1,6 @@
 """Sparse pooling modules on the conv rulebooks: ``SparseMaxPool{1..4}d``, ``SparseAvgPool{1..3}d``,
-``SparseGlobalMaxPool`` / ``SparseGlobalAvgPool``.
+``SparseGlobalMaxPool`` / ``SparseGlobalAvgPool``, and the padding-aware, capturable global pools
+``MaskedGlobalMaxPool`` / ``MaskedGlobalAvgPool`` (``spx_global_pool_fwd/bwd``).
 
 Behaviour follows ``spconv/pytorch/pool.py``: constructor arguments :36-81 / :288-318 (``stride=None``
 means ``kernel_size``), algo default :66-80, rulebook caching under ``indice_key`` :144-230, the
@@ -188,6 +189,42 @@ class SparseGlobalAvgPool(SparseGlobalMaxOrAvgPool):
 
 
 class SparseGlobalMaxPool(SparseGlobalMaxOrAvgPool):
+    def __init__(self, name=None):
+        super().__init__(is_mean=False, name=name)
+
+
+class MaskedGlobalMaxOrAvgPool(SparseModule):
+    """Per-sample reduction over the valid rows -> dense ``[batch, C]``, in CUDA (``csrc/global_pool.cu``) with no
+    host synchronisation, so a net that ends in a global pool captures as one CUDA graph.  Accepts padded and
+    unpadded tensors: only rows below ``x.num_valid`` count, and they are never read beyond it.  Rows whose batch
+    index is outside ``[0, batch_size)`` are dropped.  float32, float16 and bfloat16 features.
+
+    Max returns the value of the first row (in row order) that attains the maximum, bit for bit; a NaN counts as
+    the maximum and -0 / +0 tie.  Its gradient goes to that one row, as ``torch.max(dim)``'s does.  Mean is the
+    fp32 sum of the sample's rows divided by their count, rounded once; its gradient is ``dy / count`` on every
+    row of the sample.  Padding and dropped rows get a zero gradient.
+
+    Differences from the reference's global pools (``spconv/pytorch/pool.py:251-278``):
+      * an empty sample gives 0 (the reference's max raises, its mean gives NaN);
+      * the output is ``[batch, C]`` for the mean too (the reference's average pool returns channel 0 only);
+      * results are deterministic: the rows of a sample are reduced in a fixed order, whatever the padding."""
+
+    def __init__(self, is_mean: bool, name=None):
+        super().__init__(name=name)
+        self.is_mean = is_mean
+
+    def forward(self, input: SparseConvTensor):
+        assert isinstance(input, SparseConvTensor)
+        return Fsp.masked_global_pool(input.features, input.indices, input.batch_size, input.num_valid,
+                                      self.is_mean)
+
+
+class MaskedGlobalAvgPool(MaskedGlobalMaxOrAvgPool):
+    def __init__(self, name=None):
+        super().__init__(is_mean=True, name=name)
+
+
+class MaskedGlobalMaxPool(MaskedGlobalMaxOrAvgPool):
     def __init__(self, name=None):
         super().__init__(is_mean=False, name=name)
 
