@@ -33,6 +33,8 @@
  *        <- no kernel: the per-sample torch loop of SparseGlobalMaxPool / AvgPool, spconv/pytorch/pool.py:251-278
  *   spx_sparse_add_group / _fwd / _gather (+ spx_conv_rulebook_stage1+2 for the union)
  *        <- functional.sparse_add / sparse_add_hash_based spconv/pytorch/functional.py:441-544
+ *   spx_sparse_add_union / spx_masked_sparse_add_plan / _heads (+ _group / _fwd / _gather)
+ *        <- no counterpart: functional.masked_sparse_add / masked_remove_duplicate (padded operands, no read-back)
  *   spx_hash_clear / _insert / _query / _insert_exist / _rank
  *        <- HashTable (spconv/pytorch/hash.py)        spconv/csrc/hash/core.py
  *
@@ -455,6 +457,43 @@ int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const int32_t *o
                        int64_t M, int channels, int dtype, void *out, spx_stream_t stream);
 int spx_sparse_add_gather(const int32_t *index, const void *src, int64_t src_rows,
                           const spx_sparse_add_operands *operands, int channels, int dtype, spx_stream_t stream);
+
+/*
+ * The union with the output count kept on the device: the bounded rulebook (spx_conv_rulebook_bounded_all) of
+ * the 1x..x1, stride-1, padding-0 convolution `g` (out_dims = in_dims) over indices [N, ndim+1], without masks,
+ * mask sorts or tile tables.  out_inds [bound, ndim+1]: the distinct in-range coordinates in first-touch order,
+ * rows [M, bound) -1; dst [N] = output row of every row (-1: out of range, or ranked >= bound); *num_out = M;
+ * *status |= 1 when more than `bound` outputs existed (those ranked >= bound dropped), |= 2 on a probe-chain
+ * overflow (then M = 0).  1 <= bound <= N, bound < 2^30.  32- and 64-bit keys.
+ */
+size_t spx_sparse_add_union_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t bound);
+int spx_sparse_add_union(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int64_t bound,
+                         int32_t *out_inds, int32_t *dst, int32_t *num_out, int32_t *status, void *workspace,
+                         size_t workspace_bytes, spx_stream_t stream);
+
+/*
+ * Padded operands (functional.masked_sparse_add): the operand table and `indices` [rows, ndim+1] are in ARGUMENT
+ * order (operands->rows only is read).  num_valid: host array of operands->count device int32 pointers (an entry,
+ * or the array, NULL = every row valid); operand t's valid rows are [0, valid_t), valid_t = *num_valid[t] clamped
+ * to [0, rows_t].  Rows at and beyond valid_t are never read.  The visit order is decided on the device from the
+ * valid counts exactly as sparse_add decides it from the row counts (largest first, ties: the earliest, then the
+ * others in argument order), so rows [0, M) of every output equal sparse_add of the valid rows bit for bit.
+ *   plan:  out_inds [bound, ndim+1], *num_out, *status as spx_sparse_add_union; dst [rows] (argument order, -1
+ *          on padding, out-of-range and dropped rows); order [rows] and offsets [bound + 1] as spx_sparse_add_group
+ *          with argument-order row ids (segments in ascending visit order; offsets[o] = offsets[o+1] for o >= M).
+ *          spx_sparse_add_fwd (M = bound, argument-order operands) then gives out [bound, C] with rows [M, bound)
+ *          0, and spx_sparse_add_gather (index = dst) the gradients.  0 <= bound <= rows, bound >= 1 unless
+ *          rows == 0 (then *num_out = 0 and offsets[0] = 0).
+ *   heads: heads [bound] = order[offsets[o]] (the row that created output o) for o < *num_out, else -1;
+ *          inverse [rows] = o at heads[o], -1 elsewhere (RemoveDuplicate's gather indices).
+ */
+size_t spx_masked_sparse_add_workspace_size(const spx_conv_geometry *g, int64_t rows, int64_t bound);
+int spx_masked_sparse_add_plan(const spx_conv_geometry *g, const spx_sparse_add_operands *operands,
+                               const int32_t *const *num_valid, const int32_t *indices, int64_t bound,
+                               int32_t *out_inds, int32_t *dst, int32_t *order, int32_t *offsets, int32_t *num_out,
+                               int32_t *status, void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_masked_sparse_add_heads(const int32_t *order, const int32_t *offsets, const int32_t *num_out, int64_t bound,
+                                int64_t rows, int32_t *heads, int32_t *inverse, spx_stream_t stream);
 
 /* ------------------------------------------------------------------ padding-aware BatchNorm */
 

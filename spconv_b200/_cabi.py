@@ -152,6 +152,15 @@ SIGNATURES = {
                                    c_void_p]),
     "spx_sparse_add_gather": (c_int, [c_void_p, c_void_p, c_int64, POINTER(SparseAddOperands), c_int, c_int,
                                       c_void_p]),
+    "spx_sparse_add_union_workspace_size": (c_size_t, [POINTER(ConvGeometry), c_int64, c_int64]),
+    "spx_sparse_add_union": (c_int, [POINTER(ConvGeometry), c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_masked_sparse_add_workspace_size": (c_size_t, [POINTER(ConvGeometry), c_int64, c_int64]),
+    "spx_masked_sparse_add_plan": (c_int, [POINTER(ConvGeometry), POINTER(SparseAddOperands), POINTER(c_void_p),
+                                           c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_masked_sparse_add_heads": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
+                                            c_void_p]),
     "spx_masked_bn_fwd_train_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_masked_bn_fwd_train": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_float, c_void_p,

@@ -20,6 +20,7 @@ namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
 int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
                        int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
+int validate_sparse_add_union(const spx_conv_geometry *g, int64_t N, int64_t bound);
 }
 
 namespace spx {
@@ -1553,13 +1554,16 @@ struct BoundedWs {
     uint32_t *rank_bitmap; int *rank_tiles; int64_t rank_ntiles;
     int *state;
     void *sort_ws; size_t sort_bytes;
+    int32_t *pair_scratch;
     size_t bytes;
     RbLayout L;
 };
 
 // rank_bitmap .. state + 64 stay contiguous: conv_clear_kernel zeroes that range in one pass.
 // The table is sized from the bound alone (load <= 0.5 with `bound` outputs): there is no second attempt.
-void carve_bounded_ws(const Geom &gg, int64_t N, int64_t bound, void *workspace, size_t bytes, BoundedWs &w) {
+// `sorts`: the conv rulebook's two mask-sort scratch areas; without them (the sparse_add union) a
+// pair_fwd [bound] that the kernels write and nobody reads takes their place.
+void carve_bounded_ws(const Geom &gg, int64_t N, int64_t bound, bool sorts, void *workspace, size_t bytes, BoundedWs &w) {
     w.L = rb_layout(gg, bound, gg.out_dims, 2);
     WorkspaceCarver ws(workspace, bytes);
     w.tbl = ws.take<char>(w.L.table_bytes);
@@ -1569,8 +1573,9 @@ void carve_bounded_ws(const Geom &gg, int64_t N, int64_t bound, void *workspace,
     w.rank_tiles = (int *)(w.rank_bitmap + w.rank_ntiles * RANK_TILE_WORDS);
     w.state = ws.take<int>(64);
     const int64_t max_rows = bound > N ? bound : N;
-    w.sort_bytes = 2 * align_up(spx_mask_argsort_workspace_size(max_rows, (gg.kv + 31) / 32), 256);   // two sorts side by side
-    w.sort_ws = ws.take<char>(w.sort_bytes);
+    w.sort_bytes = sorts ? 2 * align_up(spx_mask_argsort_workspace_size(max_rows, (gg.kv + 31) / 32), 256) : 0;
+    w.sort_ws = sorts ? ws.take<char>(w.sort_bytes) : nullptr;     // two sorts side by side
+    w.pair_scratch = sorts ? nullptr : ws.take<int32_t>((size_t)bound);
     w.bytes = ws.off;
 }
 
@@ -1604,15 +1609,32 @@ int bounded_rulebook_kernels(Table t, const Geom &gg, const BoundedWs &w, const 
         else conv_pairs_kernel<Table, false><<<grid, T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd);
         SPX_CHECK_LAUNCH("conv_pairs_kernel");
     }
-    if (!mask_fwd_or) {
+    if (!mask_fwd_or && mask_fwd) {              // no masks at all for the sparse_add union
         table_mask_kernel<<<(unsigned)div_up64(bound, 256), 256, 0, stream>>>(pair_fwd, bound, gg.kv, words, mask_fwd);
         SPX_CHECK_LAUNCH("table_mask_kernel");
     }
-    if (!k3 && N > 0) {                          // the 3x3x3 pairs kernel has already written it
+    if (!k3 && N > 0 && mask_bwd) {              // the 3x3x3 pairs kernel has already written it
         table_mask_kernel<<<(unsigned)div_up64(N, 256), 256, 0, stream>>>(pair_bwd, N, gg.kv, words, mask_bwd);
         SPX_CHECK_LAUNCH("table_mask_kernel");
     }
     return 0;
+}
+
+// clear the table, the ranking scratch and the state, then the kernels above on the 32- or 64-bit-key table
+int run_bounded(const Geom &gg, const BoundedWs &w, const int32_t *indices, int64_t N, int64_t bound, int32_t *out_inds,
+                int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd, uint32_t *mask_bwd, int32_t *num_out,
+                int32_t *status, cudaStream_t stream) {
+    const int64_t zero_vec = (int64_t)(((char *)(w.state + 64) - (char *)w.rank_bitmap) / 16);
+    conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)w.L.capacity / 2,
+                                                          w.L.i64 ? (uint4 *)w.tvals : nullptr,
+                                                          w.L.i64 ? (int64_t)w.L.capacity / 4 : 0,
+                                                          (uint4 *)w.rank_bitmap, zero_vec);
+    SPX_CHECK_LAUNCH("conv_clear_kernel");
+    if (!w.L.i64)
+        return bounded_rulebook_kernels(Table32{(unsigned long long *)w.tbl, w.L.capacity - 1}, gg, w, indices, N, bound,
+                                        out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
+    return bounded_rulebook_kernels(Table64{(long long *)w.tbl, w.tvals, w.L.capacity - 1}, gg, w, indices, N, bound,
+                                    out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
 }
 
 int validate_bounded(const spx_conv_geometry *g, int64_t N, int64_t bound) {
@@ -1632,7 +1654,7 @@ int validate_bounded(const spx_conv_geometry *g, int64_t N, int64_t bound) {
 extern "C" size_t spx_conv_rulebook_bounded_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t bound) {
     if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM || N < 0 || bound <= 0 || bound >= (1ll << 30)) return 0;
     BoundedWs w;
-    carve_bounded_ws(make_geom(g, false), N, bound, nullptr, SIZE_MAX, w);
+    carve_bounded_ws(make_geom(g, false), N, bound, true, nullptr, SIZE_MAX, w);
     return align_up(w.bytes, 256) + 256;
 }
 
@@ -1656,23 +1678,46 @@ extern "C" int spx_conv_rulebook_bounded_all(const spx_conv_geometry *g, const i
     cudaStream_t stream = (cudaStream_t)stream_;
     const Geom gg = make_geom(g, false);
     BoundedWs w;
-    carve_bounded_ws(gg, N, bound, workspace, workspace_bytes, w);
-    const int64_t zero_vec = (int64_t)(((char *)(w.state + 64) - (char *)w.rank_bitmap) / 16);
-    conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)w.L.capacity / 2,
-                                                          w.L.i64 ? (uint4 *)w.tvals : nullptr,
-                                                          w.L.i64 ? (int64_t)w.L.capacity / 4 : 0,
-                                                          (uint4 *)w.rank_bitmap, zero_vec);
-    SPX_CHECK_LAUNCH("conv_clear_kernel");
-    int rc;
-    if (!w.L.i64)
-        rc = bounded_rulebook_kernels(Table32{(unsigned long long *)w.tbl, w.L.capacity - 1}, gg, w, indices, N, bound,
-                                      out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
-    else
-        rc = bounded_rulebook_kernels(Table64{(long long *)w.tbl, w.tvals, w.L.capacity - 1}, gg, w, indices, N, bound,
-                                      out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
-    if (rc) return rc;
+    carve_bounded_ws(gg, N, bound, true, workspace, workspace_bytes, w);
+    if (int rc = run_bounded(gg, w, indices, N, bound, out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status,
+                             stream)) return rc;
     return conv_sort_and_tiles(gg.kv, N, bound, pair_fwd, pair_bwd, mask_fwd, mask_bwd, argsort_fwd, argsort_bwd, do_sort,
                                table_fwd, tmask_fwd, table_bwd, tmask_bwd, w.sort_ws, w.sort_bytes, stream_);
+}
+
+// ---- the union of sparse_add: the bounded rulebook of a 1x..x1, stride-1, padding-0 convolution, without its masks,
+// mask sorts and tile tables (the union reads out_inds, dst = pair_bwd[0] and the count only)
+int spx::validate_sparse_add_union(const spx_conv_geometry *g, int64_t N, int64_t bound) {
+    if (validate_geom(g)) return 2;
+    for (int a = 0; a < g->ndim; ++a)
+        SPX_REQUIRE(g->ksize[a] == 1 && g->stride[a] == 1 && g->padding[a] == 0 && g->dilation[a] == 1 &&
+                    g->out_dims[a] == g->in_dims[a] && !g->transposed,
+                    "sparse_add_union: the geometry must be 1x..x1, stride 1, padding 0, out_dims = in_dims (axis %d)", a);
+    SPX_REQUIRE(N > 0 && N < 2147483647ll, "sparse_add_union: bad row count %lld", (long long)N);
+    SPX_REQUIRE(bound > 0 && bound <= N && bound < (1ll << 30), "sparse_add_union: bound must be in [1, min(rows, 2^30)), "
+                "got %lld for %lld rows", (long long)bound, (long long)N);
+    return 0;
+}
+
+extern "C" size_t spx_sparse_add_union_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t bound) {
+    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM || N <= 0 || bound <= 0 || bound > N || bound >= (1ll << 30)) return 0;
+    BoundedWs w;
+    carve_bounded_ws(make_geom(g, false), N, bound, false, nullptr, SIZE_MAX, w);
+    return align_up(w.bytes, 256) + 256;
+}
+
+extern "C" int spx_sparse_add_union(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int64_t bound,
+                                    int32_t *out_inds, int32_t *dst, int32_t *num_out, int32_t *status, void *workspace,
+                                    size_t workspace_bytes, spx_stream_t stream) {
+    if (validate_sparse_add_union(g, N, bound)) return 2;
+    SPX_REQUIRE(indices && out_inds && dst && num_out && status && workspace, "sparse_add_union: NULL pointer argument");
+    const size_t need = spx_sparse_add_union_workspace_size(g, N, bound);
+    SPX_REQUIRE(workspace_bytes >= need, "sparse_add_union: workspace too small: need %zu, have %zu", need, workspace_bytes);
+    const Geom gg = make_geom(g, false);
+    BoundedWs w;
+    carve_bounded_ws(gg, N, bound, false, workspace, workspace_bytes, w);
+    return run_bounded(gg, w, indices, N, bound, out_inds, w.pair_scratch, dst, nullptr, nullptr, num_out, status,
+                       (cudaStream_t)stream);
 }
 
 extern "C" int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_bytes, const int32_t *count,

@@ -19,6 +19,7 @@ namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
 int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
                        int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
+int validate_sparse_add_union(const spx_conv_geometry *g, int64_t N, int64_t bound);
 
 constexpr int SA_THREADS = 256;
 constexpr int SA_MAX = SPX_SPARSE_ADD_MAX_OPERANDS;
@@ -49,15 +50,19 @@ __global__ void sa_keys_kernel(const int32_t *__restrict__ dst, int64_t n, uint3
     keys[i] = o < 0 ? m : (uint32_t)o;
 }
 
-// keys sorted ascending: offsets[o] = first position whose key is >= o, for o = 0..m
+// keys sorted ascending: offsets[o] = first position whose key is >= o, for o = 0..m, one binary search per o.
+// (Not one thread per key filling the gap up to the next key: with a bound, outputs [M, bound) are all empty
+// and one thread would write that whole gap.)
 __global__ void sa_offsets_kernel(const uint32_t *__restrict__ keys, int64_t n, uint32_t m, int32_t *__restrict__ offsets) {
-    const int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (p >= n) return;
-    const int64_t k = keys[p];
-    const int64_t prev = p == 0 ? -1 : (int64_t)keys[p - 1];
-    for (int64_t o = prev + 1; o <= k; ++o) offsets[o] = (int32_t)p;
-    if (p == n - 1)
-        for (int64_t o = k + 1; o <= (int64_t)m; ++o) offsets[o] = (int32_t)n;
+    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (o > (int64_t)m) return;
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if ((int64_t)__ldg(keys + mid) < o) lo = mid + 1;
+        else hi = mid;
+    }
+    offsets[o] = (int32_t)lo;
 }
 
 // W elements of T per thread: W * sizeof(T) == 16 (vector path) or W == 1
@@ -187,6 +192,86 @@ static int launch_gather(const SaOperands &ops, const int32_t *index, int64_t ro
     return 0;
 }
 
+// ------------------------------------------------------------------ padded operands (masked_sparse_add)
+// Operand t's valid rows are [0, valid_t), valid_t = *num_valid[t] clamped to [0, rows_t] (NULL: every row).
+// The visit order is the one sparse_add takes for the unpadded operands: the largest valid count first (ties:
+// the earliest operand), then the others in argument order.  The counts live on the device, so every block of
+// the pack kernel decides the order itself from the <= 64 counts (no extra launch, no read-back).
+struct SaPlan {
+    int count;
+    const int32_t *num_valid[SA_MAX];
+    int64_t start[SA_MAX + 1];                 // argument order
+};
+
+// row g of the argument-order concatenation -> position pos(g) of the packed array: the valid rows of the
+// operands in visit order (exactly the concatenation sparse_add ranks), then every padding row in argument
+// order with coordinates -1 (dropped by the union).  packed[pos] = coordinates, src[pos] = g.
+__global__ void __launch_bounds__(SA_THREADS)
+sa_pack_kernel(const __grid_constant__ SaPlan plan, const int32_t *__restrict__ indices, int ncols,
+               int32_t *__restrict__ packed, int32_t *__restrict__ src) {
+    __shared__ int64_t valid[SA_MAX], vstart[SA_MAX], pstart[SA_MAX];
+    const int t = threadIdx.x;
+    if (t < plan.count) {
+        const int64_t rows = plan.start[t + 1] - plan.start[t];
+        int64_t v = rows;
+        if (plan.num_valid[t] != nullptr) {
+            v = *plan.num_valid[t];
+            v = v < 0 ? 0 : (v > rows ? rows : v);
+        }
+        valid[t] = v;
+    }
+    __syncthreads();
+    if (t == 0) {
+        int largest = 0;
+        for (int i = 1; i < plan.count; ++i)
+            if (valid[i] > valid[largest]) largest = i;
+        int64_t v = valid[largest];
+        vstart[largest] = 0;
+        for (int i = 0; i < plan.count; ++i)
+            if (i != largest) { vstart[i] = v; v += valid[i]; }
+        for (int i = 0; i < plan.count; ++i) {                 // the tail starts at V = sum of the valid counts
+            pstart[i] = v;
+            v += plan.start[i + 1] - plan.start[i] - valid[i];
+        }
+    }
+    __syncthreads();
+    const int64_t g = blockIdx.x * (int64_t)blockDim.x + t;
+    if (g >= plan.start[plan.count]) return;
+    int lo = 0, hi = plan.count - 1;                           // the last operand with start <= g
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (plan.start[mid] <= g) lo = mid;
+        else hi = mid - 1;
+    }
+    const int64_t r = g - plan.start[lo];
+    const bool ok = r < valid[lo];
+    const int64_t pos = ok ? vstart[lo] + r : pstart[lo] + (r - valid[lo]);
+    for (int a = 0; a < ncols; ++a) packed[pos * ncols + a] = ok ? __ldg(indices + g * ncols + a) : -1;
+    src[pos] = (int32_t)g;
+}
+
+// back to argument order: order_arg[p] = src[order[p]] (the segments keep their ascending visit order),
+// dst_arg[src[p]] = dst[p]
+__global__ void sa_remap_kernel(const int32_t *__restrict__ src, const int32_t *__restrict__ order,
+                                const int32_t *__restrict__ dst, int64_t n, int32_t *__restrict__ order_arg,
+                                int32_t *__restrict__ dst_arg) {
+    const int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    order_arg[p] = __ldg(src + __ldg(order + p));
+    dst_arg[__ldg(src + p)] = __ldg(dst + p);
+}
+
+// heads[o] = the row that created output o (o < M), else -1; inverse[heads[o]] = o.  inverse is -1 beforehand.
+__global__ void sa_heads_kernel(const int32_t *__restrict__ order, const int32_t *__restrict__ offsets,
+                                const int32_t *__restrict__ num_out, int64_t bound, int32_t *__restrict__ heads,
+                                int32_t *__restrict__ inverse) {
+    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (o >= bound) return;
+    const int32_t h = o < (int64_t)*num_out ? __ldg(order + __ldg(offsets + o)) : -1;
+    heads[o] = h;
+    if (h >= 0) inverse[h] = (int32_t)o;
+}
+
 }  // namespace spx
 
 using namespace spx;
@@ -221,7 +306,7 @@ extern "C" int spx_sparse_add_group(const int32_t *dst, int64_t rows, int64_t M,
     if (int rc = radix_argsort_pair(keys, order, rows, nullptr, nullptr, 0, key_bits, sort_ws,
                                     radix_argsort_workspace_bytes(rows), nullptr, 0, stream))
         return rc;
-    sa_offsets_kernel<<<blk, SA_THREADS, 0, stream>>>(keys, rows, (uint32_t)M, offsets);
+    sa_offsets_kernel<<<(unsigned)div_up64(M + 1, SA_THREADS), SA_THREADS, 0, stream>>>(keys, rows, (uint32_t)M, offsets);
     SPX_CHECK_LAUNCH("sa_offsets_kernel");
     return 0;
 }
@@ -265,4 +350,96 @@ extern "C" int spx_sparse_add_gather(const int32_t *index, const void *src, int6
     if (vec) return launch_gather<uint4>(ops, index, total, row_bytes, src, stream);
     if (dtype_bytes(dtype) == 4) return launch_gather<uint32_t>(ops, index, total, row_bytes, src, stream);
     return launch_gather<uint16_t>(ops, index, total, row_bytes, src, stream);
+}
+
+// ------------------------------------------------------------------ padded operands (masked_sparse_add)
+namespace {
+struct PlanWs {
+    int32_t *packed, *src, *dst, *order;
+    void *union_ws, *group_ws;
+    size_t union_bytes, group_bytes, bytes;
+};
+
+void carve_plan_ws(const spx_conv_geometry *g, int64_t rows, int64_t bound, void *workspace, size_t bytes, PlanWs &w) {
+    WorkspaceCarver ws(workspace, bytes);
+    w.packed = ws.take<int32_t>((size_t)rows * (g->ndim + 1));
+    w.src = ws.take<int32_t>((size_t)rows);
+    w.dst = ws.take<int32_t>((size_t)rows);
+    w.order = ws.take<int32_t>((size_t)rows);
+    w.union_bytes = spx_sparse_add_union_workspace_size(g, rows, bound);
+    w.union_ws = ws.take<char>(w.union_bytes);
+    w.group_bytes = spx_sparse_add_group_workspace_size(rows);
+    w.group_ws = ws.take<char>(w.group_bytes);
+    w.bytes = ws.off;
+}
+}  // namespace
+
+extern "C" size_t spx_masked_sparse_add_workspace_size(const spx_conv_geometry *g, int64_t rows, int64_t bound) {
+    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM || rows < 0 || bound < 0 || bound > rows) return 0;
+    if (rows == 0) return 256;
+    if (spx_sparse_add_union_workspace_size(g, rows, bound) == 0) return 0;
+    PlanWs w;
+    carve_plan_ws(g, rows, bound, nullptr, SIZE_MAX, w);
+    return align_up(w.bytes, 256) + 256;
+}
+
+extern "C" int spx_masked_sparse_add_plan(const spx_conv_geometry *g, const spx_sparse_add_operands *operands,
+                                          const int32_t *const *num_valid, const int32_t *indices, int64_t bound,
+                                          int32_t *out_inds, int32_t *dst, int32_t *order, int32_t *offsets,
+                                          int32_t *num_out, int32_t *status, void *workspace, size_t workspace_bytes,
+                                          spx_stream_t stream_) {
+    SaOperands ops;
+    int64_t rows = 0;
+    if (int rc = make_operands(operands, false, rows, ops, "masked_sparse_add_plan")) return rc;
+    SPX_REQUIRE(g != nullptr && g->ndim >= 1 && g->ndim <= SPX_MAX_NDIM, "masked_sparse_add_plan: bad geometry");
+    SPX_REQUIRE(bound >= (rows > 0 ? 1 : 0) && bound <= rows && bound < (1ll << 30),
+                "masked_sparse_add_plan: bound must be in [1, rows] and below 2^30, got %lld for %lld rows",
+                (long long)bound, (long long)rows);
+    SPX_REQUIRE(offsets && num_out && status, "masked_sparse_add_plan: NULL pointer argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (rows == 0) {                       // nothing to visit: M = 0, offsets [1] = {0}
+        SPX_CHECK_CUDA(cudaMemsetAsync(num_out, 0, sizeof(int32_t), stream));
+        SPX_CHECK_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int32_t), stream));
+        return 0;
+    }
+    if (validate_sparse_add_union(g, rows, bound)) return 2;
+    SPX_REQUIRE(indices && out_inds && dst && order && workspace, "masked_sparse_add_plan: NULL pointer argument");
+    const size_t need = spx_masked_sparse_add_workspace_size(g, rows, bound);
+    SPX_REQUIRE(workspace_bytes >= need, "masked_sparse_add_plan: workspace too small: need %zu, have %zu", need,
+                workspace_bytes);
+    PlanWs w;
+    carve_plan_ws(g, rows, bound, workspace, workspace_bytes, w);
+    SaPlan plan;
+    memset(&plan, 0, sizeof(plan));
+    plan.count = ops.count;
+    for (int t = 0; t < ops.count; ++t) plan.num_valid[t] = num_valid ? num_valid[t] : nullptr;
+    memcpy(plan.start, ops.start, sizeof(plan.start));
+    const unsigned blk = (unsigned)div_up64(rows, SA_THREADS);
+    const int ncols = g->ndim + 1;
+    sa_pack_kernel<<<blk, SA_THREADS, 0, stream>>>(plan, indices, ncols, w.packed, w.src);
+    SPX_CHECK_LAUNCH("sa_pack_kernel");
+    if (int rc = spx_sparse_add_union(g, w.packed, rows, bound, out_inds, w.dst, num_out, status, w.union_ws,
+                                      w.union_bytes, stream_)) return rc;
+    if (int rc = spx_sparse_add_group(w.dst, rows, bound, w.order, offsets, w.group_ws, w.group_bytes, stream_)) return rc;
+    sa_remap_kernel<<<blk, SA_THREADS, 0, stream>>>(w.src, w.order, w.dst, rows, order, dst);
+    SPX_CHECK_LAUNCH("sa_remap_kernel");
+    return 0;
+}
+
+extern "C" int spx_masked_sparse_add_heads(const int32_t *order, const int32_t *offsets, const int32_t *num_out,
+                                           int64_t bound, int64_t rows, int32_t *heads, int32_t *inverse,
+                                           spx_stream_t stream_) {
+    SPX_REQUIRE(rows >= 0 && rows < 2147483647ll, "masked_sparse_add_heads: bad row count %lld", (long long)rows);
+    SPX_REQUIRE(bound >= 0 && bound <= rows, "masked_sparse_add_heads: bound %lld not in [0, %lld]", (long long)bound,
+                (long long)rows);
+    if (rows == 0) return 0;
+    SPX_REQUIRE(order && offsets && num_out && inverse && (heads || bound == 0),
+                "masked_sparse_add_heads: NULL pointer argument");
+    cudaStream_t stream = (cudaStream_t)stream_;
+    SPX_CHECK_CUDA(cudaMemsetAsync(inverse, 0xff, (size_t)rows * sizeof(int32_t), stream));
+    if (bound == 0) return 0;
+    sa_heads_kernel<<<(unsigned)div_up64(bound, SA_THREADS), SA_THREADS, 0, stream>>>(order, offsets, num_out, bound,
+                                                                                       heads, inverse);
+    SPX_CHECK_LAUNCH("sa_heads_kernel");
+    return 0;
 }

@@ -14,7 +14,9 @@ from .modules import (MaskedBatchNorm1d, RemoveGrid, SparseBatchNorm, SparseIden
 from .pool import (MaskedGlobalAvgPool, MaskedGlobalMaxPool, SparseAvgPool1d,  # noqa: F401
                    SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool, SparseGlobalMaxPool, SparseMaxPool1d,
                    SparseMaxPool2d, SparseMaxPool3d, SparseMaxPool4d)
-from .tables import AddTable, ConcatTable, JoinTable  # noqa: F401
+from .tables import (AddTable, ConcatTable, JoinTable, MaskedAddTable, MaskedAddTableMisaligned,  # noqa: F401
+                     MaskedJoinTable)
+from .spatial import MaskedRemoveDuplicate  # noqa: F401
 from .utils_fuse import (fuse_act, fuse_bn, fuse_bn_act_sequential, fuse_bn_weights)  # noqa: F401
 from . import quantized  # noqa: F401
 from .graph import GraphedStep, graph_capture  # noqa: F401

@@ -1,5 +1,6 @@
 """Output bounds of the strided layers: run a net with strided convs / pools at static shapes, without a host
-synchronisation, so that a whole step replays as one CUDA graph.
+synchronisation, so that a whole step replays as one CUDA graph.  ``MaskedAddTableMisaligned`` and
+``MaskedRemoveDuplicate`` have bounds and status words too and are covered alike.
 
     bounds = spconv.set_output_bounds(net, example)       # one eager forward, sets num_out_act_bound per layer
     step = spconv.graph_capture(fn, example.pad_to(N).features, ...)
@@ -16,6 +17,11 @@ from torch import nn
 from .conv import SparseConvolution
 from .core import SparseConvTensor
 from .pool import _SparsePool
+from .spatial import MaskedRemoveDuplicate
+from .tables import MaskedAddTableMisaligned
+
+# modules whose output count depends on the data: the bound is their padded row count, num_valid the true count
+_MASKED_BOUNDED = (MaskedAddTableMisaligned, MaskedRemoveDuplicate)
 
 
 def _strided_modules(net: nn.Module):
@@ -24,6 +30,16 @@ def _strided_modules(net: nn.Module):
             yield name, mod
         elif isinstance(mod, _SparsePool) and not mod.subm:
             yield name, mod
+        elif isinstance(mod, _MASKED_BOUNDED):
+            yield name, mod
+
+
+def _out_count(mod: nn.Module, out: SparseConvTensor) -> int:
+    """the output count of one eager forward: the row count of an unbounded strided layer, the true count (one
+    read-back) of a masked module, whose unbounded output is padded to its operands' total row count"""
+    if isinstance(mod, _MASKED_BOUNDED):
+        return int(out.num_valid)
+    return out.features.shape[0]
 
 
 def set_output_bounds(net: nn.Module, example_input: SparseConvTensor, margin: float = 1.25) -> Dict[str, int]:
@@ -37,7 +53,7 @@ def set_output_bounds(net: nn.Module, example_input: SparseConvTensor, margin: f
         saved[name] = mod.num_out_act_bound
         mod.num_out_act_bound = None
         hooks.append(mod.register_forward_hook(
-            lambda m, inp, out, name=name: counts.__setitem__(name, max(counts.get(name, 0), out.features.shape[0]))))
+            lambda m, inp, out, name=name: counts.__setitem__(name, max(counts.get(name, 0), _out_count(m, out)))))
     try:
         net(example_input)
     except Exception:

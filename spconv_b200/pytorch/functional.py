@@ -349,6 +349,89 @@ def remove_duplicate(x: SparseConvTensor) -> SparseConvTensor:
     return SparseConvTensor(feats, out_inds, x.spatial_shape, x.batch_size, x.grid)
 
 
+# ---------------------------------------------------------------------------- padding-aware sparse add
+def _masked_bound(rows: int, num_out_act_bound: Optional[int]) -> int:
+    if num_out_act_bound is None:
+        return rows
+    if int(num_out_act_bound) < 1:
+        raise ValueError(f"num_out_act_bound must be positive, got {num_out_act_bound}")
+    return min(int(num_out_act_bound), rows)            # the union never has more rows than its operands
+
+
+def _merged_status(tens, name: Optional[str], status: Optional[torch.Tensor]):
+    words = {}
+    for ten in tens:
+        words.update(ten.bound_status or {})
+    if name is not None:
+        words[name] = status
+    return words or None
+
+
+def _masked_sparse_add(tens, num_out_act_bound=None, status=None, name=None) -> SparseConvTensor:
+    assert len(tens) >= 1, "masked_sparse_add needs at least one operand"
+    first = tens[0]
+    bound = _masked_bound(sum(t.features.shape[0] for t in tens), num_out_act_bound)
+    for ten in tens:
+        assert ten.spatial_shape == first.spatial_shape
+        assert ten.batch_size == first.batch_size
+        assert ten.features.shape[1] == first.features.shape[1]
+        ops._sparse_add_dtype(ten.features.dtype)
+        ops._require_cuda(ten.features, "features")
+    dtype = functools.reduce(torch.promote_types, [t.features.dtype for t in tens])
+    out_inds, dst, order, offsets, num_out, status = ops.masked_sparse_add_plan(
+        [t.indices for t in tens], [t.num_valid for t in tens], first.batch_size, first.spatial_shape, bound, status)
+    feats = [t.features if t.features.dtype == dtype else t.features.to(dtype) for t in tens]
+    res = SparseConvTensor(SparseAddFunction.apply(dst, order, offsets, bound, *feats), out_inds, first.spatial_shape,
+                           first.batch_size, benchmark=first.benchmark)
+    res.num_valid = num_out
+    res.bound_status = _merged_status(tens, name, status)
+    res.benchmark_record = first.benchmark_record
+    res._timer = first._timer
+    res.thrust_allocator = first.thrust_allocator
+    return res
+
+
+def masked_sparse_add(*tens: SparseConvTensor, num_out_act_bound: Optional[int] = None) -> SparseConvTensor:
+    """:func:`sparse_add` of padded and / or unpadded operands, with no host synchronisation (CUDA-graph capturable).
+
+    Operand ``t``'s valid rows are ``[0, t.num_valid)`` (every row when ``num_valid`` is None); rows beyond are never
+    read, neither features nor indices.  The result has ``bound`` rows and ``num_valid`` = M (device int32 ``[1]``):
+    rows ``[0, M)`` of its indices and features, M, and every operand's gradient rows ``[0, valid_t)`` equal
+    :func:`sparse_add` of the valid rows bit for bit, whatever the padding.  The visit order is decided on the device
+    from the valid counts (the largest valid count first, ties: the earliest operand, then the others in argument
+    order), as :func:`sparse_add` decides it from the row counts.  Rows ``[M, bound)`` have indices -1 and features 0;
+    padding and dropped rows get a zero gradient.
+
+    ``bound`` defaults to the operands' total row count, which the union can never exceed; a larger
+    ``num_out_act_bound`` is clamped to it.  A smaller one truncates deterministically: the outputs ranked >= bound
+    are dropped, their rows get a zero gradient, and bit 0 of the result's ``bound_status`` word is set
+    (:func:`spconv.check_bounds`).  An empty union gives M = 0.  ``indice_dict`` is not kept: deciding whether the
+    result's rows are an operand's rows would need a host read-back.  float32, float16 and bfloat16, CUDA only."""
+    return _masked_sparse_add(tens, num_out_act_bound, name="masked_sparse_add")
+
+
+def masked_remove_duplicate(x: SparseConvTensor, num_out_act_bound: Optional[int] = None) -> SparseConvTensor:
+    """:func:`remove_duplicate` of the valid rows ``[0, x.num_valid)``, with no host synchronisation.  The result has
+    ``bound`` rows (default and upper limit: ``x``'s row count) and ``num_valid`` = M; rows ``[0, M)`` equal
+    :func:`remove_duplicate` of the valid rows bit for bit, rows ``[M, bound)`` have indices -1 and features 0, and
+    the gradient goes to the kept rows only.  Truncation and ``bound_status`` as :func:`masked_sparse_add`."""
+    return _masked_remove_duplicate(x, num_out_act_bound, name="masked_remove_duplicate")
+
+
+def _masked_remove_duplicate(x: SparseConvTensor, num_out_act_bound=None, status=None, name=None) -> SparseConvTensor:
+    bound = _masked_bound(x.features.shape[0], num_out_act_bound)
+    ops._sparse_add_dtype(x.features.dtype)
+    ops._require_cuda(x.features, "features")
+    out_inds, dst, order, offsets, num_out, status = ops.masked_sparse_add_plan(
+        [x.indices], [x.num_valid], x.batch_size, x.spatial_shape, bound, status)
+    heads, inverse = ops.masked_sparse_add_heads(order, offsets, num_out)
+    res = SparseConvTensor(_RowGather.apply(x.features, heads, inverse), out_inds, x.spatial_shape, x.batch_size,
+                           x.grid)
+    res.num_valid = num_out
+    res.bound_status = _merged_status([x], name, status)
+    return res
+
+
 # ---------------------------------------------------------------------------- padding-aware BatchNorm
 class MaskedBatchNormFunction(Function):
     """``x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps`` -> training-mode

@@ -11,7 +11,10 @@ an output bound (``spconv.set_output_bounds``) and pad the inputs to one size
 (``SparseConvTensor.pad_to``): then the rulebooks keep the count on the device and a whole encoder
 step, forward and backward, captures; ``spconv.check_bounds`` tells when a bound was exceeded.  Of the
 modules, ``SparseGlobalMaxPool`` / ``SparseGlobalAvgPool`` read the per-sample counts back to the host:
-``MaskedGlobalMaxPool`` / ``MaskedGlobalAvgPool`` reduce on the device and capture.
+``MaskedGlobalMaxPool`` / ``MaskedGlobalAvgPool`` reduce on the device and capture.  Likewise
+``AddTableMisaligned`` / ``functional.sparse_add`` read the size of the union back: ``MaskedAddTableMisaligned``
+(``functional.masked_sparse_add``), ``MaskedRemoveDuplicate``, ``MaskedAddTable`` and ``MaskedJoinTable`` take
+padded tensors and capture.
 """
 from __future__ import annotations
 

@@ -1140,6 +1140,58 @@ def sparse_add_gather(index: torch.Tensor, src: torch.Tensor, rows: Sequence[int
     return outs
 
 
+def masked_sparse_add_plan(indices: Sequence[torch.Tensor], num_valid: Sequence[Optional[torch.Tensor]],
+                           batch_size: int, spatial_shape: List[int], bound: int,
+                           status: Optional[torch.Tensor] = None):
+    """Union and grouping of padded operands in ARGUMENT order (``spx_masked_sparse_add_plan``), no host read-back.
+    Operand ``t``'s valid rows are ``[0, num_valid[t])`` (None: every row); the rest are never read.  Returns
+    ``(out_inds [bound, ndim+1], dst [sum N], order [sum N], offsets [bound+1], num_out [1], status [1])``: rows
+    ``[0, num_out)`` of ``out_inds`` equal :func:`sparse_add_union` of the valid rows in sparse_add's visit order,
+    ``dst`` / ``order`` index the argument-order concatenation (-1 in ``dst`` for padding, out-of-range and dropped
+    rows), and ``status`` (ORed into when given) gets bit 0 when more than ``bound`` outputs existed and bit 1 on a
+    probe-chain overflow."""
+    for ind in indices:
+        _require_cuda(ind, "indices")
+    dev = indices[0].device
+    ndim = len(spatial_shape)
+    cat = torch.cat([i.to(torch.int32).reshape(-1, ndim + 1) for i in indices], 0).contiguous()
+    rows = [int(i.shape[0]) for i in indices]
+    n = cat.shape[0]
+    for nv in num_valid:
+        if nv is not None and (nv.dtype != torch.int32 or nv.device != dev or nv.numel() < 1):
+            raise RuntimeError("masked_sparse_add: num_valid must be a device int32 [1] on the indices' device")
+    ones, zeros = [1] * ndim, [0] * ndim
+    geo = _geometry(cat, batch_size, spatial_shape, spatial_shape, ones, ones, zeros, ones, False)
+    out_inds = torch.empty((int(bound), ndim + 1), dtype=torch.int32, device=dev)
+    dst = torch.empty((n,), dtype=torch.int32, device=dev)
+    order = torch.empty((n,), dtype=torch.int32, device=dev)
+    offsets = torch.empty((int(bound) + 1,), dtype=torch.int32, device=dev)
+    num_out = torch.empty((1,), dtype=torch.int32, device=dev)
+    if status is None:
+        status = torch.zeros((1,), dtype=torch.int32, device=dev)
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_sparse_add_workspace_size(ctypes.byref(geo), n, int(bound)), dev)
+    opnds = _sparse_add_operands(rows)
+    nv_ptrs = (ctypes.c_void_p * len(rows))(*[None if nv is None else nv.data_ptr() for nv in num_valid])
+    _cabi.check(lib.spx_masked_sparse_add_plan(
+        ctypes.byref(geo), ctypes.byref(opnds), nv_ptrs, _ptr(cat), int(bound), _ptr(out_inds), _ptr(dst), _ptr(order),
+        offsets.data_ptr(), num_out.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+        "masked_sparse_add_plan")
+    return out_inds, dst, order, offsets, num_out, status
+
+
+def masked_sparse_add_heads(order: torch.Tensor, offsets: torch.Tensor, num_out: torch.Tensor):
+    """``(heads [bound], inverse [N])`` of a one-operand plan: ``heads[o]`` is the row that created output ``o``
+    (-1 for ``o >= num_out``), ``inverse[heads[o]] = o`` and -1 on every other row."""
+    n = order.shape[0]
+    bound = offsets.shape[0] - 1
+    heads = torch.empty((bound,), dtype=torch.int32, device=order.device)
+    inverse = torch.empty((n,), dtype=torch.int32, device=order.device)
+    _cabi.check(_lib().spx_masked_sparse_add_heads(_ptr(order), offsets.data_ptr(), num_out.data_ptr(), bound, n,
+                                                   _ptr(heads), _ptr(inverse), _stream()), "masked_sparse_add_heads")
+    return heads, inverse
+
+
 # ---------------------------------------------------------------------------- misc
 def bias_add_act_inplace(x: torch.Tensor, bias: Optional[torch.Tensor], act_type=Activation.None_,
                          act_alpha: float = 0.0, act_beta: float = 0.0) -> torch.Tensor:

@@ -1,6 +1,10 @@
 """Coordinate clean-up (``spconv/pytorch/spatial.py``)."""
 from __future__ import annotations
 
+from typing import Optional
+
+import torch
+
 from . import functional as F
 from .core import SparseConvTensor
 from .modules import SparseModule
@@ -18,3 +22,24 @@ class RemoveDuplicate(SparseModule):
 
     def forward(self, x: SparseConvTensor):
         return F.remove_duplicate(x)
+
+
+class MaskedRemoveDuplicate(SparseModule):
+    """``RemoveDuplicate`` of the valid rows of a padded or unpadded tensor, with no host synchronisation
+    (:func:`functional.masked_remove_duplicate`): the result has ``num_out_act_bound`` rows (default: the input's row
+    count) and ``num_valid`` = the number of distinct in-range coordinates.  With a bound, a status word is kept for
+    ``spconv.check_bounds`` and ``spconv.set_output_bounds`` as the strided conv and pool modules keep theirs."""
+
+    def __init__(self, num_out_act_bound: Optional[int] = None, name=None):
+        super().__init__(name=name)
+        self.num_out_act_bound = num_out_act_bound
+        self._bound_status: Optional[torch.Tensor] = None
+
+    def forward(self, x: SparseConvTensor):
+        if self.num_out_act_bound is None:
+            return F._masked_remove_duplicate(x)
+        dev = x.indices.device
+        if self._bound_status is None or self._bound_status.device != dev:
+            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=dev)
+        return F._masked_remove_duplicate(x, self.num_out_act_bound, self._bound_status,
+                                          self._sparse_unique_name or self.name or type(self).__name__)
