@@ -185,9 +185,11 @@ def _restore_forced_family():
         _configure(ENV_FAMILY)
 
 
-def _launch(what, inst, launch):
-    """Run `launch` on the family `inst` says (None: FMA kernel) and check that it ran there."""
-    if SIMT:
+def _launch(what, inst, launch, fma=False):
+    """Run `launch` on the family `inst` says (None: FMA kernel) and check that it ran there.
+    fma=True pins the FMA kernels whatever the shape."""
+    fma = fma or SIMT
+    if fma:
         _configure(1)
     elif inst is not None:
         _configure(2)
@@ -198,7 +200,7 @@ def _launch(what, inst, launch):
         _configure(0)
     out = launch()
     fam = _lib().spx_last_kernel_family()
-    want = 1 if SIMT or inst is None else 2
+    want = 1 if fma or inst is None else 2
     assert fam == want, f"{what}: kernel family {fam}, expected {want} ({inst and _instance_name(inst)})"
     return out
 
@@ -260,7 +262,7 @@ class Conv:
         d.f32_mode = _cabi.SPX_F32_TF32
         return d
 
-    def fwd_call(self, x, w, inst, bias=None, act=0, alpha=0.0):
+    def fwd_call(self, x, w, inst, bias=None, act=0, alpha=0.0, fma=False):
         from spconv_b200 import _cabi
         from spconv_b200.pytorch import ops
         K, C = w.shape[0], w.shape[-1]
@@ -272,9 +274,9 @@ class Conv:
                                                      None if bias is None else bias.data_ptr(), act, alpha,
                                                      ops._stream()), "implicit_gemm_fwd")
             return out
-        return _launch("fwd", inst, launch)
+        return _launch("fwd", inst, launch, fma)
 
-    def dgrad_call(self, dout, w, inst):
+    def dgrad_call(self, dout, w, inst, fma=False):
         from spconv_b200 import _cabi
         from spconv_b200.pytorch import ops
         K, C = w.shape[0], w.shape[-1]
@@ -286,9 +288,9 @@ class Conv:
             _cabi.check(_lib().spx_implicit_gemm_dgrad(ctypes.byref(d), dout.data_ptr(), w.data_ptr(), din.data_ptr(),
                                                        ops._stream()), "implicit_gemm_dgrad")
             return din
-        return _launch("dgrad", inst, launch)
+        return _launch("dgrad", inst, launch, fma)
 
-    def wgrad_call(self, x, dout, w_shape, inst):
+    def wgrad_call(self, x, dout, w_shape, inst, fma=False):
         from spconv_b200 import _cabi
         from spconv_b200.pytorch import ops
         K, C = w_shape[0], w_shape[-1]
@@ -302,7 +304,7 @@ class Conv:
             _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d), x.data_ptr(), dout.data_ptr(), dw.data_ptr(),
                                                     ws.data_ptr(), ws.numel() * 4, ops._stream()), "implicit_gemm_wgrad")
             return dw
-        return _launch("wgrad", inst, launch)
+        return _launch("wgrad", inst, launch, fma)
 
 
 def _reference(x, w, dout, ref_pair, dev):
@@ -358,8 +360,9 @@ def _check(name, got, ref, ref_abs, terms, dt, zero=None, extra=0.0):
         assert nz == 0, f"{name}: {int(nz)} elements without any pair are not exactly 0"
 
 
-def _run_case(oracle, dev, conv, dt, C, K, seed, repeat=1, round_tf32=True):
-    """fwd + dgrad + wgrad of one conv against the float64 reference; returns the outputs"""
+def _run_case(oracle, dev, conv, dt, C, K, seed, repeat=1, round_tf32=True, fma=False):
+    """fwd + dgrad + wgrad of one conv against the float64 reference; returns the outputs.
+    fma=True runs every call on the FMA kernels."""
     rng = np.random.default_rng(seed)
     x = _exact(rng, (conv.n_in, C), dt, round_tf32=round_tf32)
     w = _exact(rng, (K, conv.kv, C), dt, round_tf32=round_tf32)
@@ -371,9 +374,9 @@ def _run_case(oracle, dev, conv, dt, C, K, seed, repeat=1, round_tf32=True):
     rel = 0.0 if round_tf32 else 2 * 2.0 ** -10             # operands rounded to tf32 by the tensor cores
     runs = []
     for _ in range(repeat):
-        out = conv.fwd_call(xd, wd, inst["fwd"])
-        din = conv.dgrad_call(dd, wd, inst["dgrad"])
-        dw = conv.wgrad_call(xd, dd, wd.shape, inst["wgrad"])
+        out = conv.fwd_call(xd, wd, inst["fwd"], fma=fma)
+        din = conv.dgrad_call(dd, wd, inst["dgrad"], fma=fma)
+        dw = conv.wgrad_call(xd, dd, wd.shape, inst["wgrad"], fma=fma)
         torch.cuda.synchronize()
         runs.append((out, din, dw))
     out, din, dw = runs[0]
