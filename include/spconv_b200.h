@@ -24,6 +24,8 @@
  *        <- InferenceOps.bias_add_act_inplace        spconv/csrc/sparse/inference.py:166-252
  *   spx_point2voxel_stage1 / _stage2
  *        <- SpconvOps.point2voxel_cuda               spconv/csrc/sparse/all.py:1349-1490
+ *   spx_point2voxel_bounded
+ *        <- no counterpart: MaskedPointToVoxel (a batch of clouds, voxel count kept on the device)
  *   spx_indice_pool_fwd / spx_indice_pool_bwd / spx_global_pool_rearrange
  *        <- SpconvOps.maxpool_forward / maxpool_backward / maxpool_implicit_gemm_forward /
  *           maxpool_implicit_gemm_backward / avgpool_implicit_gemm_forward / _backward /
@@ -368,6 +370,33 @@ int spx_point2voxel_stage2(const float *points, int64_t N, int num_features, int
                            int max_points_per_voxel, int empty_mean, float *voxels, int32_t *indices,
                            int32_t *num_per_voxel, int64_t *pc_voxel_id, void *workspace,
                            size_t workspace_bytes, spx_stream_t stream);
+
+/*
+ * A batch of clouds in one call, with the voxel count kept on the device (MaskedPointToVoxel): nothing is read
+ * back, so the call captures into a CUDA graph.  Geometry, points and the per-sample semantics as above.
+ *   point_offsets [batch_size + 1] device int32 (NULL: one sample of all N points, batch_size must be 1).  The
+ *   offsets are normalised on the device: each is clamped to [0, N], then the prefix maximum is taken; sample b
+ *   owns the points [off[b], off[b+1]), points outside every sample are padding and are never read.
+ *   Per sample, the voxels are those of spx_point2voxel_stage1/2 with max_voxels run on the sample's points
+ *   alone, bit for bit (order, cap, kept points, empty_mean fill).  Rows hold sample 0's kept voxels, then
+ *   sample 1's, .. packed; M = *num_valid = min(sum of the kept counts, bound).  Every output element is written:
+ *   voxels [bound, max_points, num_features] (unused slots: the voxel mean when empty_mean != 0, else 0),
+ *   indices [bound, ndim + 1] (batch index, then the cell in the internal axis order), num_per_voxel [bound];
+ *   rows [M, bound) hold indices -1, voxels 0, num_per_voxel 0.  pc_voxel_id [N] int64: the row of the point's
+ *   voxel, -1 for padding points, points out of range and points of dropped voxels.  *status |= 1 when more
+ *   than `bound` voxels were kept (the rows ranked >= bound are dropped); status is only ever ORed into.
+ * Limits: batch_size in [1, SPX_P2V_MAX_BATCH], N and bound below 2^31 - 1, bound >= 1, batch_size x grid
+ * volume below 2^62 (64-bit hash keys from 2^31 - 1 on).  workspace: spx_point2voxel_bounded_workspace_size
+ * bytes (0 = invalid sizes).
+ */
+#define SPX_P2V_MAX_BATCH 65536
+size_t spx_point2voxel_bounded_workspace_size(int64_t num_points, int batch_size, int64_t bound);
+int spx_point2voxel_bounded(const float *points, int64_t N, int num_features, int ndim, int zyx,
+                            const float *vsize_host, const int *grid_size_host, const float *coors_range_host,
+                            const int32_t *point_offsets, int batch_size, int64_t max_voxels, int64_t bound,
+                            int max_points_per_voxel, int empty_mean, float *voxels, int32_t *indices,
+                            int32_t *num_per_voxel, int64_t *pc_voxel_id, int32_t *num_valid, int32_t *status,
+                            void *workspace, size_t workspace_bytes, spx_stream_t stream);
 
 /* ------------------------------------------------------------------ pooling on the rulebook */
 

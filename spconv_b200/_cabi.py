@@ -42,6 +42,7 @@ class GemmDesc(Structure):
 
 
 SPX_MAX_PEERS = 16
+SPX_P2V_MAX_BATCH = 65536
 
 
 class PeerGroup(Structure):
@@ -136,6 +137,11 @@ SIGNATURES = {
     "spx_point2voxel_stage2": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, POINTER(c_float), POINTER(c_int),
                                        POINTER(c_float), c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_point2voxel_bounded_workspace_size": (c_size_t, [c_int64, c_int, c_int64]),
+    "spx_point2voxel_bounded": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, POINTER(c_float), POINTER(c_int),
+                                        POINTER(c_float), c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                        c_void_p]),
     "spx_indice_pool_fwd": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int,
                                     c_void_p, c_void_p]),
     "spx_indice_pool_bwd": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,

@@ -19,6 +19,7 @@ from .core import SparseConvTensor
 from .pool import _SparsePool
 from .spatial import MaskedRemoveDuplicate
 from .tables import MaskedAddTableMisaligned
+from .utils import MaskedPointToVoxel
 
 # modules whose output count depends on the data: the bound is their padded row count, num_valid the true count
 _MASKED_BOUNDED = (MaskedAddTableMisaligned, MaskedRemoveDuplicate)
@@ -72,13 +73,17 @@ def set_output_bounds(net: nn.Module, example_input: SparseConvTensor, margin: f
     return bounds
 
 
-def check_bounds(tensor_or_net: Union[SparseConvTensor, nn.Module]) -> None:
+def check_bounds(tensor_or_net: Union[SparseConvTensor, nn.Module, MaskedPointToVoxel]) -> None:
     """Read the status words of the bounded layers (of a net: every bounded module; of a tensor: the layers
-    it went through) and raise ``RuntimeError`` naming the first layer whose bound was exceeded.  This is
-    the one call of the bounded mode that synchronises; the words of a net are cleared by the read."""
+    it went through; of a ``MaskedPointToVoxel``: its own, whose bound is ``max_num_voxels_total``) and raise
+    ``RuntimeError`` naming the first layer whose bound was exceeded.  This is the one call of the bounded mode
+    that synchronises; the words of a net or a voxel generator are cleared by the read."""
     if isinstance(tensor_or_net, SparseConvTensor):
         words = dict(tensor_or_net.bound_status or {})
         clear = False
+    elif isinstance(tensor_or_net, MaskedPointToVoxel):
+        words = {"MaskedPointToVoxel (bound: max_num_voxels_total)": tensor_or_net._bound_status}
+        clear = True
     else:
         words = {name: mod._bound_status for name, mod in _strided_modules(tensor_or_net)
                  if mod._bound_status is not None}

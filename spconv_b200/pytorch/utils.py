@@ -11,7 +11,7 @@ point with a NaN or infinite coordinate gets ``pc_voxel_id`` -1 and makes no vox
 from __future__ import annotations
 
 import ctypes
-from typing import List, Union
+from typing import List, Optional, Union
 
 import numpy as np
 import torch
@@ -99,14 +99,119 @@ class PointToVoxel(object):
                     self.num_per_voxel[:num_voxels].clone(), pc_voxel_id)
 
 
+class MaskedPointToVoxel(object):
+    """A batch of clouds -> voxels in one call, at static shapes and with no host read-back, so a step from raw
+    points to the loss captures as one CUDA graph (``spconv.graph_capture``).
+
+    ``voxels, indices, num_per_voxel, pc_voxel_id, num_valid = gen(points, point_offsets=None, empty_mean=False)``
+
+    * ``points [P, F]`` fp32 on the device; ``point_offsets`` device int32 ``[batch_size + 1]``: sample b owns the
+      rows ``[off[b], off[b+1])``.  The offsets are not checked on the host (that would be a read-back); each is
+      clamped to ``[0, P]`` and then the prefix maximum is taken, so samples are disjoint and contiguous and a
+      decreasing offset gives an empty sample.  Rows outside every sample (e.g. at or beyond ``off[B]``) are
+      padding and are never read.  ``None``: one sample made of all P rows.
+    * Per sample, the voxels are those of ``PointToVoxel(..., max_num_voxels, ...)`` run on that sample's rows
+      alone, bit for bit: first-touch order, the per-sample cap, the first ``max_num_points_per_voxel`` points
+      of a voxel, the ``empty_mean`` fill, no voxel for NaN / infinite / out-of-range points.
+    * Outputs (``bound = max_num_voxels_total``, default ``batch_size * max_num_voxels``, which never truncates):
+      ``voxels [bound, max_points, F]``, ``indices [bound, 1 + ndim]`` int32 (batch index first, then the cell in
+      zyx order: the ``SparseConvTensor`` layout), ``num_per_voxel [bound]`` int32, ``pc_voxel_id [P]`` int64 (the
+      output row of the point's voxel, -1 for padding points, points without a voxel and points of dropped
+      voxels) and ``num_valid [1]`` int32 on the device.  Rows are sample 0's kept voxels, then sample 1's, ..,
+      packed; ``M = num_valid = min(sum_b min(count_b, max_num_voxels), bound)``.  Rows ``[M, bound)`` are padding:
+      indices -1, voxels 0, num_per_voxel 0.  Every element is written on every call.
+    * ``voxels`` / ``indices`` / ``num_per_voxel`` / ``num_valid`` are buffers allocated once by the constructor
+      and overwritten by every call (clone them to keep a result); ``pc_voxel_id`` is new per call.
+    * With ``max_num_voxels_total < batch_size * max_num_voxels``, voxels ranked at or beyond the bound are dropped
+      (deterministically: the first ``bound`` rows of the untruncated result are kept) and bit 0 of the status
+      word ``_bound_status`` is set; ``spconv.check_bounds(gen)`` reads it, clears it, and raises.
+
+    The padded ``SparseConvTensor`` of the conv path is the rows with ``num_valid`` attached, e.g. with SECOND's
+    mean features (MeanVFE; plain torch, padding rows give 0)::
+
+        voxels, indices, num_per_voxel, pc_voxel_id, num_valid = gen(points, offsets)
+        feats = voxels.sum(1) / num_per_voxel.clamp(min=1)[:, None].to(voxels.dtype)
+        x = spconv.SparseConvTensor(feats, indices, gen.grid_size, gen.batch_size)
+        x.num_valid = num_valid
+
+    At most ``SPX_P2V_MAX_BATCH`` (65536) samples; P and the bound below 2^31 - 1.  CUDA only.
+    """
+
+    def __init__(self, vsize_xyz: List[float], coors_range_xyz: List[float], num_point_features: int,
+                 max_num_voxels: int, max_num_points_per_voxel: int, batch_size: int,
+                 max_num_voxels_total: Optional[int] = None, device: torch.device = torch.device("cuda:0")):
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("spconv_b200.MaskedPointToVoxel: CUDA only")
+        if max_num_voxels <= 0 or max_num_points_per_voxel <= 0 or batch_size <= 0:
+            raise ValueError("MaskedPointToVoxel: max_num_voxels, max_num_points_per_voxel and batch_size must be "
+                             "positive")
+        if batch_size > _cabi.SPX_P2V_MAX_BATCH:
+            raise ValueError(f"MaskedPointToVoxel: batch_size {batch_size} above {_cabi.SPX_P2V_MAX_BATCH}")
+        bound = batch_size * max_num_voxels if max_num_voxels_total is None else int(max_num_voxels_total)
+        if bound <= 0 or bound >= 2 ** 31 - 1:
+            raise ValueError(f"MaskedPointToVoxel: max_num_voxels_total {bound} not in [1, 2^31 - 2]")
+        self.ndim = len(vsize_xyz)
+        self.device = device
+        self.vsize, self.grid_size, self.grid_stride, self.coors_range = calc_point2voxel_meta_data(
+            vsize_xyz, coors_range_xyz)
+        self.num_point_features = num_point_features
+        self.max_num_voxels = max_num_voxels
+        self.max_num_points_per_voxel = max_num_points_per_voxel
+        self.batch_size = batch_size
+        self.max_num_voxels_total = bound
+        self.voxels = torch.zeros([bound, max_num_points_per_voxel, num_point_features], dtype=torch.float32,
+                                  device=device)
+        self.indices = torch.full([bound, 1 + self.ndim], -1, dtype=torch.int32, device=device)
+        self.num_per_voxel = torch.zeros([bound], dtype=torch.int32, device=device)
+        self.num_valid = torch.zeros([1], dtype=torch.int32, device=device)
+        self._bound_status = torch.zeros([1], dtype=torch.int32, device=device)
+        self._c_vsize = (ctypes.c_float * self.ndim)(*self.vsize)
+        self._c_grid = (ctypes.c_int * self.ndim)(*self.grid_size)
+        self._c_range = (ctypes.c_float * (2 * self.ndim))(*self.coors_range)
+
+    def __call__(self, points: torch.Tensor, point_offsets: Optional[torch.Tensor] = None, empty_mean: bool = False):
+        if not points.is_cuda or (point_offsets is not None and not point_offsets.is_cuda):
+            raise RuntimeError("MaskedPointToVoxel: points and point_offsets must be CUDA tensors")
+        if points.dim() != 2 or points.shape[1] != self.num_point_features:
+            raise ValueError(f"MaskedPointToVoxel: points must be [P, {self.num_point_features}], got "
+                             f"{tuple(points.shape)}")
+        batch = 1
+        if point_offsets is not None:
+            if point_offsets.dtype != torch.int32 or point_offsets.shape != (self.batch_size + 1,):
+                raise ValueError(f"MaskedPointToVoxel: point_offsets must be int32 [{self.batch_size + 1}], got "
+                                 f"{point_offsets.dtype} {tuple(point_offsets.shape)}")
+            point_offsets = point_offsets.contiguous()
+            batch = self.batch_size
+        lib = _cabi.load()
+        pc = points.contiguous().float()
+        n = pc.shape[0]
+        bound = self.max_num_voxels_total
+        stream = torch.cuda.current_stream(pc.device).cuda_stream
+        with torch.no_grad():
+            pc_voxel_id = torch.empty([n], dtype=torch.int64, device=pc.device)
+            ws = torch.empty(lib.spx_point2voxel_bounded_workspace_size(n, batch, bound), dtype=torch.uint8,
+                             device=pc.device)
+            _cabi.check(lib.spx_point2voxel_bounded(
+                pc.data_ptr() if n else None, n, self.num_point_features, self.ndim, 1, self._c_vsize, self._c_grid,
+                self._c_range, point_offsets.data_ptr() if point_offsets is not None else None, batch,
+                self.max_num_voxels, bound, self.max_num_points_per_voxel, int(bool(empty_mean)),
+                self.voxels.data_ptr(), self.indices.data_ptr(), self.num_per_voxel.data_ptr(),
+                pc_voxel_id.data_ptr() if n else None, self.num_valid.data_ptr(), self._bound_status.data_ptr(),
+                ws.data_ptr(), ws.numel(), stream), "point2voxel_bounded")
+        return self.voxels, self.indices, self.num_per_voxel, pc_voxel_id, self.num_valid
+
+
 def gather_features_by_pc_voxel_id(seg_res_features: torch.Tensor, pc_voxel_id: torch.Tensor,
                                    invalid_value: Union[int, float] = 0):
     """Per-point features from per-voxel results (``utils.py:160-176``); points without a voxel get
-    ``invalid_value``."""
+    ``invalid_value``.  No host synchronisation (a ``where`` over a clamped gather instead of ``nonzero``)."""
     if seg_res_features.device != pc_voxel_id.device:
         pc_voxel_id = pc_voxel_id.to(seg_res_features.device)
     shape = (pc_voxel_id.shape[0], *seg_res_features.shape[1:])
-    res = torch.full(shape, invalid_value, dtype=seg_res_features.dtype, device=seg_res_features.device)
-    valid = torch.nonzero(pc_voxel_id != -1).view(-1)
-    res[valid] = seg_res_features[pc_voxel_id[valid]]
-    return res
+    fill = torch.full(shape, invalid_value, dtype=seg_res_features.dtype, device=seg_res_features.device)
+    if seg_res_features.shape[0] == 0:           # no voxels: every id is -1 (nothing to gather from)
+        return fill
+    valid = pc_voxel_id != -1
+    picked = seg_res_features.index_select(0, torch.where(valid, pc_voxel_id, 0))
+    return torch.where(valid.view(-1, *([1] * (len(shape) - 1))), picked, fill)
