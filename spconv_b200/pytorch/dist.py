@@ -103,9 +103,14 @@ class PeerGroup:
     weight-gradient kernel (``csrc/peer.cu``; ``include/spconv_b200.h`` ``spx_peer_group``).
 
         peers = PeerGroup()                       # after init_process_group; one process per GPU of ONE node
-        ops.set_peer_group(peers)                 # every dW now comes back summed (mean) over the ranks
+        ops.set_peer_group(peers)                 # every conv dW now comes back summed (mean) over the ranks
         ...
-        loss.backward()                           # no all-reduce call, no gradient bucket
+        loss.backward()                           # conv weight gradients: no all-reduce call
+        ops.peer_allreduce_(bucket.flat)          # everything else: biases, norms, heads (bucket = GradBucket)
+
+    Only the weight gradients of the conv ops are exchanged.  Biases (added outside the op in training)
+    and every other parameter keep rank-local gradients until ``ops.peer_allreduce_`` reduces them, one
+    call per tensor or one per :class:`GradBucket` of them, on every rank in the same order.
 
     Every rank allocates one buffer (``2 x capacity`` bytes: two epochs of its own fp32 slices), exports a CUDA IPC handle, and maps
     the others' (NVLink peer access).  ``capacity_bytes`` bounds the largest weight tensor, counted as

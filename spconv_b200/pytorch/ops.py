@@ -709,17 +709,9 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
             finish_exchange()
         main.wait_stream(side)
         return din, dfilters
-    if _WGRAD_HOOK is not None and n_in and n_out:
-        # Data-parallel overlap: weight gradient FIRST, then the hook (typically the all-reduce of dW) on
-        # a forked stream while the input gradient -- which the hook does not need -- runs on this one.
-        main = torch.cuda.current_stream()
-        side = _side_stream(features.device)
-        run_wgrad()
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            _WGRAD_HOOK(dfilters)
-        run_dgrad()
-        main.wait_stream(side)
+    if _WGRAD_HOOK is not None:
+        # also for a layer without rows (dW = 0): a rank whose shard is empty enters the same collectives
+        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
         return din, dfilters
     if timer.enable or not (n_in and n_out) or not torch._C._cuda_isCurrentStreamCapturing():
         # eager launches are host-bound (and an eager fork/join per call measured slower, not
@@ -744,12 +736,29 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
 _WGRAD_HOOK = None
 
 
+def _hooked_backward(run_wgrad, run_dgrad, dfilters, device) -> None:
+    """Data-parallel overlap: weight gradient FIRST, then the hook (typically the all-reduce of dW) on a
+    forked stream while the input gradient -- which the hook does not need -- runs on this one."""
+    main = torch.cuda.current_stream()
+    side = _side_stream(device)
+    run_wgrad()
+    side.wait_stream(main)
+    with torch.cuda.stream(side):
+        _WGRAD_HOOK(dfilters)
+    run_dgrad()
+    main.wait_stream(side)
+
+
 def set_wgrad_hook(fn) -> None:
-    """``fn(dfilters)`` is called on a forked stream right after every weight-gradient launch of
-    :func:`implicit_gemm_backward`, while the input gradient of the same layer runs on the caller's
-    stream (joined before the op returns).  This is the place for a data-parallel all-reduce of the
-    layer's dW: it overlaps the rest of the backward pass instead of trailing it (DDP-style hook).
-    ``None`` removes the hook."""
+    """``fn(dfilters)`` is called on a forked stream right after the weight gradient of every layer, while
+    the input gradient of the same layer runs on the caller's stream (joined before the op returns).  This
+    is the place for a data-parallel all-reduce of the layer's dW: it overlaps the rest of the backward pass
+    instead of trailing it (DDP-style hook).  It covers both routes, :func:`implicit_gemm_backward` and
+    :func:`indice_conv_backward` (``ConvAlgo.Native``), and every layer, also one without rows (its dW is
+    zero), so every rank enters the same collectives.  ``ConvAlgo.MaskSplitImplicitGemm`` calls it once per
+    mask split, with that split's dW, and sums what the hook left of each split over that split's kernel
+    offsets.  The hook may change ``dfilters`` in place; the op returns what it leaves there.  Ignored while
+    a peer group is installed (:func:`set_peer_group`).  ``None`` removes the hook."""
     global _WGRAD_HOOK
     _WGRAD_HOOK = fn
 
@@ -763,14 +772,19 @@ def set_peer_group(peers) -> None:
     gradient computed by :func:`implicit_gemm_backward` / :func:`indice_conv_backward` is returned
     already summed (x ``peers.scale``) over the ranks -- the exchange is the tail of the
     weight-gradient kernel (NVLink peer stores, ``csrc/peer.cu``), there is no separate all-reduce.
-    Every rank must run the same sequence of layers.  ``None`` switches it off."""
+    Every rank must run the same sequence of layers.  Only these conv weight gradients are exchanged:
+    biases (added outside the op in training) and every other parameter keep rank-local gradients until
+    :func:`peer_allreduce_` sums them (one call per tensor, or one per flat ``dist.GradBucket``), on every
+    rank in the same order.  ``None`` switches it off."""
     global _PEERS
     _PEERS = peers
 
 
 def peer_allreduce_(t: torch.Tensor) -> torch.Tensor:
-    """In-place sum (x scale) of a small tensor over the installed peer group (bias gradients, weight
-    gradients of layers that do not run the implicit-GEMM kernels); no-op without a group."""
+    """In-place sum (x scale) of a small tensor over the installed peer group: the step that reduces every
+    gradient the conv ops do not exchange (biases, other parameters; a ``dist.GradBucket``'s ``flat``
+    reduces them in one call).  Every rank calls it for the same tensors in the same order; at most the
+    group's capacity (fp32 values) per call.  No-op without a group."""
     if _PEERS is None or t.numel() == 0:
         return t
     assert t.is_contiguous(), "peer_allreduce_: contiguous tensor"
@@ -856,20 +870,30 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
     tiles_bwd = _tile_tables(t_bwd, m_bwd, None, n_in, kv) if n_in else None
     tiles_fwd = _tile_tables(t_fwd, m_fwd, None, n_out, kv) if n_out else None
     d_dg = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, t_bwd, m_bwd, None, tiles=tiles_bwd)
-    with timer.record("indice_conv_dgrad", _stream()):
-        _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
-                                                _ptr(din), _stream()), "implicit_gemm_dgrad(native)")
     d_wg = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, t_fwd, m_fwd, None, tiles=tiles_fwd)
     ws = _bytes(lib.spx_implicit_gemm_wgrad_workspace_size(ctypes.byref(d_wg)), features.device)
-    with timer.record("indice_conv_wgrad", _stream()):
-        if _PEERS is not None:
-            _cabi.check(lib.spx_implicit_gemm_wgrad_allreduce(
-                ctypes.byref(d_wg), _ptr(features), _ptr(out_bp), _ptr(dfilters), ws.data_ptr(), ws.numel(),
-                ctypes.byref(_PEERS.group), _PEERS.scale, _stream()), "implicit_gemm_wgrad_allreduce(native)")
-        else:
-            _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d_wg), _ptr(features), _ptr(out_bp),
-                                                    _ptr(dfilters), ws.data_ptr(), ws.numel(),
-                                                    _stream()), "implicit_gemm_wgrad(native)")
+
+    def run_dgrad():
+        with timer.record("indice_conv_dgrad", _stream()):
+            _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
+                                                    _ptr(din), _stream()), "implicit_gemm_dgrad(native)")
+
+    def run_wgrad():
+        with timer.record("indice_conv_wgrad", _stream()):
+            if _PEERS is not None:
+                _cabi.check(lib.spx_implicit_gemm_wgrad_allreduce(
+                    ctypes.byref(d_wg), _ptr(features), _ptr(out_bp), _ptr(dfilters), ws.data_ptr(), ws.numel(),
+                    ctypes.byref(_PEERS.group), _PEERS.scale, _stream()), "implicit_gemm_wgrad_allreduce(native)")
+            else:
+                _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d_wg), _ptr(features), _ptr(out_bp),
+                                                        _ptr(dfilters), ws.data_ptr(), ws.numel(),
+                                                        _stream()), "implicit_gemm_wgrad(native)")
+
+    if _PEERS is None and _WGRAD_HOOK is not None:
+        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
+        return din, dfilters
+    run_dgrad()
+    run_wgrad()
     return din, dfilters
 
 
