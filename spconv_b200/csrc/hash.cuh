@@ -127,6 +127,14 @@ struct Table64 {
     __device__ __forceinline__ void clear_slot(uint32_t s) const { keys[s] = -1ll; }
 };
 
+// Host side: call f with the table over `slots` (and, for 64-bit keys, `vals`), so that one launch sequence
+// serves both key widths.  f returns 0 or an error code, which is passed on.
+template <typename F>
+int visit_table(bool i64, void *slots, int32_t *vals, uint32_t capacity, F &&f) {
+    if (!i64) return f(Table32{(unsigned long long *)slots, capacity - 1});
+    return f(Table64{(long long *)slots, vals, capacity - 1});
+}
+
 // load factor <= 0.25: with linear probing the expected miss chain is ~1.4 slots and -- what
 // matters on a GPU -- the MAX chain over the 32 lanes of a warp stays ~2-3 (at 0.5 it was ~6
 // dependent L2 round trips per probe, measured with ncu on the 100 k-voxel cloud)

@@ -517,18 +517,13 @@ extern "C" int spx_point2voxel_bounded(const float *points, int64_t N, int num_f
     p2v_offsets_kernel<<<1, P2V_PLAN_THREADS, 0, stream>>>(point_offsets, batch_size, N, w.eff);
     SPX_CHECK_LAUNCH("p2v_offsets_kernel");
     const unsigned nblk = (unsigned)div_up64(N, 256);
-    if (!i64) {
-        Table32 t{(unsigned long long *)w.tbl, w.capacity - 1};
-        p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, w.eff, batch_size, w.keys);
-        SPX_CHECK_LAUNCH("p2v_insert_kernel");
-        p2v_mark_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, w.first, w.bitmap, w.tile_cnt, w.tiles, w.done);
-    } else {
-        Table64 t{(long long *)w.tbl, w.tvals, w.capacity - 1};
-        p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, w.eff, batch_size, w.keys);
-        SPX_CHECK_LAUNCH("p2v_insert_kernel");
-        p2v_mark_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, w.first, w.bitmap, w.tile_cnt, w.tiles, w.done);
-    }
-    SPX_CHECK_LAUNCH("p2v_mark_kernel");
+    if (int rc = visit_table(i64, w.tbl, w.tvals, w.capacity, [&](auto t) {
+            p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, w.eff, batch_size, w.keys);
+            SPX_CHECK_LAUNCH("p2v_insert_kernel");
+            p2v_mark_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, w.first, w.bitmap, w.tile_cnt, w.tiles, w.done);
+            SPX_CHECK_LAUNCH("p2v_mark_kernel");
+            return 0;
+        })) return rc;
     p2v_plan_kernel<<<1, P2V_PLAN_THREADS, 0, stream>>>(w.eff, batch_size, w.bitmap, w.tile_cnt, max_voxels, bound,
                                                         w.rbase, w.kept, w.base, num_valid, status);
     SPX_CHECK_LAUNCH("p2v_plan_kernel");
@@ -583,19 +578,14 @@ extern "C" int spx_point2voxel_stage1(const float *points, int64_t N, int num_fe
     SPX_CHECK_CUDA(cudaMemsetAsync(w.tbl, 0xFF, (size_t)w.capacity * 8, stream));
     SPX_CHECK_CUDA(cudaMemsetAsync(w.counter, 0, sizeof(int), stream));
     const unsigned nblk = (unsigned)div_up64(N, 256), cblk = (unsigned)div_up64(w.capacity, 256);
-    if (!w.i64) {
-        Table32 t{(unsigned long long *)w.tbl, w.capacity - 1};
-        p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, nullptr, 1, w.keys);
-        SPX_CHECK_LAUNCH("p2v_insert_kernel");
-        p2v_collect_kernel<<<cblk, 256, 0, stream>>>(t, w.capacity, w.a0, w.a1, w.counter);
-    } else {
-        SPX_CHECK_CUDA(cudaMemsetAsync(w.tvals, 0x7F, (size_t)w.capacity * 4, stream));
-        Table64 t{(long long *)w.tbl, w.tvals, w.capacity - 1};
-        p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, nullptr, 1, w.keys);
-        SPX_CHECK_LAUNCH("p2v_insert_kernel");
-        p2v_collect_kernel<<<cblk, 256, 0, stream>>>(t, w.capacity, w.a0, w.a1, w.counter);
-    }
-    SPX_CHECK_LAUNCH("p2v_collect_kernel");
+    if (w.i64) SPX_CHECK_CUDA(cudaMemsetAsync(w.tvals, 0x7F, (size_t)w.capacity * 4, stream));
+    if (int rc = visit_table(w.i64, w.tbl, w.tvals, w.capacity, [&](auto t) {
+            p2v_insert_kernel<<<nblk, 256, 0, stream>>>(t, g, points, N, num_features, nullptr, 1, w.keys);
+            SPX_CHECK_LAUNCH("p2v_insert_kernel");
+            p2v_collect_kernel<<<cblk, 256, 0, stream>>>(t, w.capacity, w.a0, w.a1, w.counter);
+            SPX_CHECK_LAUNCH("p2v_collect_kernel");
+            return 0;
+        })) return rc;
     int total = 0;
     SPX_CHECK_CUDA(cudaMemcpyAsync(&total, w.counter, sizeof(int), cudaMemcpyDeviceToHost, stream));
     SPX_CHECK_CUDA(cudaStreamSynchronize(stream));
@@ -629,22 +619,15 @@ extern "C" int spx_point2voxel_stage2(const float *points, int64_t N, int num_fe
     const unsigned nblk = (unsigned)div_up64(N, 256);
     const uint32_t M = (uint32_t)num_voxels;
     SPX_REQUIRE(num_voxels == 0 || (voxels && indices && num_per_voxel), "point2voxel: NULL output");
-    if (!w.i64) {
-        Table32 t{(unsigned long long *)w.tbl, w.capacity - 1};
-        if (total_voxels) {
-            p2v_assign_kernel<<<(unsigned)div_up64(total_voxels, 256), 256, 0, stream>>>(t, g, w.b1, total_voxels, num_voxels, indices);
-            SPX_CHECK_LAUNCH("p2v_assign_kernel");
-        }
-        p2v_lookup_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, M, pc_voxel_id, w.a0, w.a1);
-    } else {
-        Table64 t{(long long *)w.tbl, w.tvals, w.capacity - 1};
-        if (total_voxels) {
-            p2v_assign_kernel<<<(unsigned)div_up64(total_voxels, 256), 256, 0, stream>>>(t, g, w.b1, total_voxels, num_voxels, indices);
-            SPX_CHECK_LAUNCH("p2v_assign_kernel");
-        }
-        p2v_lookup_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, M, pc_voxel_id, w.a0, w.a1);
-    }
-    SPX_CHECK_LAUNCH("p2v_lookup_kernel");
+    if (int rc = visit_table(w.i64, w.tbl, w.tvals, w.capacity, [&](auto t) {
+            if (total_voxels) {
+                p2v_assign_kernel<<<(unsigned)div_up64(total_voxels, 256), 256, 0, stream>>>(t, g, w.b1, total_voxels, num_voxels, indices);
+                SPX_CHECK_LAUNCH("p2v_assign_kernel");
+            }
+            p2v_lookup_kernel<<<nblk, 256, 0, stream>>>(t, w.keys, N, M, pc_voxel_id, w.a0, w.a1);
+            SPX_CHECK_LAUNCH("p2v_lookup_kernel");
+            return 0;
+        })) return rc;
     if (num_voxels == 0) return 0;
     // stable sort of the points by voxel id: position inside a segment = rank in input order
     int end_bit = 1;

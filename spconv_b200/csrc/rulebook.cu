@@ -998,6 +998,19 @@ static int validate_geom(const spx_conv_geometry *g) {
     return 0;
 }
 
+// a regular (not SubM) conv also reads the strides and the output dims
+static int validate_strides(const spx_conv_geometry *g) {
+    for (int a = 0; a < g->ndim; ++a)
+        SPX_REQUIRE(g->stride[a] > 0 && g->out_dims[a] > 0, "bad stride/out_dims on axis %d", a);
+    return 0;
+}
+
+static int64_t kernel_volume(const spx_conv_geometry *g) {
+    int64_t kv = 1;
+    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    return kv;
+}
+
 struct RbLayout {   // workspace layout shared by the rulebook entry points
     size_t table_bytes, table_vals_bytes;
     uint32_t capacity;
@@ -1067,26 +1080,22 @@ static int subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int
     const int T = 128;
     unsigned nblk = (unsigned)div_up64(N, T);
     SPX_CHECK_CUDA(cudaMemsetAsync(tbl, 0xFF, L.table_bytes, stream));
-    if (!L.i64) {
-        Table32 t{(unsigned long long *)tbl, L.capacity - 1};
+    if (L.i64) SPX_CHECK_CUDA(cudaMemsetAsync(tvals, 0x7F, (size_t)L.capacity * 4, stream));
+    return visit_table(L.i64, tbl, tvals, L.capacity, [&](auto t) {
         subm_insert_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N);
         SPX_CHECK_LAUNCH("subm_insert_kernel");
-        if (subm_k3_path(gg)) {
-            subm_probe_k3_kernel<<<(unsigned)div_up64(N, K3_VOX), 27 * 32, 0, stream>>>(t, gg, indices, N, pair_fwd,
-                                                                                        pair_bwd, mask, row_table);
-        } else {
-            subm_probe_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N, pair_fwd, pair_bwd, mask, words);
+        if constexpr (std::is_same_v<decltype(t), Table32>) {   // subm_k3_path implies 32-bit keys
+            if (subm_k3_path(gg)) {
+                subm_probe_k3_kernel<<<(unsigned)div_up64(N, K3_VOX), 27 * 32, 0, stream>>>(t, gg, indices, N, pair_fwd,
+                                                                                            pair_bwd, mask, row_table);
+                SPX_CHECK_LAUNCH("subm_probe_kernel");
+                return 0;
+            }
         }
-        SPX_CHECK_LAUNCH("subm_probe_kernel");
-    } else {
-        SPX_CHECK_CUDA(cudaMemsetAsync(tvals, 0x7F, (size_t)L.capacity * 4, stream));
-        Table64 t{(long long *)tbl, tvals, L.capacity - 1};
-        subm_insert_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N);
-        SPX_CHECK_LAUNCH("subm_insert_kernel");
         subm_probe_kernel<<<nblk, T, 0, stream>>>(t, gg, indices, N, pair_fwd, pair_bwd, mask, words);
         SPX_CHECK_LAUNCH("subm_probe_kernel");
-    }
-    return 0;
+        return 0;
+    });
 }
 
 extern "C" int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int32_t *pair_fwd,
@@ -1138,6 +1147,56 @@ int carve_conv_ws(const spx_conv_geometry *g, const Geom &gg, int64_t N, void *w
     SPX_REQUIRE(ws.ok(), "rulebook workspace too small: need %zu, have %zu", ws.off, bytes);
     return 0;
 }
+
+// which of the insert and pairs kernels a regular conv runs
+struct ConvKind {
+    bool fast3;   // 3-D, not transposed: each block's offset precomputed once (block_taps3)
+    bool k3;      // and 3x3x3: one thread per input point walks all 27 offsets
+    explicit ConvKind(const Geom &gg)
+        : fast3(gg.ndim == 3 && !gg.transposed),
+          k3(fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3) {}
+    // 3x3x3 (one mask word): the pairs kernel ORs the forward masks too (zeroed by the assign kernel)
+    uint32_t *mask_fwd_or(uint32_t *mask_fwd) const { return k3 ? mask_fwd : nullptr; }
+};
+
+// reset the hash table of `capacity` slots and zero the ranking scratch and counters [rank_bitmap, end),
+// which the carvers keep contiguous
+int clear_conv_scratch(const RbLayout &L, uint32_t capacity, void *tbl, int32_t *tvals, uint32_t *rank_bitmap,
+                       const int *end, cudaStream_t stream) {
+    const int64_t zero_vec = (int64_t)(((const char *)end - (const char *)rank_bitmap) / 16);
+    conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)tbl, (int64_t)capacity / 2,
+                                                          L.i64 ? (uint4 *)tvals : nullptr,
+                                                          L.i64 ? (int64_t)capacity / 4 : 0,
+                                                          (uint4 *)rank_bitmap, zero_vec);
+    SPX_CHECK_LAUNCH("conv_clear_kernel");
+    return 0;
+}
+
+// After the outputs are assigned: the pair tables (pair_fwd has `rows` rows, M or the bound), then the masks that
+// the pairs kernel did not write.  A NULL mask is not wanted.
+template <typename Table>
+int conv_pairs_and_masks(Table t, const Geom &gg, ConvKind kind, const int32_t *indices, int64_t N, int64_t rows,
+                         int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd, uint32_t *mask_bwd,
+                         cudaStream_t stream) {
+    const int T = 128, words = (gg.kv + 31) / 32;
+    uint32_t *mask_fwd_or = kind.mask_fwd_or(mask_fwd);
+    if (N > 0) {
+        const dim3 grid((unsigned)div_up64(N, T), gg.kv);
+        if (kind.k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, rows, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
+        else if (kind.fast3) conv_pairs_kernel<Table, true><<<grid, T, 0, stream>>>(t, gg, indices, N, rows, pair_fwd, pair_bwd);
+        else conv_pairs_kernel<Table, false><<<grid, T, 0, stream>>>(t, gg, indices, N, rows, pair_fwd, pair_bwd);
+        SPX_CHECK_LAUNCH("conv_pairs_kernel");
+    }
+    if (mask_fwd && !mask_fwd_or) {
+        table_mask_kernel<<<(unsigned)div_up64(rows, 256), 256, 0, stream>>>(pair_fwd, rows, gg.kv, words, mask_fwd);
+        SPX_CHECK_LAUNCH("table_mask_kernel");
+    }
+    if (mask_bwd && !kind.k3 && N > 0) {        // the 3x3x3 pairs kernel has already written it
+        table_mask_kernel<<<(unsigned)div_up64(N, 256), 256, 0, stream>>>(pair_bwd, N, gg.kv, words, mask_bwd);
+        SPX_CHECK_LAUNCH("table_mask_kernel");
+    }
+    return 0;
+}
 }  // namespace
 
 extern "C" size_t spx_rulebook_workspace_size(const spx_conv_geometry *g, int64_t num_in, int64_t max_out, int is_subm) {
@@ -1164,42 +1223,29 @@ extern "C" int spx_conv_rulebook_stage1(const spx_conv_geometry *g, const int32_
     *num_out_host = 0;
     if (N == 0) return 0;
     SPX_REQUIRE(indices && workspace, "NULL pointer argument");
-    for (int a = 0; a < g->ndim; ++a)
-        SPX_REQUIRE(g->stride[a] > 0 && g->out_dims[a] > 0, "bad stride/out_dims on axis %d", a);
+    if (validate_strides(g)) return 2;
     cudaStream_t stream = (cudaStream_t)stream_;
     Geom gg = make_geom(g, false);
     SPX_REQUIRE((int64_t)gg.kv * N < 2000000000ll, "kv*N must stay below 2e9 (kv=%d, N=%lld)", gg.kv, (long long)N);
     ConvWs w;
     if (carve_conv_ws(g, gg, N, workspace, workspace_bytes, w)) return 2;
-    const int T = 128;
-    dim3 grid((unsigned)div_up64(N, T), gg.kv);
-    const bool fast3 = gg.ndim == 3 && !gg.transposed;
-    const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
+    const dim3 grid((unsigned)div_up64(N, 128), gg.kv);
+    const ConvKind kind(gg);
     g_stage1 = {workspace, w.L.capacity};
     // optimistic table, append-on-create, outputs ranked by first touch without a sort
     const int64_t max_out = spx_conv_max_out(g, N);
     int host_state[2] = {0, 0};
     uint32_t capacity = optimistic_capacity(max_out, w.L.capacity);
     for (int attempt = 0; attempt < 2; ++attempt) {
-        // ranking scratch and counters are contiguous (carve_conv_ws): one region of zeros
-        const int64_t zero_vec = (int64_t)(((char *)(w.counter + 64) - (char *)w.rank_bitmap) / 16);
-        conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)capacity / 2,
-                                                              w.L.i64 ? (uint4 *)w.tvals : nullptr,
-                                                              w.L.i64 ? (int64_t)capacity / 4 : 0,
-                                                              (uint4 *)w.rank_bitmap, zero_vec);
-        SPX_CHECK_LAUNCH("conv_clear_kernel");
-        if (!w.L.i64) {
-            Table32 t{(unsigned long long *)w.tbl, capacity - 1};
-            if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            else if (fast3) conv_insert_append_kernel<Table32, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            else conv_insert_append_kernel<Table32, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-        } else {
-            Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-            if (k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            else if (fast3) conv_insert_append_kernel<Table64, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-            else conv_insert_append_kernel<Table64, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
-        }
-        SPX_CHECK_LAUNCH("conv_insert_append_kernel");
+        if (int rc = clear_conv_scratch(w.L, capacity, w.tbl, w.tvals, w.rank_bitmap, w.counter + 64, stream)) return rc;
+        if (int rc = visit_table(w.L.i64, w.tbl, w.tvals, capacity, [&](auto t) {
+                using Table = decltype(t);
+                if (kind.k3) conv_insert_k3_append_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+                else if (kind.fast3) conv_insert_append_kernel<Table, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+                else conv_insert_append_kernel<Table, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.slot, w.counter);
+                SPX_CHECK_LAUNCH("conv_insert_append_kernel");
+                return 0;
+            })) return rc;
         SPX_CHECK_CUDA(cudaMemcpyAsync(host_state, w.counter, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
         SPX_CHECK_CUDA(cudaStreamSynchronize(stream));
         if (!host_state[1]) break;
@@ -1211,15 +1257,11 @@ extern "C" int spx_conv_rulebook_stage1(const spx_conv_geometry *g, const int32_
     *num_out_host = m_host;
     if (m_host == 0) return 0;
     const unsigned mblk = (unsigned)div_up64(m_host, MARK_THREADS);
-    if (!w.L.i64) {
-        Table32 t{(unsigned long long *)w.tbl, capacity - 1};
+    return visit_table(w.L.i64, w.tbl, w.tvals, capacity, [&](auto t) {
         conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
-    } else {
-        Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-        conv_mark_kernel<<<mblk, MARK_THREADS, 0, stream>>>(t, w.slot, m_host, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.counter + 2);
-    }
-    SPX_CHECK_LAUNCH("conv_mark_kernel");
-    return 0;
+        SPX_CHECK_LAUNCH("conv_mark_kernel");
+        return 0;
+    });
 }
 
 extern "C" int spx_conv_rulebook_stage2(const spx_conv_geometry *g, const int32_t *indices, int64_t N, int64_t M,
@@ -1233,42 +1275,14 @@ extern "C" int spx_conv_rulebook_stage2(const spx_conv_geometry *g, const int32_
     Geom gg = make_geom(g, false);
     ConvWs w;
     if (carve_conv_ws(g, gg, N, workspace, workspace_bytes, w)) return 2;
-    int words = (gg.kv + 31) / 32;
-    const int T = 128;
-    dim3 grid((unsigned)div_up64(N, T), gg.kv);
-    const bool fast3 = gg.ndim == 3 && !gg.transposed;
-    const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
+    const ConvKind kind(gg);
     SPX_REQUIRE(g_stage1.ws == workspace && g_stage1.capacity != 0,
                 "conv_rulebook_stage2 must follow conv_rulebook_stage1 on the same thread with the same workspace");
-    const uint32_t capacity = g_stage1.capacity;
-    // 3x3x3, one mask word: the pairs kernel ORs the forward masks too (zeroed by the assign kernel)
-    uint32_t *mask_fwd_or = (k3 && mask_fwd && words == 1) ? mask_fwd : nullptr;
-    if (!w.L.i64) {
-        Table32 t{(unsigned long long *)w.tbl, capacity - 1};
-        conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
+    return visit_table(w.L.i64, w.tbl, w.tvals, g_stage1.capacity, [&](auto t) {
+        conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, kind.mask_fwd_or(mask_fwd), pair_fwd, gg.kv);
         SPX_CHECK_LAUNCH("conv_assign_rank_kernel");
-        if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
-        else if (fast3) conv_pairs_kernel<Table32, true><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
-        else conv_pairs_kernel<Table32, false><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
-        SPX_CHECK_LAUNCH("conv_pairs_kernel");
-    } else {
-        Table64 t{(long long *)w.tbl, w.tvals, capacity - 1};
-        conv_assign_rank_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(t, gg, w.slot, M, w.rank_bitmap, w.rank_tiles, out_inds, mask_fwd_or, pair_fwd, gg.kv);
-        SPX_CHECK_LAUNCH("conv_assign_rank_kernel");
-        if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
-        else if (fast3) conv_pairs_kernel<Table64, true><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
-        else conv_pairs_kernel<Table64, false><<<grid, T, 0, stream>>>(t, gg, indices, N, M, pair_fwd, pair_bwd);
-        SPX_CHECK_LAUNCH("conv_pairs_kernel");
-    }
-    if (mask_fwd && !mask_fwd_or) {
-        table_mask_kernel<<<(unsigned)div_up64(M, 256), 256, 0, stream>>>(pair_fwd, M, gg.kv, words, mask_fwd);
-        SPX_CHECK_LAUNCH("table_mask_kernel");
-    }
-    if (mask_bwd && !k3) {                      // the 3x3x3 pairs kernel has already written it
-        table_mask_kernel<<<(unsigned)div_up64(N, 256), 256, 0, stream>>>(pair_bwd, N, gg.kv, words, mask_bwd);
-        SPX_CHECK_LAUNCH("table_mask_kernel");
-    }
-    return 0;
+        return conv_pairs_and_masks(t, gg, kind, indices, N, M, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+    });
 }
 
 extern "C" size_t spx_native_pairs_workspace_size(int64_t N, int kv) {
@@ -1462,8 +1476,7 @@ static size_t subm_row_table_bytes(const spx_conv_geometry *g, int64_t N) {
 
 extern "C" size_t spx_subm_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N) {
     if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
-    int kv = 1;
-    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    const int kv = (int)kernel_volume(g);
     const size_t a = spx_rulebook_workspace_size(g, N, 0, 1);
     const size_t b = spx_mask_argsort_workspace_size(N, (kv + 31) / 32);
     return align_up(a > b ? a : b, 256) + subm_row_table_bytes(g, N) + 256;
@@ -1477,8 +1490,7 @@ extern "C" int spx_subm_rulebook_all(const spx_conv_geometry *g, const int32_t *
     if (N == 0) return 0;
     SPX_REQUIRE(mask && argsort && tile_table && tile_mask && workspace, "subm_rulebook_all: NULL pointer argument");
     SPX_REQUIRE(workspace_bytes >= spx_subm_rulebook_all_workspace_size(g, N), "subm_rulebook_all: workspace too small");
-    int kv = 1;
-    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    const int kv = (int)kernel_volume(g);
     const int words = (kv + 31) / 32;
     const size_t rb = spx_rulebook_workspace_size(g, N, 0, 1), as = spx_mask_argsort_workspace_size(N, words);
     const size_t shared = align_up(rb > as ? rb : as, 256);          // rulebook and sort scratch are used one after the other
@@ -1514,8 +1526,7 @@ static int conv_sort_and_tiles(int kv, int64_t N, int64_t M, int32_t *pair_fwd, 
 
 extern "C" size_t spx_conv_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N) {
     if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM) return 0;
-    int kv = 1;
-    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    const int kv = (int)kernel_volume(g);
     const int64_t max_rows = spx_conv_max_out(g, N) > N ? spx_conv_max_out(g, N) : N;
     return align_up(spx_rulebook_workspace_size(g, N, 0, 0), 256) +
            2 * align_up(spx_mask_argsort_workspace_size(max_rows, (kv + 31) / 32), 256) + 256;   // two sorts side by side
@@ -1537,8 +1548,7 @@ extern "C" int spx_conv_rulebook_stage2_all(const spx_conv_geometry *g, const in
                 "conv_rulebook_stage2_all: argsort_bwd, table_bwd and tmask_bwd must all be given (training) or all be "
                 "NULL (inference)");
     SPX_REQUIRE(workspace_bytes >= spx_conv_rulebook_all_workspace_size(g, N), "conv_rulebook_stage2_all: workspace too small");
-    int kv = 1;
-    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    const int kv = (int)kernel_volume(g);
     const size_t rb = spx_rulebook_workspace_size(g, N, 0, 0);
     void *sort_ws = (char *)workspace + align_up(rb, 256);
     const size_t sort_bytes = workspace_bytes - align_up(rb, 256);
@@ -1579,72 +1589,39 @@ void carve_bounded_ws(const Geom &gg, int64_t N, int64_t bound, bool sorts, void
     w.bytes = ws.off;
 }
 
-template <typename Table>
-int bounded_rulebook_kernels(Table t, const Geom &gg, const BoundedWs &w, const int32_t *indices, int64_t N, int64_t bound,
-                             int32_t *out_inds, int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd,
-                             uint32_t *mask_bwd, int32_t *num_out, int32_t *status, cudaStream_t stream) {
-    const int T = 128, words = (gg.kv + 31) / 32;
-    const dim3 grid((unsigned)div_up64(N > 0 ? N : 1, T), gg.kv);
-    const bool fast3 = gg.ndim == 3 && !gg.transposed;
-    const bool k3 = fast3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
-    const int64_t capacity = w.L.capacity;
-    if (N > 0) {
-        if (k3) conv_insert_k3_bounded_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
-        else if (fast3) conv_insert_bounded_kernel<Table, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
-        else conv_insert_bounded_kernel<Table, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
-        SPX_CHECK_LAUNCH("conv_insert_bounded_kernel");
-    }
-    conv_mark_table_kernel<<<(unsigned)div_up64(capacity, MARK_THREADS), MARK_THREADS, 0, stream>>>(
-        t, capacity, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.state);
-    SPX_CHECK_LAUNCH("conv_mark_table_kernel");
-    // 3x3x3, one mask word: the pairs kernel ORs the forward masks too (zeroed by the assign kernel)
-    uint32_t *mask_fwd_or = (k3 && words == 1) ? mask_fwd : nullptr;
-    const int64_t span = capacity > bound ? capacity : bound;
-    conv_assign_table_kernel<<<(unsigned)div_up64(span, 256), 256, 0, stream>>>(
-        t, gg, capacity, bound, w.rank_bitmap, w.rank_tiles, w.state, out_inds, mask_fwd_or, pair_fwd, gg.kv, num_out, status);
-    SPX_CHECK_LAUNCH("conv_assign_table_kernel");
-    if (N > 0) {
-        if (k3) conv_pairs_k3_kernel<<<(unsigned)div_up64(N, T), T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd, mask_bwd, mask_fwd_or);
-        else if (fast3) conv_pairs_kernel<Table, true><<<grid, T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd);
-        else conv_pairs_kernel<Table, false><<<grid, T, 0, stream>>>(t, gg, indices, N, bound, pair_fwd, pair_bwd);
-        SPX_CHECK_LAUNCH("conv_pairs_kernel");
-    }
-    if (!mask_fwd_or && mask_fwd) {              // no masks at all for the sparse_add union
-        table_mask_kernel<<<(unsigned)div_up64(bound, 256), 256, 0, stream>>>(pair_fwd, bound, gg.kv, words, mask_fwd);
-        SPX_CHECK_LAUNCH("table_mask_kernel");
-    }
-    if (!k3 && N > 0 && mask_bwd) {              // the 3x3x3 pairs kernel has already written it
-        table_mask_kernel<<<(unsigned)div_up64(N, 256), 256, 0, stream>>>(pair_bwd, N, gg.kv, words, mask_bwd);
-        SPX_CHECK_LAUNCH("table_mask_kernel");
-    }
-    return 0;
-}
-
-// clear the table, the ranking scratch and the state, then the kernels above on the 32- or 64-bit-key table
+// clear the table, the ranking scratch and the state, then insert, rank, assign and pair on the table
 int run_bounded(const Geom &gg, const BoundedWs &w, const int32_t *indices, int64_t N, int64_t bound, int32_t *out_inds,
                 int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd, uint32_t *mask_bwd, int32_t *num_out,
                 int32_t *status, cudaStream_t stream) {
-    const int64_t zero_vec = (int64_t)(((char *)(w.state + 64) - (char *)w.rank_bitmap) / 16);
-    conv_clear_kernel<<<sm_count() * 4, 256, 0, stream>>>((uint4 *)w.tbl, (int64_t)w.L.capacity / 2,
-                                                          w.L.i64 ? (uint4 *)w.tvals : nullptr,
-                                                          w.L.i64 ? (int64_t)w.L.capacity / 4 : 0,
-                                                          (uint4 *)w.rank_bitmap, zero_vec);
-    SPX_CHECK_LAUNCH("conv_clear_kernel");
-    if (!w.L.i64)
-        return bounded_rulebook_kernels(Table32{(unsigned long long *)w.tbl, w.L.capacity - 1}, gg, w, indices, N, bound,
-                                        out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
-    return bounded_rulebook_kernels(Table64{(long long *)w.tbl, w.tvals, w.L.capacity - 1}, gg, w, indices, N, bound,
-                                    out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd, num_out, status, stream);
+    if (int rc = clear_conv_scratch(w.L, w.L.capacity, w.tbl, w.tvals, w.rank_bitmap, w.state + 64, stream)) return rc;
+    const ConvKind kind(gg);
+    const int64_t capacity = w.L.capacity;
+    return visit_table(w.L.i64, w.tbl, w.tvals, w.L.capacity, [&](auto t) {
+        using Table = decltype(t);
+        if (N > 0) {
+            const dim3 grid((unsigned)div_up64(N, 128), gg.kv);
+            if (kind.k3) conv_insert_k3_bounded_kernel<<<(unsigned)div_up64(N, APPEND_THREADS), APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+            else if (kind.fast3) conv_insert_bounded_kernel<Table, true><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+            else conv_insert_bounded_kernel<Table, false><<<grid, APPEND_THREADS, 0, stream>>>(t, gg, indices, N, w.state);
+            SPX_CHECK_LAUNCH("conv_insert_bounded_kernel");
+        }
+        conv_mark_table_kernel<<<(unsigned)div_up64(capacity, MARK_THREADS), MARK_THREADS, 0, stream>>>(
+            t, capacity, w.rank_bitmap, w.rank_tiles, w.rank_ntiles, w.state);
+        SPX_CHECK_LAUNCH("conv_mark_table_kernel");
+        const int64_t span = capacity > bound ? capacity : bound;
+        conv_assign_table_kernel<<<(unsigned)div_up64(span, 256), 256, 0, stream>>>(
+            t, gg, capacity, bound, w.rank_bitmap, w.rank_tiles, w.state, out_inds, kind.mask_fwd_or(mask_fwd), pair_fwd,
+            gg.kv, num_out, status);
+        SPX_CHECK_LAUNCH("conv_assign_table_kernel");
+        return conv_pairs_and_masks(t, gg, kind, indices, N, bound, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+    });
 }
 
 int validate_bounded(const spx_conv_geometry *g, int64_t N, int64_t bound) {
-    if (validate_geom(g)) return 2;
-    for (int a = 0; a < g->ndim; ++a)
-        SPX_REQUIRE(g->stride[a] > 0 && g->out_dims[a] > 0, "bad stride/out_dims on axis %d", a);
+    if (validate_geom(g) || validate_strides(g)) return 2;
     SPX_REQUIRE(bound > 0 && bound < (1ll << 30), "bound must be in [1, 2^30), got %lld", (long long)bound);
     SPX_REQUIRE(N >= 0, "bad N");
-    int64_t kv = 1;
-    for (int a = 0; a < g->ndim; ++a) kv *= g->ksize[a];
+    const int64_t kv = kernel_volume(g);
     SPX_REQUIRE(kv <= 128, "conv_rulebook_bounded: kernel volume %lld not in [1,128]", (long long)kv);
     SPX_REQUIRE(kv * N < 2000000000ll, "kv*N must stay below 2e9 (kv=%lld, N=%lld)", (long long)kv, (long long)N);
     return 0;

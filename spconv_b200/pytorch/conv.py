@@ -22,7 +22,7 @@ from .. import constants as _constants
 from ..core import Activation, ConvAlgo
 from . import functional as Fsp
 from . import ops
-from .core import (ImplicitGemmIndiceData, IndiceData, SparseConvTensor, expand_nd)
+from .core import (ImplicitGemmIndiceData, IndiceData, SparseConvTensor, expand_nd, rulebook_num_valid)
 from .modules import SparseModule
 
 _MAX_NUM_VOXELS_DURING_TRAINING = "max_num_voxels_during_training"
@@ -76,7 +76,6 @@ class SparseConvolution(SparseModule):
         # When set the rulebook runs without a host read-back, the output has exactly this many rows and
         # carries ``num_valid`` (spconv.set_output_bounds finds the value).  None: exact shapes, one sync.
         self.num_out_act_bound: Optional[int] = None
-        self._bound_status: Optional[torch.Tensor] = None
         self.fp32_accum = fp32_accum
         self.act_type, self.act_alpha, self.act_beta = act_type, act_alpha, act_beta
         kv = int(np.prod(self.kernel_size))
@@ -169,13 +168,6 @@ class SparseConvolution(SparseModule):
         return (self.num_out_act_bound is not None and self.num_out_act_bound > 0 and not self.subm
                 and not self.inverse and algo == ConvAlgo.MaskImplicitGemm)
 
-    def _status_word(self, device) -> torch.Tensor:
-        """This layer's bounded-rulebook status word.  It lives on the module, outside any captured step, so
-        the bits stay set across graph replays until spconv.check_bounds reads them."""
-        if self._bound_status is None or self._bound_status.device != device:
-            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=device)
-        return self._bound_status
-
     # ------------------------------------------------------------------ cache validity
     def _check_subm_reuse_valid(self, inp: SparseConvTensor, spatial_shape: List[int], datas):
         assert datas.is_subm, "only support reuse subm indices"
@@ -234,9 +226,6 @@ class SparseConvolution(SparseModule):
                                               self.padding, self.dilation, self.output_padding)
         return ops.get_conv_output_size(spatial_shape, self.kernel_size, self.stride,
                                         self.padding, self.dilation)
-
-    def _layer_name(self) -> str:
-        return self._sparse_unique_name or self.name or self.indice_key or type(self).__name__
 
     def _rulebook_error(self, tag, indices, batch_size, spatial_shape, algo):
         print(f"[Exception|{tag}]indices={indices.shape},bs={batch_size},ss={spatial_shape},"
@@ -372,24 +361,14 @@ class SparseConvolution(SparseModule):
                         raise
                 (outids, _num_per_loc, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd,
                  masks) = res
-                in_valid = input.num_valid
-                if not self.subm:
-                    # a bounded rulebook leaves the count on the device; an unbounded one has exact rows
-                    num_valid = getattr(outids, "_spx_num_valid", None)
-                    if num_valid is not None:
-                        out_tensor.bound_status = {**(input.bound_status or {}),
-                                                   self._layer_name(): outids._spx_bound_status}
+                num_valid = rulebook_num_valid(outids, input, out_tensor, self.subm, self)
                 if self.indice_key is not None:
                     assert self.indice_key not in indice_dict, \
                         f"your indice key {self.indice_key} already exists in this sparse tensor."
-                    indice_dict[self.indice_key] = ImplicitGemmIndiceData(
-                        outids, indices, pair_fwd, pair_bwd, pair_mask_fwd_splits=mask_fwd,
-                        pair_mask_bwd_splits=mask_bwd, mask_argsort_fwd_splits=sort_fwd,
-                        mask_argsort_bwd_splits=sort_bwd, masks=masks, is_subm=self.subm,
-                        spatial_shape=spatial_shape, out_spatial_shape=out_spatial_shape,
-                        algo=algo, ksize=self.kernel_size, stride=self.stride,
-                        dilation=self.dilation, padding=self.padding, in_voxel_num=in_valid,
-                        out_voxel_num=num_valid)
+                    indice_dict[self.indice_key] = ImplicitGemmIndiceData.from_rulebook(
+                        res, indices, input.num_valid, self.subm, spatial_shape=spatial_shape,
+                        out_spatial_shape=out_spatial_shape, algo=algo, ksize=self.kernel_size,
+                        stride=self.stride, dilation=self.dilation, padding=self.padding)
             num_activate_out = outids.shape[0]
             if training:
                 out_features = Fsp.implicit_gemm(features, weight, pair_fwd, pair_bwd, mask_fwd,

@@ -151,6 +151,28 @@ class ImplicitGemmIndiceData:
     # pick its rulebook up from the indice_dict (the reference lets SubM layers alone reuse a key)
     prefetched: bool = False
 
+    @classmethod
+    def from_rulebook(cls, res, indices: torch.Tensor, in_voxel_num, is_subm: bool, **geometry):
+        """The entry of the 9-tuple ``res`` of ``ops.get_indice_pairs_implicit_gemm`` built on ``indices``."""
+        outids, _, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
+        return cls(outids, indices, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks, is_subm=is_subm,
+                   in_voxel_num=in_voxel_num, out_voxel_num=_out_voxel_num(outids, in_voxel_num, is_subm), **geometry)
+
+
+def _out_voxel_num(outids: torch.Tensor, in_voxel_num, is_subm: bool):
+    # SubM keeps its input's rows; a bounded rulebook leaves its output count on the device (None: all rows valid)
+    return in_voxel_num if is_subm else getattr(outids, "_spx_num_valid", None)
+
+
+def rulebook_num_valid(outids: torch.Tensor, inp: "SparseConvTensor", out: "SparseConvTensor", is_subm: bool,
+                       layer) -> Optional[torch.Tensor]:
+    """``num_valid`` of the output ``out`` of a conv / pool ``layer`` on ``inp`` whose rows are ``outids``.  A
+    bounded rulebook's status word joins ``out.bound_status`` under the layer's name."""
+    num_valid = _out_voxel_num(outids, inp.num_valid, is_subm)
+    if num_valid is not None and not is_subm:
+        out.bound_status = {**(inp.bound_status or {}), layer._layer_name(): outids._spx_bound_status}
+    return num_valid
+
 
 def scatter_nd(indices: torch.Tensor, updates: torch.Tensor, shape: Sequence[int]) -> torch.Tensor:
     """Dense tensor of ``shape`` with ``updates`` written at integer coordinates ``indices``

@@ -29,6 +29,19 @@ class SparseModule(nn.Module):
         super().__init__()
         self.name = name
         self._sparse_unique_name = ""
+        # the status word of a module with an output bound (strided conv / pool, masked sparse add, remove duplicate)
+        self._bound_status: Optional[torch.Tensor] = None
+
+    def _status_word(self, device) -> torch.Tensor:
+        """This module's output-bound status word.  It lives on the module, outside any captured step, so the bits
+        stay set across graph replays until spconv.check_bounds reads them."""
+        if self._bound_status is None or self._bound_status.device != device:
+            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=device)
+        return self._bound_status
+
+    def _layer_name(self) -> str:
+        """The name under which this module's status word appears in ``SparseConvTensor.bound_status``."""
+        return self._sparse_unique_name or self.name or getattr(self, "indice_key", None) or type(self).__name__
 
 
 def assign_name_for_sparse_modules(module: nn.Module):

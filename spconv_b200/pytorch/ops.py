@@ -174,37 +174,48 @@ def _conv_stage1(geo, indices, n_in, ws) -> int:
 
 
 def _conv_rulebook(geo, indices, n_in, kv, words, want_masks, alloc):
-    """Two-phase regular-conv rulebook; returns (out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd)."""
+    """Two-phase regular-conv rulebook; returns (out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd).  With no outputs
+    (M == 0) stage 2 does not run and pair_bwd is left unwritten: the caller decides what M == 0 means."""
     lib = _lib()
     dev = indices.device
     ws_bytes = lib.spx_rulebook_workspace_size(ctypes.byref(geo), n_in, 0, 0)
     ws = _bytes(ws_bytes, dev, alloc)
     m = _conv_stage1(geo, indices, n_in, ws)
-    if m == 0:
-        raise ValueError(_VANISHED)
     ndim = indices.shape[1] - 1
     out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
     pair_fwd = torch.empty((kv, m), dtype=torch.int32, device=dev)
     pair_bwd = torch.empty((kv, n_in), dtype=torch.int32, device=dev)
     mask_fwd = torch.empty((1, m, words), dtype=torch.int32, device=dev) if want_masks else None
     mask_bwd = torch.empty((1, n_in, words), dtype=torch.int32, device=dev) if want_masks else None
-    _cabi.check(lib.spx_conv_rulebook_stage2(ctypes.byref(geo), _ptr(indices), n_in, m,
-                                             out_inds.data_ptr(), pair_fwd.data_ptr(),
-                                             pair_bwd.data_ptr(), _ptr(mask_fwd), _ptr(mask_bwd),
-                                             ws.data_ptr(), ws.numel(), _stream()),
-                "conv_rulebook_stage2")
+    if m:
+        _cabi.check(lib.spx_conv_rulebook_stage2(ctypes.byref(geo), _ptr(indices), n_in, m,
+                                                 out_inds.data_ptr(), pair_fwd.data_ptr(),
+                                                 pair_bwd.data_ptr(), _ptr(mask_fwd), _ptr(mask_bwd),
+                                                 ws.data_ptr(), ws.numel(), _stream()),
+                    "conv_rulebook_stage2")
     return out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd
 
 
-def _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks):
-    """Regular-conv implicit-GEMM rulebook in two native calls (stage 1 with its host read-back of the
-    output count, then stage 2 + both mask sorts + both tile tables)."""
+def _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks, bound=0,
+                       status=None):
+    """Regular-conv implicit-GEMM rulebook with its mask sorts and tile tables, as the reference's 9-tuple.
+
+    ``bound == 0``: two native calls, stage 1 with its host read-back of the output count M, then stage 2.
+    ``bound > 0`` (``spx_conv_rulebook_bounded_all``): one native call and no host read-back; every output-side
+    tensor has ``bound`` rows, and the true count (device int32 ``[1]``) and the status word ride on ``out_inds`` as
+    ``_spx_num_valid`` / ``_spx_bound_status``."""
     lib = _lib()
     dev = indices.device
-    ws = _bytes(lib.spx_conv_rulebook_all_workspace_size(ctypes.byref(geo), n_in), dev, alloc)
-    m = _conv_stage1(geo, indices, n_in, ws)
-    if m == 0:
-        raise ValueError(_VANISHED)
+    if bound:
+        m = bound
+        if n_in == 0:                    # host-known: the unbounded path raises the same error for M == 0
+            raise ValueError(_VANISHED)
+        ws = _bytes(lib.spx_conv_rulebook_bounded_workspace_size(ctypes.byref(geo), n_in, m), dev, alloc)
+    else:
+        ws = _bytes(lib.spx_conv_rulebook_all_workspace_size(ctypes.byref(geo), n_in), dev, alloc)
+        m = _conv_stage1(geo, indices, n_in, ws)
+        if m == 0:
+            raise ValueError(_VANISHED)
     ndim = indices.shape[1] - 1
     out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
     pair_fwd = torch.empty((kv, m), dtype=torch.int32, device=dev)
@@ -215,51 +226,20 @@ def _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, 
     sort_bwd = torch.empty((1, n_in), dtype=torch.int32, device=dev) if is_train else None
     t_fwd, tm_fwd = _alloc_tile_tables(m, kv, dev)
     t_bwd, tm_bwd = _alloc_tile_tables(n_in, kv, dev) if is_train else (None, None)
-    _cabi.check(lib.spx_conv_rulebook_stage2_all(
-        ctypes.byref(geo), _ptr(indices), n_in, m, out_inds.data_ptr(), pair_fwd.data_ptr(), pair_bwd.data_ptr(),
-        mask_fwd.data_ptr(), mask_bwd.data_ptr(), sort_fwd.data_ptr(), _ptr(sort_bwd), int(bool(do_sort)),
-        _ptr(t_fwd), _ptr(tm_fwd), _ptr(t_bwd), _ptr(tm_bwd), ws.data_ptr(), ws.numel(), _stream()),
-        "conv_rulebook_stage2_all")
-    sf = sort_fwd[0]
-    sf._spx_tile_cache = (_tile_key(pair_fwd, sf, m), t_fwd, tm_fwd)
-    if not is_train:
-        return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [], [sf], [], masks)
-    sb = sort_bwd[0]
-    sb._spx_tile_cache = (_tile_key(pair_bwd, sb, n_in), t_bwd, tm_bwd)
-    return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, [mask_fwd[0]], [mask_bwd[0]], [sf], [sb], masks)
-
-
-def _conv_rulebook_bounded(geo, indices, n_in, kv, words, bound, is_train, do_sort, alloc, indice_num_per_loc, masks,
-                           status):
-    """Bounded regular-conv implicit-GEMM rulebook (``spx_conv_rulebook_bounded_all``): one native call, no host
-    read-back.  Every output-side tensor has ``bound`` rows; the true count (device int32 ``[1]``) and the status
-    word ride on ``out_inds`` as ``_spx_num_valid`` / ``_spx_bound_status``."""
-    lib = _lib()
-    dev = indices.device
-    m = int(bound)
-    if n_in == 0:                        # host-known: the unbounded path raises the same error for M == 0
-        raise ValueError(_VANISHED)
-    ws = _bytes(lib.spx_conv_rulebook_bounded_workspace_size(ctypes.byref(geo), n_in, m), dev, alloc)
-    ndim = indices.shape[1] - 1
-    out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
-    pair_fwd = torch.empty((kv, m), dtype=torch.int32, device=dev)
-    pair_bwd = torch.empty((kv, n_in), dtype=torch.int32, device=dev)
-    mask_fwd = torch.empty((1, m, words), dtype=torch.int32, device=dev)
-    mask_bwd = torch.empty((1, n_in, words), dtype=torch.int32, device=dev)
-    sort_fwd = torch.empty((1, m), dtype=torch.int32, device=dev)
-    sort_bwd = torch.empty((1, n_in), dtype=torch.int32, device=dev) if is_train else None
-    t_fwd, tm_fwd = _alloc_tile_tables(m, kv, dev)
-    t_bwd, tm_bwd = _alloc_tile_tables(n_in, kv, dev) if is_train else (None, None)
-    num_out = torch.empty((1,), dtype=torch.int32, device=dev)
-    if status is None:
-        status = torch.zeros((1,), dtype=torch.int32, device=dev)
-    _cabi.check(lib.spx_conv_rulebook_bounded_all(
-        ctypes.byref(geo), _ptr(indices), n_in, m, out_inds.data_ptr(), pair_fwd.data_ptr(), _ptr(pair_bwd),
-        mask_fwd.data_ptr(), _ptr(mask_bwd), sort_fwd.data_ptr(), _ptr(sort_bwd), int(bool(do_sort)),
-        _ptr(t_fwd), _ptr(tm_fwd), _ptr(t_bwd), _ptr(tm_bwd), num_out.data_ptr(), status.data_ptr(),
-        ws.data_ptr(), ws.numel(), _stream()), "conv_rulebook_bounded_all")
-    out_inds._spx_num_valid = num_out
-    out_inds._spx_bound_status = status
+    args = (ctypes.byref(geo), _ptr(indices), n_in, m, out_inds.data_ptr(), pair_fwd.data_ptr(), _ptr(pair_bwd),
+            mask_fwd.data_ptr(), _ptr(mask_bwd), sort_fwd.data_ptr(), _ptr(sort_bwd), int(bool(do_sort)),
+            _ptr(t_fwd), _ptr(tm_fwd), _ptr(t_bwd), _ptr(tm_bwd))
+    if bound:
+        num_out = torch.empty((1,), dtype=torch.int32, device=dev)
+        if status is None:
+            status = torch.zeros((1,), dtype=torch.int32, device=dev)
+        _cabi.check(lib.spx_conv_rulebook_bounded_all(*args, num_out.data_ptr(), status.data_ptr(), ws.data_ptr(),
+                                                      ws.numel(), _stream()), "conv_rulebook_bounded_all")
+        out_inds._spx_num_valid = num_out
+        out_inds._spx_bound_status = status
+    else:
+        _cabi.check(lib.spx_conv_rulebook_stage2_all(*args, ws.data_ptr(), ws.numel(), _stream()),
+                    "conv_rulebook_stage2_all")
     sf = sort_fwd[0]
     sf._spx_tile_cache = (_tile_key(pair_fwd, sf, m), t_fwd, tm_fwd)
     if not is_train:
@@ -333,6 +313,8 @@ def get_indice_pairs(indices: torch.Tensor, batch_size: int, spatial_shape: List
     else:
         out_inds, pair_fwd, pair_bwd, _, _ = _conv_rulebook(geo, indices, n_in, kv,
                                                             (kv + 31) // 32, False, None)
+        if out_inds.shape[0] == 0:
+            raise ValueError(_VANISHED)
     ws2 = _bytes(lib.spx_native_pairs_workspace_size(n_in, kv), dev)
     _cabi.check(lib.spx_native_pairs(_ptr(pair_bwd), n_in, kv, int(subm), pairs.data_ptr(),
                                      num.data_ptr(), ws2.data_ptr(), ws2.numel(), _stream()),
@@ -421,16 +403,16 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
         with timer.record("gen_conv_inds", _stream()):
             out_inds, pair_fwd, pair_bwd, mask_fwd, mask_bwd = _conv_rulebook(
                 geo, indices, n_in, kv, words, True, alloc)
+            if out_inds.shape[0] == 0:
+                raise ValueError(_VANISHED)
         with timer.record("gen_conv_inds_sort", _stream()):
             mf, sf = _split_and_sort(mask_fwd, masks, kv, do_sort, alloc)
             mb, sb = _split_and_sort(mask_bwd, masks, kv, do_sort, alloc) if is_train else ([], [])
         return (out_inds, indice_num_per_loc, pair_fwd, pair_bwd, mf, mb, sf, sb, masks)
-    if num_out_act_bound is not None and int(num_out_act_bound) > 0:
-        with timer.record("gen_conv_inds", _stream()):
-            return _conv_rulebook_bounded(geo, indices, n_in, kv, words, int(num_out_act_bound), is_train, do_sort,
-                                          alloc, indice_num_per_loc, masks, bound_status)
+    bound = int(num_out_act_bound) if num_out_act_bound is not None and int(num_out_act_bound) > 0 else 0
     with timer.record("gen_conv_inds", _stream()):
-        return _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks)
+        return _conv_rulebook_all(geo, indices, n_in, kv, words, is_train, do_sort, alloc, indice_num_per_loc, masks,
+                                  bound, bound_status)
 
 
 # ---------------------------------------------------------------------------- GEMM descriptor
@@ -1079,17 +1061,10 @@ def sparse_add_union(indices: Sequence[torch.Tensor], batch_size: int, spatial_s
         return torch.empty((0, ndim + 1), dtype=torch.int32, device=dev), torch.empty((0,), dtype=torch.int32, device=dev)
     ones, zeros = [1] * ndim, [0] * ndim
     geo = _geometry(cat, batch_size, spatial_shape, spatial_shape, ones, ones, zeros, ones, False)
-    lib = _lib()
-    ws = _bytes(lib.spx_rulebook_workspace_size(ctypes.byref(geo), n, 0, 0), dev)
-    m = _conv_stage1(geo, cat, n, ws)
-    out_inds = torch.empty((m, ndim + 1), dtype=torch.int32, device=dev)
-    dst = torch.empty((n,), dtype=torch.int32, device=dev)
-    if m == 0:
-        return out_inds, dst.fill_(-1)
-    pair_fwd = torch.empty((1, m), dtype=torch.int32, device=dev)        # written by stage 2, not read
-    _cabi.check(lib.spx_conv_rulebook_stage2(ctypes.byref(geo), cat.data_ptr(), n, m, out_inds.data_ptr(),
-                                             pair_fwd.data_ptr(), dst.data_ptr(), None, None, ws.data_ptr(),
-                                             ws.numel(), _stream()), "conv_rulebook_stage2(sparse_add)")
+    out_inds, _, pair_bwd, _, _ = _conv_rulebook(geo, cat, n, 1, 1, False, None)
+    dst = pair_bwd[0]
+    if out_inds.shape[0] == 0:
+        dst.fill_(-1)
     return out_inds, dst
 
 

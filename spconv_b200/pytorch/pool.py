@@ -17,7 +17,7 @@ import torch
 from ..core import ConvAlgo
 from . import functional as Fsp
 from . import ops
-from .core import ImplicitGemmIndiceData, IndiceData, SparseConvTensor, expand_nd
+from .core import ImplicitGemmIndiceData, IndiceData, SparseConvTensor, expand_nd, rulebook_num_valid
 from .modules import SparseModule
 
 _MAX_NUM_VOXELS_DURING_TRAINING = "max_num_voxels_during_training"
@@ -42,7 +42,6 @@ class _SparsePool(SparseModule):
         self.record_voxel_count = record_voxel_count
         # as SparseConvolution.num_out_act_bound: bounded implicit-GEMM rulebook, padded output, no host sync
         self.num_out_act_bound: Optional[int] = None
-        self._bound_status: Optional[torch.Tensor] = None
         if record_voxel_count and not subm:
             self.register_buffer(_MAX_NUM_VOXELS_DURING_TRAINING, torch.zeros(1, dtype=torch.int32))
         self.algo = algo
@@ -66,8 +65,6 @@ class _SparsePool(SparseModule):
     def _implicit_rulebook(self, input: SparseConvTensor, out_spatial_shape, indice_dict):
         bounded = (self.num_out_act_bound is not None and self.num_out_act_bound > 0 and not self.subm
                    and self.algo == ConvAlgo.MaskImplicitGemm)
-        if bounded and (self._bound_status is None or self._bound_status.device != input.indices.device):
-            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=input.indices.device)
         with input._timer.namespace("gen_pairs"):
             res = ops.get_indice_pairs_implicit_gemm(
                 input.indices, input.batch_size, input.spatial_shape, self.algo, ksize=self.kernel_size,
@@ -75,31 +72,23 @@ class _SparsePool(SparseModule):
                 out_padding=[0] * self.ndim, subm=self.subm, is_train=(not self.subm) or self.training,
                 alloc=input.thrust_allocator, timer=input._timer,
                 num_out_act_bound=self.num_out_act_bound if bounded else -1,
-                bound_status=self._bound_status if bounded else None)
-        outids, _, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
+                bound_status=self._status_word(input.indices.device) if bounded else None)
         if self.indice_key is not None:
             assert self.indice_key not in indice_dict, \
                 f"your indice key {self.indice_key} already exists in this sparse tensor."
-            indice_dict[self.indice_key] = ImplicitGemmIndiceData(
-                outids, input.indices, pair_fwd, pair_bwd, pair_mask_fwd_splits=mask_fwd,
-                pair_mask_bwd_splits=mask_bwd, mask_argsort_fwd_splits=sort_fwd,
-                mask_argsort_bwd_splits=sort_bwd, masks=masks, is_subm=self.subm,
-                spatial_shape=input.spatial_shape, out_spatial_shape=out_spatial_shape, algo=self.algo,
-                ksize=self.kernel_size, stride=self.stride, dilation=self.dilation, padding=self.padding,
-                in_voxel_num=input.num_valid,
-                out_voxel_num=input.num_valid if self.subm else getattr(outids, "_spx_num_valid", None))
-        return outids, pair_fwd, pair_bwd
+            indice_dict[self.indice_key] = ImplicitGemmIndiceData.from_rulebook(
+                res, input.indices, input.num_valid, self.subm, spatial_shape=input.spatial_shape,
+                out_spatial_shape=out_spatial_shape, algo=self.algo, ksize=self.kernel_size, stride=self.stride,
+                dilation=self.dilation, padding=self.padding)
+        return res[0], res[2], res[3]                       # out_inds, pair_fwd, pair_bwd
 
     def _finish(self, input: SparseConvTensor, out_features, outids, indice_dict, out_spatial_shape):
-        num_valid = input.num_valid if self.subm else getattr(outids, "_spx_num_valid", None)
+        out = input.shadow_copy().replace_feature(out_features)
+        num_valid = rulebook_num_valid(outids, input, out, self.subm, self)
         if not self.subm and self.record_voxel_count and hasattr(self, _MAX_NUM_VOXELS_DURING_TRAINING):
             ops.maximum_value_int_(getattr(self, _MAX_NUM_VOXELS_DURING_TRAINING),
                                    outids.shape[0] if num_valid is None else num_valid)
-        out = input.shadow_copy().replace_feature(out_features)
         out.num_valid = num_valid
-        if num_valid is not None and not self.subm:
-            name = self._sparse_unique_name or self.name or self.indice_key or type(self).__name__
-            out.bound_status = {**(input.bound_status or {}), name: outids._spx_bound_status}
         out.indices = outids
         out.indice_dict = indice_dict
         out.spatial_shape = out_spatial_shape

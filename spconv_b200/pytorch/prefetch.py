@@ -86,13 +86,10 @@ class RulebookPrefetcher:
                         inds, x.batch_size, shape, algo, ksize=m.kernel_size, stride=m.stride, padding=m.padding,
                         dilation=m.dilation, out_padding=m.output_padding, subm=m.subm, transpose=False,
                         is_train=(not m.subm) or self.training)
-                    outids, _, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
                     out_shape = shape if m.subm else ops.get_conv_output_size(shape, m.kernel_size, m.stride,
                                                                              m.padding, m.dilation)
-                    done = ImplicitGemmIndiceData(
-                        outids, inds, pair_fwd, pair_bwd, pair_mask_fwd_splits=mask_fwd, pair_mask_bwd_splits=mask_bwd,
-                        mask_argsort_fwd_splits=sort_fwd, mask_argsort_bwd_splits=sort_bwd, masks=masks,
-                        is_subm=m.subm, spatial_shape=shape, out_spatial_shape=out_shape, algo=algo,
+                    done = ImplicitGemmIndiceData.from_rulebook(
+                        res, inds, None, m.subm, spatial_shape=shape, out_spatial_shape=out_shape, algo=algo,
                         ksize=m.kernel_size, stride=m.stride, dilation=m.dilation, padding=m.padding, prefetched=True)
                     x.indice_dict[m.indice_key] = done
                 elif not done.is_subm and not m.subm:

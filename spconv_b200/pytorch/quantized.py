@@ -113,14 +113,12 @@ class QuantizedSparseConv(SparseConvolution):
                 stride=self.stride, padding=self.padding, dilation=self.dilation, out_padding=self.output_padding,
                 subm=self.subm, transpose=self.transposed, is_train=not self.subm, alloc=input.thrust_allocator,
                 timer=input._timer)
-            outids, _, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = res
+            outids, _, pair_fwd, _, mask_fwd, _, sort_fwd, _, masks = res
             if self.indice_key is not None:
-                indice_dict[self.indice_key] = ImplicitGemmIndiceData(
-                    outids, input.indices, pair_fwd, pair_bwd, pair_mask_fwd_splits=mask_fwd,
-                    pair_mask_bwd_splits=mask_bwd, mask_argsort_fwd_splits=sort_fwd,
-                    mask_argsort_bwd_splits=sort_bwd, masks=masks, is_subm=self.subm,
-                    spatial_shape=input.spatial_shape, out_spatial_shape=out_spatial_shape, algo=self.algo,
-                    ksize=self.kernel_size, stride=self.stride, dilation=self.dilation, padding=self.padding)
+                indice_dict[self.indice_key] = ImplicitGemmIndiceData.from_rulebook(
+                    res, input.indices, None, self.subm, spatial_shape=input.spatial_shape,
+                    out_spatial_shape=out_spatial_shape, algo=self.algo, ksize=self.kernel_size, stride=self.stride,
+                    dilation=self.dilation, padding=self.padding)
         add_scale = 0.0
         add_feats = None
         if add_input is not None:                 # residual enters the epilogue (conv.py:511-512)

@@ -3,8 +3,6 @@ from __future__ import annotations
 
 from typing import Optional
 
-import torch
-
 from . import functional as F
 from .core import SparseConvTensor
 from .modules import SparseModule
@@ -33,13 +31,9 @@ class MaskedRemoveDuplicate(SparseModule):
     def __init__(self, num_out_act_bound: Optional[int] = None, name=None):
         super().__init__(name=name)
         self.num_out_act_bound = num_out_act_bound
-        self._bound_status: Optional[torch.Tensor] = None
 
     def forward(self, x: SparseConvTensor):
         if self.num_out_act_bound is None:
             return F._masked_remove_duplicate(x)
-        dev = x.indices.device
-        if self._bound_status is None or self._bound_status.device != dev:
-            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=dev)
-        return F._masked_remove_duplicate(x, self.num_out_act_bound, self._bound_status,
-                                          self._sparse_unique_name or self.name or type(self).__name__)
+        return F._masked_remove_duplicate(x, self.num_out_act_bound, self._status_word(x.indices.device),
+                                          self._layer_name())

@@ -121,16 +121,12 @@ class MaskedAddTableMisaligned(SparseModule):
     def __init__(self, num_out_act_bound: Optional[int] = None, name=None):
         super().__init__(name=name)
         self.num_out_act_bound = num_out_act_bound
-        self._bound_status: Optional[torch.Tensor] = None
 
     def forward(self, input: List[SparseConvTensor]):
         if self.num_out_act_bound is None:
             return F._masked_sparse_add(input)
-        dev = input[0].indices.device
-        if self._bound_status is None or self._bound_status.device != dev:
-            self._bound_status = torch.zeros((1,), dtype=torch.int32, device=dev)
-        return F._masked_sparse_add(input, self.num_out_act_bound, self._bound_status,
-                                    self._sparse_unique_name or self.name or type(self).__name__)
+        return F._masked_sparse_add(input, self.num_out_act_bound, self._status_word(input[0].indices.device),
+                                    self._layer_name())
 
     def input_spatial_size(self, out_size):
         return out_size
