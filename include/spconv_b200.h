@@ -37,6 +37,8 @@
  *        <- functional.sparse_add / sparse_add_hash_based spconv/pytorch/functional.py:441-544
  *   spx_sparse_add_union / spx_masked_sparse_add_plan / _heads (+ _group / _fwd / _gather)
  *        <- no counterpart: functional.masked_sparse_add / masked_remove_duplicate (padded operands, no read-back)
+ *   spx_point_scatter_group / _fwd / _bwd (+ spx_sparse_add_gather for the sum's backward)
+ *        <- no counterpart: PointVoxelScatter (per-voxel max / mean / sum of point features, no read-back)
  *   spx_hash_clear / _insert / _query / _insert_exist / _rank
  *        <- HashTable (spconv/pytorch/hash.py)        spconv/csrc/hash/core.py
  *
@@ -523,6 +525,40 @@ int spx_masked_sparse_add_plan(const spx_conv_geometry *g, const spx_sparse_add_
                                int32_t *status, void *workspace, size_t workspace_bytes, spx_stream_t stream);
 int spx_masked_sparse_add_heads(const int32_t *order, const int32_t *offsets, const int32_t *num_out, int64_t bound,
                                 int64_t rows, int32_t *heads, int32_t *inverse, spx_stream_t stream);
+
+/* ------------------------------------------------------------------ point -> voxel reductions */
+
+/*
+ * Per-row reductions of point features x [num_points, channels] (PointVoxelScatter: the scatter of a dynamic
+ * VFE), with no host read-back.  ids [num_points] (id_bytes 4: int32, 8: int64; e.g. the pc_voxel_id of
+ * spx_point2voxel_bounded) give every point's output row; a point whose id is outside [0, rows) is dropped.
+ *   group: row32 [num_points] = the id, or -1 for a dropped point; order [num_points] and offsets [rows + 1] as
+ *          spx_sparse_add_group: the points of row r are order[offsets[r] .. offsets[r+1]) in ascending point
+ *          index, dropped points last.  rows may exceed num_points; num_points == 0 gives rows + 1 zero offsets.
+ *          workspace: spx_point_scatter_group_workspace_size(num_points) bytes.
+ *   fwd:   out [rows, channels]; a row without points gives 0 and every element is written:
+ *          mode 0 max:  out[r, c] = x[a, c] bit for bit, a = argmax[r, c] ([rows, channels] int32, -1 on an empty
+ *                       row) the first point in ascending order that attains the maximum; a NaN counts as the
+ *                       maximum, -0 and +0 tie;
+ *          mode 1 mean: the fp32 sum of the row's points in ascending order divided by their count, rounded once;
+ *          mode 2 sum:  the fp32 sum in ascending order, rounded once (the kernel of spx_sparse_add_fwd).
+ *   bwd:   dx [num_points, channels], every element written once, 0 for a dropped point:
+ *          mode 0 dx[p, c] = dy[r, c] where argmax[r, c] == p, else 0;  mode 1 dy[r, c] / count[r] in fp32,
+ *          rounded once (count [rows] int32 = offsets[r+1] - offsets[r]);  mode 2 dy[r, c]
+ *          (spx_sparse_add_gather with index = row32).
+ * No float atomics: every result is bit-reproducible and independent of the dropped points, wherever they sit.
+ * dtype: f32 / f16 / bf16, any channels >= 1 (16-byte vectors when the row size and pointers allow them).
+ * num_points and rows below 2^31 - 1.
+ */
+size_t spx_point_scatter_group_workspace_size(int64_t num_points);
+int spx_point_scatter_group(const void *ids, int id_bytes, int64_t num_points, int64_t rows, int32_t *row32,
+                            int32_t *order, int32_t *offsets, void *workspace, size_t workspace_bytes,
+                            spx_stream_t stream);
+int spx_point_scatter_fwd(int mode, const void *x, int64_t num_points, int channels, int dtype, const int32_t *order,
+                          const int32_t *offsets, int64_t rows, void *out, int32_t *argmax, spx_stream_t stream);
+int spx_point_scatter_bwd(int mode, const void *dy, const int32_t *row32, int64_t num_points, int64_t rows,
+                          int channels, int dtype, const int32_t *argmax, const int32_t *count, void *dx,
+                          spx_stream_t stream);
 
 /* ------------------------------------------------------------------ padding-aware BatchNorm */
 

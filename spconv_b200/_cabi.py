@@ -167,6 +167,13 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_masked_sparse_add_heads": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p,
                                             c_void_p]),
+    "spx_point_scatter_group_workspace_size": (c_size_t, [c_int64]),
+    "spx_point_scatter_group": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_size_t, c_void_p]),
+    "spx_point_scatter_fwd": (c_int, [c_int, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p,
+                                      c_void_p, c_void_p]),
+    "spx_point_scatter_bwd": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
     "spx_masked_bn_fwd_train_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_masked_bn_fwd_train": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_float, c_void_p,

@@ -106,6 +106,18 @@ template <> __device__ __forceinline__ float from_float<float>(float v) { return
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
+// The max rule of the global pool and the point scatter: does (v, r) beat (bv, br)?  r < 0 marks an empty side.
+// A NaN beats every number, then the greater value, then, on equality (-0 == +0), the lower row: a total order
+// whose winner is the first row in ascending order that attains the maximum (np.argmax).
+__device__ __forceinline__ bool max_beats(float v, int r, float bv, int br) {
+    if (r < 0) return false;
+    if (br < 0) return true;
+    const bool n = isnan(v), bn = isnan(bv);
+    if (n != bn) return n;
+    if (!n && v != bv) return v > bv;
+    return r < br;
+}
+
 __device__ __forceinline__ float apply_act(float v, int act, float alpha) {
     // InferenceOps activations: spconv/csrc/sparse/inference.py:26-146
     switch (act) {

@@ -14,7 +14,7 @@
 //              order, then the lanes merge in a fixed binary tree; the partial goes to workspace [chunk][C];
 //   finalize : per (sample, channel) 32 lanes merge the sample's chunks p, p + 32, ... in order, then a fixed
 //              tree; writes out, and argmax [B, C] (max) or count [B] (mean) for the backward.
-// Max partials are (value, row) pairs ordered by gp_beats: a NaN beats every number, then the greater value,
+// Max partials are (value, row) pairs ordered by max_beats: a NaN beats every number, then the greater value,
 // then, on equality (-0 == +0), the lower row; that is a total order, so the winner is the first row in
 // ascending order that attains the maximum (np.argmax).  out is copied from x[argmax] bit for bit.
 // Mean partials are fp32 sums; out = sum / count, rounded once.
@@ -41,16 +41,6 @@ __device__ __forceinline__ int64_t gp_valid_rows(const int32_t *num_valid, int64
     if (num_valid == nullptr) return rows;
     const int64_t m = __ldg(num_valid);
     return m < 0 ? 0 : (m > rows ? rows : m);
-}
-
-// does (v, r) beat (bv, br)?  r < 0 marks an empty side.
-__device__ __forceinline__ bool gp_beats(float v, int r, float bv, int br) {
-    if (r < 0) return false;
-    if (br < 0) return true;
-    const bool n = isnan(v), bn = isnan(bv);
-    if (n != bn) return n;
-    if (!n && v != bv) return v > bv;
-    return r < br;
 }
 
 template <typename T, int W> __device__ __forceinline__ void gp_load(const T *p, float (&f)[W]) {
@@ -180,7 +170,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
             for (int j = 0; j < W; ++j) {
                 if constexpr (MEAN) {
                     acc[j] += f[j];
-                } else if (gp_beats(f[j], r, acc[j], arg[j])) {
+                } else if (max_beats(f[j], r, acc[j], arg[j])) {
                     acc[j] = f[j];
                     arg[j] = r;
                 }
@@ -219,7 +209,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
             for (int j = 0; j < W; ++j) {
                 if constexpr (MEAN) {
                     s_v[slot * W + j] = acc[j] = acc[j] + s_v[o * W + j];
-                } else if (gp_beats(s_v[o * W + j], s_r[o * W + j], acc[j], arg[j])) {
+                } else if (max_beats(s_v[o * W + j], s_r[o * W + j], acc[j], arg[j])) {
                     s_v[slot * W + j] = acc[j] = s_v[o * W + j];
                     s_r[slot * W + j] = arg[j] = s_r[o * W + j];
                 }
@@ -251,7 +241,7 @@ gp_finalize_kernel(const T *__restrict__ x, const float2 *__restrict__ partials,
         for (int32_t k = k0 + pl; k < k1; k += GP_FIN_LANES) {
             const float2 p = partials[(int64_t)k * channels + c];
             if constexpr (MEAN) acc += p.x;
-            else if (gp_beats(p.x, __float_as_int(p.y), acc, arg)) { acc = p.x; arg = __float_as_int(p.y); }
+            else if (max_beats(p.x, __float_as_int(p.y), acc, arg)) { acc = p.x; arg = __float_as_int(p.y); }
         }
     s_v[pl][cl] = acc;
     s_r[pl][cl] = arg;
@@ -260,7 +250,7 @@ gp_finalize_kernel(const T *__restrict__ x, const float2 *__restrict__ partials,
         if (pl < s) {
             if constexpr (MEAN) {
                 s_v[pl][cl] = acc = acc + s_v[pl + s][cl];
-            } else if (gp_beats(s_v[pl + s][cl], s_r[pl + s][cl], acc, arg)) {
+            } else if (max_beats(s_v[pl + s][cl], s_r[pl + s][cl], acc, arg)) {
                 s_v[pl][cl] = acc = s_v[pl + s][cl];
                 s_r[pl][cl] = arg = s_r[pl + s][cl];
             }

@@ -281,19 +281,19 @@ extern "C" size_t spx_sparse_add_group_workspace_size(int64_t rows) {
     return align_up((size_t)rows * 4, 256) + radix_argsort_workspace_bytes(rows) + 1024;
 }
 
-extern "C" int spx_sparse_add_group(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets,
-                                    void *workspace, size_t workspace_bytes, spx_stream_t stream_) {
-    SPX_REQUIRE(rows >= 0 && rows < 2147483647ll, "sparse_add_group: bad row count %lld", (long long)rows);
-    SPX_REQUIRE(M >= 0 && M <= rows, "sparse_add_group: output count %lld not in [0, %lld]", (long long)M, (long long)rows);
-    SPX_REQUIRE(offsets != nullptr, "sparse_add_group: offsets is NULL");
-    cudaStream_t stream = (cudaStream_t)stream_;
+namespace spx {
+// The grouping of spx_sparse_add_group and spx_point_scatter_group: order [rows] and offsets [M + 1] of dst [rows].
+// M may exceed rows here; with rows == 0 all M + 1 offsets are 0.  0 <= rows < 2^31 - 1, 0 <= M < 2^31 - 1.
+int group_rows(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets, void *workspace,
+               size_t workspace_bytes, cudaStream_t stream, const char *who) {
+    SPX_REQUIRE(offsets != nullptr, "%s: offsets is NULL", who);
     if (rows == 0) {
-        SPX_CHECK_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int32_t), stream));
+        SPX_CHECK_CUDA(cudaMemsetAsync(offsets, 0, (size_t)(M + 1) * sizeof(int32_t), stream));
         return 0;
     }
-    SPX_REQUIRE(dst && order && workspace, "sparse_add_group: NULL pointer argument");
+    SPX_REQUIRE(dst && order && workspace, "%s: NULL pointer argument", who);
     SPX_REQUIRE(workspace_bytes >= spx_sparse_add_group_workspace_size(rows),
-                "sparse_add_group: workspace too small: need %zu, have %zu", spx_sparse_add_group_workspace_size(rows),
+                "%s: workspace too small: need %zu, have %zu", who, spx_sparse_add_group_workspace_size(rows),
                 workspace_bytes);
     WorkspaceCarver ws(workspace, workspace_bytes);
     uint32_t *keys = ws.take<uint32_t>((size_t)rows);
@@ -311,6 +311,37 @@ extern "C" int spx_sparse_add_group(const int32_t *dst, int64_t rows, int64_t M,
     return 0;
 }
 
+static int sum_dtype(const SaOperands &ops, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
+                     int dtype, void *out, cudaStream_t stream) {
+    switch (dtype) {
+        case SPX_F32: return dispatch_sum<float>(ops, order, offsets, M, channels, out, stream);
+        case SPX_F16: return dispatch_sum<__half>(ops, order, offsets, M, channels, out, stream);
+        case SPX_BF16: return dispatch_sum<__nv_bfloat16>(ops, order, offsets, M, channels, out, stream);
+    }
+    return 2;
+}
+
+// The sum of spx_point_scatter_fwd: one operand x [rows, channels] and M segments, M may exceed rows.  The caller
+// has checked every argument.
+int sum_segments(const void *x, int64_t rows, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
+                 int dtype, void *out, cudaStream_t stream) {
+    SaOperands ops;
+    memset(&ops, 0, sizeof(ops));
+    ops.count = 1;
+    ops.features[0] = x;
+    ops.start[1] = rows;
+    return sum_dtype(ops, order, offsets, M, channels, dtype, out, stream);
+}
+}  // namespace spx
+
+extern "C" int spx_sparse_add_group(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets,
+                                    void *workspace, size_t workspace_bytes, spx_stream_t stream_) {
+    SPX_REQUIRE(rows >= 0 && rows < 2147483647ll, "sparse_add_group: bad row count %lld", (long long)rows);
+    SPX_REQUIRE(M >= 0 && M <= rows, "sparse_add_group: output count %lld not in [0, %lld]", (long long)M, (long long)rows);
+    return group_rows(dst, rows, M, order, offsets, workspace, workspace_bytes, (cudaStream_t)stream_,
+                      "sparse_add_group");
+}
+
 extern "C" int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const int32_t *order, const int32_t *offsets,
                                   int64_t M, int channels, int dtype, void *out, spx_stream_t stream_) {
     SaOperands ops;
@@ -320,13 +351,7 @@ extern "C" int spx_sparse_add_fwd(const spx_sparse_add_operands *operands, const
     SPX_REQUIRE(M >= 0 && M <= total, "sparse_add_fwd: output count %lld not in [0, %lld]", (long long)M, (long long)total);
     if (M == 0) return 0;
     SPX_REQUIRE(order && offsets && out, "sparse_add_fwd: NULL pointer argument");
-    cudaStream_t stream = (cudaStream_t)stream_;
-    switch (dtype) {
-        case SPX_F32: return dispatch_sum<float>(ops, order, offsets, M, channels, out, stream);
-        case SPX_F16: return dispatch_sum<__half>(ops, order, offsets, M, channels, out, stream);
-        case SPX_BF16: return dispatch_sum<__nv_bfloat16>(ops, order, offsets, M, channels, out, stream);
-    }
-    return 2;
+    return sum_dtype(ops, order, offsets, M, channels, dtype, out, (cudaStream_t)stream_);
 }
 
 extern "C" int spx_sparse_add_gather(const int32_t *index, const void *src, int64_t src_rows,

@@ -480,3 +480,26 @@ class MaskedGlobalPoolFunction(Function):
 
 
 masked_global_pool = MaskedGlobalPoolFunction.apply
+
+
+# ---------------------------------------------------------------------------- point -> voxel reductions
+class PointScatterFunction(Function):
+    """``x, row32, order, offsets, count, mode`` -> ``[rows, C]``: per-row max, mean or sum of the points
+    (:func:`ops.point_scatter_fwd`).  The backward gives ``x``'s gradient: ``dy`` at the argmax point (max),
+    ``dy / count`` (mean) or ``dy`` (sum) on the row's points, 0 on dropped points."""
+
+    @staticmethod
+    def forward(ctx, x, row32, order, offsets, count, mode):
+        out, argmax = ops.point_scatter_fwd(x, order, offsets, mode)
+        ctx.save_for_backward(row32, argmax if mode == "max" else (count if mode == "mean" else None))
+        ctx.mode = mode
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        row32, aux = ctx.saved_tensors
+        return ops.point_scatter_bwd(grad_output, row32, aux, ctx.mode), None, None, None, None, None
+
+
+point_scatter = PointScatterFunction.apply

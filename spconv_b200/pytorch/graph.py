@@ -15,8 +15,10 @@ modules, ``SparseGlobalMaxPool`` / ``SparseGlobalAvgPool`` read the per-sample c
 ``AddTableMisaligned`` / ``functional.sparse_add`` read the size of the union back: ``MaskedAddTableMisaligned``
 (``functional.masked_sparse_add``), ``MaskedRemoveDuplicate``, ``MaskedAddTable`` and ``MaskedJoinTable`` take
 padded tensors and capture.  In front of the first layer, ``PointToVoxel`` reads each cloud's voxel count back:
-``MaskedPointToVoxel`` voxelises a padded batch of clouds with the count on the device and captures, and
-``gather_features_by_pc_voxel_id`` (the per-point read-out) does not synchronise.
+``MaskedPointToVoxel`` voxelises a padded batch of clouds with the count on the device and captures,
+``PointVoxelScatter`` (a dynamic VFE's per-voxel max / mean / sum of point features, in place of
+``torch.unique`` + scatter) captures, and ``gather_features_by_pc_voxel_id`` (the per-point read-out) does not
+synchronise.
 """
 from __future__ import annotations
 

@@ -1191,6 +1191,72 @@ def masked_sparse_add_heads(order: torch.Tensor, offsets: torch.Tensor, num_out:
     return heads, inverse
 
 
+# ---------------------------------------------------------------------------- point -> voxel reductions
+POINT_SCATTER_MODES = {"max": 0, "mean": 1, "sum": 2}
+
+
+def point_scatter_group(ids: torch.Tensor, rows: int):
+    """``(row32 [P], order [P], offsets [rows + 1])`` of the int32 / int64 ids ``[P]`` (``spx_point_scatter_group``):
+    ``row32[p]`` is the id, or -1 when it is outside ``[0, rows)`` (the point is dropped); the points of row ``r``
+    are ``order[offsets[r]:offsets[r + 1]]`` in ascending point index.  No host synchronisation."""
+    _require_cuda(ids, "pc_voxel_id")
+    if ids.dim() != 1 or ids.dtype not in (torch.int32, torch.int64):
+        raise RuntimeError(f"point scatter: the ids must be an int32 or int64 vector [P], got {ids.dtype} "
+                           f"{tuple(ids.shape)}")
+    ids = ids.contiguous()
+    n, rows = ids.shape[0], int(rows)
+    row32 = torch.empty((n,), dtype=torch.int32, device=ids.device)
+    order = torch.empty((n,), dtype=torch.int32, device=ids.device)
+    offsets = torch.empty((rows + 1,), dtype=torch.int32, device=ids.device)
+    lib = _lib()
+    ws = _bytes(lib.spx_point_scatter_group_workspace_size(n), ids.device)
+    _cabi.check(lib.spx_point_scatter_group(_ptr(ids), ids.element_size(), n, rows, _ptr(row32), _ptr(order),
+                                            offsets.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+                "point_scatter_group")
+    return row32, order, offsets
+
+
+def _point_scatter_dtype(x: torch.Tensor) -> int:
+    if x.dtype not in _GLOBAL_POOL_DTYPES:
+        raise RuntimeError(f"PointVoxelScatter supports float32, float16 and bfloat16 features, got {x.dtype}")
+    return _DTYPE_CODE[x.dtype]
+
+
+def point_scatter_fwd(x: torch.Tensor, order: torch.Tensor, offsets: torch.Tensor, mode: str):
+    """``(out [rows, C], argmax)`` of the points ``x [P, C]`` grouped by :func:`point_scatter_group`: per row the max
+    (``argmax [rows, C]`` int32: the first point that attains it, a NaN counting as the maximum; bit copy), the
+    mean (fp32 sum in ascending point order / count, rounded once) or the sum (fp32, rounded once).  ``argmax``
+    is None unless ``mode`` is ``"max"``.  A row without points gives 0 (argmax -1)."""
+    code = _point_scatter_dtype(x)
+    _require_cuda(x, "features")
+    if x.dim() != 2 or x.shape[0] != order.shape[0]:
+        raise RuntimeError(f"point scatter: features must be [{order.shape[0]}, C], got {tuple(x.shape)}")
+    x = x.contiguous()
+    n, c = x.shape
+    rows = offsets.shape[0] - 1
+    out = torch.empty((rows, c), dtype=x.dtype, device=x.device)
+    argmax = torch.empty((rows, c), dtype=torch.int32, device=x.device) if mode == "max" else None
+    _cabi.check(_lib().spx_point_scatter_fwd(POINT_SCATTER_MODES[mode], _ptr(x), n, c, code, _ptr(order),
+                                             offsets.data_ptr(), rows, _ptr(out), _ptr(argmax), _stream()),
+                "point_scatter_fwd")
+    return out, argmax
+
+
+def point_scatter_bwd(dy: torch.Tensor, row32: torch.Tensor, aux: Optional[torch.Tensor], mode: str) -> torch.Tensor:
+    """``dx [P, C]`` of :func:`point_scatter_fwd`: ``dy[r]`` at the argmax point (max), ``dy[r] / count[r]`` (mean,
+    ``aux`` = count) or ``dy[r]`` (sum) on every point of row ``r``; 0 for dropped points."""
+    code = _point_scatter_dtype(dy)
+    dy = dy.contiguous()
+    n = row32.shape[0]
+    rows, c = dy.shape
+    dx = torch.empty((n, c), dtype=dy.dtype, device=dy.device)
+    _cabi.check(_lib().spx_point_scatter_bwd(POINT_SCATTER_MODES[mode], _ptr(dy), _ptr(row32), n, rows, c, code,
+                                             _ptr(aux) if mode == "max" else None,
+                                             _ptr(aux) if mode == "mean" else None, _ptr(dx), _stream()),
+                "point_scatter_bwd")
+    return dx
+
+
 # ---------------------------------------------------------------------------- misc
 def bias_add_act_inplace(x: torch.Tensor, bias: Optional[torch.Tensor], act_type=Activation.None_,
                          act_alpha: float = 0.0, act_beta: float = 0.0) -> torch.Tensor:

@@ -1,5 +1,6 @@
 """Point cloud -> voxel front end (``spconv/pytorch/utils.py:23-176``): ``PointToVoxel`` and
-``gather_features_by_pc_voxel_id``.  CUDA only; the kernels live in ``csrc/pointops.cu``.
+``gather_features_by_pc_voxel_id``, plus ``MaskedPointToVoxel`` and ``PointVoxelScatter``.  CUDA only; the
+kernels live in ``csrc/pointops.cu`` and ``csrc/point_scatter.cu``.
 
 Unlike the reference's GPU generator (atomic appends: voxel order and the points kept per voxel
 depend on scheduling) the result is deterministic and equal to the reference's CPU generator
@@ -17,6 +18,8 @@ import numpy as np
 import torch
 
 from .. import _cabi
+from . import functional as Fsp
+from . import ops
 
 
 def calc_point2voxel_meta_data(vsize_xyz: List[float], coors_range_xyz: List[float]):
@@ -134,6 +137,9 @@ class MaskedPointToVoxel(object):
         x = spconv.SparseConvTensor(feats, indices, gen.grid_size, gen.batch_size)
         x.num_valid = num_valid
 
+    A dynamic VFE, which reduces every point of a voxel rather than the first ``max_num_points_per_voxel``, uses
+    ``pc_voxel_id`` with :class:`PointVoxelScatter` instead (see its docstring).
+
     At most ``SPX_P2V_MAX_BATCH`` (65536) samples; P and the bound below 2^31 - 1.  CUDA only.
     """
 
@@ -200,6 +206,66 @@ class MaskedPointToVoxel(object):
                 pc_voxel_id.data_ptr() if n else None, self.num_valid.data_ptr(), self._bound_status.data_ptr(),
                 ws.data_ptr(), ws.numel(), stream), "point2voxel_bounded")
         return self.voxels, self.indices, self.num_per_voxel, pc_voxel_id, self.num_valid
+
+
+class PointVoxelScatter(object):
+    """Per-voxel max / mean / sum of point features, in CUDA (``csrc/point_scatter.cu``) with no host read-back: the
+    point -> voxel reduction of a dynamic VFE (OpenPCDet's ``DynamicVoxelVFE`` / ``DynamicPillarVFE``), which keeps
+    every point of a voxel.
+
+    ``scatter = PointVoxelScatter(pc_voxel_id, num_rows)`` groups the points once: point ``p`` belongs to output row
+    ``pc_voxel_id[p]`` (int32 or int64 ``[P]``, e.g. from :class:`MaskedPointToVoxel`, which sets it for every point
+    of a kept voxel, including those beyond ``max_num_points_per_voxel``); a point whose id is outside
+    ``[0, num_rows)`` (-1, padding, dropped voxels) is dropped.  Every reduction over the same ids then reuses the
+    one sort:
+
+    * ``scatter.max(x)``, ``scatter.mean(x)``, ``scatter.sum(x)``: ``[num_rows, C]`` from ``x [P, C]``,
+      differentiable in ``x``.  ``sum`` adds a row's points in fp32 in ascending point index and rounds once;
+      ``mean`` divides that sum by the count in fp32 and rounds once.  ``max`` returns the value of the first point
+      (in point order) that attains the maximum, bit for bit; a NaN counts as the maximum and -0 / +0 tie.  Its
+      gradient goes to that one point per row and channel, as ``torch.max(dim)``'s does (not to a thread-timing
+      winner, as ``torch_scatter.scatter_max``, nor split between ties, as ``scatter_reduce("amax")``).  The mean's
+      gradient is ``dy / count``, the sum's ``dy``.  A row without points gives 0; dropped points get a zero
+      gradient.
+    * ``scatter.count``: int32 ``[num_rows]``, the number of points of every row (not capped by
+      ``max_num_points_per_voxel``).
+
+    No float atomics: results are bit-reproducible and do not depend on dropped points, wherever they sit.  Nothing
+    is read back to the host, so a step captures as one CUDA graph.  float32, float16 and bfloat16 features; P and
+    ``num_rows`` below 2^31 - 1.  CUDA only.
+
+    A dynamic-VFE front end (``max_num_points_per_voxel`` only caps the ``voxels`` buffer and may be 1)::
+
+        gen = spconv.MaskedPointToVoxel(vsize, coors_range, 4, max_voxels, 1, batch_size)
+        voxels, indices, num_per_voxel, pc_voxel_id, num_valid = gen(points, offsets)
+        scatter = spconv.PointVoxelScatter(pc_voxel_id, gen.max_num_voxels_total)
+        xyz_mean = scatter.mean(points[:, :3])
+        f_cluster = points[:, :3] - spconv.gather_features_by_pc_voxel_id(xyz_mean, pc_voxel_id)
+        feats = scatter.max(pfn(torch.cat([points, f_cluster], 1)))   # per-point layers, then the voxel max
+        x = spconv.SparseConvTensor(feats, indices, gen.grid_size, gen.batch_size)
+        x.num_valid = num_valid
+    """
+
+    def __init__(self, pc_voxel_id: torch.Tensor, num_rows: int):
+        if int(num_rows) < 0 or int(num_rows) >= 2 ** 31 - 1:
+            raise ValueError(f"PointVoxelScatter: num_rows {num_rows} not in [0, 2^31 - 2]")
+        self.num_rows = int(num_rows)
+        self.row32, self.order, self.offsets = ops.point_scatter_group(pc_voxel_id, self.num_rows)
+        self.count = self.offsets.diff()
+
+    def _reduce(self, x: torch.Tensor, mode: str) -> torch.Tensor:
+        ops._point_scatter_dtype(x)
+        ops._require_cuda(x, "features")
+        return Fsp.point_scatter(x, self.row32, self.order, self.offsets, self.count, mode)
+
+    def max(self, x: torch.Tensor) -> torch.Tensor:
+        return self._reduce(x, "max")
+
+    def mean(self, x: torch.Tensor) -> torch.Tensor:
+        return self._reduce(x, "mean")
+
+    def sum(self, x: torch.Tensor) -> torch.Tensor:
+        return self._reduce(x, "sum")
 
 
 def gather_features_by_pc_voxel_id(seg_res_features: torch.Tensor, pc_voxel_id: torch.Tensor,
