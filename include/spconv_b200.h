@@ -41,6 +41,8 @@
  *        <- no counterpart: PointVoxelScatter (per-voxel max / mean / sum of point features, no read-back)
  *   spx_hash_clear / _insert / _query / _insert_exist / _rank
  *        <- HashTable (spconv/pytorch/hash.py)        spconv/csrc/hash/core.py
+ *   spx_depthwise_fwd / _dgrad / _wgrad (+ _wgrad_workspace_size)
+ *        <- no counterpart: the conv modules with groups = in_channels = out_channels (the reference refuses groups)
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless the name ends in `_host`;
@@ -559,6 +561,39 @@ int spx_point_scatter_fwd(int mode, const void *x, int64_t num_points, int chann
 int spx_point_scatter_bwd(int mode, const void *dy, const int32_t *row32, int64_t num_points, int64_t rows,
                           int channels, int dtype, const int32_t *argmax, const int32_t *count, void *dx,
                           spx_stream_t stream);
+
+/* ------------------------------------------------------------------ depthwise convolution */
+
+/*
+ * Depthwise sparse convolution (groups = in_channels = out_channels = channels) on a dense rulebook table
+ * T [kv, rows] int32 (row stride table_stride >= rows, -1 = no pair): pair_fwd / pair_bwd of the masked
+ * implicit-GEMM rulebooks, or the tables of spx_pairs_to_table for ConvAlgo.Native.  weight is KRSC with one input
+ * channel per group, [channels, kv], read as given.  Kernel offsets are visited in ascending k; every sum is fp32
+ * from +0, rounded once to dtype; no float atomics, so every result is bit-reproducible.
+ *   fwd:   out[o, c] = act(sum_k W[c, k] * x[T[k][o], c] + bias[c]) for o < n_out; bias may be NULL, act is
+ *          SPX_ACT_NONE / RELU / SIGMOID / LEAKY_RELU (alpha = act_alpha).
+ *   dgrad: din[i, c] = sum_k W[c, k] * dy[T[k'][i], c] for i < n_in, every row written once; k' = k (pair_bwd),
+ *          or k' = kv - 1 - k with reverse_offsets != 0 (SubM: T is pair_fwd, whose mirrored offset gives pair_bwd).
+ *   wgrad: dweight[c, k] = sum over o < n_out with T[k][o] >= 0 of dy[o, c] * x[T[k][o], c]: per chunk of 512 rows
+ *          a fixed fold (ascending rows per lane, then a binary tree over lanes) into the workspace, then the
+ *          chunks in ascending order.  Depends on the row indices alone: trailing rows without pairs or with
+ *          dy = 0 leave it unchanged bit for bit.  n_out = 0 writes dweight = 0.
+ *          workspace: spx_depthwise_wgrad_workspace_size(n_out, kv, channels) bytes (may be 0).
+ * The gathered operand (features, out_bp; features in wgrad) is only read through table entries >= 0 and may be
+ * NULL when it has no rows.
+ * dtype: f32 / f16 / bf16.  kv in [1, 4096], channels in [1, 2^20], rows below 2^31 - 1.  Rows move as 16-byte
+ * vectors when channels * element size is a multiple of 16 and the feature pointers are 16-byte aligned, else
+ * one element per thread.
+ */
+int spx_depthwise_fwd(const void *features, const void *weight, const void *bias, void *out, const int32_t *table,
+                      int64_t table_stride, int kv, int64_t n_out, int channels, int dtype, int act, float act_alpha,
+                      spx_stream_t stream);
+int spx_depthwise_dgrad(const void *out_bp, const void *weight, void *din, const int32_t *table, int64_t table_stride,
+                        int kv, int64_t n_in, int channels, int dtype, int reverse_offsets, spx_stream_t stream);
+size_t spx_depthwise_wgrad_workspace_size(int64_t n_out, int kv, int channels);
+int spx_depthwise_wgrad(const void *features, const void *out_bp, void *dweight, const int32_t *table,
+                        int64_t table_stride, int kv, int64_t n_out, int channels, int dtype, void *workspace,
+                        size_t workspace_bytes, spx_stream_t stream);
 
 /* ------------------------------------------------------------------ padding-aware BatchNorm */
 

@@ -174,6 +174,13 @@ SIGNATURES = {
                                       c_void_p, c_void_p]),
     "spx_point_scatter_bwd": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
+    "spx_depthwise_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int,
+                                  c_int, c_int, c_float, c_void_p]),
+    "spx_depthwise_dgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int,
+                                    c_int, c_void_p]),
+    "spx_depthwise_wgrad_workspace_size": (c_size_t, [c_int64, c_int, c_int]),
+    "spx_depthwise_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int,
+                                    c_void_p, c_size_t, c_void_p]),
     "spx_masked_bn_fwd_train_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_masked_bn_fwd_train": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_float, c_void_p,

@@ -57,7 +57,10 @@ class SparseConvolution(SparseModule):
                  act_beta: float = 0, large_kernel_fast_algo: bool = False,
                  name=None, device=None, dtype=None):
         super().__init__(name=name)
-        assert groups == 1, "don't support groups for now"
+        # groups: 1, or depthwise (groups == in_channels == out_channels > 1); general groups are not supported
+        assert groups == 1 or (groups > 1 and groups == in_channels == out_channels), \
+            f"groups must be 1 or in_channels == out_channels (depthwise), got groups={groups} for " \
+            f"{in_channels} -> {out_channels} channels"
         self.ndim = ndim
         self.in_channels = in_channels
         self.out_channels = out_channels
@@ -67,6 +70,7 @@ class SparseConvolution(SparseModule):
         self.padding = expand_nd(ndim, padding)
         self.output_padding = expand_nd(ndim, output_padding)
         self.groups = groups
+        self.depthwise = groups > 1
         self.subm = subm
         self.transposed = transposed
         self.inverse = inverse
@@ -91,7 +95,7 @@ class SparseConvolution(SparseModule):
             algo = (ConvAlgo.MaskImplicitGemm if kv <= (128 if large_kernel_fast_algo else 32)
                     else ConvAlgo.Native)
         self.algo = algo
-        self.weight_shape = [out_channels, *self.kernel_size, in_channels]
+        self.weight_shape = [out_channels, *self.kernel_size, in_channels // groups]
         factory = {"device": device, "dtype": dtype}
         self.weight = Parameter(torch.empty(*self.weight_shape, **factory))
         if bias:
@@ -137,8 +141,8 @@ class SparseConvolution(SparseModule):
 
     # ------------------------------------------------------------------ parameters
     def reset_parameters(self):
-        """kaiming-uniform(a=sqrt(5)) on fan_in = C * kv, bias U(+-1/sqrt(fan_in))."""
-        fan_in = self.in_channels * int(np.prod(self.kernel_size))
+        """kaiming-uniform(a=sqrt(5)) on fan_in = (C / groups) * kv, bias U(+-1/sqrt(fan_in))."""
+        fan_in = self.in_channels // self.groups * int(np.prod(self.kernel_size))
         gain = math.sqrt(2.0 / (1 + 5.0))
         bound = gain * math.sqrt(3.0 / fan_in)
         with torch.no_grad():
@@ -156,6 +160,8 @@ class SparseConvolution(SparseModule):
             parts.append(f"dilation={self.dilation}")
         if self.output_padding != [0] * self.ndim:
             parts.append(f"output_padding={self.output_padding}")
+        if self.groups != 1:
+            parts.append(f"groups={self.groups}")
         if self.bias is None:
             parts.append("bias=False")
         parts.append(f"algo={self.algo}")
@@ -212,6 +218,20 @@ class SparseConvolution(SparseModule):
                              "please check Inverse Convolution in docs/USAGE.md.")
 
     # ------------------------------------------------------------------ forward
+    def _depthwise_native(self, features, weight, indice_pairs, indice_pair_num, n_out, timer, bias, act_alpha,
+                          act_type):
+        """Depthwise conv on ConvAlgo.Native compact pairs: scattered into the dense tables the kernels walk (the
+        backward table only when a gradient can flow; SubM mirrors the forward table instead)."""
+        kv = int(indice_pairs.shape[1])
+        need_bwd = (not self.subm and torch.is_grad_enabled()
+                    and (features.requires_grad or weight.requires_grad))
+        with timer.record("depthwise_conv_table", ops._stream()):
+            t_fwd, _, t_bwd, _ = ops._native_tables(indice_pairs.contiguous(), indice_pair_num, features.shape[0],
+                                                    int(n_out), kv, self.subm, self.inverse, True, need_bwd)
+        if not self.subm and t_bwd is None:
+            t_bwd = torch.empty((kv, 0), dtype=torch.int32, device=features.device)     # no backward will run
+        return Fsp.depthwise_conv(features, weight, t_fwd, t_bwd, n_out, timer, bias, act_alpha, act_type)
+
     def forward(self, input: SparseConvTensor, add_input: Optional[SparseConvTensor] = None):
         return self._conv_forward(self.training, input, self.weight, self.bias, add_input,
                                   name=self.name, sparse_unique_name=self._sparse_unique_name,
@@ -258,8 +278,11 @@ class SparseConvolution(SparseModule):
         num_valid = input.num_valid
 
         if self.conv1x1:
-            w2d = weight.view(self.out_channels, self.in_channels)
-            feats = torch.mm(features, w2d.t())
+            if self.depthwise:
+                feats = features * weight.view(self.out_channels)
+            else:
+                w2d = weight.view(self.out_channels, self.in_channels)
+                feats = torch.mm(features, w2d.t())
             if bias is not None:
                 feats = feats + bias
             out_tensor = out_tensor.replace_feature(feats)
@@ -310,11 +333,15 @@ class SparseConvolution(SparseModule):
                         stride=self.stride, padding=self.padding, dilation=self.dilation)
             if indice_pairs.device != features.device:
                 indice_pairs = indice_pairs.to(features.device)
-            conv_fn = (Fsp.indice_subm_conv if self.subm else
-                       Fsp.indice_inverse_conv if self.inverse else Fsp.indice_conv)
-            out_features = conv_fn(features, weight, indice_pairs, indice_pair_num,
-                                   outids.shape[0], algo, timer, bias_infer, act_alpha, act_beta,
-                                   act_type)
+            if self.depthwise:
+                out_features = self._depthwise_native(features, weight, indice_pairs, indice_pair_num,
+                                                      outids.shape[0], timer, bias_infer, act_alpha, act_type)
+            else:
+                conv_fn = (Fsp.indice_subm_conv if self.subm else
+                           Fsp.indice_inverse_conv if self.inverse else Fsp.indice_conv)
+                out_features = conv_fn(features, weight, indice_pairs, indice_pair_num,
+                                       outids.shape[0], algo, timer, bias_infer, act_alpha, act_beta,
+                                       act_type)
         else:
             if datas is not None:
                 assert isinstance(datas, ImplicitGemmIndiceData)
@@ -370,7 +397,12 @@ class SparseConvolution(SparseModule):
                         out_spatial_shape=out_spatial_shape, algo=algo, ksize=self.kernel_size,
                         stride=self.stride, dilation=self.dilation, padding=self.padding)
             num_activate_out = outids.shape[0]
-            if training:
+            if self.depthwise:
+                # the whole dense table is walked: no tile table, mask sort or split is needed.  SubM (whose
+                # inference rulebook has no pair_bwd) walks pair_fwd with mirrored offsets in the backward
+                out_features = Fsp.depthwise_conv(features, weight, pair_fwd, None if self.subm else pair_bwd,
+                                                  num_activate_out, timer, bias_infer, act_alpha, act_type)
+            elif training:
                 out_features = Fsp.implicit_gemm(features, weight, pair_fwd, pair_bwd, mask_fwd,
                                                  mask_bwd, sort_fwd, sort_bwd, num_activate_out,
                                                  masks, training, self.subm, timer,

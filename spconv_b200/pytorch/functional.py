@@ -231,6 +231,50 @@ def indice_subm_conv(features, filters, indice_pairs, indice_pair_num, num_activ
                    bias, act_alpha, act_beta, act_type, False, True)
 
 
+class DepthwiseConvFunction(Function):
+    """``features, filters [C, *ksize, 1], table_fwd, table_bwd, num_activate_out, timer, bias, act_alpha,
+    act_type`` -> depthwise conv over the dense tables (:func:`ops.depthwise_conv`); ``table_bwd`` None walks the
+    forward table with mirrored offsets in the backward (SubM)."""
+
+    @staticmethod
+    @_amp_fwd
+    def forward(ctx, features, filters, table_fwd, table_bwd, num_activate_out, timer, bias, act_alpha, act_type):
+        try:
+            out = ops.depthwise_conv(features, filters, table_fwd, num_activate_out, bias, act_type, act_alpha,
+                                     timer=timer)
+        except Exception:
+            _report("depthwise_conv", feat=tuple(features.shape), w=tuple(filters.shape),
+                    pair=tuple(table_fwd.shape), act=num_activate_out)
+            raise
+        ctx.save_for_backward(features, filters, table_fwd, table_bwd)
+        ctx.spx = (timer, timer.snapshot())
+        return out
+
+    @staticmethod
+    @once_differentiable
+    @_amp_bwd
+    def backward(ctx, grad_output):
+        features, filters, table_fwd, table_bwd = ctx.saved_tensors
+        timer, scope = ctx.spx
+        try:
+            with timer.scoped(scope):
+                din, dw = ops.depthwise_conv_backward(features, filters, grad_output, table_fwd, table_bwd,
+                                                      timer=timer)
+        except Exception:
+            _report("depthwise_conv_backward", feat=tuple(features.shape), w=tuple(filters.shape),
+                    pair=tuple(table_fwd.shape), do=tuple(grad_output.shape))
+            raise
+        return (din, dw) + (None,) * 7
+
+
+def depthwise_conv(features, filters, table_fwd, table_bwd, num_activate_out, timer=None, bias=None,
+                   act_alpha=0.0, act_type=Activation.None_):
+    if timer is None:
+        timer = CUDAKernelTimer(False)
+    return DepthwiseConvFunction.apply(features, filters, table_fwd, table_bwd, num_activate_out, timer, bias,
+                                       act_alpha, act_type)
+
+
 implicit_gemm = SparseImplicitGemmFunction.apply
 zero_padding_grad = ZeroPaddingGrad.apply
 indice_maxpool = SparseMaxPoolFunction.apply

@@ -735,9 +735,9 @@ def set_wgrad_hook(fn) -> None:
     """``fn(dfilters)`` is called on a forked stream right after the weight gradient of every layer, while
     the input gradient of the same layer runs on the caller's stream (joined before the op returns).  This
     is the place for a data-parallel all-reduce of the layer's dW: it overlaps the rest of the backward pass
-    instead of trailing it (DDP-style hook).  It covers both routes, :func:`implicit_gemm_backward` and
-    :func:`indice_conv_backward` (``ConvAlgo.Native``), and every layer, also one without rows (its dW is
-    zero), so every rank enters the same collectives.  ``ConvAlgo.MaskSplitImplicitGemm`` calls it once per
+    instead of trailing it (DDP-style hook).  It covers every route, :func:`implicit_gemm_backward`,
+    :func:`indice_conv_backward` (``ConvAlgo.Native``) and :func:`depthwise_conv_backward`, and every layer, also one
+    without rows (its dW is zero), so every rank enters the same collectives.  ``ConvAlgo.MaskSplitImplicitGemm`` calls it once per
     mask split, with that split's dW, and sums what the hook left of each split over that split's kernel
     offsets.  The hook may change ``dfilters`` in place; the op returns what it leaves there.  Ignored while
     a peer group is installed (:func:`set_peer_group`).  ``None`` removes the hook."""
@@ -753,7 +753,8 @@ def set_peer_group(peers) -> None:
     """Data-parallel mode: with a :class:`spconv_b200.pytorch.dist.PeerGroup` installed, every weight
     gradient computed by :func:`implicit_gemm_backward` / :func:`indice_conv_backward` is returned
     already summed (x ``peers.scale``) over the ranks -- the exchange is the tail of the
-    weight-gradient kernel (NVLink peer stores, ``csrc/peer.cu``), there is no separate all-reduce.
+    weight-gradient kernel (NVLink peer stores, ``csrc/peer.cu``), there is no separate all-reduce.  A depthwise
+    layer's dW (:func:`depthwise_conv_backward`) is summed by :func:`peer_allreduce_` right after its kernels.
     Every rank must run the same sequence of layers.  Only these conv weight gradients are exchanged:
     biases (added outside the op in training) and every other parameter keep rank-local gradients until
     :func:`peer_allreduce_` sums them (one call per tensor, or one per flat ``dist.GradBucket``), on every
@@ -870,6 +871,92 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
                 _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d_wg), _ptr(features), _ptr(out_bp),
                                                         _ptr(dfilters), ws.data_ptr(), ws.numel(),
                                                         _stream()), "implicit_gemm_wgrad(native)")
+
+    if _PEERS is None and _WGRAD_HOOK is not None:
+        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
+        return din, dfilters
+    run_dgrad()
+    run_wgrad()
+    return din, dfilters
+
+
+# ---------------------------------------------------------------------------- depthwise conv
+def _depthwise_check(features: torch.Tensor, filters: torch.Tensor, table: torch.Tensor) -> Tuple[int, int]:
+    _require_cuda(features, "features")
+    if filters.dtype != features.dtype:
+        raise RuntimeError(f"features ({features.dtype}) and filters ({filters.dtype}) must have the same dtype")
+    if features.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+        raise RuntimeError(f"depthwise conv: unsupported dtype {features.dtype}")
+    c = int(filters.shape[0])
+    if filters.shape[-1] != 1 or features.shape[1] != c:
+        raise RuntimeError(f"depthwise conv: filters [C, *ksize, 1] with C = features' channels, got "
+                           f"{tuple(filters.shape)} for {tuple(features.shape)}")
+    kv = _prod(filters.shape[1:-1])
+    if (table.dim() != 2 or table.shape[0] != kv or table.dtype != torch.int32
+            or (table.shape[1] > 1 and table.stride(1) != 1)):
+        raise RuntimeError(f"depthwise conv: table must be int32 [kv = {kv}, rows] with unit column stride, got "
+                           f"{tuple(table.shape)} {table.dtype}")
+    return kv, c
+
+
+def depthwise_conv(features: torch.Tensor, filters: torch.Tensor, table: torch.Tensor, num_activate_out: int,
+                   bias: Optional[torch.Tensor] = None, act_type=Activation.None_, act_alpha: float = 0.0,
+                   timer: CUDAKernelTimer = CUDAKernelTimer(False)) -> torch.Tensor:
+    """Depthwise forward ``out[o, c] = act(sum_k W[c, k] x[table[k][o], c] + bias[c])`` over a dense table
+    ``[kv, >= num_activate_out]`` (``pair_fwd``, or the Native forward table).  ``filters`` is KRSC
+    ``[C, *ksize, 1]``.  Offsets in ascending order, fp32 sums, no atomics (``spx_depthwise_fwd``)."""
+    features = features.contiguous()
+    filters = filters.contiguous()
+    kv, c = _depthwise_check(features, filters, table)
+    n_out = int(num_activate_out)
+    out = torch.empty((n_out, c), dtype=features.dtype, device=features.device)
+    if bias is not None:
+        bias = bias.to(features.dtype).contiguous()
+    with timer.record("depthwise_conv", _stream()):
+        _cabi.check(_lib().spx_depthwise_fwd(_ptr(features), _ptr(filters), _ptr(bias), _ptr(out), _ptr(table),
+                                             int(table.stride(0)), kv, n_out, c, _DTYPE_CODE[features.dtype],
+                                             _act_code(act_type), float(act_alpha), _stream()), "depthwise_fwd")
+    return out
+
+
+def depthwise_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: torch.Tensor,
+                            table_fwd: torch.Tensor, table_bwd: Optional[torch.Tensor],
+                            timer: CUDAKernelTimer = CUDAKernelTimer(False)):
+    """Backward of :func:`depthwise_conv` -> ``(din, dfilters)``.  ``table_bwd`` ``[kv, >= N]`` maps inputs to
+    outputs; ``None`` (SubM) walks ``table_fwd`` with the mirrored offset instead.  The weight gradient is summed
+    in a fixed order of the row indices (bit-reproducible, unchanged by trailing padding rows).  Data-parallel as
+    the other convs: the wgrad hook receives dW (:func:`set_wgrad_hook`); with a peer group installed dW is summed
+    over the ranks by :func:`peer_allreduce_`."""
+    features = features.contiguous()
+    filters = filters.contiguous()
+    out_bp = out_bp.contiguous()
+    if out_bp.dtype != features.dtype:
+        out_bp = out_bp.to(features.dtype)
+    kv, c = _depthwise_check(features, filters, table_fwd)
+    n_in, n_out = features.shape[0], out_bp.shape[0]
+    reverse = table_bwd is None
+    table_dg = table_fwd if reverse else table_bwd
+    if not reverse:
+        _depthwise_check(features, filters, table_bwd)
+    lib = _lib()
+    dtype = _DTYPE_CODE[features.dtype]
+    din = torch.empty_like(features)
+    dfilters = torch.empty_like(filters)
+    ws = _bytes(lib.spx_depthwise_wgrad_workspace_size(n_out, kv, c), features.device)
+
+    def run_dgrad():
+        with timer.record("depthwise_conv_dgrad", _stream()):
+            _cabi.check(lib.spx_depthwise_dgrad(_ptr(out_bp), _ptr(filters), _ptr(din), _ptr(table_dg),
+                                                int(table_dg.stride(0)), kv, n_in, c, dtype, int(reverse), _stream()),
+                        "depthwise_dgrad")
+
+    def run_wgrad():
+        with timer.record("depthwise_conv_wgrad", _stream()):
+            _cabi.check(lib.spx_depthwise_wgrad(_ptr(features), _ptr(out_bp), _ptr(dfilters), _ptr(table_fwd),
+                                                int(table_fwd.stride(0)), kv, n_out, c, dtype, ws.data_ptr(),
+                                                ws.numel(), _stream()), "depthwise_wgrad")
+            if _PEERS is not None:
+                peer_allreduce_(dfilters)
 
     if _PEERS is None and _WGRAD_HOOK is not None:
         _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)

@@ -66,6 +66,9 @@ class QuantizedSparseConv(SparseConvolution):
     @classmethod
     def from_float(cls, mod: SparseConvolution, output_scale: float) -> "QuantizedSparseConv":
         assert isinstance(mod, SparseConvolution) and not mod.conv1x1
+        if getattr(mod, "depthwise", False):
+            raise NotImplementedError(f"int8 depthwise convolution is not supported (groups={mod.groups}); "
+                                      "keep this layer in floating point")
         q = cls(mod.ndim, mod.in_channels, mod.out_channels, mod.kernel_size, mod.stride, mod.padding,
                 mod.dilation, mod.groups, mod.bias is not None, subm=mod.subm,
                 output_padding=mod.output_padding, transposed=mod.transposed, inverse=mod.inverse,
