@@ -179,11 +179,11 @@ def scatter_nd(indices: torch.Tensor, updates: torch.Tensor, shape: Sequence[int
     (last-writer-wins on duplicates, as the reference's ``scatter_nd``)."""
     lead = indices.shape[-1]
     dims = [int(s) for s in shape]
-    weights = [1] * lead
-    for a in range(lead - 2, -1, -1):
-        weights[a] = weights[a + 1] * dims[a + 1]
-    flat = (indices.reshape(-1, lead).long() *
-            torch.tensor(weights, device=indices.device, dtype=torch.long)).sum(dim=1)
+    # row-major linear index with host scalars: no host-to-device copy, so a padded ToDense captures
+    rows = indices.reshape(-1, lead).long()
+    flat = rows[:, 0]
+    for a in range(1, lead):
+        flat = flat * dims[a] + rows[:, a]
     cells = int(np.prod(dims[:lead]))
     out = updates.new_zeros((cells, *dims[lead:]))
     out[flat] = updates.reshape(-1, *dims[lead:])
@@ -324,7 +324,7 @@ class SparseConvTensor:
         if self.num_valid is not None:
             # padding rows go to one spare sample that is cut off again: no sync, valid cells untouched
             spare = torch.zeros_like(self.indices[:1])
-            spare[0, 0] = self.batch_size
+            spare[:, 0].fill_(self.batch_size)
             inds = torch.where(self.valid_mask().unsqueeze(1), self.indices, spare)
             full[0] += 1
             grid = scatter_nd(inds, self._features, full)[:self.batch_size]

@@ -270,8 +270,8 @@ def _split_and_sort(mask: torch.Tensor, masks: List[np.ndarray], kv: int, do_sor
     (``ops.py:494-503,538-549``: every split is sorted on its own)."""
     mask_s, sort_s = [], []
     for m in masks:
-        const = torch.from_numpy(m.view(np.int32).copy()).to(mask.device)
-        part = torch.bitwise_and(mask, const.view(1, 1, 1)).contiguous()
+        # a scalar operand, not a device tensor: no host-to-device copy, so the rulebook captures
+        part = torch.bitwise_and(mask, int(m.view(np.int32)[0])).contiguous()
         sort_s.append(_argsort_masks(part, kv, do_sort, alloc)[0])
         mask_s.append(part[0])
     return mask_s, sort_s
@@ -585,6 +585,19 @@ def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_spli
     return out, mask_output, MASK_WIDTH
 
 
+def _zero_runs(mask: np.ndarray, kv: int):
+    """``[(a, b), ...]``: the runs of kernel offsets ``a <= k < b`` whose bit is clear in the split mask words"""
+    runs, start = [], None
+    for k in range(kv + 1):
+        clear = k < kv and not (int(mask[k >> 5]) >> (k & 31)) & 1
+        if clear and start is None:
+            start = k
+        elif not clear and start is not None:
+            runs.append((start, k))
+            start = None
+    return runs
+
+
 def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: torch.Tensor,
                            pair_fwd: torch.Tensor, pair_bwd: torch.Tensor,
                            pair_mask_fwd_splits: List[torch.Tensor],
@@ -617,10 +630,12 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
                                             [pair_mask_fwd_splits[j]], bwd_m, [mask_argsort_fwd_splits[j]],
                                             bwd_s, None, masks, mask_width, is_subm, timer, fp32_accum)
             # dW of split j is only meaningful on ITS offsets: the tensor-core kernel leaves the others zero, the
-            # generic FMA kernel (odd channel counts) walks the whole pair table -- mask either way
-            keep = torch.tensor([(int(masks[j][k >> 5]) >> (k & 31)) & 1 for k in range(kv)], dtype=dw.dtype,
-                                device=dw.device).view(1, kv, 1)
-            dw = dw.view(c_out, kv, c_in) * keep
+            # generic FMA kernel (odd channel counts) walks the whole pair table -- zero them either way.  The
+            # offsets come from the host-side split constant, so no mask tensor is copied to the device (a
+            # blocking copy per layer eagerly, refused under CUDA-graph capture)
+            dw = dw.view(c_out, kv, c_in)
+            for a, b in _zero_runs(masks[j], kv):
+                dw[:, a:b].zero_()
             din = di if din is None else din.add_(di)
             dfilters = dw if dfilters is None else dfilters.add_(dw)
         return din, dfilters.view(filters.shape)
