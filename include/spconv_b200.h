@@ -109,6 +109,8 @@ int64_t spx_conv_max_out(const spx_conv_geometry *g, int64_t num_in);
  *   pair_bwd [kv, N]   pair_bwd[k][i] = o  (may be NULL)
  *   mask     [N, words] uint32, bit k%32 of word k/32 set iff pair_fwd[k][o] != -1  (may be NULL)
  * `words` = ceil(kv/32).
+ * Every rulebook entry point that takes `indices` (here and below, spx_sparse_add_union too) reads its rows as
+ * 16-byte vectors and refuses (returns 2) an `indices` pointer that is not 16-byte aligned.
  */
 int spx_subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int64_t N,
                       int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask, void *workspace,
@@ -268,6 +270,9 @@ int spx_build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, const
 /*
  * out[o, :] = act( sum_k x[pair[k][o], :] @ W[:, k, :]^T  + bias )      rows = n_out
  * filters: KRSC [c_out, kv, c_in].  bias (same dtype as features) may be NULL.
+ * The tensor-core kernels also need features, filters and out 16-byte aligned; otherwise the call runs on the
+ * FMA kernels (under SPX_FORCE_TC=1 it returns 3).  The same holds for out_bp, filters, din of the input
+ * gradient, features and out_bp of the weight gradient, and features, filters, out of the int8 forward.
  */
 int spx_implicit_gemm_fwd(const spx_gemm_desc *d, const void *features, const void *filters,
                           void *out, const void *bias, int act, float act_alpha,
@@ -413,7 +418,9 @@ int spx_point2voxel_bounded(const float *points, int64_t N, int num_features, in
  *           made by spx_pairs_to_table from the compact pairs
  *   mode 2  mean over the valid inputs; count_out [n_out] int32 (may be NULL) receives their number
  *           (SparseAvgPool: maxpool.py:211-259)
- * channels * element size must be a multiple of 16 bytes.  dtype: f32 / f16 / bf16, int8 for max.
+ * channels * element size must be a multiple of 16 bytes, and features / out 16-byte aligned (returns 2
+ * otherwise; spx_indice_pool_bwd likewise for features, out_features, out_bp and din).  dtype: f32 / f16 /
+ * bf16, int8 for max.
  */
 int spx_indice_pool_fwd(int mode, const void *features, void *out, const int32_t *pair_fwd,
                         int64_t pair_stride, int kv, int64_t n_out, int channels, int dtype,

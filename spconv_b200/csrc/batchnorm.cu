@@ -35,8 +35,10 @@ __device__ __forceinline__ float bn_chunk_count(int64_t k, int64_t M) {
     return (float)(n < 0 ? 0 : (n > BN_CHUNK ? BN_CHUNK : n));
 }
 
-template <typename T, int W> __device__ __forceinline__ void bn_load(const T *p, float (&f)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
+// V: one 16-byte access per W elements (the pointers are 16-byte aligned); otherwise W element accesses.  W alone
+// decides which rows and channels a thread folds, so both give the same bits.
+template <typename T, int W, bool V> __device__ __forceinline__ void bn_load(const T *p, float (&f)[W]) {
+    if constexpr (V && W * sizeof(T) == 16) {
         const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
         const T *e = reinterpret_cast<const T *>(&v);
 #pragma unroll
@@ -46,8 +48,8 @@ template <typename T, int W> __device__ __forceinline__ void bn_load(const T *p,
         for (int j = 0; j < W; ++j) f[j] = to_float(__ldg(p + j));
     }
 }
-template <typename T, int W> __device__ __forceinline__ void bn_store(T *p, const float (&f)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
+template <typename T, int W, bool V> __device__ __forceinline__ void bn_store(T *p, const float (&f)[W]) {
+    if constexpr (V && W * sizeof(T) == 16) {
         uint4 v;
         T *e = reinterpret_cast<T *>(&v);
 #pragma unroll
@@ -84,7 +86,7 @@ __device__ __forceinline__ BnRowThread bn_row_thread(int vecs, int tpr) {
 }
 
 // ---------------------------------------------------------------- forward
-template <typename T, int W>
+template <typename T, int W, bool V>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_stats_kernel(const T *__restrict__ x, int64_t rows, int channels, int vecs, int tpr,
                 const int32_t *__restrict__ num_valid, float2 *__restrict__ partials) {
@@ -114,13 +116,13 @@ bn_stats_kernel(const T *__restrict__ x, int64_t rows, int channels, int vecs, i
         for (; r + 3 * lanes < end; r += 4 * lanes) {     // four loads in flight, folded in row order
             float f[4][W];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) bn_load<T, W>(base + (r + (int64_t)u * lanes) * channels, f[u]);
+            for (int u = 0; u < 4; ++u) bn_load<T, W, V>(base + (r + (int64_t)u * lanes) * channels, f[u]);
 #pragma unroll
             for (int u = 0; u < 4; ++u) fold(f[u]);
         }
         for (; r < end; r += lanes) {
             float f[W];
-            bn_load<T, W>(base + r * channels, f);
+            bn_load<T, W, V>(base + r * channels, f);
             fold(f);
         }
     }
@@ -211,7 +213,7 @@ bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
     }
 }
 
-template <typename T, int W>
+template <typename T, int W, bool V>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, int channels, int vecs,
                     const int32_t *__restrict__ num_valid, const float *__restrict__ coef) {
@@ -222,7 +224,7 @@ bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, in
     const int64_t M = bn_valid_rows(num_valid, rows);
     float f[W];
     if (r < M) {
-        bn_load<T, W>(x + r * channels + v * W, f);
+        bn_load<T, W, V>(x + r * channels + v * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -232,11 +234,11 @@ bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, in
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    bn_store<T, W>(y + r * channels + v * W, f);
+    bn_store<T, W, V>(y + r * channels + v * W, f);
 }
 
 // ---------------------------------------------------------------- backward
-template <typename T, int W>
+template <typename T, int W, bool V>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t rows, int channels, int vecs, int tpr,
                      const int32_t *__restrict__ num_valid, const float *__restrict__ save_mean,
@@ -272,16 +274,16 @@ bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t 
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int64_t o = (r + (int64_t)u * lanes) * channels + off;
-                bn_load<T, W>(x + o, fx[u]);
-                bn_load<T, W>(dy + o, fd[u]);
+                bn_load<T, W, V>(x + o, fx[u]);
+                bn_load<T, W, V>(dy + o, fd[u]);
             }
 #pragma unroll
             for (int u = 0; u < 2; ++u) fold(fx[u], fd[u]);
         }
         for (; r < end; r += lanes) {
             float fx[W], fd[W];
-            bn_load<T, W>(x + r * channels + off, fx);
-            bn_load<T, W>(dy + r * channels + off, fd);
+            bn_load<T, W, V>(x + r * channels + off, fx);
+            bn_load<T, W, V>(dy + r * channels + off, fd);
             fold(fx, fd);
         }
     }
@@ -337,7 +339,7 @@ bn_bwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
     coef[2 * channels + c] = M > 0 ? __fdiv_rn(sdyx, Mf) : 0.f;
 }
 
-template <typename T, int W>
+template <typename T, int W, bool V>
 __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__restrict__ dx, int64_t rows, int channels,
                     int vecs, const int32_t *__restrict__ num_valid, const float *__restrict__ save_mean,
@@ -350,8 +352,8 @@ bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
     float f[W];
     if (r < M) {
         float fx[W];
-        bn_load<T, W>(x + r * channels + v * W, fx);
-        bn_load<T, W>(dy + r * channels + v * W, f);
+        bn_load<T, W, V>(x + r * channels + v * W, fx);
+        bn_load<T, W, V>(dy + r * channels + v * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -362,7 +364,7 @@ bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    bn_store<T, W>(dx + r * channels + v * W, f);
+    bn_store<T, W, V>(dx + r * channels + v * W, f);
 }
 
 // ---------------------------------------------------------------- host side
@@ -383,8 +385,6 @@ static int bn_check(const char *who, int64_t rows, int channels, int dtype, int 
                 "%s: parameter dtype %d must be float32 or the feature dtype %d", who, param_dtype, dtype);
     return 0;
 }
-
-static bool bn_aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
 
 static int bn_tpr(int vecs) {
     int tpr = 1;
@@ -409,16 +409,16 @@ struct BnFwdArgs {
     float *coef;
 };
 
-template <typename T, int W> static int bn_fwd_rows(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
+template <typename T, int W, bool V> static int bn_fwd_rows(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (stats) {
         const int tpr = bn_tpr(vecs);
         const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
-        bn_stats_kernel<T, W><<<grid, BN_THREADS, 0, stream>>>(static_cast<const T *>(a.x), a.rows, a.channels, vecs,
+        bn_stats_kernel<T, W, V><<<grid, BN_THREADS, 0, stream>>>(static_cast<const T *>(a.x), a.rows, a.channels, vecs,
                                                                tpr, a.num_valid, a.partials);
         SPX_CHECK_LAUNCH("bn_stats_kernel");
     } else {
-        bn_fwd_apply_kernel<T, W><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
+        bn_fwd_apply_kernel<T, W, V><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<T *>(a.y), a.rows, a.channels, vecs, a.num_valid, a.coef);
         SPX_CHECK_LAUNCH("bn_fwd_apply_kernel");
     }
@@ -427,8 +427,9 @@ template <typename T, int W> static int bn_fwd_rows(const BnFwdArgs &a, bool sta
 
 template <typename T> static int bn_fwd_rows_dispatch(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && bn_aligned16(a.x) && bn_aligned16(a.y);
-    return vec ? bn_fwd_rows<T, W>(a, stats, stream) : bn_fwd_rows<T, 1>(a, stats, stream);
+    if ((a.channels * (int)sizeof(T)) % 16) return bn_fwd_rows<T, 1, false>(a, stats, stream);
+    return aligned16(a.x) && aligned16(a.y) ? bn_fwd_rows<T, W, true>(a, stats, stream)
+                                            : bn_fwd_rows<T, W, false>(a, stats, stream);
 }
 
 static int bn_fwd_rows_typed(int dtype, const BnFwdArgs &a, bool stats, cudaStream_t stream) {
@@ -461,17 +462,17 @@ struct BnBwdArgs {
     float *coef;
 };
 
-template <typename T, int W> static int bn_bwd_rows(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
+template <typename T, int W, bool V> static int bn_bwd_rows(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (reduce) {
         const int tpr = bn_tpr(vecs);
         const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
-        bn_bwd_reduce_kernel<T, W><<<grid, BN_THREADS, 0, stream>>>(
+        bn_bwd_reduce_kernel<T, W, V><<<grid, BN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<const T *>(a.dy), a.rows, a.channels, vecs, tpr, a.num_valid,
             a.save_mean, a.save_invstd, a.partials);
         SPX_CHECK_LAUNCH("bn_bwd_reduce_kernel");
     } else {
-        bn_bwd_apply_kernel<T, W><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
+        bn_bwd_apply_kernel<T, W, V><<<(unsigned)div_up64(a.rows * vecs, BN_THREADS), BN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<const T *>(a.dy), static_cast<T *>(a.dx), a.rows, a.channels, vecs,
             a.num_valid, a.save_mean, a.save_invstd, a.coef);
         SPX_CHECK_LAUNCH("bn_bwd_apply_kernel");
@@ -481,9 +482,9 @@ template <typename T, int W> static int bn_bwd_rows(const BnBwdArgs &a, bool red
 
 template <typename T> static int bn_bwd_rows_dispatch(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && bn_aligned16(a.x) && bn_aligned16(a.dy) &&
-                     bn_aligned16(a.dx);
-    return vec ? bn_bwd_rows<T, W>(a, reduce, stream) : bn_bwd_rows<T, 1>(a, reduce, stream);
+    if ((a.channels * (int)sizeof(T)) % 16) return bn_bwd_rows<T, 1, false>(a, reduce, stream);
+    return aligned16(a.x) && aligned16(a.dy) && aligned16(a.dx) ? bn_bwd_rows<T, W, true>(a, reduce, stream)
+                                                                : bn_bwd_rows<T, W, false>(a, reduce, stream);
 }
 
 static int bn_bwd_rows_typed(int dtype, const BnBwdArgs &a, bool reduce, cudaStream_t stream) {

@@ -68,6 +68,16 @@ bool func_configured(const void *fn, int dev);   // returns the previous state a
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int64_t div_up64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// 16-byte vector accesses (cp.async, uint4 / float4 / int4 loads and stores, tensor maps) fault on an address
+// that is not a multiple of 16.  Every caller pointer a kernel reads or writes that way is checked with this
+// before that kernel is chosen; NULL passes.
+static inline bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
+
+// for kernels without an element-wise path: refuse the call, naming the argument
+#define SPX_REQUIRE_ALIGNED16(ptr, who)                                                   \
+    SPX_REQUIRE(spx::aligned16(ptr), "%s: %s must be 16-byte aligned (got %p)", who, #ptr, \
+                (const void *)(ptr))
+
 // carve a caller-provided workspace
 struct WorkspaceCarver {
     char *base;

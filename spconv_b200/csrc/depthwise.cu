@@ -27,8 +27,10 @@ constexpr int DW_U = 4;          // fwd / dgrad: gathers in flight per thread
 constexpr int DW_CHUNK = 512;    // wgrad: rows per partial
 constexpr int DW_FIN = 16;       // finalize: partial loads in flight per thread
 
-template <typename T, int V> __device__ __forceinline__ void dw_load(const T *p, float (&f)[V]) {
-    if constexpr (V * sizeof(T) == 16) {
+// A: the pointer is 16-byte aligned, so V elements move as one 16-byte access; otherwise V element accesses.  V
+// alone decides which rows and channels a thread folds, so both give the same bits.
+template <typename T, int V, bool A = true> __device__ __forceinline__ void dw_load(const T *p, float (&f)[V]) {
+    if constexpr (A && V * sizeof(T) == 16) {
         const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
         const T *e = reinterpret_cast<const T *>(&v);
 #pragma unroll
@@ -151,7 +153,7 @@ depthwise_dgrad_kernel(const T *__restrict__ dy, const T *__restrict__ weight, T
 // ---------------------------------------------------------------- wgrad: per-chunk partials, then finalize
 template <int V> struct DwKw { static constexpr int value = V == 1 ? 16 : 32 / V; };   // offsets per wgrad block
 
-template <typename T, int V>
+template <typename T, int V, bool A>
 __global__ void __launch_bounds__(DW_THREADS)
 depthwise_wgrad_partial_kernel(const T *__restrict__ x, const T *__restrict__ dy, const int32_t *__restrict__ table,
                                int64_t stride, int kv, int64_t rows, int channels, int vecs, int tpr,
@@ -178,12 +180,12 @@ depthwise_wgrad_partial_kernel(const T *__restrict__ x, const T *__restrict__ dy
             for (int kw = 0; kw < KW; ++kw) any |= idx[kw] >= 0;
             if (!any) continue;
             float g[V];
-            dw_load<T, V>(dy + r * channels + t.c0, g);
+            dw_load<T, V, A>(dy + r * channels + t.c0, g);
 #pragma unroll
             for (int kw = 0; kw < KW; ++kw) {
                 if (idx[kw] < 0) continue;
                 float f[V];
-                dw_load<T, V>(x + (int64_t)idx[kw] * channels + t.c0, f);
+                dw_load<T, V, A>(x + (int64_t)idx[kw] * channels + t.c0, f);
 #pragma unroll
                 for (int j = 0; j < V; ++j) acc[kw][j] = fmaf(g[j], f[j], acc[kw][j]);
             }
@@ -244,8 +246,6 @@ static int dw_tpr(int vecs) {
     return tpr;
 }
 
-static bool aligned16(const void *p) { return p == nullptr || ((uintptr_t)p & 15u) == 0; }
-
 template <typename T, int V>
 static int launch_gather(bool fwd, bool rev, const void *src, const void *weight, const void *bias, void *dst,
                          const int32_t *table, int64_t stride, int kv, int64_t rows, int channels, int act, float alpha,
@@ -281,14 +281,14 @@ static int dispatch_gather(bool vec, bool fwd, bool rev, const void *src, const 
 
 static int64_t dw_chunks(int64_t rows) { return (rows + DW_CHUNK - 1) / DW_CHUNK; }
 
-template <typename T, int V>
+template <typename T, int V, bool A>
 static int launch_wgrad(const void *x, const void *dy, void *dweight, const int32_t *table, int64_t stride, int kv,
                         int64_t rows, int channels, float *partials, cudaStream_t stream) {
     const int64_t chunks = dw_chunks(rows);
     if (chunks > 0) {
         const int vecs = channels / V, tpr = dw_tpr(vecs);
         const dim3 grid((unsigned)chunks, (unsigned)div_up64(vecs, tpr), (unsigned)div_up64(kv, DwKw<V>::value));
-        depthwise_wgrad_partial_kernel<T, V><<<grid, DW_THREADS, 0, stream>>>((const T *)x, (const T *)dy, table, stride,
+        depthwise_wgrad_partial_kernel<T, V, A><<<grid, DW_THREADS, 0, stream>>>((const T *)x, (const T *)dy, table, stride,
                                                                               kv, rows, channels, vecs, tpr, partials);
         SPX_CHECK_LAUNCH("depthwise_wgrad_partial_kernel");
     }
@@ -299,11 +299,15 @@ static int launch_wgrad(const void *x, const void *dy, void *dweight, const int3
     return 0;
 }
 
+// The partial sums' order follows the vector width: a misaligned x or dy keeps the width of the aligned call and
+// only loads element by element, so the weight gradient does not depend on where the operands start.
 template <typename T>
-static int dispatch_wgrad(bool vec, const void *x, const void *dy, void *dweight, const int32_t *table, int64_t stride,
-                          int kv, int64_t rows, int channels, float *partials, cudaStream_t stream) {
-    if (vec) return launch_wgrad<T, 16 / sizeof(T)>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
-    return launch_wgrad<T, 1>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
+static int dispatch_wgrad(bool wide, bool aligned, const void *x, const void *dy, void *dweight, const int32_t *table,
+                          int64_t stride, int kv, int64_t rows, int channels, float *partials, cudaStream_t stream) {
+    constexpr int W = 16 / sizeof(T);
+    if (!wide) return launch_wgrad<T, 1, false>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
+    if (aligned) return launch_wgrad<T, W, true>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
+    return launch_wgrad<T, W, false>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
 }
 
 }  // namespace spx
@@ -373,13 +377,14 @@ extern "C" int spx_depthwise_wgrad(const void *features, const void *out_bp, voi
     const size_t need = spx_depthwise_wgrad_workspace_size(n_out, kv, channels);
     SPX_REQUIRE(workspace_bytes >= need && (need == 0 || workspace != nullptr),
                 "depthwise_wgrad: workspace of %zu bytes, %zu needed", workspace_bytes, need);
-    const bool vec = use_vectors(channels, dtype, features, out_bp, nullptr);
+    const bool wide = ((int64_t)channels * dtype_bytes(dtype)) % 16 == 0;
+    const bool aligned = aligned16(features) && aligned16(out_bp);
     float *partials = (float *)workspace;
     cudaStream_t stream = (cudaStream_t)stream_;
     switch (dtype) {
-        case SPX_F32: return dispatch_wgrad<float>(vec, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
-        case SPX_F16: return dispatch_wgrad<__half>(vec, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
-        case SPX_BF16: return dispatch_wgrad<__nv_bfloat16>(vec, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
+        case SPX_F32: return dispatch_wgrad<float>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
+        case SPX_F16: return dispatch_wgrad<__half>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
+        case SPX_BF16: return dispatch_wgrad<__nv_bfloat16>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
     }
     return 2;
 }

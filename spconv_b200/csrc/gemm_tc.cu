@@ -525,9 +525,15 @@ static bool tc_shape_ok(int dtype, int kv, int c_in, int c_out, int transpose_w)
     return true;
 }
 
+// The producers gather x rows with 16-byte cp.async, the weight slice comes through a tensor map (or as
+// float4 for the fp32 input gradient) and the epilogue stores column pairs: a call whose x, w or y is not
+// 16-byte aligned runs on the FMA kernels, which access them element by element.
+static bool tc_operands_aligned(const GatherGemmArgs &a) { return aligned16(a.x) && aligned16(a.w) && aligned16(a.y); }
+
 bool tc_gather_gemm_supported(const GatherGemmArgs &a) {
     if (a.dtype == SPX_I8) return false;
     if (!a.tile_table || !a.tile_mask) return false;   // built by spx_build_tile_table
+    if (!tc_operands_aligned(a)) return false;
     // tf32 input gradient: the weight loader writes the filter slice transposed (tf32 wgmma reads K-major
     // operands only); it is served for whole 128-byte filter rows, otherwise fp32 dgrad runs on the FMA
     // kernel; spx_debug_configure bit 256 switches the tensor-core route off (A/B against the FMA kernel).
@@ -537,6 +543,7 @@ bool tc_gather_gemm_supported(const GatherGemmArgs &a) {
 }
 bool tc_gather_gemm_int8_supported(const Int8Args &q) {
     if (!q.g.tile_table || !q.g.tile_mask) return false;
+    if (!tc_operands_aligned(q.g)) return false;
     if (((size_t)q.g.kv * q.g.c_in) % 16) return false;
     return tc_shape_ok(SPX_I8, q.g.kv, q.g.c_in, q.g.c_out, 0);
 }

@@ -535,6 +535,7 @@ struct WgPlan { WgParams p; int passes, chunks; size_t smem; };
 static bool make_plan(const WgradArgs &a, WgPlan &pl) {
     if (a.dtype != SPX_F16 && a.dtype != SPX_BF16 && a.dtype != SPX_F32) return false;
     if (!a.tile_table || !a.tile_mask) return false;                 // built by spx_build_tile_table
+    if (!aligned16(a.x) || !aligned16(a.dout)) return false;         // 16-byte cp.async / float4 row gathers
     const bool tf32 = a.dtype == SPX_F32;       // fp32 reaches here only in TF32 mode (api_gemm.cu)
     const int e = tf32 ? 4 : 2;
     if (a.c_in % 16 || a.c_out % 16 || a.c_in > 256 || a.c_out > 256) return false;
@@ -615,7 +616,7 @@ int tc_wgrad(const WgradArgs &a, cudaStream_t stream) {
     pl.p.partial = (float *)a.workspace;
     SPX_REQUIRE((size_t)pl.chunks * pl.p.partial_stride * sizeof(float) <= a.workspace_bytes,
                 "tc_wgrad: workspace too small");
-    SPX_REQUIRE(((uintptr_t)a.workspace & 15u) == 0, "tc_wgrad: workspace must be 16-byte aligned");
+    SPX_REQUIRE(aligned16(a.workspace), "tc_wgrad: workspace must be 16-byte aligned");
     dim3 grid(pl.chunks, pl.passes);
     const int cpa = pl.p.span_x >> 4, cpd = pl.p.db >> 4;
     using KernelFn = void (*)(const WgParams);

@@ -43,8 +43,10 @@ __device__ __forceinline__ int64_t gp_valid_rows(const int32_t *num_valid, int64
     return m < 0 ? 0 : (m > rows ? rows : m);
 }
 
-template <typename T, int W> __device__ __forceinline__ void gp_load(const T *p, float (&f)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
+// A: the pointer is 16-byte aligned, so W elements move as one 16-byte access; otherwise W element accesses.  W
+// alone decides which rows and channels a thread folds, so both give the same bits.
+template <typename T, int W, bool A = true> __device__ __forceinline__ void gp_load(const T *p, float (&f)[W]) {
+    if constexpr (A && W * sizeof(T) == 16) {
         const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
         const T *e = reinterpret_cast<const T *>(&v);
 #pragma unroll
@@ -139,7 +141,7 @@ __device__ __forceinline__ int gp_sample_of_chunk(const int32_t *cstart, int bat
 
 // Block layout as batchnorm.cu: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
 // `lanes` = GP_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
-template <typename T, int W, bool MEAN>
+template <typename T, int W, bool MEAN, bool A>
 __global__ void __launch_bounds__(GP_THREADS)
 gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, const int32_t *__restrict__ offsets,
                  const int32_t *__restrict__ cstart, int batch_size, int channels, int vecs, int tpr,
@@ -183,14 +185,14 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
 #pragma unroll
             for (int u = 0; u < 2; ++u) r[u] = __ldg(order + p + u * lanes);
 #pragma unroll
-            for (int u = 0; u < 2; ++u) gp_load<T, W>(base + (int64_t)r[u] * channels, f[u]);
+            for (int u = 0; u < 2; ++u) gp_load<T, W, A>(base + (int64_t)r[u] * channels, f[u]);
 #pragma unroll
             for (int u = 0; u < 2; ++u) fold(f[u], r[u]);
         }
         for (; p < end; p += lanes) {
             const int r = __ldg(order + p);
             float f[W];
-            gp_load<T, W>(base + (int64_t)r * channels, f);
+            gp_load<T, W, A>(base + (int64_t)r * channels, f);
             fold(f, r);
         }
     }
@@ -306,8 +308,6 @@ static int64_t gp_max_chunks(int64_t rows, int batch_size) {
     return (rows + GP_CHUNK - 1) / GP_CHUNK + batch_size;
 }
 
-static bool gp_aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
-
 static int gp_tpr(int vecs) {
     int tpr = 1;
     while (tpr < vecs && tpr < 32) tpr <<= 1;
@@ -339,12 +339,12 @@ struct GpFwdArgs {
     int32_t *argmax;
 };
 
-template <typename T, int W, bool MEAN> static int gp_fwd_launch(const GpFwdArgs &a, cudaStream_t stream) {
+template <typename T, int W, bool MEAN, bool A> static int gp_fwd_launch(const GpFwdArgs &a, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (a.rows > 0) {
         const int tpr = gp_tpr(vecs);
         const dim3 grid((unsigned)gp_max_chunks(a.rows, a.batch_size), (unsigned)div_up64(vecs, tpr));
-        gp_reduce_kernel<T, W, MEAN><<<grid, GP_THREADS, 0, stream>>>(
+        gp_reduce_kernel<T, W, MEAN, A><<<grid, GP_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), a.order, a.offsets, a.cstart, a.batch_size, a.channels, vecs, tpr,
             a.partials);
         SPX_CHECK_LAUNCH("gp_reduce_kernel");
@@ -358,9 +358,12 @@ template <typename T, int W, bool MEAN> static int gp_fwd_launch(const GpFwdArgs
 
 template <typename T> static int gp_fwd_dispatch(const GpFwdArgs &a, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && (a.rows == 0 || gp_aligned16(a.x));
-    if (a.mode == 1) return vec ? gp_fwd_launch<T, W, true>(a, stream) : gp_fwd_launch<T, 1, true>(a, stream);
-    return vec ? gp_fwd_launch<T, W, false>(a, stream) : gp_fwd_launch<T, 1, false>(a, stream);
+    // a misaligned x keeps the row layout (and so the order of the sums) of the aligned call
+    if ((a.channels * (int)sizeof(T)) % 16)
+        return a.mode == 1 ? gp_fwd_launch<T, 1, true, false>(a, stream) : gp_fwd_launch<T, 1, false, false>(a, stream);
+    if (a.rows == 0 || aligned16(a.x))
+        return a.mode == 1 ? gp_fwd_launch<T, W, true, true>(a, stream) : gp_fwd_launch<T, W, false, true>(a, stream);
+    return a.mode == 1 ? gp_fwd_launch<T, W, true, false>(a, stream) : gp_fwd_launch<T, W, false, false>(a, stream);
 }
 
 struct GpBwdArgs {
@@ -384,7 +387,7 @@ template <typename T, int W, bool MEAN> static int gp_bwd_launch(const GpBwdArgs
 
 template <typename T> static int gp_bwd_dispatch(const GpBwdArgs &a, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && gp_aligned16(a.dy) && gp_aligned16(a.din);
+    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && aligned16(a.dy) && aligned16(a.din);
     if (a.mode == 1) return vec ? gp_bwd_launch<T, W, true>(a, stream) : gp_bwd_launch<T, 1, true>(a, stream);
     return vec ? gp_bwd_launch<T, W, false>(a, stream) : gp_bwd_launch<T, 1, false>(a, stream);
 }

@@ -148,7 +148,6 @@ ps_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ row32, int64
 }
 
 // ---------------------------------------------------------------- host side
-static bool ps_aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
 
 static int ps_check(const char *who, int mode, int64_t n, int64_t rows, int channels, int dtype) {
     SPX_REQUIRE(mode >= 0 && mode <= 2, "%s: mode must be 0 (max), 1 (mean) or 2 (sum), got %d", who, mode);
@@ -177,7 +176,7 @@ template <typename T>
 static int ps_fwd_dispatch(bool mean, const void *x, const int32_t *order, const int32_t *offsets, int64_t rows,
                            int channels, void *out, int32_t *argmax, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && ps_aligned16(x) && ps_aligned16(out);
+    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && aligned16(x) && aligned16(out);
     if (mean) return vec ? ps_fwd_launch<T, W, true>(x, order, offsets, rows, channels, out, argmax, stream)
                          : ps_fwd_launch<T, 1, true>(x, order, offsets, rows, channels, out, argmax, stream);
     return vec ? ps_fwd_launch<T, W, false>(x, order, offsets, rows, channels, out, argmax, stream)
@@ -198,7 +197,7 @@ template <typename T>
 static int ps_bwd_dispatch(bool mean, const void *dy, const int32_t *row32, int64_t n, int channels,
                            const int32_t *argmax, const int32_t *count, void *dx, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && ps_aligned16(dy) && ps_aligned16(dx);
+    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && aligned16(dy) && aligned16(dx);
     if (mean) return vec ? ps_bwd_launch<T, W, true>(dy, row32, n, channels, argmax, count, dx, stream)
                          : ps_bwd_launch<T, 1, true>(dy, row32, n, channels, argmax, count, dx, stream);
     return vec ? ps_bwd_launch<T, W, false>(dy, row32, n, channels, argmax, count, dx, stream)

@@ -6,9 +6,10 @@
 //   forward_kernel / backward_kernel                                      (ConvAlgo.Native, compact pairs)
 // Pure HBM-bound gather work: one thread owns one 16-byte channel chunk of one output row and walks
 // the kv table entries of that row; the row indices are warp-broadcast loads, the feature rows are
-// read and written as 16-byte vectors.  The Native variants run on the same kernels after the
-// compact pairs have been scattered into a dense table (spx_pairs_to_table) -- no atomics on
-// features, results independent of the pair order.
+// read and written as 16-byte vectors, so the entry points refuse a feature pointer that is not
+// 16-byte aligned.  The Native variants run on the same kernels after the compact pairs have been
+// scattered into a dense table (spx_pairs_to_table) -- no atomics on features, results independent
+// of the pair order.
 #include "common.cuh"
 
 namespace spx {
@@ -195,6 +196,8 @@ extern "C" int spx_indice_pool_fwd(int mode, const void *features, void *out, co
     if (check_pool("indice_pool_fwd", kv, channels, dtype, n_out, mode != 2)) return 2;
     if (n_out == 0) return 0;
     SPX_REQUIRE(features && out && pair_fwd, "indice_pool_fwd: NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(features, "indice_pool_fwd");
+    SPX_REQUIRE_ALIGNED16(out, "indice_pool_fwd");
     cudaStream_t stream = (cudaStream_t)stream_;
     switch (dtype) {
         case SPX_F32: return launch_fwd<float>(mode, features, out, pair_fwd, pair_stride, kv, n_out, channels, count_out, stream);
@@ -215,6 +218,10 @@ extern "C" int spx_indice_pool_bwd(int mode, const void *features, const void *o
     SPX_REQUIRE(out_bp && din && pair_bwd, "indice_pool_bwd: NULL pointer argument");
     SPX_REQUIRE(avg ? count_out != nullptr : (features && out_features), "indice_pool_bwd: missing %s",
                 avg ? "count_out" : "features / out_features");
+    SPX_REQUIRE_ALIGNED16(features, "indice_pool_bwd");
+    SPX_REQUIRE_ALIGNED16(out_features, "indice_pool_bwd");
+    SPX_REQUIRE_ALIGNED16(out_bp, "indice_pool_bwd");
+    SPX_REQUIRE_ALIGNED16(din, "indice_pool_bwd");
     cudaStream_t stream = (cudaStream_t)stream_;
     switch (dtype) {
         case SPX_F32: return launch_bwd<float>(avg, features, out_features, out_bp, din, pair_bwd, pair_stride, kv, n_in, channels, count_out, stream);

@@ -1068,6 +1068,7 @@ static int subm_rulebook(const spx_conv_geometry *g, const int32_t *indices, int
     SPX_REQUIRE(N >= 0 && N < 2147483647ll, "bad N");
     if (N == 0) return 0;
     SPX_REQUIRE(indices && pair_fwd && workspace, "NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(indices, "subm_rulebook");
     cudaStream_t stream = (cudaStream_t)stream_;
     Geom gg = make_geom(g, true);
     SPX_REQUIRE((int64_t)gg.kv * N < 2147483647ll * 4, "kv*N too large");
@@ -1223,6 +1224,7 @@ extern "C" int spx_conv_rulebook_stage1(const spx_conv_geometry *g, const int32_
     *num_out_host = 0;
     if (N == 0) return 0;
     SPX_REQUIRE(indices && workspace, "NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(indices, "conv_rulebook_stage1");
     if (validate_strides(g)) return 2;
     cudaStream_t stream = (cudaStream_t)stream_;
     Geom gg = make_geom(g, false);
@@ -1271,6 +1273,7 @@ extern "C" int spx_conv_rulebook_stage2(const spx_conv_geometry *g, const int32_
     if (validate_geom(g)) return 2;
     if (N == 0 || M == 0) return 0;
     SPX_REQUIRE(indices && out_inds && pair_fwd && pair_bwd && workspace, "NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(indices, "conv_rulebook_stage2");
     cudaStream_t stream = (cudaStream_t)stream_;
     Geom gg = make_geom(g, false);
     ConvWs w;
@@ -1407,7 +1410,7 @@ static int build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, co
     int words = (kv + 31) / 32;
     if (row_table) {
         SPX_REQUIRE(kv <= 32, "build_tile_table: row_table holds at most 32 offsets per row, kv = %d", kv);
-        SPX_REQUIRE(((uintptr_t)row_table & 15u) == 0, "build_tile_table: row_table must be 16-byte aligned");
+        SPX_REQUIRE(aligned16(row_table), "build_tile_table: row_table must be 16-byte aligned");
         build_tile_table_rows_kernel<<<(unsigned)div_up64(rows, 128), 128 * TT_SPLIT, 0, stream>>>(
             row_table, kv, argsort, mask, rows, table, tile_mask);
         SPX_CHECK_LAUNCH("build_tile_table_rows_kernel");
@@ -1420,7 +1423,7 @@ static int build_tile_table(const int32_t *pair, int64_t pair_stride, int kv, co
     }
     const int64_t tiles = div_up64(rows, 128);
     SPX_REQUIRE(tiles < 2147483647ll, "build_tile_table: too many tiles");
-    SPX_REQUIRE(((uintptr_t)table & 15u) == 0, "build_tile_table: table must be 16-byte aligned");
+    SPX_REQUIRE(aligned16(table), "build_tile_table: table must be 16-byte aligned");
     int32_t *rec = table + tt_blocks_elems(tiles, kv);
     ToJobs oj;
     memset(&oj, 0, sizeof(oj));
@@ -1445,7 +1448,7 @@ static int build_tile_tables_pair(int kv, const int32_t *pair0, const int32_t *a
     const int words = (kv + 31) / 32;
     const int64_t tiles0 = div_up64(rows0, 128), tiles1 = div_up64(rows1, 128);
     SPX_REQUIRE(tiles0 < 2147483647ll && tiles1 < 2147483647ll, "build_tile_table: too many tiles");
-    SPX_REQUIRE((((uintptr_t)table0 | (uintptr_t)table1) & 15u) == 0, "build_tile_table: table must be 16-byte aligned");
+    SPX_REQUIRE(aligned16(table0) && aligned16(table1), "build_tile_table: table must be 16-byte aligned");
     TtJobs jobs;
     memset(&jobs, 0, sizeof(jobs));
     jobs.j[0] = TtJob{pair0, rows0, argsort0, mask0, rows0, table0, tmask0};
@@ -1645,6 +1648,7 @@ extern "C" int spx_conv_rulebook_bounded_all(const spx_conv_geometry *g, const i
     SPX_REQUIRE(out_inds && pair_fwd && mask_fwd && argsort_fwd && table_fwd && tmask_fwd && num_out && status && workspace,
                 "conv_rulebook_bounded_all: NULL pointer argument");
     SPX_REQUIRE(N == 0 || (indices && pair_bwd && mask_bwd), "conv_rulebook_bounded_all: NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(indices, "conv_rulebook_bounded_all");
     const bool train = argsort_bwd != nullptr;
     SPX_REQUIRE((table_bwd != nullptr) == train && (tmask_bwd != nullptr) == train,
                 "conv_rulebook_bounded_all: argsort_bwd, table_bwd and tmask_bwd must all be given (training) or all be "
@@ -1688,6 +1692,7 @@ extern "C" int spx_sparse_add_union(const spx_conv_geometry *g, const int32_t *i
                                     size_t workspace_bytes, spx_stream_t stream) {
     if (validate_sparse_add_union(g, N, bound)) return 2;
     SPX_REQUIRE(indices && out_inds && dst && num_out && status && workspace, "sparse_add_union: NULL pointer argument");
+    SPX_REQUIRE_ALIGNED16(indices, "sparse_add_union");
     const size_t need = spx_sparse_add_union_workspace_size(g, N, bound);
     SPX_REQUIRE(workspace_bytes >= need, "sparse_add_union: workspace too small: need %zu, have %zu", need, workspace_bytes);
     const Geom gg = make_geom(g, false);
@@ -1704,7 +1709,7 @@ extern "C" int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_byt
     SPX_REQUIRE(ptr && count, "zero_rows_from_count: NULL pointer argument");
     cudaStream_t stream = (cudaStream_t)stream_;
     const unsigned blocks = (unsigned)sm_count() * 4;
-    if (row_bytes % 16 == 0 && ((uintptr_t)ptr & 15u) == 0)
+    if (row_bytes % 16 == 0 && aligned16(ptr))
         zero_rows_from_count_kernel<<<blocks, 256, 0, stream>>>((uint4 *)ptr, rows, row_bytes / 16, count);
     else
         zero_rows_from_count_kernel<<<blocks, 256, 0, stream>>>((uint16_t *)ptr, rows, row_bytes / 2, count);

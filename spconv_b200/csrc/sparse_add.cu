@@ -160,8 +160,6 @@ static int check_features(int channels, int dtype, const char *who) {
     return 0;
 }
 
-static bool aligned16(const void *p) { return ((uintptr_t)p & 15u) == 0; }
-
 template <typename T, int W>
 static int launch_sum(const SaOperands &ops, const int32_t *order, const int32_t *offsets, int64_t M, int channels, void *out,
                       cudaStream_t stream) {

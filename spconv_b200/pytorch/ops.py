@@ -78,6 +78,17 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return t.data_ptr()
 
 
+def _dense(t: torch.Tensor) -> torch.Tensor:
+    """``t`` itself when it is contiguous and 16-byte aligned, else a contiguous copy.  The tensor-core GEMMs, the
+    pooling and the rulebook kernels read rows as 16-byte vectors; a contiguous view at an odd element offset
+    (an autograd gradient sliced out of a ``torch.cat``, a parameter in a flat buffer) would send the GEMMs to
+    the FMA kernels and make the others refuse the call.  The copy keeps every public call on the same kernels,
+    with the same bits, as an aligned one."""
+    if t.is_contiguous() and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
+
+
 def _require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise RuntimeError(
@@ -290,7 +301,7 @@ def get_indice_pairs(indices: torch.Tensor, batch_size: int, spatial_shape: List
     _require_cuda(indices, "indices")
     lib = _lib()
     dev = indices.device
-    indices = indices.contiguous()
+    indices = _dense(indices)
     n_in = indices.shape[0]
     kv = _prod(ksize)
     out_shape = _out_shape(spatial_shape, ksize, stride, padding, dilation, out_padding, subm,
@@ -348,7 +359,7 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
     assert algo in (ConvAlgo.MaskImplicitGemm, ConvAlgo.MaskSplitImplicitGemm), "TODO"
     lib = _lib()
     dev = indices.device
-    indices = indices.contiguous()
+    indices = _dense(indices)
     n_in = indices.shape[0]
     kv = _prod(ksize)
     words = (kv + 31) // 32
@@ -502,8 +513,8 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     (``fp32_accum`` is accepted and ignored)."""
     _require_cuda(features, "features")
     lib = _lib()
-    features = features.contiguous()
-    filters = filters.contiguous()
+    features = _dense(features)
+    filters = _dense(filters)
     kv, c_in, c_out = _check_filter(features, filters)
     assert features.shape[1] == c_in, "channel size mismatch"
     n_in, n_out = features.shape[0], int(num_activate_out)
@@ -530,6 +541,13 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
         # accumulator, the residual enters with beta = output_add_scale / output_scale
         scale_f = scale.float().contiguous()
         bias_f = bias.float().contiguous() if bias is not None else None
+        if output_add is not None:
+            # the epilogue reads the residual as int8 [n_out, c_out] rows
+            _require_cuda(output_add, "output_add")
+            if output_add.dtype != torch.int8 or tuple(output_add.shape) != (n_out, c_out):
+                raise RuntimeError(f"int8 implicit gemm: output_add must be int8 of shape {(n_out, c_out)}, got "
+                                   f"{output_add.dtype} {tuple(output_add.shape)}")
+            output_add = _dense(output_add)
         with timer.record("implicit_gemm_int8", _stream()):
             _cabi.check(lib.spx_implicit_gemm_fwd_int8(
                 ctypes.byref(d), _ptr(features), _ptr(filters), _ptr(out), _DTYPE_CODE[output_dtype],
@@ -612,9 +630,9 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
     (``ops.py:1667-1681`` / ``convops.py:2247-2440``)."""
     _require_cuda(features, "features")
     lib = _lib()
-    features = features.contiguous()
-    filters = filters.contiguous()
-    out_bp = out_bp.contiguous()
+    features = _dense(features)
+    filters = _dense(filters)
+    out_bp = _dense(out_bp)
     if out_bp.dtype != features.dtype:
         out_bp = out_bp.to(features.dtype)
     kv, c_in, c_out = _check_filter(features, filters)
@@ -821,8 +839,8 @@ def indice_conv(features: torch.Tensor, filters: torch.Tensor, indice_pairs: tor
     accumulates every offset in registers -- no atomics, deterministic."""
     _require_cuda(features, "features")
     lib = _lib()
-    features = features.contiguous()
-    filters = filters.contiguous()
+    features = _dense(features)
+    filters = _dense(filters)
     indice_pairs = indice_pairs.contiguous()
     kv, c_in, c_out = _check_filter(features, filters)
     assert features.shape[1] == c_in, "channel size mismatch"
@@ -853,9 +871,9 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
     ``convops.py:1751-2071``)."""
     _require_cuda(features, "features")
     lib = _lib()
-    features = features.contiguous()
-    filters = filters.contiguous()
-    out_bp = out_bp.contiguous()
+    features = _dense(features)
+    filters = _dense(filters)
+    out_bp = _dense(out_bp)
     if out_bp.dtype != features.dtype:
         out_bp = out_bp.to(features.dtype)
     indice_pairs = indice_pairs.contiguous()
@@ -996,7 +1014,7 @@ def _pool_check(features: torch.Tensor):
 
 
 def _pool_fwd(mode, features, table, n_out, count_out=None):
-    features = features.contiguous()
+    features = _dense(features)
     _pool_check(features)
     out = torch.empty((int(n_out), features.shape[1]), dtype=features.dtype, device=features.device)
     _cabi.check(_lib().spx_indice_pool_fwd(mode, _ptr(features), _ptr(out), _ptr(table), int(table.stride(0)),
@@ -1007,7 +1025,7 @@ def _pool_fwd(mode, features, table, n_out, count_out=None):
 
 
 def _pool_bwd(mode, features, out_features, out_bp, table_bwd, n_in, count_out=None):
-    out_bp = out_bp.contiguous()
+    out_bp = _dense(out_bp)
     _pool_check(out_bp)
     din = torch.empty((int(n_in), out_bp.shape[1]), dtype=out_bp.dtype, device=out_bp.device)
     _cabi.check(_lib().spx_indice_pool_bwd(mode, _ptr(features), _ptr(out_features), _ptr(out_bp), _ptr(din),
@@ -1034,7 +1052,7 @@ def indice_maxpool_backward(features, out_features, out_bp, indice_pairs, indice
     kv = int(indice_pairs.shape[1])
     _, _, t_bwd, _ = _native_tables(indice_pairs.contiguous(), indice_pair_num, features.shape[0],
                                     out_features.shape[0], kv, False, False, False, True)
-    return _pool_bwd(_POOL_MAX, features.contiguous(), out_features.contiguous(), out_bp, t_bwd,
+    return _pool_bwd(_POOL_MAX, _dense(features), _dense(out_features), out_bp, t_bwd,
                      features.shape[0])
 
 
@@ -1045,7 +1063,7 @@ def indice_maxpool_implicit_gemm(features: torch.Tensor, indice_pairs: torch.Ten
 
 def indice_maxpool_implicit_gemm_backward(features, out_features, out_bp, indice_pairs):
     """``indice_pairs`` is the backward table ``pair_bwd [kv, N]`` (``ops.py:2009-2030``)."""
-    return _pool_bwd(_POOL_MAX, features.contiguous(), out_features.contiguous(), out_bp, indice_pairs,
+    return _pool_bwd(_POOL_MAX, _dense(features), _dense(out_features), out_bp, indice_pairs,
                      features.shape[0])
 
 
