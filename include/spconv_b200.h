@@ -343,6 +343,11 @@ int spx_peer_push(const spx_peer_group *pg, const void *data, int64_t count, int
 int spx_peer_finish(const spx_peer_group *pg, void *out, int64_t count, int dtype, float scale, spx_stream_t stream);
 int spx_peer_allreduce(const spx_peer_group *pg, void *data, int64_t count, int dtype, float scale,
                        spx_stream_t stream);
+/* gather: every rank's `count` 32-bit words of src land, unchanged, in dst[r * count, (r + 1) * count) for r in
+ * rank order, on every rank.  The same push and finish protocol (one exchange in flight); a timed-out peer
+ * leaves dst NaN (0x7fc00000) and sets spx_peer_error. */
+int spx_peer_allgather(const spx_peer_group *pg, const uint32_t *src, int64_t count, uint32_t *dst,
+                       spx_stream_t stream);
 
 /* x[r, j] = act(x[r, j] + bias[j])   in place; bias may be NULL */
 int spx_bias_act_inplace(void *x, const void *bias, int64_t rows, int cols, int dtype, int act,
@@ -631,6 +636,56 @@ int spx_masked_bn_bwd(const void *x, const void *dy, void *dx, int64_t rows, int
                       const int32_t *num_valid, const void *weight, int param_dtype, const float *save_mean,
                       const float *save_invstd, void *dweight, void *dbias, void *workspace, size_t workspace_bytes,
                       spx_stream_t stream);
+
+/*
+ * Cross-rank training-mode BatchNorm (MaskedSyncBatchNorm1d): the statistics cover the valid rows of every rank.
+ * A forward or backward is two calls on each rank around an exchange the caller runs (spx_peer_allgather or an
+ * NCCL all-gather, both move the bits unchanged):
+ *   *_local  reduces this rank's rows [0, M_r) as spx_masked_bn_* does and writes local = [M_r, A[C], B[C]] (fp32);
+ *   exchange local of every rank into gathered = [world][2 C + 1] in rank order;
+ *   *_merge  folds the gathered vectors in rank order, the same on every rank, then writes y / dx.
+ * Forward:  A = sum of the rank's valid rows, B = their M2 about the rank's own mean.  The merge takes
+ *           M = sum M_r (int64), mean = sum A_r / M, M2 = sum [B_r + M_r (A_r / M_r - mean)^2], and writes
+ *           save_mean / save_invstd, y and the running stats exactly as spx_masked_bn_fwd_train does for M rows.
+ * Backward: A = sum(dy), B = sum(dy * xhat) over the rank's rows with the global mean / invstd; dbias = A and
+ *           dweight = B are the RANK-LOCAL sums (bwd_local writes them; average them like any other parameter
+ *           gradient).  The merge sums A_r, B_r in rank order and writes dx with the global sums over M.
+ * With one rank (gathered = local) every result equals spx_masked_bn_fwd_train / spx_masked_bn_bwd bit for bit.
+ * A gathered count outside [0, 2^24] (NaN after a timed-out exchange) makes the statistics, the running stats and
+ * y / dx NaN.  rows <= 2^24 per call.  One descriptor holds the operands of the layer call, so the local and the
+ * merge call of one pass read the same ones; the workspace (spx_masked_sync_bn_workspace_size) is also shared
+ * by the two calls of one pass.  Fields a call does not use may be anything.
+ */
+typedef struct spx_masked_sync_bn {
+    int64_t rows;
+    int channels, dtype, param_dtype;
+    int world;                              /* vectors in `gathered` (merge calls), 1..SPX_MAX_PEERS */
+    const int32_t *num_valid;               /* device int32, clamped to [0, rows]; NULL = every row */
+    const void *x;                          /* [rows, channels] */
+    void *y;                                /* fwd: [rows, channels] */
+    const void *dy;                         /* bwd: [rows, channels] */
+    void *dx;                               /* bwd: [rows, channels] */
+    const void *weight, *bias;              /* [channels] param_dtype, or NULL (1 / 0) */
+    void *running_mean, *running_var;       /* fwd: both or neither */
+    const int64_t *num_batches_tracked;     /* fwd, cumulative != 0: device int64, already incremented */
+    float momentum;
+    int cumulative;
+    float eps;
+    float *save_mean, *save_invstd;         /* [channels] fp32: written by fwd_merge, read by the backward */
+    void *dweight, *dbias;                  /* bwd: [channels] param_dtype or NULL */
+    float *local;                           /* [2 channels + 1]: written by the local calls */
+    const float *gathered;                  /* [world][2 channels + 1]: read by the merge calls */
+} spx_masked_sync_bn;
+
+size_t spx_masked_sync_bn_workspace_size(int64_t rows, int channels);
+int spx_masked_sync_bn_fwd_local(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                 spx_stream_t stream);
+int spx_masked_sync_bn_fwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                 spx_stream_t stream);
+int spx_masked_sync_bn_bwd_local(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                 spx_stream_t stream);
+int spx_masked_sync_bn_bwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                 spx_stream_t stream);
 
 /* ------------------------------------------------------------------ hash table */
 

@@ -67,6 +67,18 @@ class SparseAddOperands(Structure):
     ]
 
 
+class MaskedSyncBN(Structure):
+    """``spx_masked_sync_bn``: the operands of one MaskedSyncBatchNorm1d pass on this rank."""
+    _fields_ = [
+        ("rows", c_int64), ("channels", c_int), ("dtype", c_int), ("param_dtype", c_int), ("world", c_int),
+        ("num_valid", c_void_p), ("x", c_void_p), ("y", c_void_p), ("dy", c_void_p), ("dx", c_void_p),
+        ("weight", c_void_p), ("bias", c_void_p), ("running_mean", c_void_p), ("running_var", c_void_p),
+        ("num_batches_tracked", c_void_p), ("momentum", c_float), ("cumulative", c_int), ("eps", c_float),
+        ("save_mean", c_void_p), ("save_invstd", c_void_p), ("dweight", c_void_p), ("dbias", c_void_p),
+        ("local", c_void_p), ("gathered", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); also the list the CPU test checks against the header
 SIGNATURES = {
     "spx_last_error": (c_char_p, []),
@@ -125,6 +137,7 @@ SIGNATURES = {
     "spx_peer_push": (c_int, [POINTER(PeerGroup), c_void_p, c_int64, c_int, c_void_p]),
     "spx_peer_finish": (c_int, [POINTER(PeerGroup), c_void_p, c_int64, c_int, c_float, c_void_p]),
     "spx_peer_allreduce": (c_int, [POINTER(PeerGroup), c_void_p, c_int64, c_int, c_float, c_void_p]),
+    "spx_peer_allgather": (c_int, [POINTER(PeerGroup), c_void_p, c_int64, c_void_p, c_void_p]),
     "spx_bias_act_inplace": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_float,
                                      c_void_p]),
     "spx_implicit_gemm_fwd_int8": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p,
@@ -188,6 +201,9 @@ SIGNATURES = {
     "spx_masked_bn_bwd_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_masked_bn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "spx_masked_sync_bn_workspace_size": (c_size_t, [c_int64, c_int]),
+    **{f"spx_masked_sync_bn_{p}": (c_int, [POINTER(MaskedSyncBN), c_void_p, c_size_t, c_void_p])
+       for p in ("fwd_local", "fwd_merge", "bwd_local", "bwd_merge")},
     "spx_hash_workspace_size": (c_size_t, [c_int64, c_int64]),
     "spx_hash_clear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     "spx_hash_insert": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,

@@ -166,25 +166,18 @@ __device__ __forceinline__ float bn_lane_sum(float v, float (*buf)[BN_FIN_CH], i
     return total;
 }
 
-template <typename P>
-__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
-bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
-                       const int32_t *__restrict__ num_valid, const P *__restrict__ weight, const P *__restrict__ bias,
-                       P *__restrict__ running_mean, P *__restrict__ running_var,
-                       const int64_t *__restrict__ num_batches_tracked, float momentum, int cumulative, float eps,
-                       float *__restrict__ save_mean, float *__restrict__ save_invstd, float *__restrict__ coef) {
-    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
-    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
-    const int c = blockIdx.x * BN_FIN_CH + cl;
-    const bool active = c < channels;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+// Sum of the valid rows and M2 about their mean, from the chunk partials: sum = lane tree of n_k * mean_k, mean =
+// sum / M, m2 = lane tree of q_k + n_k * (mean_k - mean)^2.  Every thread of the channel gets all three.
+__device__ __forceinline__ void bn_fwd_sums(const float2 *__restrict__ partials, int64_t M, int channels, int c,
+                                            bool active, float (*buf)[BN_FIN_CH], int pl, int cl, float &sum,
+                                            float &mean, float &m2) {
     const int64_t K = (M + BN_CHUNK - 1) / BN_CHUNK;
     float s = 0.f;
     if (active)
         for (int64_t k = pl; k < K; k += BN_FIN_LANES) s = fmaf(bn_chunk_count(k, M), partials[k * channels + c].x, s);
     const float Mf = (float)M;
-    const float sum = bn_lane_sum(s, buf, pl, cl);
-    const float mean = M > 0 ? __fdiv_rn(sum, Mf) : 0.f;
+    sum = bn_lane_sum(s, buf, pl, cl);
+    mean = M > 0 ? __fdiv_rn(sum, Mf) : 0.f;
     float q = 0.f;
     if (active)
         for (int64_t k = pl; k < K; k += BN_FIN_LANES) {
@@ -192,8 +185,19 @@ bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
             const float d = p.x - mean;
             q += fmaf(bn_chunk_count(k, M) * d, d, p.y);
         }
-    const float m2 = bn_lane_sum(q, buf, pl, cl);
-    if (pl != 0 || !active) return;
+    m2 = bn_lane_sum(q, buf, pl, cl);
+}
+
+// Channel c of a batch of M rows with this mean and M2: save_mean / save_invstd, the apply coefficients and the
+// running-stat update.
+template <typename P>
+__device__ __forceinline__ void bn_fwd_write(int c, int channels, int64_t M, float mean, float m2,
+                                             const P *__restrict__ weight, const P *__restrict__ bias,
+                                             P *__restrict__ running_mean, P *__restrict__ running_var,
+                                             const int64_t *__restrict__ num_batches_tracked, float momentum,
+                                             int cumulative, float eps, float *__restrict__ save_mean,
+                                             float *__restrict__ save_invstd, float *__restrict__ coef) {
+    const float Mf = (float)M;
     const float var = M > 0 ? __fdiv_rn(m2, Mf) : 0.f;
     const float invstd = __frsqrt_rn(var + eps);
     const float gamma = weight ? to_float(weight[c]) : 1.f;
@@ -211,6 +215,25 @@ bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
         running_mean[c] = from_float<P>((1.f - f) * to_float(running_mean[c]) + f * mean);
         running_var[c] = from_float<P>((1.f - f) * to_float(running_var[c]) + f * unbiased);
     }
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
+bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
+                       const int32_t *__restrict__ num_valid, const P *__restrict__ weight, const P *__restrict__ bias,
+                       P *__restrict__ running_mean, P *__restrict__ running_var,
+                       const int64_t *__restrict__ num_batches_tracked, float momentum, int cumulative, float eps,
+                       float *__restrict__ save_mean, float *__restrict__ save_invstd, float *__restrict__ coef) {
+    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
+    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
+    const int c = blockIdx.x * BN_FIN_CH + cl;
+    const bool active = c < channels;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    float sum, mean, m2;
+    bn_fwd_sums(partials, M, channels, c, active, buf, pl, cl, sum, mean, m2);
+    if (pl != 0 || !active) return;
+    bn_fwd_write<P>(c, channels, M, mean, m2, weight, bias, running_mean, running_var, num_batches_tracked, momentum,
+                    cumulative, eps, save_mean, save_invstd, coef);
 }
 
 template <typename T, int W, bool V>
@@ -308,6 +331,34 @@ bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t 
     }
 }
 
+// Lane trees of the backward partials: sum(dy) and sum(dy * xhat) over the valid rows.
+__device__ __forceinline__ void bn_bwd_sums(const float2 *__restrict__ partials, int64_t M, int channels, int c,
+                                            bool active, float (*buf)[BN_FIN_CH], int pl, int cl, float &sdy,
+                                            float &sdyx) {
+    const int64_t K = (M + BN_CHUNK - 1) / BN_CHUNK;
+    float a = 0.f, b = 0.f;
+    if (active)
+        for (int64_t k = pl; k < K; k += BN_FIN_LANES) {
+            const float2 p = partials[k * channels + c];
+            a += p.x;
+            b += p.y;
+        }
+    sdy = bn_lane_sum(a, buf, pl, cl);
+    sdyx = bn_lane_sum(b, buf, pl, cl);
+}
+
+// the dx coefficients of channel c from the sums over a batch of M rows
+template <typename P>
+__device__ __forceinline__ void bn_bwd_write(int c, int channels, int64_t M, float sdy, float sdyx,
+                                             const P *__restrict__ weight, const float *__restrict__ save_invstd,
+                                             float *__restrict__ coef) {
+    const float Mf = (float)M;
+    const float gamma = weight ? to_float(weight[c]) : 1.f;
+    coef[c] = gamma * save_invstd[c];
+    coef[channels + c] = M > 0 ? __fdiv_rn(sdy, Mf) : 0.f;
+    coef[2 * channels + c] = M > 0 ? __fdiv_rn(sdyx, Mf) : 0.f;
+}
+
 template <typename P>
 __global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
 bn_bwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
@@ -319,24 +370,12 @@ bn_bwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
     const int c = blockIdx.x * BN_FIN_CH + cl;
     const bool active = c < channels;
     const int64_t M = bn_valid_rows(num_valid, rows);
-    const int64_t K = (M + BN_CHUNK - 1) / BN_CHUNK;
-    float a = 0.f, b = 0.f;
-    if (active)
-        for (int64_t k = pl; k < K; k += BN_FIN_LANES) {
-            const float2 p = partials[k * channels + c];
-            a += p.x;
-            b += p.y;
-        }
-    const float sdy = bn_lane_sum(a, buf, pl, cl);
-    const float sdyx = bn_lane_sum(b, buf, pl, cl);
+    float sdy, sdyx;
+    bn_bwd_sums(partials, M, channels, c, active, buf, pl, cl, sdy, sdyx);
     if (pl != 0 || !active) return;
     if (dbias) dbias[c] = from_float<P>(sdy);
     if (dweight) dweight[c] = from_float<P>(sdyx);
-    const float Mf = (float)M;
-    const float gamma = weight ? to_float(weight[c]) : 1.f;
-    coef[c] = gamma * save_invstd[c];
-    coef[channels + c] = M > 0 ? __fdiv_rn(sdy, Mf) : 0.f;
-    coef[2 * channels + c] = M > 0 ? __fdiv_rn(sdyx, Mf) : 0.f;
+    bn_bwd_write<P>(c, channels, M, sdy, sdyx, weight, save_invstd, coef);
 }
 
 template <typename T, int W, bool V>
@@ -365,6 +404,127 @@ bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
     bn_store<T, W, V>(dx + r * channels + v * W, f);
+}
+
+// ---------------------------------------------------------------- cross-rank statistics (MaskedSyncBatchNorm1d)
+// Each rank reduces its own rows with the kernels above, then a local kernel writes its vector
+// [M_r, A_r[C], B_r[C]] (fp32, M_r exact below 2^24).  The vectors of all ranks are gathered in rank order, and a
+// merge kernel (one thread per channel) folds them in rank order, the same on every rank:
+//   forward : A_r = sum of the rank's rows, B_r = M2 about the rank's own mean A_r / M_r; M = sum of M_r in int64,
+//             mean = (sum A_r) / M, M2 = sum [B_r + M_r (A_r / M_r - mean)^2].
+//   backward: A_r = sum(dy), B_r = sum(dy * xhat) about the global mean / invstd; the merge sums them.  dweight /
+//             dbias are the rank-local A_r / B_r, written by the local kernel.
+// One rank: the merge is the finalize above operation for operation (its extra term is M_0 * 0^2 = +0), so the
+// results equal MaskedBatchNorm1d bit for bit.  A count that is not a number in [0, 2^24] (a timed-out exchange
+// delivers NaN) makes every statistic and coefficient NaN.
+constexpr float BN_SYNC_MAX_ROWS = 16777216.f;        // 2^24: every count is an exact fp32 integer
+
+__device__ __forceinline__ void bn_sync_write_local(float *__restrict__ local, int channels, int64_t M, int c,
+                                                    bool active, int pl, float a, float b) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) local[0] = (float)M;
+    if (pl != 0 || !active) return;
+    local[1 + c] = a;
+    local[1 + channels + c] = b;
+}
+
+__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
+bn_sync_fwd_local_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
+                         const int32_t *__restrict__ num_valid, float *__restrict__ local) {
+    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
+    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
+    const int c = blockIdx.x * BN_FIN_CH + cl;
+    const bool active = c < channels;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    float sum, mean, m2;
+    bn_fwd_sums(partials, M, channels, c, active, buf, pl, cl, sum, mean, m2);
+    bn_sync_write_local(local, channels, M, c, active, pl, sum, m2);
+}
+
+// rank-order total of the gathered counts; false when one is not a count
+__device__ __forceinline__ bool bn_sync_count(const float *__restrict__ gathered, int world, int64_t stride,
+                                              int64_t &M) {
+    M = 0;
+    bool ok = true;
+    for (int r = 0; r < world; ++r) {
+        const float n = gathered[r * stride];
+        ok = ok && n >= 0.f && n <= BN_SYNC_MAX_ROWS;
+        M += ok ? (int64_t)n : 0;
+    }
+    return ok;
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_sync_fwd_merge_kernel(const float *__restrict__ gathered, int world, int channels, const P *__restrict__ weight,
+                         const P *__restrict__ bias, P *__restrict__ running_mean, P *__restrict__ running_var,
+                         const int64_t *__restrict__ num_batches_tracked, float momentum, int cumulative, float eps,
+                         float *__restrict__ save_mean, float *__restrict__ save_invstd, float *__restrict__ coef) {
+    const int c = blockIdx.x * BN_THREADS + threadIdx.x;
+    if (c >= channels) return;
+    const int64_t stride = 2 * (int64_t)channels + 1;
+    int64_t M;
+    if (!bn_sync_count(gathered, world, stride, M)) {
+        const float nan = __int_as_float(0x7fc00000);
+        save_mean[c] = save_invstd[c] = coef[c] = coef[channels + c] = coef[2 * channels + c] = nan;
+        if (running_mean != nullptr) running_mean[c] = running_var[c] = from_float<P>(nan);
+        return;
+    }
+    float sum = 0.f;
+    for (int r = 0; r < world; ++r) {
+        const float a = gathered[r * stride + 1 + c];
+        sum = r == 0 ? a : sum + a;
+    }
+    const float mean = M > 0 ? __fdiv_rn(sum, (float)M) : 0.f;
+    float m2 = 0.f;
+    for (int r = 0; r < world; ++r) {
+        const float *v = gathered + r * stride;
+        const float n = v[0];
+        const float d = (n > 0.f ? __fdiv_rn(v[1 + c], n) : 0.f) - mean;
+        const float t = fmaf(n * d, d, v[1 + channels + c]);
+        m2 = r == 0 ? t : m2 + t;
+    }
+    bn_fwd_write<P>(c, channels, M, mean, m2, weight, bias, running_mean, running_var, num_batches_tracked, momentum,
+                    cumulative, eps, save_mean, save_invstd, coef);
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_FIN_CH * BN_FIN_LANES)
+bn_sync_bwd_local_kernel(const float2 *__restrict__ partials, int64_t rows, int channels,
+                         const int32_t *__restrict__ num_valid, P *__restrict__ dweight, P *__restrict__ dbias,
+                         float *__restrict__ local) {
+    __shared__ float buf[BN_FIN_LANES][BN_FIN_CH];
+    const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
+    const int c = blockIdx.x * BN_FIN_CH + cl;
+    const bool active = c < channels;
+    const int64_t M = bn_valid_rows(num_valid, rows);
+    float sdy, sdyx;
+    bn_bwd_sums(partials, M, channels, c, active, buf, pl, cl, sdy, sdyx);
+    if (pl == 0 && active) {
+        if (dbias) dbias[c] = from_float<P>(sdy);
+        if (dweight) dweight[c] = from_float<P>(sdyx);
+    }
+    bn_sync_write_local(local, channels, M, c, active, pl, sdy, sdyx);
+}
+
+template <typename P>
+__global__ void __launch_bounds__(BN_THREADS)
+bn_sync_bwd_merge_kernel(const float *__restrict__ gathered, int world, int channels, const P *__restrict__ weight,
+                         const float *__restrict__ save_invstd, float *__restrict__ coef) {
+    const int c = blockIdx.x * BN_THREADS + threadIdx.x;
+    if (c >= channels) return;
+    const int64_t stride = 2 * (int64_t)channels + 1;
+    int64_t M;
+    if (!bn_sync_count(gathered, world, stride, M)) {
+        coef[c] = coef[channels + c] = coef[2 * channels + c] = __int_as_float(0x7fc00000);
+        return;
+    }
+    float sdy = 0.f, sdyx = 0.f;
+    for (int r = 0; r < world; ++r) {
+        const float a = gathered[r * stride + 1 + c], b = gathered[r * stride + 1 + channels + c];
+        sdy = r == 0 ? a : sdy + a;
+        sdyx = r == 0 ? b : sdyx + b;
+    }
+    bn_bwd_write<P>(c, channels, M, sdy, sdyx, weight, save_invstd, coef);
 }
 
 // ---------------------------------------------------------------- host side
@@ -577,4 +737,149 @@ extern "C" int spx_masked_bn_bwd(const void *x, const void *dy, void *dx, int64_
     }
     if (rc || rows == 0) return rc;
     return bn_bwd_rows_typed(dtype, a, false, stream);
+}
+
+// ---------------------------------------------------------------- cross-rank BatchNorm (MaskedSyncBatchNorm1d)
+namespace spx {
+
+static int bn_sync_check(const char *who, const spx_masked_sync_bn *d, bool merge, size_t workspace_bytes,
+                         const void *workspace) {
+    SPX_REQUIRE(d != nullptr, "%s: descriptor is NULL", who);
+    if (int rc = bn_check(who, d->rows, d->channels, d->dtype, d->param_dtype)) return rc;
+    SPX_REQUIRE(d->rows <= (1 << 24), "%s: %lld rows, at most 2^24 per rank and call", who, (long long)d->rows);
+    SPX_REQUIRE(workspace != nullptr, "%s: NULL pointer argument (workspace)", who);
+    const size_t need = spx_masked_sync_bn_workspace_size(d->rows, d->channels);
+    SPX_REQUIRE(workspace_bytes >= need, "%s: workspace too small: need %zu, have %zu", who, need, workspace_bytes);
+    if (merge) {
+        SPX_REQUIRE(d->world >= 1 && d->world <= SPX_MAX_PEERS, "%s: world %d out of range (1..%d)", who, d->world,
+                    SPX_MAX_PEERS);
+        SPX_REQUIRE(d->gathered != nullptr, "%s: NULL pointer argument (gathered)", who);
+    } else {
+        SPX_REQUIRE(d->local != nullptr, "%s: NULL pointer argument (local)", who);
+    }
+    return 0;
+}
+
+static BnFwdArgs bn_sync_fwd_args(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes) {
+    BnFwdArgs a{d->x, d->y, d->rows, d->channels, d->num_valid, d->weight, d->bias, d->running_mean,
+                d->running_var, d->num_batches_tracked, d->momentum, d->cumulative, d->eps, d->save_mean,
+                d->save_invstd, nullptr, nullptr};
+    WorkspaceCarver ws(workspace, workspace_bytes);
+    a.partials = ws.take<float2>((size_t)bn_chunks(d->rows) * d->channels);
+    a.coef = ws.take<float>((size_t)3 * d->channels);
+    return a;
+}
+
+static BnBwdArgs bn_sync_bwd_args(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes) {
+    BnBwdArgs a{d->x, d->dy, d->dx, d->rows, d->channels, d->num_valid, d->weight, d->save_mean, d->save_invstd,
+                d->dweight, d->dbias, nullptr, nullptr};
+    WorkspaceCarver ws(workspace, workspace_bytes);
+    a.partials = ws.take<float2>((size_t)bn_chunks(d->rows) * d->channels);
+    a.coef = ws.take<float>((size_t)3 * d->channels);
+    return a;
+}
+
+static unsigned bn_fin_blocks(int channels) { return (unsigned)div_up64(channels, BN_FIN_CH); }
+static unsigned bn_merge_blocks(int channels) { return (unsigned)div_up64(channels, BN_THREADS); }
+
+template <typename P> static int bn_sync_fwd_merge(const spx_masked_sync_bn *d, const BnFwdArgs &a, cudaStream_t stream) {
+    bn_sync_fwd_merge_kernel<P><<<bn_merge_blocks(a.channels), BN_THREADS, 0, stream>>>(
+        d->gathered, d->world, a.channels, static_cast<const P *>(a.weight), static_cast<const P *>(a.bias),
+        static_cast<P *>(a.running_mean), static_cast<P *>(a.running_var), a.nbt, a.momentum, a.cumulative, a.eps,
+        a.save_mean, a.save_invstd, a.coef);
+    SPX_CHECK_LAUNCH("bn_sync_fwd_merge_kernel");
+    return 0;
+}
+
+template <typename P> static int bn_sync_bwd_local(const spx_masked_sync_bn *d, const BnBwdArgs &a, cudaStream_t stream) {
+    bn_sync_bwd_local_kernel<P><<<bn_fin_blocks(a.channels), BN_FIN_CH * BN_FIN_LANES, 0, stream>>>(
+        a.partials, a.rows, a.channels, a.num_valid, static_cast<P *>(a.dweight), static_cast<P *>(a.dbias), d->local);
+    SPX_CHECK_LAUNCH("bn_sync_bwd_local_kernel");
+    return 0;
+}
+
+template <typename P> static int bn_sync_bwd_merge(const spx_masked_sync_bn *d, const BnBwdArgs &a, cudaStream_t stream) {
+    bn_sync_bwd_merge_kernel<P><<<bn_merge_blocks(a.channels), BN_THREADS, 0, stream>>>(
+        d->gathered, d->world, a.channels, static_cast<const P *>(a.weight), a.save_invstd, a.coef);
+    SPX_CHECK_LAUNCH("bn_sync_bwd_merge_kernel");
+    return 0;
+}
+
+}  // namespace spx
+
+extern "C" size_t spx_masked_sync_bn_workspace_size(int64_t rows, int channels) {
+    return bn_workspace(rows, channels, 3);
+}
+
+extern "C" int spx_masked_sync_bn_fwd_local(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                            spx_stream_t stream_) {
+    const char *who = "masked_sync_bn_fwd_local";
+    if (int rc = bn_sync_check(who, d, false, workspace_bytes, workspace)) return rc;
+    SPX_REQUIRE(d->rows == 0 || d->x, "%s: NULL pointer argument (x)", who);
+    const BnFwdArgs a = bn_sync_fwd_args(d, workspace, workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (d->rows > 0)
+        if (int rc = bn_fwd_rows_typed(d->dtype, a, true, stream)) return rc;
+    bn_sync_fwd_local_kernel<<<bn_fin_blocks(a.channels), BN_FIN_CH * BN_FIN_LANES, 0, stream>>>(
+        a.partials, a.rows, a.channels, a.num_valid, d->local);
+    SPX_CHECK_LAUNCH("bn_sync_fwd_local_kernel");
+    return 0;
+}
+
+extern "C" int spx_masked_sync_bn_fwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                            spx_stream_t stream_) {
+    const char *who = "masked_sync_bn_fwd_merge";
+    if (int rc = bn_sync_check(who, d, true, workspace_bytes, workspace)) return rc;
+    SPX_REQUIRE(d->save_mean && d->save_invstd, "%s: NULL pointer argument (save_mean, save_invstd)", who);
+    SPX_REQUIRE(d->rows == 0 || (d->x && d->y), "%s: NULL pointer argument (x, y)", who);
+    SPX_REQUIRE((d->running_mean == nullptr) == (d->running_var == nullptr),
+                "%s: running_mean and running_var must both be given or both be NULL", who);
+    SPX_REQUIRE(!(d->running_mean && d->cumulative && d->num_batches_tracked == nullptr),
+                "%s: a cumulative average (momentum None) needs num_batches_tracked", who);
+    SPX_REQUIRE(d->eps > 0.f, "%s: eps must be positive", who);
+    const BnFwdArgs a = bn_sync_fwd_args(d, workspace, workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int rc = 0;
+    switch (d->param_dtype) {
+        case SPX_F32: rc = bn_sync_fwd_merge<float>(d, a, stream); break;
+        case SPX_F16: rc = bn_sync_fwd_merge<__half>(d, a, stream); break;
+        default: rc = bn_sync_fwd_merge<__nv_bfloat16>(d, a, stream); break;
+    }
+    if (rc || d->rows == 0) return rc;
+    return bn_fwd_rows_typed(d->dtype, a, false, stream);
+}
+
+extern "C" int spx_masked_sync_bn_bwd_local(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                            spx_stream_t stream_) {
+    const char *who = "masked_sync_bn_bwd_local";
+    if (int rc = bn_sync_check(who, d, false, workspace_bytes, workspace)) return rc;
+    SPX_REQUIRE(d->save_mean && d->save_invstd, "%s: NULL pointer argument (save_mean, save_invstd)", who);
+    SPX_REQUIRE(d->rows == 0 || (d->x && d->dy), "%s: NULL pointer argument (x, dy)", who);
+    const BnBwdArgs a = bn_sync_bwd_args(d, workspace, workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (d->rows > 0)
+        if (int rc = bn_bwd_rows_typed(d->dtype, a, true, stream)) return rc;
+    switch (d->param_dtype) {
+        case SPX_F32: return bn_sync_bwd_local<float>(d, a, stream);
+        case SPX_F16: return bn_sync_bwd_local<__half>(d, a, stream);
+        default: return bn_sync_bwd_local<__nv_bfloat16>(d, a, stream);
+    }
+}
+
+extern "C" int spx_masked_sync_bn_bwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
+                                            spx_stream_t stream_) {
+    const char *who = "masked_sync_bn_bwd_merge";
+    if (int rc = bn_sync_check(who, d, true, workspace_bytes, workspace)) return rc;
+    SPX_REQUIRE(d->save_mean && d->save_invstd, "%s: NULL pointer argument (save_mean, save_invstd)", who);
+    SPX_REQUIRE(d->rows == 0 || (d->x && d->dy && d->dx), "%s: NULL pointer argument (x, dy, dx)", who);
+    const BnBwdArgs a = bn_sync_bwd_args(d, workspace, workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int rc = 0;
+    switch (d->param_dtype) {
+        case SPX_F32: rc = bn_sync_bwd_merge<float>(d, a, stream); break;
+        case SPX_F16: rc = bn_sync_bwd_merge<__half>(d, a, stream); break;
+        default: rc = bn_sync_bwd_merge<__nv_bfloat16>(d, a, stream); break;
+    }
+    if (rc || d->rows == 0) return rc;
+    return bn_bwd_rows_typed(d->dtype, a, false, stream);
 }

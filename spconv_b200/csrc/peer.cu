@@ -29,6 +29,10 @@
 // layer instead of a collective launch).  bench.py therefore defaults to the NCCL hook for the graph-replayed
 // headline and keeps this path selectable (--allreduce fused).
 //
+// Gather mode (spx_peer_allgather, MaskedSyncBatchNorm1d's statistics): the same push and the same finish with
+// GATHER set, which copies every rank's slice to dst[r] as 32-bit words instead of summing them.  Publish, wait,
+// timeout and the epoch advance are the one code path of the sum, so the slot protocol below covers both.
+//
 // No grid-wide barrier, no host involvement.  Neither kernel waits for a peer before it has published, so ranks
 // cannot deadlock each other; a peer that never shows up trips the group's timeout in finish (error word +
 // NaN result) instead of hanging the GPU.  Two slots alternate by epoch: rank r overwrites slot e&1 in its
@@ -125,7 +129,8 @@ peer_push_kernel(const float *__restrict__ partial, int64_t stride, int chunks, 
 constexpr int FIN_CHUNK_BYTES = 8192;              // per source rank per step: world x 8 KB in flight per CTA
 constexpr int FIN_MAX_CTAS = 64;               // 0.44 MB per peer = 54 chunks: one round trip for the whole tensor
 
-template <typename T>
+// GATHER: dst is [world][total] 32-bit words (T = uint32_t), rank r's slice copied unchanged to dst[r]; scale unused.
+template <typename T, bool GATHER>
 __global__ void __launch_bounds__(PX_THREADS)
 peer_finish_kernel(T *__restrict__ dst, int64_t total, PeerPtrs peers, int world, int rank, int64_t capacity, float scale,
                    unsigned long long timeout_ns) {
@@ -176,18 +181,33 @@ peer_finish_kernel(T *__restrict__ dst, int64_t total, PeerPtrs peers, int world
         }
         mbar_wait(&bar, phase);
         phase ^= 1u;
-        for (int j = threadIdx.x * 4; j < nfl; j += PX_THREADS * 4) {
-            float4 t = *reinterpret_cast<const float4 *>(fin_smem + (size_t)j * 4);
-            for (int r = 1; r < world; ++r) {                          // rank order: identical bits on every rank
-                const float4 v = *reinterpret_cast<const float4 *>(fin_smem + (size_t)r * FIN_CHUNK_BYTES + (size_t)j * 4);
-                t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+        if constexpr (GATHER) {
+            for (int j = threadIdx.x * 4; j < nfl; j += PX_THREADS * 4) {
+                const int64_t i = f0 + j;
+                for (int r = 0; r < world; ++r) {                      // word copies: the bits every rank sent
+                    uint4 w = *reinterpret_cast<const uint4 *>(fin_smem + (size_t)r * FIN_CHUNK_BYTES + (size_t)j * 4);
+                    if (bad) w = make_uint4(0x7fc00000u, 0x7fc00000u, 0x7fc00000u, 0x7fc00000u);
+                    T *d = dst + (int64_t)r * total + i;
+                    d[0] = w.x;
+                    if (i + 1 < total) d[1] = w.y;
+                    if (i + 2 < total) d[2] = w.z;
+                    if (i + 3 < total) d[3] = w.w;
+                }
             }
-            if (bad) t = make_float4(nan, nan, nan, nan);
-            const int64_t i = f0 + j;
-            dst[i] = from_float<T>(t.x * scale);
-            if (i + 1 < total) dst[i + 1] = from_float<T>(t.y * scale);
-            if (i + 2 < total) dst[i + 2] = from_float<T>(t.z * scale);
-            if (i + 3 < total) dst[i + 3] = from_float<T>(t.w * scale);
+        } else {
+            for (int j = threadIdx.x * 4; j < nfl; j += PX_THREADS * 4) {
+                float4 t = *reinterpret_cast<const float4 *>(fin_smem + (size_t)j * 4);
+                for (int r = 1; r < world; ++r) {                      // rank order: identical bits on every rank
+                    const float4 v = *reinterpret_cast<const float4 *>(fin_smem + (size_t)r * FIN_CHUNK_BYTES + (size_t)j * 4);
+                    t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w;
+                }
+                if (bad) t = make_float4(nan, nan, nan, nan);
+                const int64_t i = f0 + j;
+                dst[i] = from_float<T>(t.x * scale);
+                if (i + 1 < total) dst[i + 1] = from_float<T>(t.y * scale);
+                if (i + 2 < total) dst[i + 2] = from_float<T>(t.z * scale);
+                if (i + 3 < total) dst[i + 3] = from_float<T>(t.w * scale);
+            }
         }
         __syncthreads();                                               // the chunk is consumed before it is overwritten
     }
@@ -239,8 +259,10 @@ int peer_push(const float *partial, int64_t stride, int chunks, const void *src,
     return 0;
 }
 
-int peer_finish(void *dst, int64_t total, int dtype, const spx_peer_group *pg, float scale, cudaStream_t stream) {
-    if (int rc = check_group(pg, total, "peer finish")) return rc;
+// gather: dst [world][total] 32-bit words; dtype and scale are ignored
+static int peer_finish_any(void *dst, int64_t total, int dtype, const spx_peer_group *pg, float scale, bool gather,
+                           cudaStream_t stream) {
+    if (int rc = check_group(pg, total, gather ? "peer allgather" : "peer finish")) return rc;
     if (total == 0) return 0;
     const PeerPtrs pp = peer_ptrs(pg);
     const int64_t cap = (int64_t)(pg->capacity_bytes / 4);
@@ -250,21 +272,26 @@ int peer_finish(void *dst, int64_t total, int dtype, const spx_peer_group *pg, f
     const unsigned grid = (unsigned)(nchunks < max_ctas ? nchunks : max_ctas);
     const size_t smem = (size_t)pg->world * FIN_CHUNK_BYTES;
     const unsigned long long timeout_ns = (unsigned long long)(pg->timeout_ms > 0 ? pg->timeout_ms : 20000) * 1000000ull;
-#define PX_LAUNCH(T)                                                                                                  \
+#define PX_LAUNCH(T, G)                                                                                               \
     do {                                                                                                              \
-        auto fn = peer_finish_kernel<T>;                                                                              \
+        auto fn = peer_finish_kernel<T, G>;                                                                            \
         if (smem > 48 * 1024 && !func_configured((const void *)fn, current_device()))                                 \
             SPX_CHECK_CUDA(cudaFuncSetAttribute((const void *)fn, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
                                                 SPX_MAX_PEERS * FIN_CHUNK_BYTES));                                    \
         fn<<<grid, PX_THREADS, smem, stream>>>((T *)dst, total, pp, pg->world, pg->rank, cap, scale, timeout_ns);     \
     } while (0)
-    if (dtype == SPX_F16) PX_LAUNCH(__half);
-    else if (dtype == SPX_BF16) PX_LAUNCH(__nv_bfloat16);
-    else if (dtype == SPX_F32) PX_LAUNCH(float);
+    if (gather) PX_LAUNCH(uint32_t, true);
+    else if (dtype == SPX_F16) PX_LAUNCH(__half, false);
+    else if (dtype == SPX_BF16) PX_LAUNCH(__nv_bfloat16, false);
+    else if (dtype == SPX_F32) PX_LAUNCH(float, false);
     else { set_error("peer finish: dtype %d not supported", dtype); return 2; }
 #undef PX_LAUNCH
     SPX_CHECK_LAUNCH("peer_finish_kernel");
     return 0;
+}
+
+int peer_finish(void *dst, int64_t total, int dtype, const spx_peer_group *pg, float scale, cudaStream_t stream) {
+    return peer_finish_any(dst, total, dtype, pg, scale, false, stream);
 }
 
 }  // namespace spx
@@ -339,4 +366,13 @@ extern "C" int spx_peer_allreduce(const spx_peer_group *pg, void *data, int64_t 
                                   spx_stream_t stream) {
     if (int rc = spx_peer_push(pg, data, count, dtype, stream)) return rc;
     return spx_peer_finish(pg, data, count, dtype, scale, stream);
+}
+
+extern "C" int spx_peer_allgather(const spx_peer_group *pg, const uint32_t *src, int64_t count, uint32_t *dst,
+                                  spx_stream_t stream) {
+    SPX_REQUIRE(count == 0 || (src != nullptr && dst != nullptr), "peer_allgather: NULL src or dst");
+    if (int rc = check_group(pg, count, "peer allgather")) return rc;
+    // the fp32 push reads and stores each word without arithmetic, so the bits arrive unchanged
+    if (int rc = peer_push(nullptr, 0, 0, src, count, SPX_F32, pg, (cudaStream_t)stream)) return rc;
+    return peer_finish_any(dst, count, SPX_F32, pg, 1.f, true, (cudaStream_t)stream);
 }

@@ -501,6 +501,39 @@ class MaskedBatchNormFunction(Function):
 masked_batch_norm = MaskedBatchNormFunction.apply
 
 
+class MaskedSyncBatchNormFunction(Function):
+    """``x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps, transport`` ->
+    training-mode BatchNorm whose statistics cover rows ``[0, num_valid)`` of every rank of ``transport``
+    (:func:`ops.masked_sync_batch_norm_forward`).  The backward exchanges again over the same transport and gives
+    dx (0 on padding rows) and this rank's dweight and dbias."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps,
+                transport):
+        y, mean, invstd = ops.masked_sync_batch_norm_forward(x, num_valid, weight, bias, running_mean, running_var,
+                                                             num_batches_tracked, momentum, eps, transport)
+        ctx.save_for_backward(x, weight, mean, invstd, num_valid)
+        ctx.transport = transport
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        x, weight, mean, invstd, num_valid = ctx.saved_tensors
+        dx, dw, db = ops.masked_sync_batch_norm_backward(x, grad_output, num_valid, weight, mean, invstd,
+                                                         ctx.transport, ctx.needs_input_grad[1],
+                                                         ctx.needs_input_grad[2])
+        return dx, dw, db, None, None, None, None, None, None, None
+
+
+def masked_sync_batch_norm(x, weight, bias, running_mean, running_var, num_batches_tracked, num_valid, momentum, eps,
+                           process_group=None):
+    """:class:`MaskedSyncBatchNormFunction` over the transport :func:`ops.sync_bn_transport` picks for
+    ``process_group``: the installed peer group, else ``torch.distributed``, else this rank alone."""
+    return MaskedSyncBatchNormFunction.apply(x, weight, bias, running_mean, running_var, num_batches_tracked,
+                                             num_valid, momentum, eps, ops.sync_bn_transport(process_group))
+
+
 # ---------------------------------------------------------------------------- padding-aware global pooling
 class MaskedGlobalPoolFunction(Function):
     """``features, indices, batch_size, num_valid, is_mean`` -> ``[batch_size, C]``: per-sample max or mean over

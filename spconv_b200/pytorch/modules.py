@@ -136,10 +136,27 @@ class SparseBatchNorm(_FeatureWise):
         super().__init__(nn.BatchNorm1d(num_features, eps, momentum, affine, track_running_stats))
 
     def forward(self, x: SparseConvTensor):
-        if isinstance(self.inner, MaskedBatchNorm1d):
+        if isinstance(self.inner, (MaskedBatchNorm1d, MaskedSyncBatchNorm1d)):
             return self.inner(x)
         if self.inner.training:
             x.require_unpadded("SparseBatchNorm in training mode")
+        return super().forward(x)
+
+
+class SparseSyncBatchNorm(_FeatureWise):
+    """``nn.SyncBatchNorm`` on the features (``spconv.pytorch.SparseSyncBatchNorm``).  It counts every row as
+    data, so it refuses a padded tensor in training; :meth:`MaskedSyncBatchNorm1d.convert_masked_sync_batchnorm`
+    turns its ``inner`` into the padding-aware :class:`MaskedSyncBatchNorm1d`."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True,
+                 process_group=None):
+        super().__init__(nn.SyncBatchNorm(num_features, eps, momentum, affine, track_running_stats, process_group))
+
+    def forward(self, x: SparseConvTensor):
+        if isinstance(self.inner, MaskedSyncBatchNorm1d):
+            return self.inner(x)
+        if self.inner.training:
+            x.require_unpadded("SparseSyncBatchNorm in training mode")
         return super().forward(x)
 
 
@@ -208,6 +225,89 @@ class MaskedBatchNorm1d(SparseModule, nn.BatchNorm1d):
     @classmethod
     def _from_batchnorm(cls, bn: nn.BatchNorm1d) -> "MaskedBatchNorm1d":
         out = cls(bn.num_features, bn.eps, bn.momentum, bn.affine, bn.track_running_stats, device="meta")
+        if bn.affine:
+            out.weight = bn.weight
+            out.bias = bn.bias
+        out.running_mean = bn.running_mean
+        out.running_var = bn.running_var
+        out.num_batches_tracked = bn.num_batches_tracked
+        out.training = bn.training
+        return out
+
+
+class MaskedSyncBatchNorm1d(SparseModule, nn.SyncBatchNorm):
+    """:class:`MaskedBatchNorm1d` whose training statistics cover the valid rows of every data-parallel rank, as
+    ``nn.SyncBatchNorm`` does for dense tensors, but padding-aware.  Same constructor, parameters, buffers and
+    ``state_dict`` keys as ``nn.SyncBatchNorm``; convert a net with :meth:`convert_masked_sync_batchnorm`.
+
+    Each rank reduces its own valid rows (``x.num_valid``) with the kernels of ``csrc/batchnorm.cu`` into a vector
+    of its count, sum and M2; the vectors are gathered in rank order and merged in that order on every rank, so
+    mean, invstd, the running stats and y are computed from the same bits everywhere.  The exchange runs over the
+    installed peer group (:func:`ops.set_peer_group`) when there is one, else over ``torch.distributed``
+    (``process_group``, default the world) when it has more than one rank; with one rank there is no exchange
+    and every result equals :class:`MaskedBatchNorm1d` bit for bit.  Nothing is read back to the host, so a
+    training step captures as one CUDA graph.
+
+    The backward exchanges the sums of dy and dy * xhat the same way, so dx uses the global sums.  The
+    parameter gradients dweight / dbias are this rank's own sums, as in ``nn.SyncBatchNorm``: reduce them with
+    the other parameter gradients (DDP, ``GradBucket``, ``ops.peer_allreduce_``).
+
+    Every rank must call every training forward and backward, in the same order as its other exchanges: a
+    rank whose tensor has no rows still joins, takes its running stats from the others, and gets zero
+    dweight / dbias.  ``num_batches_tracked`` counts every training call.  The edge cases of the total count
+    are :class:`MaskedBatchNorm1d`'s.  Eval mode with running stats is torch's ``F.batch_norm``; eval mode
+    without them normalises with this rank's rows alone, like ``nn.SyncBatchNorm``."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True,
+                 process_group=None, device=None, dtype=None):
+        nn.SyncBatchNorm.__init__(self, num_features, eps, momentum, affine, track_running_stats, process_group,
+                                  device, dtype)
+        self.name = None
+        self._sparse_unique_name = ""
+
+    def forward(self, x: SparseConvTensor):
+        feats = x.features
+        if feats.dim() != 2 or feats.shape[1] != self.num_features:
+            raise ValueError(f"MaskedSyncBatchNorm1d({self.num_features}): features of shape {tuple(feats.shape)}")
+        if not self.training:
+            if feats.shape[0] == 0:
+                return x
+            if self.running_mean is not None or self.running_var is not None:
+                return x.replace_feature(nn.functional.batch_norm(
+                    feats, self.running_mean, self.running_var, self.weight, self.bias, False, 0.0, self.eps))
+            return x.replace_feature(functional.masked_batch_norm(
+                feats, self.weight, self.bias, None, None, None, x.num_valid, self.momentum, self.eps))
+        track = self.track_running_stats
+        if track and self.num_batches_tracked is not None:
+            self.num_batches_tracked.add_(1)
+        rm = self.running_mean if track else None
+        rv = self.running_var if track else None
+        return x.replace_feature(functional.masked_sync_batch_norm(
+            feats, self.weight, self.bias, rm, rv, self.num_batches_tracked if rm is not None else None,
+            x.num_valid, self.momentum, self.eps, self.process_group))
+
+    @classmethod
+    def convert_masked_sync_batchnorm(cls, module: nn.Module, process_group=None) -> nn.Module:
+        """Replace, in place, every ``nn.BatchNorm1d``, ``nn.SyncBatchNorm`` and :class:`MaskedBatchNorm1d` (those
+        exact types) that is a direct child of a :class:`SparseSequential`, and the ``inner`` BatchNorm of every
+        :class:`SparseBatchNorm` / :class:`SparseSyncBatchNorm`, by a ``MaskedSyncBatchNorm1d`` that takes over its
+        parameters and buffers; returns ``module``.  ``process_group`` None keeps a ``SyncBatchNorm``'s own group.
+        Other subclasses and BatchNorm layers outside sparse containers (dense heads) are left alone."""
+        kinds = (nn.BatchNorm1d, nn.SyncBatchNorm, MaskedBatchNorm1d)
+        if isinstance(module, SparseSequential):
+            for key, child in list(module._modules.items()):
+                if type(child) in kinds:
+                    module._modules[key] = cls._from_batchnorm(child, process_group)
+        elif isinstance(module, (SparseBatchNorm, SparseSyncBatchNorm)) and type(module.inner) in kinds:
+            module.inner = cls._from_batchnorm(module.inner, process_group)
+        for child in module.children():
+            cls.convert_masked_sync_batchnorm(child, process_group)
+        return module
+
+    @classmethod
+    def _from_batchnorm(cls, bn: nn.modules.batchnorm._BatchNorm, process_group=None) -> "MaskedSyncBatchNorm1d":
+        group = process_group if process_group is not None else getattr(bn, "process_group", None)
+        out = cls(bn.num_features, bn.eps, bn.momentum, bn.affine, bn.track_running_stats, group, device="meta")
         if bn.affine:
             out.weight = bn.weight
             out.bias = bn.bias

@@ -1488,6 +1488,144 @@ def masked_batch_norm_backward(x: torch.Tensor, dy: torch.Tensor, num_valid: Opt
     return dx, dw, db
 
 
+# ---------------------------------------------------------------------------- cross-rank BatchNorm
+SYNC_BN_MAX_ROWS = 1 << 24          # rows per rank and call: every count crosses the exchange as an exact fp32 value
+
+
+class SyncBNTransport:
+    """How the per-rank BatchNorm vectors of one :class:`MaskedSyncBatchNorm1d` call reach every rank.  ``kind`` is
+    "peer" (the installed :class:`~spconv_b200.pytorch.dist.PeerGroup`, ``spx_peer_allgather``), "dist"
+    (``torch.distributed.all_gather_into_tensor`` on ``group``) or "local" (one rank, no exchange).  The forward
+    picks it and its backward reuses it."""
+
+    __slots__ = ("kind", "peers", "group", "world")
+
+    def __init__(self, kind: str, peers=None, group=None, world: int = 1):
+        self.kind, self.peers, self.group, self.world = kind, peers, group, world
+
+
+def sync_bn_transport(process_group=None) -> SyncBNTransport:
+    """The peer route when a group is installed (:func:`set_peer_group`), else ``torch.distributed`` when
+    ``process_group`` (default: the world) has more than one rank, else one rank.  Raises when ``process_group``
+    and the installed peer group disagree on the number of ranks."""
+    import torch.distributed as dist
+    initialized = dist.is_available() and dist.is_initialized()
+    if _PEERS is not None:
+        if process_group is not None and initialized and dist.get_world_size(process_group) != _PEERS.world:
+            raise RuntimeError(f"masked_sync_batch_norm: process_group has {dist.get_world_size(process_group)} ranks, "
+                               f"the installed peer group {_PEERS.world}")
+        return SyncBNTransport("peer", peers=_PEERS, world=_PEERS.world)
+    if initialized:
+        world = dist.get_world_size(process_group)
+        if world > 1:
+            return SyncBNTransport("dist", group=process_group, world=world)
+    return SyncBNTransport("local")
+
+
+def _sync_bn_check(x: torch.Tensor, transport: SyncBNTransport) -> None:
+    rows, c = x.shape
+    if rows > SYNC_BN_MAX_ROWS:
+        raise RuntimeError(f"masked_sync_batch_norm: {rows} rows, at most 2^24 per rank and call")
+    if transport.kind == "peer":
+        if transport.world > _cabi.SPX_MAX_PEERS or not 0 <= transport.peers.rank < transport.world:
+            raise RuntimeError(f"masked_sync_batch_norm: bad peer group (world {transport.world}, "
+                               f"rank {transport.peers.rank})")
+        need = (2 * c + 1 + 3) // 4 * 16
+        if need > transport.peers.group.capacity_bytes:
+            raise RuntimeError(f"masked_sync_batch_norm: {2 * c + 1} fp32 values exceed the peer group's exchange "
+                               f"capacity of {transport.peers.group.capacity_bytes} bytes")
+
+
+def _sync_bn_gather(local: torch.Tensor, transport: SyncBNTransport) -> torch.Tensor:
+    """[world, 2 C + 1]: every rank's vector in rank order, the same bits on every rank."""
+    if transport.kind == "local":
+        return local.view(1, -1)
+    out = torch.empty((transport.world, local.numel()), dtype=torch.float32, device=local.device)
+    if transport.kind == "peer":
+        _cabi.check(_lib().spx_peer_allgather(ctypes.byref(transport.peers.group), local.data_ptr(), local.numel(),
+                                              out.data_ptr(), _stream()), "peer_allgather")
+    else:
+        import torch.distributed as dist
+        dist.all_gather_into_tensor(out, local, group=transport.group)
+    return out
+
+
+def _sync_bn_desc(x, num_valid, weight, code, world=1) -> "_cabi.MaskedSyncBN":
+    d = _cabi.MaskedSyncBN()
+    d.rows, d.channels = x.shape
+    d.dtype, d.param_dtype, d.world = _DTYPE_CODE[x.dtype], code, world
+    d.num_valid, d.x, d.weight = _ptr(num_valid), _ptr(x), _ptr(weight)
+    return d
+
+
+def masked_sync_batch_norm_forward(x: torch.Tensor, num_valid: Optional[torch.Tensor], weight: Optional[torch.Tensor],
+                                   bias: Optional[torch.Tensor], running_mean: Optional[torch.Tensor],
+                                   running_var: Optional[torch.Tensor], num_batches_tracked: Optional[torch.Tensor],
+                                   momentum: Optional[float], eps: float, transport: SyncBNTransport):
+    """:func:`masked_batch_norm_forward` with statistics over the valid rows of every rank of ``transport``:
+    ``(y, mean, invstd)``, where mean / invstd and the running stats come out bit-identical on every rank.  Every
+    rank must call it, also one with no rows, in the same order as its other exchanges."""
+    x = _bn_features(x, num_valid)
+    code = _bn_param_code(x, [weight, bias, running_mean, running_var])
+    _sync_bn_check(x, transport)
+    rows, c = x.shape
+    cumulative = momentum is None
+    if cumulative and running_mean is not None and num_batches_tracked is None:
+        raise RuntimeError("masked_sync_batch_norm: momentum=None needs num_batches_tracked")
+    y = torch.empty_like(x)
+    mean = torch.empty((c,), dtype=torch.float32, device=x.device)
+    invstd = torch.empty((c,), dtype=torch.float32, device=x.device)
+    local = torch.empty((2 * c + 1,), dtype=torch.float32, device=x.device)
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_sync_bn_workspace_size(rows, c), x.device)
+    d = _sync_bn_desc(x, num_valid, weight, code)
+    d.local = local.data_ptr()
+    _cabi.check(lib.spx_masked_sync_bn_fwd_local(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_sync_bn_fwd_local")
+    gathered = _sync_bn_gather(local, transport)
+    d.world, d.gathered, d.y = gathered.shape[0], gathered.data_ptr(), _ptr(y)
+    d.bias, d.running_mean, d.running_var = _ptr(bias), _ptr(running_mean), _ptr(running_var)
+    d.num_batches_tracked = _ptr(num_batches_tracked)
+    d.momentum, d.cumulative, d.eps = 0.0 if cumulative else float(momentum), int(cumulative), float(eps)
+    d.save_mean, d.save_invstd = mean.data_ptr(), invstd.data_ptr()
+    _cabi.check(lib.spx_masked_sync_bn_fwd_merge(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_sync_bn_fwd_merge")
+    return y, mean, invstd
+
+
+def masked_sync_batch_norm_backward(x: torch.Tensor, dy: torch.Tensor, num_valid: Optional[torch.Tensor],
+                                    weight: Optional[torch.Tensor], mean: torch.Tensor, invstd: torch.Tensor,
+                                    transport: SyncBNTransport, need_weight_grad: bool = True,
+                                    need_bias_grad: bool = True):
+    """``(dx, dweight, dbias)`` of :func:`masked_sync_batch_norm_forward`: dx with the sums over every rank,
+    dweight / dbias the sums over this rank's rows only (they are averaged later like any other parameter
+    gradient).  Every rank must call it."""
+    x = _bn_features(x, num_valid)
+    dy = dy.contiguous()
+    if dy.shape != x.shape or dy.dtype != x.dtype:
+        raise RuntimeError("masked_sync_batch_norm: the output gradient must match the features' shape and dtype")
+    code = _bn_param_code(x, [weight])
+    _sync_bn_check(x, transport)
+    pdt = weight.dtype if weight is not None else torch.float32
+    rows, c = x.shape
+    dx = torch.empty_like(x)
+    dw = torch.empty((c,), dtype=pdt, device=x.device) if need_weight_grad else None
+    db = torch.empty((c,), dtype=pdt, device=x.device) if need_bias_grad else None
+    local = torch.empty((2 * c + 1,), dtype=torch.float32, device=x.device)
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_sync_bn_workspace_size(rows, c), x.device)
+    d = _sync_bn_desc(x, num_valid, weight, code)
+    d.dy, d.dx, d.dweight, d.dbias = _ptr(dy), _ptr(dx), _ptr(dw), _ptr(db)
+    d.save_mean, d.save_invstd, d.local = mean.data_ptr(), invstd.data_ptr(), local.data_ptr()
+    _cabi.check(lib.spx_masked_sync_bn_bwd_local(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_sync_bn_bwd_local")
+    gathered = _sync_bn_gather(local, transport)
+    d.world, d.gathered = gathered.shape[0], gathered.data_ptr()
+    _cabi.check(lib.spx_masked_sync_bn_bwd_merge(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_sync_bn_bwd_merge")
+    return dx, dw, db
+
+
 def last_kernel_family() -> int:
     """0 none, 1 generic FMA kernels, 2 wgmma tensor-core kernels (what served the last GEMM call)."""
     return int(_lib().spx_last_kernel_family())
