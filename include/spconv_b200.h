@@ -687,6 +687,57 @@ int spx_masked_sync_bn_bwd_local(const spx_masked_sync_bn *d, void *workspace, s
 int spx_masked_sync_bn_bwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
                                  spx_stream_t stream);
 
+/* ------------------------------------------------------------------ padding-aware GroupNorm */
+
+/*
+ * Per-sample GroupNorm / InstanceNorm (MaskedGroupNorm) over x [rows, channels], with no host read-back.  One
+ * descriptor holds the operands of a layer call; the forward and the backward of one call read the same one.
+ * M = *num_valid (device int32, clamped to [0, rows]; NULL = every row).  Row r belongs to sample b when r < M and
+ * coords[r * row_ints] == b with 0 <= b < batch_size; every other row is dropped: rows [M, rows) are never read
+ * (features nor coords), and y and dx are 0 on dropped rows.  groups divides channels; group g holds channels
+ * [g Cg, (g + 1) Cg), Cg = channels / groups, and sample b has n = count_b * Cg values in it.
+ * fwd: mean [batch_size, groups] and the biased variance over those n values (fp32; an empty sample gives mean 0),
+ *      invstd = rsqrt(var + eps) [batch_size, groups]; y = (x - mean) * (weight * invstd) + bias, in fp32, rounded
+ *      once.  weight / bias may be NULL (1 / 0).  Also writes the grouping the backward reuses: order [rows] (the
+ *      kept rows of sample b are order[offsets[b] .. offsets[b+1]) in ascending row order), offsets [batch_size + 1]
+ *      and cstart [batch_size + 1] (the sample's first chunk of 512 rows; cstart[batch_size] = chunks).
+ * bwd: with those outputs of the forward (nothing is sorted again): dbias = sum(dy), dweight = sum(dy * xhat) over
+ *      every kept row (either may be NULL); dx = invstd * (weight dy - S1 / n - xhat * S2 / n) with
+ *      S1 = sum over the group's channels of weight_c sum(dy), S2 = sum of weight_c sum(dy * xhat).  Every element of
+ *      dx is written once.
+ * Every sum is fp32 in an order fixed by the sample's kept rows (chunks of 512 rows merged in chunk order, the
+ * channels of a group in ascending order, the samples in ascending order), with no float atomics, so every result
+ * is bit-reproducible and independent of `rows` (padding) and of dropped rows.
+ * dtype: f32 / f16 / bf16 features; param_dtype (weight, bias, dweight, dbias): f32 or dtype.  batch_size in
+ * [1, 2^20], channels in [1, 65536], rows < 2^31 - 1, row_ints >= 1, eps > 0.  Rows move as 16-byte vectors when
+ * channels * element size is a multiple of 16 and the feature pointers are 16-byte aligned, else element by element
+ * with the same bits.
+ * workspace (fwd and bwd): spx_masked_group_norm_workspace_size(rows, batch_size, channels) bytes.  Fields a
+ * call does not use may be anything.
+ */
+typedef struct spx_masked_group_norm {
+    int64_t rows;
+    int row_ints, batch_size, channels, groups, dtype, param_dtype;
+    float eps;                              /* fwd: > 0 */
+    const int32_t *coords;                  /* [rows, row_ints], the batch index first */
+    const int32_t *num_valid;               /* device int32, clamped to [0, rows]; NULL = every row */
+    const void *x;                          /* [rows, channels] */
+    void *y;                                /* fwd: [rows, channels] */
+    const void *dy;                         /* bwd: [rows, channels] */
+    void *dx;                               /* bwd: [rows, channels] */
+    const void *weight, *bias;              /* [channels] param_dtype, or NULL (1 / 0) */
+    void *dweight, *dbias;                  /* bwd: [channels] param_dtype, or NULL */
+    float *mean, *invstd;                   /* [batch_size, groups] fp32: written by fwd, read by bwd */
+    int32_t *order;                         /* [rows]: written by fwd, read by bwd */
+    int32_t *offsets, *cstart;              /* [batch_size + 1]: written by fwd, read by bwd */
+} spx_masked_group_norm;
+
+size_t spx_masked_group_norm_workspace_size(int64_t rows, int batch_size, int channels);
+int spx_masked_group_norm_fwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
+                              spx_stream_t stream);
+int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
+                              spx_stream_t stream);
+
 /* ------------------------------------------------------------------ hash table */
 
 /*

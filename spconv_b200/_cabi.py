@@ -79,6 +79,17 @@ class MaskedSyncBN(Structure):
     ]
 
 
+class MaskedGroupNorm(Structure):
+    """``spx_masked_group_norm``: the operands of one MaskedGroupNorm call (forward and backward)."""
+    _fields_ = [
+        ("rows", c_int64), ("row_ints", c_int), ("batch_size", c_int), ("channels", c_int), ("groups", c_int),
+        ("dtype", c_int), ("param_dtype", c_int), ("eps", c_float),
+        ("coords", c_void_p), ("num_valid", c_void_p), ("x", c_void_p), ("y", c_void_p), ("dy", c_void_p),
+        ("dx", c_void_p), ("weight", c_void_p), ("bias", c_void_p), ("dweight", c_void_p), ("dbias", c_void_p),
+        ("mean", c_void_p), ("invstd", c_void_p), ("order", c_void_p), ("offsets", c_void_p), ("cstart", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); also the list the CPU test checks against the header
 SIGNATURES = {
     "spx_last_error": (c_char_p, []),
@@ -204,6 +215,9 @@ SIGNATURES = {
     "spx_masked_sync_bn_workspace_size": (c_size_t, [c_int64, c_int]),
     **{f"spx_masked_sync_bn_{p}": (c_int, [POINTER(MaskedSyncBN), c_void_p, c_size_t, c_void_p])
        for p in ("fwd_local", "fwd_merge", "bwd_local", "bwd_merge")},
+    "spx_masked_group_norm_workspace_size": (c_size_t, [c_int64, c_int, c_int]),
+    **{f"spx_masked_group_norm_{p}": (c_int, [POINTER(MaskedGroupNorm), c_void_p, c_size_t, c_void_p])
+       for p in ("fwd", "bwd")},
     "spx_hash_workspace_size": (c_size_t, [c_int64, c_int64]),
     "spx_hash_clear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
     "spx_hash_insert": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,

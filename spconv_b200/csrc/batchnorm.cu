@@ -61,16 +61,6 @@ template <typename T, int W, bool V> __device__ __forceinline__ void bn_store(T 
     }
 }
 
-// Chan et al.: fold (nb, mb, qb) into (na, ma, qa).  An empty side changes nothing, bit for bit.
-__device__ __forceinline__ void chan_merge(float &na, float &ma, float &qa, float nb, float mb, float qb) {
-    if (nb == 0.f) return;
-    if (na == 0.f) { na = nb; ma = mb; qa = qb; return; }
-    const float n = na + nb, d = mb - ma, f = __fdiv_rn(nb, n);
-    ma = fmaf(d, f, ma);
-    qa = qa + qb + d * d * na * f;
-    na = n;
-}
-
 // Block layout of the row kernels: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
 // `lanes` = BN_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
 struct BnRowThread {

@@ -30,18 +30,11 @@ int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t 
                        int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
 
 constexpr int GP_THREADS = 256;
-constexpr int GP_CHUNK = 512;        // rows per partial
 constexpr int GP_SEG_THREADS = 1024; // the one block of the segments kernel
 constexpr int GP_FIN_CH = 8;         // finalize: channels per block
 constexpr int GP_FIN_LANES = 32;     // finalize: partial lanes per channel
 constexpr int GP_MAX_BATCH = 1 << 20;
 constexpr int GP_MAX_CHANNELS = 1 << 16;   // finalize grid.y = C / GP_FIN_CH must stay below 2^16
-
-__device__ __forceinline__ int64_t gp_valid_rows(const int32_t *num_valid, int64_t rows) {
-    if (num_valid == nullptr) return rows;
-    const int64_t m = __ldg(num_valid);
-    return m < 0 ? 0 : (m > rows ? rows : m);
-}
 
 // A: the pointer is 16-byte aligned, so W elements move as one 16-byte access; otherwise W element accesses.  W
 // alone decides which rows and channels a thread folds, so both give the same bits.
@@ -126,17 +119,6 @@ gp_segments_kernel(const uint32_t *__restrict__ keys, int32_t n, int batch_size,
         offsets[batch_size] = gp_lower_bound(keys, n, (uint32_t)batch_size);
         cstart[batch_size] = s_scan[t];
     }
-}
-
-// the sample whose chunks hold chunk k: the last b with cstart[b] <= k (empty samples own no chunk)
-__device__ __forceinline__ int gp_sample_of_chunk(const int32_t *cstart, int batch_size, int32_t k) {
-    int lo = 0, hi = batch_size - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(cstart + mid) <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
 }
 
 // Block layout as batchnorm.cu: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
@@ -314,6 +296,27 @@ static int gp_tpr(int vecs) {
     return tpr;
 }
 
+// keys -> stable argsort -> segments: order [rows], offsets [B+1], cstart [B+1] and, when count != NULL, count [B]
+// (see the top of this file).  keys [rows] and sort_ws (radix_argsort_workspace_bytes(rows)) are scratch.  Shared
+// with group_norm.cu.
+int group_samples(const int32_t *coords, int64_t rows, int row_ints, int batch_size, const int32_t *num_valid,
+                  uint32_t *keys, int32_t *order, void *sort_ws, int32_t *offsets, int32_t *cstart, int32_t *count,
+                  cudaStream_t stream) {
+    if (rows > 0) {
+        gp_keys_kernel<<<(unsigned)div_up64(rows, GP_THREADS), GP_THREADS, 0, stream>>>(
+            coords, rows, row_ints, batch_size, num_valid, keys);
+        SPX_CHECK_LAUNCH("gp_keys_kernel");
+        int key_bits = 1;                                  // enough bits for the keys 0..B
+        while (key_bits < 32 && (batch_size >> key_bits) != 0) ++key_bits;
+        if (int rc = radix_argsort_pair(keys, order, rows, nullptr, nullptr, 0, key_bits, sort_ws,
+                                        radix_argsort_workspace_bytes(rows), nullptr, 0, stream))
+            return rc;
+    }
+    gp_segments_kernel<<<1, GP_SEG_THREADS, 0, stream>>>(keys, (int32_t)rows, batch_size, offsets, cstart, count);
+    SPX_CHECK_LAUNCH("gp_segments_kernel");
+    return 0;
+}
+
 static int gp_check(const char *who, int mode, int64_t rows, int row_ints, int batch_size, int channels,
                     int dtype) {
     SPX_REQUIRE(mode == 0 || mode == 1, "%s: mode must be 0 (max) or 1 (mean), got %d", who, mode);
@@ -423,19 +426,9 @@ extern "C" int spx_global_pool_fwd(int mode, const void *features, const int32_t
     int32_t *cstart = ws.take<int32_t>((size_t)batch_size + 1);
     float2 *partials = ws.take<float2>((size_t)gp_max_chunks(rows, batch_size) * channels);
     cudaStream_t stream = (cudaStream_t)stream_;
-    if (rows > 0) {
-        gp_keys_kernel<<<(unsigned)div_up64(rows, GP_THREADS), GP_THREADS, 0, stream>>>(
-            coords, rows, row_ints, batch_size, num_valid, keys);
-        SPX_CHECK_LAUNCH("gp_keys_kernel");
-        int key_bits = 1;                                  // enough bits for the keys 0..B
-        while (key_bits < 32 && (batch_size >> key_bits) != 0) ++key_bits;
-        if (int rc = radix_argsort_pair(keys, order, rows, nullptr, nullptr, 0, key_bits, sort_ws,
-                                        radix_argsort_workspace_bytes(rows), nullptr, 0, stream))
-            return rc;
-    }
-    gp_segments_kernel<<<1, GP_SEG_THREADS, 0, stream>>>(keys, (int32_t)rows, batch_size, offsets, cstart,
-                                                         mode == 1 ? count : nullptr);
-    SPX_CHECK_LAUNCH("gp_segments_kernel");
+    if (int rc = group_samples(coords, rows, row_ints, batch_size, num_valid, keys, order, sort_ws, offsets, cstart,
+                               mode == 1 ? count : nullptr, stream))
+        return rc;
     GpFwdArgs a{mode, features, order, offsets, cstart, rows, batch_size, channels, partials, out, argmax};
     switch (dtype) {
         case SPX_F32: return gp_fwd_dispatch<float>(a, stream);

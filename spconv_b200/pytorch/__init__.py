@@ -9,8 +9,8 @@ from .conv import (SparseConv1d, SparseConv2d, SparseConv3d, SparseConv4d,  # no
 from .identity import Identity  # noqa: F401
 from .core import (CUDAKernelTimer, ImplicitGemmIndiceData, IndiceData,  # noqa: F401
                    SparseConvTensor, scatter_nd)
-from .modules import (MaskedBatchNorm1d, MaskedSyncBatchNorm1d, RemoveGrid, SparseBatchNorm,  # noqa: F401
-                      SparseIdentity, SparseModule, SparseReLU, SparseSequential, SparseSyncBatchNorm, ToDense,
+from .modules import (MaskedBatchNorm1d, MaskedGroupNorm, MaskedSyncBatchNorm1d, RemoveGrid,  # noqa: F401
+                      SparseBatchNorm, SparseIdentity, SparseModule, SparseReLU, SparseSequential, SparseSyncBatchNorm, ToDense,
                       assign_name_for_sparse_modules)
 from .pool import (MaskedGlobalAvgPool, MaskedGlobalMaxPool, SparseAvgPool1d,  # noqa: F401
                    SparseAvgPool2d, SparseAvgPool3d, SparseGlobalAvgPool, SparseGlobalMaxPool, SparseMaxPool1d,

@@ -534,6 +534,33 @@ def masked_sync_batch_norm(x, weight, bias, running_mean, running_var, num_batch
                                              num_valid, momentum, eps, ops.sync_bn_transport(process_group))
 
 
+# ---------------------------------------------------------------------------- per-sample GroupNorm
+class MaskedGroupNormFunction(Function):
+    """``x, weight, bias, indices, batch_size, num_valid, num_groups, eps`` -> per-sample GroupNorm over the rows
+    ``[0, num_valid)`` whose batch index is in range (:func:`ops.masked_group_norm_forward`).  The backward reuses
+    the forward's grouping and gives dx (0 on padding and dropped rows), dweight and dbias."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, indices, batch_size, num_valid, num_groups, eps):
+        y, mean, invstd, order, offsets, cstart = ops.masked_group_norm_forward(
+            x, indices, batch_size, num_valid, num_groups, weight, bias, eps)
+        ctx.save_for_backward(x, weight, indices, num_valid, mean, invstd, order, offsets, cstart)
+        ctx.batch_size, ctx.num_groups = batch_size, num_groups
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        x, weight, indices, num_valid, mean, invstd, order, offsets, cstart = ctx.saved_tensors
+        dx, dw, db = ops.masked_group_norm_backward(x, grad_output, indices, ctx.batch_size, num_valid,
+                                                    ctx.num_groups, weight, mean, invstd, order, offsets, cstart,
+                                                    ctx.needs_input_grad[1], ctx.needs_input_grad[2])
+        return dx, dw, db, None, None, None, None, None
+
+
+masked_group_norm = MaskedGroupNormFunction.apply
+
+
 # ---------------------------------------------------------------------------- padding-aware global pooling
 class MaskedGlobalPoolFunction(Function):
     """``features, indices, batch_size, num_valid, is_mean`` -> ``[batch_size, C]``: per-sample max or mean over

@@ -318,6 +318,49 @@ class MaskedSyncBatchNorm1d(SparseModule, nn.SyncBatchNorm):
         return out
 
 
+class MaskedGroupNorm(SparseModule, nn.GroupNorm):
+    """``nn.GroupNorm`` applied per sample of a :class:`SparseConvTensor`: the statistics of sample ``b`` and group
+    ``g`` (channels ``[g C/G, (g+1) C/G)``) are the mean and biased variance over every value of that group in the
+    rows of sample ``b``, as ``F.group_norm(x[rows_b].T[None], G, weight, bias, eps)`` computes them.
+    ``MaskedGroupNorm(C, C)`` is InstanceNorm.  Same constructor, parameters and ``state_dict`` keys as
+    ``nn.GroupNorm``; :meth:`from_groupnorm` takes over an existing module's parameters.
+
+    Row ``r`` belongs to sample ``b`` when ``r < x.num_valid`` (every row of an unpadded tensor) and
+    ``x.indices[r, 0] == b`` with ``0 <= b < x.batch_size``.  Every other row (padding, or a batch index out of
+    range) is dropped: never read, and 0 in the output and in the input gradient.  The kernels of
+    ``csrc/group_norm.cu`` sum in fp32 in an order fixed by each sample's rows, with no float atomics and no host
+    read-back, so results are bit-reproducible, independent of the padding, and a padded step captures as one CUDA
+    graph.  An empty sample computes nothing; one row with one channel per group normalises to 0, so its output is
+    ``bias``, as in torch.  GroupNorm has no running statistics: eval mode is the same computation.
+
+    A plain ``nn.GroupNorm`` inside :class:`SparseSequential` sees ``x.features`` ``[N, C]`` and so treats every row
+    as its own batch element, normalising it over its own C/G channels; that behaviour of dense layers is left as it
+    is.  Use this module for per-sample statistics."""
+
+    def __init__(self, num_groups, num_channels, eps=1e-5, affine=True, device=None, dtype=None):
+        nn.GroupNorm.__init__(self, num_groups, num_channels, eps, affine, device, dtype)
+        self.name = None
+        self._sparse_unique_name = ""
+
+    def forward(self, x: SparseConvTensor):
+        feats = x.features
+        if feats.dim() != 2 or feats.shape[1] != self.num_channels:
+            raise ValueError(f"MaskedGroupNorm({self.num_groups}, {self.num_channels}): features of shape "
+                             f"{tuple(feats.shape)}")
+        return x.replace_feature(functional.masked_group_norm(
+            feats, self.weight, self.bias, x.indices, x.batch_size, x.num_valid, self.num_groups, self.eps))
+
+    @classmethod
+    def from_groupnorm(cls, gn: nn.GroupNorm) -> "MaskedGroupNorm":
+        """A ``MaskedGroupNorm`` with ``gn``'s configuration that shares its parameters (the same objects)."""
+        out = cls(gn.num_groups, gn.num_channels, gn.eps, gn.affine, device="meta")
+        if gn.affine:
+            out.weight = gn.weight
+            out.bias = gn.bias
+        out.training = gn.training
+        return out
+
+
 class SparseIdentity(SparseModule):
     def forward(self, x: SparseConvTensor):
         return x

@@ -1413,17 +1413,17 @@ def zero_rows_from_count_(x: torch.Tensor, num_valid: torch.Tensor) -> torch.Ten
 _BN_DTYPES = (torch.float32, torch.float16, torch.bfloat16)
 
 
-def _bn_param_code(x: torch.Tensor, params: Sequence[Optional[torch.Tensor]]) -> int:
-    """dtype code of the BatchNorm parameters / buffers: all float32, or all the feature dtype."""
+def _bn_param_code(x: torch.Tensor, params: Sequence[Optional[torch.Tensor]], who: str = "masked_batch_norm") -> int:
+    """dtype code of the BatchNorm / GroupNorm parameters and buffers: all float32, or all the feature dtype."""
     given = [p for p in params if p is not None]
     dt = given[0].dtype if given else torch.float32
     for p in given:
-        _require_cuda(p, "BatchNorm parameters and buffers")
+        _require_cuda(p, "BatchNorm parameters and buffers" if who == "masked_batch_norm" else "GroupNorm parameters")
         if p.dtype != dt or p.dim() != 1 or p.shape[0] != x.shape[1] or not p.is_contiguous():
-            raise RuntimeError(f"masked_batch_norm: parameters and buffers must be contiguous [{x.shape[1]}] tensors "
+            raise RuntimeError(f"{who}: parameters and buffers must be contiguous [{x.shape[1]}] tensors "
                                "of one dtype")
     if dt not in (torch.float32, x.dtype):
-        raise RuntimeError(f"masked_batch_norm: parameter dtype {dt} must be float32 or the feature dtype {x.dtype}")
+        raise RuntimeError(f"{who}: parameter dtype {dt} must be float32 or the feature dtype {x.dtype}")
     return _DTYPE_CODE[dt]
 
 
@@ -1485,6 +1485,104 @@ def masked_batch_norm_backward(x: torch.Tensor, dy: torch.Tensor, num_valid: Opt
         _ptr(x), _ptr(dy), _ptr(dx), rows, c, _DTYPE_CODE[x.dtype], _ptr(num_valid), _ptr(weight), code,
         mean.data_ptr(), invstd.data_ptr(), _ptr(dw), _ptr(db), ws.data_ptr(), ws.numel(), _stream()),
         "masked_bn_bwd")
+    return dx, dw, db
+
+
+# ---------------------------------------------------------------------------- per-sample GroupNorm
+GROUP_NORM_MAX_BATCH = 1 << 20
+GROUP_NORM_MAX_CHANNELS = 1 << 16
+
+
+def _gn_check(x: torch.Tensor, indices: torch.Tensor, batch_size: int, num_groups: int,
+              num_valid: Optional[torch.Tensor]) -> None:
+    _require_cuda(x, "features")
+    _require_cuda(indices, "indices")
+    if x.dim() != 2 or x.dtype not in _BN_DTYPES:
+        raise RuntimeError(f"masked_group_norm: features must be a [rows, C] float32 / float16 / bfloat16 matrix, got "
+                           f"{tuple(x.shape)} {x.dtype}")
+    if indices.dim() != 2 or indices.dtype != torch.int32 or indices.shape[0] != x.shape[0] or indices.shape[1] < 1:
+        raise RuntimeError(f"masked_group_norm: int32 indices [rows, ndim + 1] expected, got {tuple(indices.shape)} "
+                           f"{indices.dtype}")
+    if num_valid is not None and (num_valid.dtype != torch.int32 or num_valid.device != x.device):
+        raise RuntimeError("masked_group_norm: num_valid must be an int32 tensor on the features' device")
+    c = x.shape[1]
+    if not 1 <= int(batch_size) <= GROUP_NORM_MAX_BATCH:
+        raise RuntimeError(f"masked_group_norm: batch_size must be in [1, 2^20], got {batch_size}")
+    if not 1 <= c <= GROUP_NORM_MAX_CHANNELS:
+        raise RuntimeError(f"masked_group_norm: channels must be in [1, 65536], got {c}")
+    if int(num_groups) < 1 or c % int(num_groups):
+        raise RuntimeError(f"masked_group_norm: num_groups {num_groups} must divide the channels {c}")
+
+
+def _gn_desc(x, indices, batch_size, num_groups, num_valid, code) -> "_cabi.MaskedGroupNorm":
+    d = _cabi.MaskedGroupNorm()
+    d.rows, d.row_ints, d.batch_size, d.channels = x.shape[0], indices.shape[1], int(batch_size), x.shape[1]
+    d.groups, d.dtype, d.param_dtype = int(num_groups), _DTYPE_CODE[x.dtype], code
+    d.coords, d.num_valid, d.x = _ptr(indices), _ptr(num_valid), _ptr(x)
+    return d
+
+
+def masked_group_norm_forward(x: torch.Tensor, indices: torch.Tensor, batch_size: int, num_valid: Optional[torch.Tensor],
+                              num_groups: int, weight: Optional[torch.Tensor], bias: Optional[torch.Tensor],
+                              eps: float):
+    """Per-sample GroupNorm of the rows ``r < num_valid`` (all rows when ``num_valid`` is None) whose batch index
+    ``indices[r, 0]`` is in ``[0, batch_size)``; every other row of ``y`` is 0.  Returns ``(y, mean, invstd, order,
+    offsets, cstart)``: the fp32 statistics ``[batch_size, num_groups]`` and the grouping of the rows by sample,
+    which :func:`masked_group_norm_backward` reuses.  No host synchronisation; bit-reproducible whatever the
+    padding."""
+    _gn_check(x, indices, batch_size, num_groups, num_valid)
+    x, indices = x.contiguous(), indices.contiguous()
+    code = _bn_param_code(x, [weight, bias], "masked_group_norm")
+    if not eps > 0:
+        raise RuntimeError(f"masked_group_norm: eps must be positive, got {eps}")
+    rows, c = x.shape
+    b, g = int(batch_size), int(num_groups)
+    y = torch.empty_like(x)
+    mean = torch.empty((b, g), dtype=torch.float32, device=x.device)
+    invstd = torch.empty((b, g), dtype=torch.float32, device=x.device)
+    order = torch.empty((rows,), dtype=torch.int32, device=x.device)
+    offsets = torch.empty((b + 1,), dtype=torch.int32, device=x.device)
+    cstart = torch.empty((b + 1,), dtype=torch.int32, device=x.device)
+    d = _gn_desc(x, indices, b, g, num_valid, code)
+    d.eps, d.y, d.weight, d.bias = float(eps), _ptr(y), _ptr(weight), _ptr(bias)
+    d.mean, d.invstd, d.order, d.offsets, d.cstart = (mean.data_ptr(), invstd.data_ptr(), _ptr(order),
+                                                      offsets.data_ptr(), cstart.data_ptr())
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_group_norm_workspace_size(rows, b, c), x.device)
+    _cabi.check(lib.spx_masked_group_norm_fwd(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_group_norm_fwd")
+    return y, mean, invstd, order, offsets, cstart
+
+
+def masked_group_norm_backward(x: torch.Tensor, dy: torch.Tensor, indices: torch.Tensor, batch_size: int,
+                               num_valid: Optional[torch.Tensor], num_groups: int, weight: Optional[torch.Tensor],
+                               mean: torch.Tensor, invstd: torch.Tensor, order: torch.Tensor, offsets: torch.Tensor,
+                               cstart: torch.Tensor, need_weight_grad: bool = True, need_bias_grad: bool = True):
+    """``(dx, dweight, dbias)`` of :func:`masked_group_norm_forward`, from its statistics and grouping (nothing is
+    sorted again).  dx is 0 on padding and dropped rows; the parameter gradients (None when not needed) have the
+    parameters' dtype (float32 without ``weight``)."""
+    _gn_check(x, indices, batch_size, num_groups, num_valid)
+    x, indices, dy = x.contiguous(), indices.contiguous(), dy.contiguous()
+    if dy.shape != x.shape or dy.dtype != x.dtype:
+        raise RuntimeError("masked_group_norm: the output gradient must match the features' shape and dtype")
+    code = _bn_param_code(x, [weight], "masked_group_norm")
+    pdt = weight.dtype if weight is not None else torch.float32
+    rows, c = x.shape
+    b, g = int(batch_size), int(num_groups)
+    for t, shape in ((mean, (b, g)), (invstd, (b, g)), (order, (rows,)), (offsets, (b + 1,)), (cstart, (b + 1,))):
+        if tuple(t.shape) != shape or not t.is_contiguous() or t.device != x.device:
+            raise RuntimeError("masked_group_norm: the saved statistics and grouping do not match the features")
+    dx = torch.empty_like(x)
+    dw = torch.empty((c,), dtype=pdt, device=x.device) if need_weight_grad else None
+    db = torch.empty((c,), dtype=pdt, device=x.device) if need_bias_grad else None
+    d = _gn_desc(x, indices, b, g, num_valid, code)
+    d.dy, d.dx, d.weight, d.dweight, d.dbias = _ptr(dy), _ptr(dx), _ptr(weight), _ptr(dw), _ptr(db)
+    d.mean, d.invstd, d.order, d.offsets, d.cstart = (mean.data_ptr(), invstd.data_ptr(), _ptr(order),
+                                                      offsets.data_ptr(), cstart.data_ptr())
+    lib = _lib()
+    ws = _bytes(lib.spx_masked_group_norm_workspace_size(rows, b, c), x.device)
+    _cabi.check(lib.spx_masked_group_norm_bwd(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+                "masked_group_norm_bwd")
     return dx, dw, db
 
 
