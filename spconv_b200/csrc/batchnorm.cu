@@ -14,7 +14,7 @@
 // Backward: reduce (per-chunk sums of dy and dy * xhat) -> finalize (dbeta, dgamma, coefficients) ->
 // apply dx = gamma * invstd * (dy - sum(dy) / M - xhat * sum(dy * xhat) / M).
 // Feature rows move as 16-byte vectors when the row length and the pointers allow it, else per element.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 
@@ -23,56 +23,10 @@ constexpr int BN_CHUNK = 512;        // rows per partial
 constexpr int BN_FIN_CH = 8;         // finalize: channels per block
 constexpr int BN_FIN_LANES = 32;     // finalize: partial lanes per channel
 
-__device__ __forceinline__ int64_t bn_valid_rows(const int32_t *num_valid, int64_t rows) {
-    if (num_valid == nullptr) return rows;
-    const int64_t m = __ldg(num_valid);
-    return m < 0 ? 0 : (m > rows ? rows : m);
-}
-
 // rows of chunk k that are valid
 __device__ __forceinline__ float bn_chunk_count(int64_t k, int64_t M) {
     const int64_t n = M - k * BN_CHUNK;
     return (float)(n < 0 ? 0 : (n > BN_CHUNK ? BN_CHUNK : n));
-}
-
-// V: one 16-byte access per W elements (the pointers are 16-byte aligned); otherwise W element accesses.  W alone
-// decides which rows and channels a thread folds, so both give the same bits.
-template <typename T, int W, bool V> __device__ __forceinline__ void bn_load(const T *p, float (&f)[W]) {
-    if constexpr (V && W * sizeof(T) == 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-        const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(e[j]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(__ldg(p + j));
-    }
-}
-template <typename T, int W, bool V> __device__ __forceinline__ void bn_store(T *p, const float (&f)[W]) {
-    if constexpr (V && W * sizeof(T) == 16) {
-        uint4 v;
-        T *e = reinterpret_cast<T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) e[j] = from_float<T>(f[j]);
-        *reinterpret_cast<uint4 *>(p) = v;
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) p[j] = from_float<T>(f[j]);
-    }
-}
-
-// Block layout of the row kernels: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
-// `lanes` = BN_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
-struct BnRowThread {
-    int lane, v;
-    bool active;
-};
-__device__ __forceinline__ BnRowThread bn_row_thread(int vecs, int tpr) {
-    BnRowThread t;
-    t.lane = threadIdx.x / tpr;
-    t.v = blockIdx.y * tpr + (threadIdx.x % tpr);
-    t.active = t.v < vecs;
-    return t;
 }
 
 // ---------------------------------------------------------------- forward
@@ -81,11 +35,11 @@ __global__ void __launch_bounds__(BN_THREADS)
 bn_stats_kernel(const T *__restrict__ x, int64_t rows, int channels, int vecs, int tpr,
                 const int32_t *__restrict__ num_valid, float2 *__restrict__ partials) {
     __shared__ float s_mean[BN_THREADS * W], s_q[BN_THREADS * W], s_n[BN_THREADS];
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     const int64_t r0 = (int64_t)blockIdx.x * BN_CHUNK;
     if (r0 >= M) return;                                   // the whole block: nothing valid here
     const int lanes = BN_THREADS / tpr;
-    const BnRowThread t = bn_row_thread(vecs, tpr);
+    const RowThread t = row_thread(vecs, tpr);
     const int64_t end = M < r0 + BN_CHUNK ? M : r0 + BN_CHUNK;
     float n = 0.f, mean[W], q[W];
 #pragma unroll
@@ -106,36 +60,17 @@ bn_stats_kernel(const T *__restrict__ x, int64_t rows, int channels, int vecs, i
         for (; r + 3 * lanes < end; r += 4 * lanes) {     // four loads in flight, folded in row order
             float f[4][W];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) bn_load<T, W, V>(base + (r + (int64_t)u * lanes) * channels, f[u]);
+            for (int u = 0; u < 4; ++u) row_load<T, W, V>(base + (r + (int64_t)u * lanes) * channels, f[u]);
 #pragma unroll
             for (int u = 0; u < 4; ++u) fold(f[u]);
         }
         for (; r < end; r += lanes) {
             float f[W];
-            bn_load<T, W, V>(base + r * channels, f);
+            row_load<T, W, V>(base + r * channels, f);
             fold(f);
         }
     }
-    // fixed tree over the row lanes: at step s, lanes [0, s) fold lanes [s, 2s) into their own slots
-    const int slot = threadIdx.x;
-#pragma unroll
-    for (int j = 0; j < W; ++j) { s_mean[slot * W + j] = mean[j]; s_q[slot * W + j] = q[j]; }
-    s_n[slot] = n;
-    for (int s = lanes >> 1; s >= 1; s >>= 1) {
-        __syncthreads();
-        if (t.lane < s) {
-            const int o = slot + s * tpr;
-            const float nb = s_n[o];
-#pragma unroll
-            for (int j = 0; j < W; ++j) {
-                float na = n;
-                chan_merge(na, mean[j], q[j], nb, s_mean[o * W + j], s_q[o * W + j]);
-                s_mean[slot * W + j] = mean[j];
-                s_q[slot * W + j] = q[j];
-            }
-            s_n[slot] = n = n + nb;
-        }
-    }
+    welford_lane_tree<W>(s_mean, s_q, s_n, lanes, tpr, n, mean, q);
     if (t.lane == 0 && t.active) {
         float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
 #pragma unroll
@@ -218,7 +153,7 @@ bn_fwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
     const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
     const int c = blockIdx.x * BN_FIN_CH + cl;
     const bool active = c < channels;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float sum, mean, m2;
     bn_fwd_sums(partials, M, channels, c, active, buf, pl, cl, sum, mean, m2);
     if (pl != 0 || !active) return;
@@ -234,10 +169,10 @@ bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, in
     const int64_t r = idx / vecs;
     const int v = (int)(idx - r * vecs);
     if (r >= rows) return;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float f[W];
     if (r < M) {
-        bn_load<T, W, V>(x + r * channels + v * W, f);
+        row_load<T, W, V>(x + r * channels + v * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -247,7 +182,7 @@ bn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, int64_t rows, in
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    bn_store<T, W, V>(y + r * channels + v * W, f);
+    row_store<T, W, V>(y + r * channels + v * W, f);
 }
 
 // ---------------------------------------------------------------- backward
@@ -257,11 +192,11 @@ bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t 
                      const int32_t *__restrict__ num_valid, const float *__restrict__ save_mean,
                      const float *__restrict__ save_invstd, float2 *__restrict__ partials) {
     __shared__ float s_a[BN_THREADS * W], s_b[BN_THREADS * W];
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     const int64_t r0 = (int64_t)blockIdx.x * BN_CHUNK;
     if (r0 >= M) return;
     const int lanes = BN_THREADS / tpr;
-    const BnRowThread t = bn_row_thread(vecs, tpr);
+    const RowThread t = row_thread(vecs, tpr);
     const int64_t end = M < r0 + BN_CHUNK ? M : r0 + BN_CHUNK;
     float sdy[W], sdyx[W];
 #pragma unroll
@@ -287,33 +222,20 @@ bn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, int64_t 
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int64_t o = (r + (int64_t)u * lanes) * channels + off;
-                bn_load<T, W, V>(x + o, fx[u]);
-                bn_load<T, W, V>(dy + o, fd[u]);
+                row_load<T, W, V>(x + o, fx[u]);
+                row_load<T, W, V>(dy + o, fd[u]);
             }
 #pragma unroll
             for (int u = 0; u < 2; ++u) fold(fx[u], fd[u]);
         }
         for (; r < end; r += lanes) {
             float fx[W], fd[W];
-            bn_load<T, W, V>(x + r * channels + off, fx);
-            bn_load<T, W, V>(dy + r * channels + off, fd);
+            row_load<T, W, V>(x + r * channels + off, fx);
+            row_load<T, W, V>(dy + r * channels + off, fd);
             fold(fx, fd);
         }
     }
-    const int slot = threadIdx.x;
-#pragma unroll
-    for (int j = 0; j < W; ++j) { s_a[slot * W + j] = sdy[j]; s_b[slot * W + j] = sdyx[j]; }
-    for (int s = lanes >> 1; s >= 1; s >>= 1) {
-        __syncthreads();
-        if (t.lane < s) {
-            const int o = slot + s * tpr;
-#pragma unroll
-            for (int j = 0; j < W; ++j) {
-                s_a[slot * W + j] = sdy[j] = sdy[j] + s_a[o * W + j];
-                s_b[slot * W + j] = sdyx[j] = sdyx[j] + s_b[o * W + j];
-            }
-        }
-    }
+    pair_sum_lane_tree<W>(s_a, s_b, lanes, tpr, sdy, sdyx);
     if (t.lane == 0 && t.active) {
         float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
 #pragma unroll
@@ -359,7 +281,7 @@ bn_bwd_finalize_kernel(const float2 *__restrict__ partials, int64_t rows, int ch
     const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
     const int c = blockIdx.x * BN_FIN_CH + cl;
     const bool active = c < channels;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float sdy, sdyx;
     bn_bwd_sums(partials, M, channels, c, active, buf, pl, cl, sdy, sdyx);
     if (pl != 0 || !active) return;
@@ -377,12 +299,12 @@ bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
     const int64_t r = idx / vecs;
     const int v = (int)(idx - r * vecs);
     if (r >= rows) return;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float f[W];
     if (r < M) {
         float fx[W];
-        bn_load<T, W, V>(x + r * channels + v * W, fx);
-        bn_load<T, W, V>(dy + r * channels + v * W, f);
+        row_load<T, W, V>(x + r * channels + v * W, fx);
+        row_load<T, W, V>(dy + r * channels + v * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -393,7 +315,7 @@ bn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    bn_store<T, W, V>(dx + r * channels + v * W, f);
+    row_store<T, W, V>(dx + r * channels + v * W, f);
 }
 
 // ---------------------------------------------------------------- cross-rank statistics (MaskedSyncBatchNorm1d)
@@ -424,7 +346,7 @@ bn_sync_fwd_local_kernel(const float2 *__restrict__ partials, int64_t rows, int 
     const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
     const int c = blockIdx.x * BN_FIN_CH + cl;
     const bool active = c < channels;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float sum, mean, m2;
     bn_fwd_sums(partials, M, channels, c, active, buf, pl, cl, sum, mean, m2);
     bn_sync_write_local(local, channels, M, c, active, pl, sum, m2);
@@ -486,7 +408,7 @@ bn_sync_bwd_local_kernel(const float2 *__restrict__ partials, int64_t rows, int 
     const int cl = threadIdx.x % BN_FIN_CH, pl = threadIdx.x / BN_FIN_CH;
     const int c = blockIdx.x * BN_FIN_CH + cl;
     const bool active = c < channels;
-    const int64_t M = bn_valid_rows(num_valid, rows);
+    const int64_t M = valid_rows(num_valid, rows);
     float sdy, sdyx;
     bn_bwd_sums(partials, M, channels, c, active, buf, pl, cl, sdy, sdyx);
     if (pl == 0 && active) {
@@ -536,12 +458,6 @@ static int bn_check(const char *who, int64_t rows, int channels, int dtype, int 
     return 0;
 }
 
-static int bn_tpr(int vecs) {
-    int tpr = 1;
-    while (tpr < vecs && tpr < 32) tpr <<= 1;
-    return tpr;
-}
-
 struct BnFwdArgs {
     const void *x;
     void *y;
@@ -562,7 +478,7 @@ struct BnFwdArgs {
 template <typename T, int W, bool V> static int bn_fwd_rows(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (stats) {
-        const int tpr = bn_tpr(vecs);
+        const int tpr = row_tpr(vecs);
         const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
         bn_stats_kernel<T, W, V><<<grid, BN_THREADS, 0, stream>>>(static_cast<const T *>(a.x), a.rows, a.channels, vecs,
                                                                tpr, a.num_valid, a.partials);
@@ -575,19 +491,14 @@ template <typename T, int W, bool V> static int bn_fwd_rows(const BnFwdArgs &a, 
     return 0;
 }
 
-template <typename T> static int bn_fwd_rows_dispatch(const BnFwdArgs &a, bool stats, cudaStream_t stream) {
-    constexpr int W = 16 / sizeof(T);
-    if ((a.channels * (int)sizeof(T)) % 16) return bn_fwd_rows<T, 1, false>(a, stats, stream);
-    return aligned16(a.x) && aligned16(a.y) ? bn_fwd_rows<T, W, true>(a, stats, stream)
-                                            : bn_fwd_rows<T, W, false>(a, stats, stream);
-}
-
 static int bn_fwd_rows_typed(int dtype, const BnFwdArgs &a, bool stats, cudaStream_t stream) {
-    switch (dtype) {
-        case SPX_F32: return bn_fwd_rows_dispatch<float>(a, stats, stream);
-        case SPX_F16: return bn_fwd_rows_dispatch<__half>(a, stats, stream);
-        default: return bn_fwd_rows_dispatch<__nv_bfloat16>(a, stats, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int W = 16 / sizeof(T);
+        const RowWidth w = row_width(a.channels * sizeof(T), a.x, a.y);   // a reduction: W whenever wide
+        if (!w.wide) return bn_fwd_rows<T, 1, false>(a, stats, stream);
+        return w.aligned ? bn_fwd_rows<T, W, true>(a, stats, stream) : bn_fwd_rows<T, W, false>(a, stats, stream);
+    });
 }
 
 template <typename P> static int bn_fwd_finalize(const BnFwdArgs &a, cudaStream_t stream) {
@@ -615,7 +526,7 @@ struct BnBwdArgs {
 template <typename T, int W, bool V> static int bn_bwd_rows(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (reduce) {
-        const int tpr = bn_tpr(vecs);
+        const int tpr = row_tpr(vecs);
         const dim3 grid((unsigned)bn_chunks(a.rows), (unsigned)div_up64(vecs, tpr));
         bn_bwd_reduce_kernel<T, W, V><<<grid, BN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<const T *>(a.dy), a.rows, a.channels, vecs, tpr, a.num_valid,
@@ -630,19 +541,14 @@ template <typename T, int W, bool V> static int bn_bwd_rows(const BnBwdArgs &a, 
     return 0;
 }
 
-template <typename T> static int bn_bwd_rows_dispatch(const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
-    constexpr int W = 16 / sizeof(T);
-    if ((a.channels * (int)sizeof(T)) % 16) return bn_bwd_rows<T, 1, false>(a, reduce, stream);
-    return aligned16(a.x) && aligned16(a.dy) && aligned16(a.dx) ? bn_bwd_rows<T, W, true>(a, reduce, stream)
-                                                                : bn_bwd_rows<T, W, false>(a, reduce, stream);
-}
-
 static int bn_bwd_rows_typed(int dtype, const BnBwdArgs &a, bool reduce, cudaStream_t stream) {
-    switch (dtype) {
-        case SPX_F32: return bn_bwd_rows_dispatch<float>(a, reduce, stream);
-        case SPX_F16: return bn_bwd_rows_dispatch<__half>(a, reduce, stream);
-        default: return bn_bwd_rows_dispatch<__nv_bfloat16>(a, reduce, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int W = 16 / sizeof(T);
+        const RowWidth w = row_width(a.channels * sizeof(T), a.x, a.dy, a.dx);   // a reduction: W whenever wide
+        if (!w.wide) return bn_bwd_rows<T, 1, false>(a, reduce, stream);
+        return w.aligned ? bn_bwd_rows<T, W, true>(a, reduce, stream) : bn_bwd_rows<T, W, false>(a, reduce, stream);
+    });
 }
 
 template <typename P> static int bn_bwd_finalize(const BnBwdArgs &a, cudaStream_t stream) {
@@ -691,12 +597,8 @@ extern "C" int spx_masked_bn_fwd_train(const void *x, void *y, int64_t rows, int
     cudaStream_t stream = (cudaStream_t)stream_;
     if (rows > 0)
         if (int rc = bn_fwd_rows_typed(dtype, a, true, stream)) return rc;
-    int rc = 0;
-    switch (param_dtype) {
-        case SPX_F32: rc = bn_fwd_finalize<float>(a, stream); break;
-        case SPX_F16: rc = bn_fwd_finalize<__half>(a, stream); break;
-        default: rc = bn_fwd_finalize<__nv_bfloat16>(a, stream); break;
-    }
+    const int rc =
+        dispatch_dtype(param_dtype, [&](auto p) { return bn_fwd_finalize<typename decltype(p)::type>(a, stream); });
     if (rc || rows == 0) return rc;
     return bn_fwd_rows_typed(dtype, a, false, stream);
 }
@@ -719,12 +621,8 @@ extern "C" int spx_masked_bn_bwd(const void *x, const void *dy, void *dx, int64_
     cudaStream_t stream = (cudaStream_t)stream_;
     if (rows > 0)
         if (int rc = bn_bwd_rows_typed(dtype, a, true, stream)) return rc;
-    int rc = 0;
-    switch (param_dtype) {
-        case SPX_F32: rc = bn_bwd_finalize<float>(a, stream); break;
-        case SPX_F16: rc = bn_bwd_finalize<__half>(a, stream); break;
-        default: rc = bn_bwd_finalize<__nv_bfloat16>(a, stream); break;
-    }
+    const int rc =
+        dispatch_dtype(param_dtype, [&](auto p) { return bn_bwd_finalize<typename decltype(p)::type>(a, stream); });
     if (rc || rows == 0) return rc;
     return bn_bwd_rows_typed(dtype, a, false, stream);
 }
@@ -829,12 +727,8 @@ extern "C" int spx_masked_sync_bn_fwd_merge(const spx_masked_sync_bn *d, void *w
     SPX_REQUIRE(d->eps > 0.f, "%s: eps must be positive", who);
     const BnFwdArgs a = bn_sync_fwd_args(d, workspace, workspace_bytes);
     cudaStream_t stream = (cudaStream_t)stream_;
-    int rc = 0;
-    switch (d->param_dtype) {
-        case SPX_F32: rc = bn_sync_fwd_merge<float>(d, a, stream); break;
-        case SPX_F16: rc = bn_sync_fwd_merge<__half>(d, a, stream); break;
-        default: rc = bn_sync_fwd_merge<__nv_bfloat16>(d, a, stream); break;
-    }
+    const int rc = dispatch_dtype(d->param_dtype,
+                                  [&](auto p) { return bn_sync_fwd_merge<typename decltype(p)::type>(d, a, stream); });
     if (rc || d->rows == 0) return rc;
     return bn_fwd_rows_typed(d->dtype, a, false, stream);
 }
@@ -849,11 +743,8 @@ extern "C" int spx_masked_sync_bn_bwd_local(const spx_masked_sync_bn *d, void *w
     cudaStream_t stream = (cudaStream_t)stream_;
     if (d->rows > 0)
         if (int rc = bn_bwd_rows_typed(d->dtype, a, true, stream)) return rc;
-    switch (d->param_dtype) {
-        case SPX_F32: return bn_sync_bwd_local<float>(d, a, stream);
-        case SPX_F16: return bn_sync_bwd_local<__half>(d, a, stream);
-        default: return bn_sync_bwd_local<__nv_bfloat16>(d, a, stream);
-    }
+    return dispatch_dtype(d->param_dtype,
+                          [&](auto p) { return bn_sync_bwd_local<typename decltype(p)::type>(d, a, stream); });
 }
 
 extern "C" int spx_masked_sync_bn_bwd_merge(const spx_masked_sync_bn *d, void *workspace, size_t workspace_bytes,
@@ -864,12 +755,8 @@ extern "C" int spx_masked_sync_bn_bwd_merge(const spx_masked_sync_bn *d, void *w
     SPX_REQUIRE(d->rows == 0 || (d->x && d->dy && d->dx), "%s: NULL pointer argument (x, dy, dx)", who);
     const BnBwdArgs a = bn_sync_bwd_args(d, workspace, workspace_bytes);
     cudaStream_t stream = (cudaStream_t)stream_;
-    int rc = 0;
-    switch (d->param_dtype) {
-        case SPX_F32: rc = bn_sync_bwd_merge<float>(d, a, stream); break;
-        case SPX_F16: rc = bn_sync_bwd_merge<__half>(d, a, stream); break;
-        default: rc = bn_sync_bwd_merge<__nv_bfloat16>(d, a, stream); break;
-    }
+    const int rc = dispatch_dtype(d->param_dtype,
+                                  [&](auto p) { return bn_sync_bwd_merge<typename decltype(p)::type>(d, a, stream); });
     if (rc || d->rows == 0) return rc;
     return bn_bwd_rows_typed(d->dtype, a, false, stream);
 }

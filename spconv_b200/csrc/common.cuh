@@ -116,49 +116,6 @@ template <> __device__ __forceinline__ float from_float<float>(float v) { return
 template <> __device__ __forceinline__ __half from_float<__half>(float v) { return __float2half_rn(v); }
 template <> __device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
-// The max rule of the global pool and the point scatter: does (v, r) beat (bv, br)?  r < 0 marks an empty side.
-// A NaN beats every number, then the greater value, then, on equality (-0 == +0), the lower row: a total order
-// whose winner is the first row in ascending order that attains the maximum (np.argmax).
-__device__ __forceinline__ bool max_beats(float v, int r, float bv, int br) {
-    if (r < 0) return false;
-    if (br < 0) return true;
-    const bool n = isnan(v), bn = isnan(bv);
-    if (n != bn) return n;
-    if (!n && v != bv) return v > bv;
-    return r < br;
-}
-
-// ---- per-sample row grouping (global_pool.cu, group_norm.cu)
-constexpr int GP_CHUNK = 512;        // rows per partial
-
-// M = *num_valid clamped to [0, rows]; NULL: every row
-__device__ __forceinline__ int64_t gp_valid_rows(const int32_t *num_valid, int64_t rows) {
-    if (num_valid == nullptr) return rows;
-    const int64_t m = __ldg(num_valid);
-    return m < 0 ? 0 : (m > rows ? rows : m);
-}
-
-// the sample whose chunks hold chunk k: the last b with cstart[b] <= k (empty samples own no chunk)
-__device__ __forceinline__ int gp_sample_of_chunk(const int32_t *cstart, int batch_size, int32_t k) {
-    int lo = 0, hi = batch_size - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(cstart + mid) <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
-// Chan et al.: fold (nb, mb, qb) into (na, ma, qa).  An empty side changes nothing, bit for bit.
-__device__ __forceinline__ void chan_merge(float &na, float &ma, float &qa, float nb, float mb, float qb) {
-    if (nb == 0.f) return;
-    if (na == 0.f) { na = nb; ma = mb; qa = qb; return; }
-    const float n = na + nb, d = mb - ma, f = __fdiv_rn(nb, n);
-    ma = fmaf(d, f, ma);
-    qa = qa + qb + d * d * na * f;
-    na = n;
-}
-
 __device__ __forceinline__ float apply_act(float v, int act, float alpha) {
     // InferenceOps activations: spconv/csrc/sparse/inference.py:26-146
     switch (act) {

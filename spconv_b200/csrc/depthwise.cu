@@ -17,7 +17,7 @@
 // r0 + l, r0 + l + lanes, ... in ascending order, the lanes merge in a fixed binary tree, and the chunk's partial
 // goes to workspace [chunks][C][kv]; the finalize kernel sums the partials in ascending chunk order.  The result
 // depends on the row indices alone: a chunk of padding rows (no pair, or dy = 0) adds +0.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 
@@ -26,47 +26,6 @@ constexpr int DW_KT = 16;        // fwd / dgrad: offsets per shared-memory tile
 constexpr int DW_U = 4;          // fwd / dgrad: gathers in flight per thread
 constexpr int DW_CHUNK = 512;    // wgrad: rows per partial
 constexpr int DW_FIN = 16;       // finalize: partial loads in flight per thread
-
-// A: the pointer is 16-byte aligned, so V elements move as one 16-byte access; otherwise V element accesses.  V
-// alone decides which rows and channels a thread folds, so both give the same bits.
-template <typename T, int V, bool A = true> __device__ __forceinline__ void dw_load(const T *p, float (&f)[V]) {
-    if constexpr (A && V * sizeof(T) == 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-        const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-        for (int j = 0; j < V; ++j) f[j] = to_float(e[j]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < V; ++j) f[j] = to_float(__ldg(p + j));
-    }
-}
-template <typename T, int V> __device__ __forceinline__ void dw_store(T *p, const float (&f)[V]) {
-    if constexpr (V * sizeof(T) == 16) {
-        uint4 v;
-        T *e = reinterpret_cast<T *>(&v);
-#pragma unroll
-        for (int j = 0; j < V; ++j) e[j] = from_float<T>(f[j]);
-        *reinterpret_cast<uint4 *>(p) = v;
-    } else {
-#pragma unroll
-        for (int j = 0; j < V; ++j) p[j] = from_float<T>(f[j]);
-    }
-}
-
-// Block layout: tpr threads per row (a power of two >= the row's vectors, at most 32); blockIdx.y selects the
-// slice of tpr vectors = tpr * V channels.
-struct DwThread {
-    int lane, v, c0;     // row lane, vector index in the row, first channel of the thread
-    bool active;
-};
-template <int V> __device__ __forceinline__ DwThread dw_thread(int vecs, int tpr) {
-    DwThread t;
-    t.lane = threadIdx.x / tpr;
-    t.v = blockIdx.y * tpr + (threadIdx.x % tpr);
-    t.c0 = t.v * V;
-    t.active = t.v < vecs;
-    return t;
-}
 
 // ---------------------------------------------------------------- fwd / dgrad: gather over the offsets
 template <typename T, int V, bool REV>
@@ -79,7 +38,8 @@ __device__ __forceinline__ void dw_gather(const T *__restrict__ src, const T *__
     const int slice_ch = tpr * V;
     const int ch_base = blockIdx.y * slice_ch;
     const int64_t r0 = (int64_t)blockIdx.x * rpb;
-    const DwThread t = dw_thread<V>(vecs, tpr);
+    const RowThread t = row_thread(vecs, tpr);
+    const int c0 = t.v * V;                              // first channel of the thread
     const int64_t row = r0 + t.lane;
     const bool live = t.active && row < rows;
     float acc[V];
@@ -101,7 +61,7 @@ __device__ __forceinline__ void dw_gather(const T *__restrict__ src, const T *__
         }
         __syncthreads();
         if (!live) continue;
-        const int cl0 = t.c0 - ch_base;
+        const int cl0 = c0 - ch_base;
         for (int kk = 0; kk < kt; kk += DW_U) {
             int32_t idx[DW_U];
             float f[DW_U][V];
@@ -109,7 +69,7 @@ __device__ __forceinline__ void dw_gather(const T *__restrict__ src, const T *__
             for (int u = 0; u < DW_U; ++u) {
                 idx[u] = kk + u < kt ? s_t[kk + u][t.lane] : -1;
                 if (idx[u] >= 0) {
-                    dw_load<T, V>(src + (int64_t)idx[u] * channels + t.c0, f[u]);
+                    row_load<T, V>(src + (int64_t)idx[u] * channels + c0, f[u]);
                 } else {
 #pragma unroll
                     for (int j = 0; j < V; ++j) f[u][j] = 0.f;
@@ -127,11 +87,11 @@ __device__ __forceinline__ void dw_gather(const T *__restrict__ src, const T *__
     if (bias != nullptr || act != SPX_ACT_NONE) {
 #pragma unroll
         for (int j = 0; j < V; ++j) {
-            const float b = bias != nullptr ? to_float(__ldg(bias + t.c0 + j)) : 0.f;
+            const float b = bias != nullptr ? to_float(__ldg(bias + c0 + j)) : 0.f;
             acc[j] = apply_act(acc[j] + b, act, alpha);
         }
     }
-    dw_store<T, V>(dst + row * channels + t.c0, acc);
+    row_store<T, V>(dst + row * channels + c0, acc);
 }
 
 template <typename T, int V>
@@ -161,7 +121,8 @@ depthwise_wgrad_partial_kernel(const T *__restrict__ x, const T *__restrict__ dy
     constexpr int KW = DwKw<V>::value;
     __shared__ float s_red[KW * V][DW_THREADS];
     const int lanes = DW_THREADS / tpr;
-    const DwThread t = dw_thread<V>(vecs, tpr);
+    const RowThread t = row_thread(vecs, tpr);
+    const int c0 = t.v * V;
     const int64_t r0 = (int64_t)blockIdx.x * DW_CHUNK;
     const int k0 = blockIdx.z * KW;
     const int64_t end = rows < r0 + DW_CHUNK ? rows : r0 + DW_CHUNK;
@@ -180,12 +141,12 @@ depthwise_wgrad_partial_kernel(const T *__restrict__ x, const T *__restrict__ dy
             for (int kw = 0; kw < KW; ++kw) any |= idx[kw] >= 0;
             if (!any) continue;
             float g[V];
-            dw_load<T, V, A>(dy + r * channels + t.c0, g);
+            row_load<T, V, A>(dy + r * channels + c0, g);
 #pragma unroll
             for (int kw = 0; kw < KW; ++kw) {
                 if (idx[kw] < 0) continue;
                 float f[V];
-                dw_load<T, V, A>(x + (int64_t)idx[kw] * channels + t.c0, f);
+                row_load<T, V, A>(x + (int64_t)idx[kw] * channels + c0, f);
 #pragma unroll
                 for (int j = 0; j < V; ++j) acc[kw][j] = fmaf(g[j], f[j], acc[kw][j]);
             }
@@ -213,7 +174,7 @@ depthwise_wgrad_partial_kernel(const T *__restrict__ x, const T *__restrict__ dy
     float *dst = partials + (int64_t)blockIdx.x * channels * kv;
 #pragma unroll
     for (int j = 0; j < V; ++j) {
-        const int c = t.c0 + j;
+        const int c = c0 + j;
 #pragma unroll
         for (int kw = 0; kw < KW; ++kw)
             if (k0 + kw < kv) dst[(int64_t)c * kv + k0 + kw] = acc[kw][j];
@@ -240,17 +201,11 @@ depthwise_wgrad_finalize_kernel(const float *__restrict__ partials, int64_t chun
 }
 
 // ---------------------------------------------------------------- launchers
-static int dw_tpr(int vecs) {
-    int tpr = 1;
-    while (tpr < vecs && tpr < 32) tpr <<= 1;
-    return tpr;
-}
-
 template <typename T, int V>
 static int launch_gather(bool fwd, bool rev, const void *src, const void *weight, const void *bias, void *dst,
                          const int32_t *table, int64_t stride, int kv, int64_t rows, int channels, int act, float alpha,
                          cudaStream_t stream) {
-    const int vecs = channels / V, tpr = dw_tpr(vecs);
+    const int vecs = channels / V, tpr = row_tpr(vecs);
     const dim3 grid((unsigned)div_up64(rows, DW_THREADS / tpr), (unsigned)div_up64(vecs, tpr));
     if (fwd) {
         depthwise_fwd_kernel<T, V><<<grid, DW_THREADS, 0, stream>>>((const T *)src, (const T *)weight, (const T *)bias,
@@ -286,7 +241,7 @@ static int launch_wgrad(const void *x, const void *dy, void *dweight, const int3
                         int64_t rows, int channels, float *partials, cudaStream_t stream) {
     const int64_t chunks = dw_chunks(rows);
     if (chunks > 0) {
-        const int vecs = channels / V, tpr = dw_tpr(vecs);
+        const int vecs = channels / V, tpr = row_tpr(vecs);
         const dim3 grid((unsigned)chunks, (unsigned)div_up64(vecs, tpr), (unsigned)div_up64(kv, DwKw<V>::value));
         depthwise_wgrad_partial_kernel<T, V, A><<<grid, DW_THREADS, 0, stream>>>((const T *)x, (const T *)dy, table, stride,
                                                                               kv, rows, channels, vecs, tpr, partials);
@@ -302,11 +257,11 @@ static int launch_wgrad(const void *x, const void *dy, void *dweight, const int3
 // The partial sums' order follows the vector width: a misaligned x or dy keeps the width of the aligned call and
 // only loads element by element, so the weight gradient does not depend on where the operands start.
 template <typename T>
-static int dispatch_wgrad(bool wide, bool aligned, const void *x, const void *dy, void *dweight, const int32_t *table,
+static int dispatch_wgrad(RowWidth w, const void *x, const void *dy, void *dweight, const int32_t *table,
                           int64_t stride, int kv, int64_t rows, int channels, float *partials, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    if (!wide) return launch_wgrad<T, 1, false>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
-    if (aligned) return launch_wgrad<T, W, true>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
+    if (!w.wide) return launch_wgrad<T, 1, false>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
+    if (w.aligned) return launch_wgrad<T, W, true>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
     return launch_wgrad<T, W, false>(x, dy, dweight, table, stride, kv, rows, channels, partials, stream);
 }
 
@@ -324,10 +279,6 @@ static int check_depthwise(const char *who, int64_t stride, int kv, int64_t rows
     return 0;
 }
 
-static bool use_vectors(int channels, int dtype, const void *a, const void *b, const void *c) {
-    return ((int64_t)channels * dtype_bytes(dtype)) % 16 == 0 && aligned16(a) && aligned16(b) && aligned16(c);
-}
-
 extern "C" int spx_depthwise_fwd(const void *features, const void *weight, const void *bias, void *out,
                                  const int32_t *table, int64_t table_stride, int kv, int64_t n_out, int channels,
                                  int dtype, int act, float act_alpha, spx_stream_t stream_) {
@@ -336,14 +287,13 @@ extern "C" int spx_depthwise_fwd(const void *features, const void *weight, const
                 "depthwise_fwd: bad activation %d", act);
     if (n_out == 0) return 0;
     SPX_REQUIRE(weight && out && table, "depthwise_fwd: NULL pointer argument");
-    const bool vec = use_vectors(channels, dtype, features, out, nullptr);
+    const RowWidth w = row_width((int64_t)channels * dtype_bytes(dtype), features, out);
     cudaStream_t stream = (cudaStream_t)stream_;
-    switch (dtype) {
-        case SPX_F32: return dispatch_gather<float>(vec, true, false, features, weight, bias, out, table, table_stride, kv, n_out, channels, act, act_alpha, stream);
-        case SPX_F16: return dispatch_gather<__half>(vec, true, false, features, weight, bias, out, table, table_stride, kv, n_out, channels, act, act_alpha, stream);
-        case SPX_BF16: return dispatch_gather<__nv_bfloat16>(vec, true, false, features, weight, bias, out, table, table_stride, kv, n_out, channels, act, act_alpha, stream);
-    }
-    return 2;
+    return dispatch_dtype(dtype, [&](auto t) {
+        return dispatch_gather<typename decltype(t)::type>(w.wide && w.aligned, true, false, features, weight, bias, out,
+                                                           table, table_stride, kv, n_out, channels, act, act_alpha,
+                                                           stream);
+    });
 }
 
 extern "C" int spx_depthwise_dgrad(const void *out_bp, const void *weight, void *din, const int32_t *table,
@@ -352,15 +302,14 @@ extern "C" int spx_depthwise_dgrad(const void *out_bp, const void *weight, void 
     if (check_depthwise("depthwise_dgrad", table_stride, kv, n_in, channels, dtype)) return 2;
     if (n_in == 0) return 0;
     SPX_REQUIRE(weight && din && table, "depthwise_dgrad: NULL pointer argument");
-    const bool vec = use_vectors(channels, dtype, out_bp, din, nullptr);
+    const RowWidth w = row_width((int64_t)channels * dtype_bytes(dtype), out_bp, din);
     const bool rev = reverse_offsets != 0;
     cudaStream_t stream = (cudaStream_t)stream_;
-    switch (dtype) {
-        case SPX_F32: return dispatch_gather<float>(vec, false, rev, out_bp, weight, nullptr, din, table, table_stride, kv, n_in, channels, SPX_ACT_NONE, 0.f, stream);
-        case SPX_F16: return dispatch_gather<__half>(vec, false, rev, out_bp, weight, nullptr, din, table, table_stride, kv, n_in, channels, SPX_ACT_NONE, 0.f, stream);
-        case SPX_BF16: return dispatch_gather<__nv_bfloat16>(vec, false, rev, out_bp, weight, nullptr, din, table, table_stride, kv, n_in, channels, SPX_ACT_NONE, 0.f, stream);
-    }
-    return 2;
+    return dispatch_dtype(dtype, [&](auto t) {
+        return dispatch_gather<typename decltype(t)::type>(w.wide && w.aligned, false, rev, out_bp, weight, nullptr, din,
+                                                           table, table_stride, kv, n_in, channels, SPX_ACT_NONE, 0.f,
+                                                           stream);
+    });
 }
 
 extern "C" size_t spx_depthwise_wgrad_workspace_size(int64_t n_out, int kv, int channels) {
@@ -377,14 +326,11 @@ extern "C" int spx_depthwise_wgrad(const void *features, const void *out_bp, voi
     const size_t need = spx_depthwise_wgrad_workspace_size(n_out, kv, channels);
     SPX_REQUIRE(workspace_bytes >= need && (need == 0 || workspace != nullptr),
                 "depthwise_wgrad: workspace of %zu bytes, %zu needed", workspace_bytes, need);
-    const bool wide = ((int64_t)channels * dtype_bytes(dtype)) % 16 == 0;
-    const bool aligned = aligned16(features) && aligned16(out_bp);
+    const RowWidth w = row_width((int64_t)channels * dtype_bytes(dtype), features, out_bp);
     float *partials = (float *)workspace;
     cudaStream_t stream = (cudaStream_t)stream_;
-    switch (dtype) {
-        case SPX_F32: return dispatch_wgrad<float>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
-        case SPX_F16: return dispatch_wgrad<__half>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
-        case SPX_BF16: return dispatch_wgrad<__nv_bfloat16>(wide, aligned, features, out_bp, dweight, table, table_stride, kv, n_out, channels, partials, stream);
-    }
-    return 2;
+    return dispatch_dtype(dtype, [&](auto t) {
+        return dispatch_wgrad<typename decltype(t)::type>(w, features, out_bp, dweight, table, table_stride, kv, n_out,
+                                                          channels, partials, stream);
+    });
 }

@@ -22,7 +22,7 @@
 // (mean), and 0 on padding and dropped rows: every element of din is written once, nothing is scattered.
 // The summation order depends only on the sample's valid rows, never on `rows`, M beyond them or the grid,
 // and no float atomics are used, so every result is bit-reproducible and independent of padding.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
@@ -36,34 +36,12 @@ constexpr int GP_FIN_LANES = 32;     // finalize: partial lanes per channel
 constexpr int GP_MAX_BATCH = 1 << 20;
 constexpr int GP_MAX_CHANNELS = 1 << 16;   // finalize grid.y = C / GP_FIN_CH must stay below 2^16
 
-// A: the pointer is 16-byte aligned, so W elements move as one 16-byte access; otherwise W element accesses.  W
-// alone decides which rows and channels a thread folds, so both give the same bits.
-template <typename T, int W, bool A = true> __device__ __forceinline__ void gp_load(const T *p, float (&f)[W]) {
-    if constexpr (A && W * sizeof(T) == 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-        const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(e[j]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(__ldg(p + j));
-    }
-}
-template <typename T, int W> __device__ __forceinline__ void gp_store(T *p, const T (&e)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
-        *reinterpret_cast<uint4 *>(p) = *reinterpret_cast<const uint4 *>(e);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) p[j] = e[j];
-    }
-}
-
 __global__ void gp_keys_kernel(const int32_t *__restrict__ coords, int64_t rows, int row_ints, int batch_size,
                                const int32_t *__restrict__ num_valid, uint32_t *__restrict__ keys) {
     const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (r >= rows) return;
     uint32_t key = (uint32_t)batch_size;
-    if (r < gp_valid_rows(num_valid, rows)) {
+    if (r < valid_rows(num_valid, rows)) {
         const int32_t b = __ldg(coords + r * row_ints);
         if (b >= 0 && b < batch_size) key = (uint32_t)b;
     }
@@ -121,8 +99,6 @@ gp_segments_kernel(const uint32_t *__restrict__ keys, int32_t n, int batch_size,
     }
 }
 
-// Block layout as batchnorm.cu: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
-// `lanes` = GP_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
 template <typename T, int W, bool MEAN, bool A>
 __global__ void __launch_bounds__(GP_THREADS)
 gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, const int32_t *__restrict__ offsets,
@@ -130,6 +106,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
                  float2 *__restrict__ partials) {
     __shared__ float s_v[GP_THREADS * W];
     __shared__ int s_r[MEAN ? 1 : GP_THREADS * W];
+    // sample_chunk (rows.cuh) written out: called, it gives these kernels a different register allocation
     const int32_t k = (int32_t)blockIdx.x;
     if (k >= __ldg(cstart + batch_size)) return;
     const int b = gp_sample_of_chunk(cstart, batch_size, k);
@@ -137,9 +114,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
     const int32_t seg_end = __ldg(offsets + b + 1);
     const int32_t end = seg_end < p0 + GP_CHUNK ? seg_end : p0 + GP_CHUNK;
     const int lanes = GP_THREADS / tpr;
-    const int lane = threadIdx.x / tpr;
-    const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
-    const bool active = v < vecs;
+    const RowThread t = row_thread(vecs, tpr);
     float acc[W];
     int arg[W];
 #pragma unroll
@@ -147,8 +122,8 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
         acc[j] = MEAN ? 0.f : -INFINITY;
         arg[j] = -1;
     }
-    if (active) {
-        const T *base = x + (int64_t)v * W;
+    if (t.active) {
+        const T *base = x + (int64_t)t.v * W;
         auto fold = [&](const float (&f)[W], int r) {        // rows of a lane come in ascending order
 #pragma unroll
             for (int j = 0; j < W; ++j) {
@@ -160,21 +135,21 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
                 }
             }
         };
-        int64_t p = p0 + lane;
+        int64_t p = p0 + t.lane;
         for (; p + lanes < end; p += 2 * lanes) {             // two rows in flight (four spill), folded in row order
             int r[2];
             float f[2][W];
 #pragma unroll
             for (int u = 0; u < 2; ++u) r[u] = __ldg(order + p + u * lanes);
 #pragma unroll
-            for (int u = 0; u < 2; ++u) gp_load<T, W, A>(base + (int64_t)r[u] * channels, f[u]);
+            for (int u = 0; u < 2; ++u) row_load<T, W, A>(base + (int64_t)r[u] * channels, f[u]);
 #pragma unroll
             for (int u = 0; u < 2; ++u) fold(f[u], r[u]);
         }
         for (; p < end; p += lanes) {
             const int r = __ldg(order + p);
             float f[W];
-            gp_load<T, W, A>(base + (int64_t)r * channels, f);
+            row_load<T, W, A>(base + (int64_t)r * channels, f);
             fold(f, r);
         }
     }
@@ -187,7 +162,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
     }
     for (int s = lanes >> 1; s >= 1; s >>= 1) {
         __syncthreads();
-        if (lane < s) {
+        if (t.lane < s) {
             const int o = slot + s * tpr;
 #pragma unroll
             for (int j = 0; j < W; ++j) {
@@ -200,8 +175,8 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
             }
         }
     }
-    if (lane == 0 && active) {
-        float2 *dst = partials + (int64_t)k * channels + (int64_t)v * W;
+    if (t.lane == 0 && t.active) {
+        float2 *dst = partials + (int64_t)k * channels + (int64_t)t.v * W;
 #pragma unroll
         for (int j = 0; j < W; ++j) dst[j] = make_float2(acc[j], __int_as_float(arg[j]));
     }
@@ -261,7 +236,7 @@ gp_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ coords, int6
     const int v = (int)(idx - r * vecs);
     if (r >= rows) return;
     int b = -1;
-    if (r < gp_valid_rows(num_valid, rows)) {
+    if (r < valid_rows(num_valid, rows)) {
         b = __ldg(coords + r * row_ints);
         if (b >= batch_size) b = -1;
     }
@@ -272,7 +247,7 @@ gp_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ coords, int6
         const int64_t o = (int64_t)b * channels + (int64_t)v * W;
         if constexpr (MEAN) {
             float f[W];
-            gp_load<T, W>(dy + o, f);
+            row_load<T, W>(dy + o, f);
             const float n = (float)__ldg(count + b);           // >= 1: row r itself counts
 #pragma unroll
             for (int j = 0; j < W; ++j) e[j] = from_float<T>(__fdiv_rn(f[j], n));
@@ -282,18 +257,12 @@ gp_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ coords, int6
                 if (__ldg(argmax + o + j) == (int32_t)r) e[j] = dy[o + j];
         }
     }
-    gp_store<T, W>(din + r * channels + (int64_t)v * W, e);
+    row_store_raw<T, W>(din + r * channels + (int64_t)v * W, e);
 }
 
 // ---------------------------------------------------------------- host side
 static int64_t gp_max_chunks(int64_t rows, int batch_size) {
     return (rows + GP_CHUNK - 1) / GP_CHUNK + batch_size;
-}
-
-static int gp_tpr(int vecs) {
-    int tpr = 1;
-    while (tpr < vecs && tpr < 32) tpr <<= 1;
-    return tpr;
 }
 
 // keys -> stable argsort -> segments: order [rows], offsets [B+1], cstart [B+1] and, when count != NULL, count [B]
@@ -345,7 +314,7 @@ struct GpFwdArgs {
 template <typename T, int W, bool MEAN, bool A> static int gp_fwd_launch(const GpFwdArgs &a, cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (a.rows > 0) {
-        const int tpr = gp_tpr(vecs);
+        const int tpr = row_tpr(vecs);
         const dim3 grid((unsigned)gp_max_chunks(a.rows, a.batch_size), (unsigned)div_up64(vecs, tpr));
         gp_reduce_kernel<T, W, MEAN, A><<<grid, GP_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), a.order, a.offsets, a.cstart, a.batch_size, a.channels, vecs, tpr,
@@ -361,10 +330,10 @@ template <typename T, int W, bool MEAN, bool A> static int gp_fwd_launch(const G
 
 template <typename T> static int gp_fwd_dispatch(const GpFwdArgs &a, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    // a misaligned x keeps the row layout (and so the order of the sums) of the aligned call
-    if ((a.channels * (int)sizeof(T)) % 16)
+    const RowWidth w = row_width(a.channels * sizeof(T), a.x);     // a reduction: W whenever wide
+    if (!w.wide)
         return a.mode == 1 ? gp_fwd_launch<T, 1, true, false>(a, stream) : gp_fwd_launch<T, 1, false, false>(a, stream);
-    if (a.rows == 0 || aligned16(a.x))
+    if (a.rows == 0 || w.aligned)
         return a.mode == 1 ? gp_fwd_launch<T, W, true, true>(a, stream) : gp_fwd_launch<T, W, false, true>(a, stream);
     return a.mode == 1 ? gp_fwd_launch<T, W, true, false>(a, stream) : gp_fwd_launch<T, W, false, false>(a, stream);
 }
@@ -390,7 +359,8 @@ template <typename T, int W, bool MEAN> static int gp_bwd_launch(const GpBwdArgs
 
 template <typename T> static int gp_bwd_dispatch(const GpBwdArgs &a, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (a.channels * (int)sizeof(T)) % 16 == 0 && aligned16(a.dy) && aligned16(a.din);
+    const RowWidth w = row_width(a.channels * sizeof(T), a.dy, a.din);
+    const bool vec = w.wide && w.aligned;
     if (a.mode == 1) return vec ? gp_bwd_launch<T, W, true>(a, stream) : gp_bwd_launch<T, 1, true>(a, stream);
     return vec ? gp_bwd_launch<T, W, false>(a, stream) : gp_bwd_launch<T, 1, false>(a, stream);
 }
@@ -430,11 +400,7 @@ extern "C" int spx_global_pool_fwd(int mode, const void *features, const int32_t
                                mode == 1 ? count : nullptr, stream))
         return rc;
     GpFwdArgs a{mode, features, order, offsets, cstart, rows, batch_size, channels, partials, out, argmax};
-    switch (dtype) {
-        case SPX_F32: return gp_fwd_dispatch<float>(a, stream);
-        case SPX_F16: return gp_fwd_dispatch<__half>(a, stream);
-        default: return gp_fwd_dispatch<__nv_bfloat16>(a, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) { return gp_fwd_dispatch<typename decltype(t)::type>(a, stream); });
 }
 
 extern "C" int spx_global_pool_bwd(int mode, const void *dy, const int32_t *coords, int64_t rows, int row_ints,
@@ -449,9 +415,5 @@ extern "C" int spx_global_pool_bwd(int mode, const void *dy, const int32_t *coor
     if (rows == 0) return 0;
     GpBwdArgs a{mode, dy, coords, rows, row_ints, batch_size, channels, num_valid, argmax, count, din};
     cudaStream_t stream = (cudaStream_t)stream_;
-    switch (dtype) {
-        case SPX_F32: return gp_bwd_dispatch<float>(a, stream);
-        case SPX_F16: return gp_bwd_dispatch<__half>(a, stream);
-        default: return gp_bwd_dispatch<__nv_bfloat16>(a, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) { return gp_bwd_dispatch<typename decltype(t)::type>(a, stream); });
 }

@@ -23,7 +23,7 @@
 //   apply    : dx = invstd_bg * (gamma_c dy - S1 / n - xhat * S2 / n); every element of dx is written once.
 // The order of every sum depends only on the sample's kept rows, never on `rows`, the padding or the grid, and no
 // float atomics are used, so every result is bit-reproducible and independent of padding and dropped rows.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
@@ -37,32 +37,6 @@ constexpr int GN_FIN_LANES = 32;     // finalize: partial lanes per channel
 constexpr int GN_MAX_BATCH = 1 << 20;
 constexpr int GN_MAX_CHANNELS = 1 << 16;
 
-// A: one 16-byte access per W elements; otherwise W element accesses.  W alone decides which rows and channels a
-// thread folds, so both give the same bits.
-template <typename T, int W, bool A> __device__ __forceinline__ void gn_load(const T *p, float (&f)[W]) {
-    if constexpr (A && W * sizeof(T) == 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-        const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(e[j]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(__ldg(p + j));
-    }
-}
-template <typename T, int W, bool A> __device__ __forceinline__ void gn_store(T *p, const float (&f)[W]) {
-    if constexpr (A && W * sizeof(T) == 16) {
-        uint4 v;
-        T *e = reinterpret_cast<T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) e[j] = from_float<T>(f[j]);
-        *reinterpret_cast<uint4 *>(p) = v;
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) p[j] = from_float<T>(f[j]);
-    }
-}
-
 // sample of row r, or -1 for a padding or dropped row
 __device__ __forceinline__ int gn_row_sample(const int32_t *coords, int64_t r, int row_ints, int batch_size,
                                              int64_t M) {
@@ -71,21 +45,7 @@ __device__ __forceinline__ int gn_row_sample(const int32_t *coords, int64_t r, i
     return b >= 0 && b < batch_size ? b : -1;
 }
 
-// The chunk of block blockIdx.x: its sample and sorted positions [p0, end).  False past the last chunk.
-__device__ __forceinline__ bool gn_chunk(const int32_t *offsets, const int32_t *cstart, int batch_size, int &b,
-                                         int32_t &p0, int32_t &end) {
-    const int32_t k = (int32_t)blockIdx.x;
-    if (k >= __ldg(cstart + batch_size)) return false;
-    b = gp_sample_of_chunk(cstart, batch_size, k);
-    p0 = __ldg(offsets + b) + (k - __ldg(cstart + b)) * GP_CHUNK;
-    const int32_t seg_end = __ldg(offsets + b + 1);
-    end = seg_end < p0 + GP_CHUNK ? seg_end : p0 + GP_CHUNK;
-    return true;
-}
-
 // ---------------------------------------------------------------- forward
-// Block layout of gp_reduce_kernel: `tpr` threads per row (a power of two >= the row's vectors, at most 32),
-// `lanes` = GN_THREADS / tpr rows in flight; blockIdx.y selects a slice of tpr vectors.
 template <typename T, int W, bool A>
 __global__ void __launch_bounds__(GN_THREADS)
 gn_stats_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, const int32_t *__restrict__ offsets,
@@ -94,16 +54,14 @@ gn_stats_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, cons
     __shared__ float s_mean[GN_THREADS * W], s_q[GN_THREADS * W], s_n[GN_THREADS];
     int b;
     int32_t p0, end;
-    if (!gn_chunk(offsets, cstart, batch_size, b, p0, end)) return;
+    if (!sample_chunk(offsets, cstart, batch_size, b, p0, end)) return;
     const int lanes = GN_THREADS / tpr;
-    const int lane = threadIdx.x / tpr;
-    const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
-    const bool active = v < vecs;
+    const RowThread t = row_thread(vecs, tpr);
     float n = 0.f, mean[W], q[W];
 #pragma unroll
     for (int j = 0; j < W; ++j) mean[j] = q[j] = 0.f;
-    if (active) {
-        const T *base = x + (int64_t)v * W;
+    if (t.active) {
+        const T *base = x + (int64_t)t.v * W;
         auto fold = [&](const float (&f)[W], float inv) {  // Welford, in ascending sorted position; inv = 1 / n
             n += 1.f;
 #pragma unroll
@@ -113,7 +71,7 @@ gn_stats_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, cons
                 q[j] = fmaf(d, f[j] - mean[j], q[j]);
             }
         };
-        int32_t p = p0 + lane;
+        int32_t p = p0 + t.lane;
         for (; p + lanes < end; p += 2 * lanes) {          // two rows in flight, folded in order
             // the reciprocals first: their slow path is a call, and nothing of the rows is live across it
             const float inv0 = __frcp_rn(n + 1.f), inv1 = __frcp_rn(n + 2.f);
@@ -122,39 +80,20 @@ gn_stats_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, cons
 #pragma unroll
             for (int u = 0; u < 2; ++u) r[u] = __ldg(order + p + u * lanes);
 #pragma unroll
-            for (int u = 0; u < 2; ++u) gn_load<T, W, A>(base + (int64_t)r[u] * channels, f[u]);
+            for (int u = 0; u < 2; ++u) row_load<T, W, A>(base + (int64_t)r[u] * channels, f[u]);
             fold(f[0], inv0);
             fold(f[1], inv1);
         }
         for (; p < end; p += lanes) {
             const float inv = __frcp_rn(n + 1.f);
             float f[W];
-            gn_load<T, W, A>(base + (int64_t)__ldg(order + p) * channels, f);
+            row_load<T, W, A>(base + (int64_t)__ldg(order + p) * channels, f);
             fold(f, inv);
         }
     }
-    // fixed tree over the row lanes: at step s, lanes [0, s) fold lanes [s, 2s) into their own slots
-    const int slot = threadIdx.x;
-#pragma unroll
-    for (int j = 0; j < W; ++j) { s_mean[slot * W + j] = mean[j]; s_q[slot * W + j] = q[j]; }
-    s_n[slot] = n;
-    for (int s = lanes >> 1; s >= 1; s >>= 1) {
-        __syncthreads();
-        if (lane < s) {
-            const int o = slot + s * tpr;
-            const float nb = s_n[o];
-#pragma unroll
-            for (int j = 0; j < W; ++j) {
-                float na = n;
-                chan_merge(na, mean[j], q[j], nb, s_mean[o * W + j], s_q[o * W + j]);
-                s_mean[slot * W + j] = mean[j];
-                s_q[slot * W + j] = q[j];
-            }
-            s_n[slot] = n = n + nb;
-        }
-    }
-    if (lane == 0 && active) {
-        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)v * W;
+    welford_lane_tree<W>(s_mean, s_q, s_n, lanes, tpr, n, mean, q);
+    if (t.lane == 0 && t.active) {
+        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
 #pragma unroll
         for (int j = 0; j < W; ++j) dst[j] = make_float2(mean[j], q[j]);
     }
@@ -233,11 +172,11 @@ gn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, const int32_t *_
     const int64_t r = blockIdx.x * (int64_t)lanes + threadIdx.x / tpr;
     const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
     if (r >= rows || v >= vecs) return;
-    const int b = gn_row_sample(coords, r, row_ints, batch_size, gp_valid_rows(num_valid, rows));
+    const int b = gn_row_sample(coords, r, row_ints, batch_size, valid_rows(num_valid, rows));
     const int cg = channels / groups;
     float f[W];
     if (b >= 0) {
-        gn_load<T, W, A>(x + r * channels + (int64_t)v * W, f);
+        row_load<T, W, A>(x + r * channels + (int64_t)v * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -249,7 +188,7 @@ gn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, const int32_t *_
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    gn_store<T, W, A>(y + r * channels + (int64_t)v * W, f);
+    row_store<T, W, A>(y + r * channels + (int64_t)v * W, f);
 }
 
 // ---------------------------------------------------------------- backward
@@ -262,24 +201,22 @@ gn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, const in
     __shared__ float s_a[GN_THREADS * W], s_b[GN_THREADS * W];
     int b;
     int32_t p0, end;
-    if (!gn_chunk(offsets, cstart, batch_size, b, p0, end)) return;
+    if (!sample_chunk(offsets, cstart, batch_size, b, p0, end)) return;
     const int lanes = GN_THREADS / tpr;
-    const int lane = threadIdx.x / tpr;
-    const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
-    const bool active = v < vecs;
+    const RowThread t = row_thread(vecs, tpr);
     float sdy[W], sdyx[W];
 #pragma unroll
     for (int j = 0; j < W; ++j) sdy[j] = sdyx[j] = 0.f;
-    if (active) {
+    if (t.active) {
         const int cg = channels / groups;
         float mean[W], invstd[W];
 #pragma unroll
         for (int j = 0; j < W; ++j) {
-            const int64_t bg = (int64_t)b * groups + (v * W + j) / cg;
+            const int64_t bg = (int64_t)b * groups + (t.v * W + j) / cg;
             mean[j] = __ldg(mean_bg + bg);
             invstd[j] = __ldg(invstd_bg + bg);
         }
-        const int64_t off = (int64_t)v * W;
+        const int64_t off = (int64_t)t.v * W;
         auto fold = [&](const float (&fx)[W], const float (&fd)[W]) {
 #pragma unroll
             for (int j = 0; j < W; ++j) {
@@ -287,14 +224,14 @@ gn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, const in
                 sdyx[j] = fmaf(fd[j], (fx[j] - mean[j]) * invstd[j], sdyx[j]);
             }
         };
-        int32_t p = p0 + lane;
+        int32_t p = p0 + t.lane;
         for (; p + lanes < end; p += 2 * lanes) {          // two rows of x and dy in flight
             float fx[2][W], fd[2][W];
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const int64_t o = (int64_t)__ldg(order + p + u * lanes) * channels + off;
-                gn_load<T, W, A>(x + o, fx[u]);
-                gn_load<T, W, A>(dy + o, fd[u]);
+                row_load<T, W, A>(x + o, fx[u]);
+                row_load<T, W, A>(dy + o, fd[u]);
             }
 #pragma unroll
             for (int u = 0; u < 2; ++u) fold(fx[u], fd[u]);
@@ -302,27 +239,14 @@ gn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, const in
         for (; p < end; p += lanes) {
             const int64_t o = (int64_t)__ldg(order + p) * channels + off;
             float fx[W], fd[W];
-            gn_load<T, W, A>(x + o, fx);
-            gn_load<T, W, A>(dy + o, fd);
+            row_load<T, W, A>(x + o, fx);
+            row_load<T, W, A>(dy + o, fd);
             fold(fx, fd);
         }
     }
-    const int slot = threadIdx.x;
-#pragma unroll
-    for (int j = 0; j < W; ++j) { s_a[slot * W + j] = sdy[j]; s_b[slot * W + j] = sdyx[j]; }
-    for (int s = lanes >> 1; s >= 1; s >>= 1) {
-        __syncthreads();
-        if (lane < s) {
-            const int o = slot + s * tpr;
-#pragma unroll
-            for (int j = 0; j < W; ++j) {
-                s_a[slot * W + j] = sdy[j] = sdy[j] + s_a[o * W + j];
-                s_b[slot * W + j] = sdyx[j] = sdyx[j] + s_b[o * W + j];
-            }
-        }
-    }
-    if (lane == 0 && active) {
-        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)v * W;
+    pair_sum_lane_tree<W>(s_a, s_b, lanes, tpr, sdy, sdyx);
+    if (t.lane == 0 && t.active) {
+        float2 *dst = partials + (int64_t)blockIdx.x * channels + (int64_t)t.v * W;
 #pragma unroll
         for (int j = 0; j < W; ++j) dst[j] = make_float2(sdy[j], sdyx[j]);
     }
@@ -403,14 +327,14 @@ gn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
     const int64_t r = blockIdx.x * (int64_t)lanes + threadIdx.x / tpr;
     const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
     if (r >= rows || v >= vecs) return;
-    const int b = gn_row_sample(coords, r, row_ints, batch_size, gp_valid_rows(num_valid, rows));
+    const int b = gn_row_sample(coords, r, row_ints, batch_size, valid_rows(num_valid, rows));
     const int cg = channels / groups;
     float f[W];
     if (b >= 0) {
         float fx[W];
         const int64_t o = r * channels + (int64_t)v * W;
-        gn_load<T, W, A>(x + o, fx);
-        gn_load<T, W, A>(dy + o, f);
+        row_load<T, W, A>(x + o, fx);
+        row_load<T, W, A>(dy + o, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
@@ -425,18 +349,12 @@ gn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
 #pragma unroll
         for (int j = 0; j < W; ++j) f[j] = 0.f;
     }
-    gn_store<T, W, A>(dx + r * channels + (int64_t)v * W, f);
+    row_store<T, W, A>(dx + r * channels + (int64_t)v * W, f);
 }
 
 // ---------------------------------------------------------------- host side
 static int64_t gn_max_chunks(int64_t rows, int batch_size) {
     return (rows + GP_CHUNK - 1) / GP_CHUNK + batch_size;
-}
-
-static int gn_tpr(int vecs) {
-    int tpr = 1;
-    while (tpr < vecs && tpr < 32) tpr <<= 1;
-    return tpr;
 }
 
 static int gn_check(const char *who, int64_t rows, int row_ints, int batch_size, int channels, int groups, int dtype,
@@ -493,7 +411,7 @@ template <typename T, typename P, int W, bool A> static int gn_rows(const GnArgs
                                                                    cudaStream_t stream) {
     const int vecs = a.channels / W;
     if (reduce) {
-        const int tpr = gn_tpr(vecs);
+        const int tpr = row_tpr(vecs);
         const dim3 grid((unsigned)gn_max_chunks(a.rows, a.batch_size), (unsigned)div_up64(vecs, tpr));
         if (fwd) {
             gn_stats_kernel<T, W, A><<<grid, GN_THREADS, 0, stream>>>(
@@ -508,7 +426,7 @@ template <typename T, typename P, int W, bool A> static int gn_rows(const GnArgs
         }
         return 0;
     }
-    const int tpr = gn_tpr(vecs);
+    const int tpr = row_tpr(vecs);
     const dim3 blocks((unsigned)div_up64(a.rows, GN_THREADS / tpr), (unsigned)div_up64(vecs, tpr));
     if (fwd) {
         gn_fwd_apply_kernel<T, P, W, A><<<blocks, GN_THREADS, 0, stream>>>(
@@ -527,27 +445,21 @@ template <typename T, typename P, int W, bool A> static int gn_rows(const GnArgs
     return 0;
 }
 
-// 16-byte vectors when the row size allows them; a misaligned operand keeps that width (and so the order of the
-// sums) and only loads and stores element by element
-template <typename T, typename P> static int gn_rows_dispatch(const GnArgs &a, bool fwd, bool reduce,
-                                                              cudaStream_t stream) {
-    constexpr int W = 16 / sizeof(T);
-    if ((a.channels * (int)sizeof(T)) % 16) return gn_rows<T, P, 1, false>(a, fwd, reduce, stream);
-    const bool aligned = fwd ? aligned16(a.x) && aligned16(a.y)
-                             : aligned16(a.x) && aligned16(a.dy) && aligned16(a.dx);
-    return aligned ? gn_rows<T, P, W, true>(a, fwd, reduce, stream) : gn_rows<T, P, W, false>(a, fwd, reduce, stream);
-}
-
 static int gn_rows_typed(int dtype, int param_dtype, const GnArgs &a, bool fwd, bool reduce, cudaStream_t stream) {
-    switch (dtype) {
-        case SPX_F32: return gn_rows_dispatch<float, float>(a, fwd, reduce, stream);
-        case SPX_F16:
-            return param_dtype == SPX_F32 ? gn_rows_dispatch<__half, float>(a, fwd, reduce, stream)
-                                          : gn_rows_dispatch<__half, __half>(a, fwd, reduce, stream);
-        default:
-            return param_dtype == SPX_F32 ? gn_rows_dispatch<__nv_bfloat16, float>(a, fwd, reduce, stream)
-                                          : gn_rows_dispatch<__nv_bfloat16, __nv_bfloat16>(a, fwd, reduce, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int W = 16 / sizeof(T);
+        // the reductions and the applies share one width: W whenever wide
+        const RowWidth w = fwd ? row_width(a.channels * sizeof(T), a.x, a.y)
+                               : row_width(a.channels * sizeof(T), a.x, a.dy, a.dx);
+        auto rows = [&](auto p) {
+            using P = typename decltype(p)::type;
+            if (!w.wide) return gn_rows<T, P, 1, false>(a, fwd, reduce, stream);
+            return w.aligned ? gn_rows<T, P, W, true>(a, fwd, reduce, stream)
+                             : gn_rows<T, P, W, false>(a, fwd, reduce, stream);
+        };
+        return param_dtype == SPX_F32 ? rows(Type<float>{}) : rows(Type<T>{});
+    });
 }
 
 template <typename P> static int gn_bwd_coef(const GnArgs &a, cudaStream_t stream) {
@@ -651,12 +563,8 @@ extern "C" int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *w
     gn_bwd_finalize_kernel<<<dim3((unsigned)a.batch_size, (unsigned)div_up64(a.channels, GN_FIN_CH)),
                              GN_FIN_CH * GN_FIN_LANES, 0, stream>>>(a.ws.partials, a.cstart, a.channels, a.ws.bc);
     SPX_CHECK_LAUNCH("gn_bwd_finalize_kernel");
-    int rc = 0;
-    switch (d->param_dtype) {
-        case SPX_F32: rc = gn_bwd_coef<float>(a, stream); break;
-        case SPX_F16: rc = gn_bwd_coef<__half>(a, stream); break;
-        default: rc = gn_bwd_coef<__nv_bfloat16>(a, stream); break;
-    }
+    const int rc =
+        dispatch_dtype(d->param_dtype, [&](auto p) { return gn_bwd_coef<typename decltype(p)::type>(a, stream); });
     if (rc || a.rows == 0) return rc;
     return gn_rows_typed(d->dtype, d->param_dtype, a, false, false, stream);
 }

@@ -14,7 +14,7 @@
 //             count[r] (mean), dy[r] (sum: spx_sparse_add_gather with index = row32), 0 for a dropped point.
 // The order of every reduction depends only on the row's points, and no float atomics are used, so results are
 // bit-reproducible and independent of dropped points, wherever they sit.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 int group_rows(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets, void *workspace,
@@ -33,24 +33,6 @@ __global__ void ps_rows_kernel(const I *__restrict__ ids, int64_t n, int64_t row
     if (p >= n) return;
     const int64_t id = (int64_t)__ldg(ids + p);
     row32[p] = id >= 0 && id < rows ? (int32_t)id : -1;
-}
-
-// W elements of T: one 16-byte vector (W * sizeof(T) == 16) or W == 1
-template <typename T, int W> __device__ __forceinline__ void ps_load(const T *p, T (&e)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
-        *reinterpret_cast<uint4 *>(e) = __ldg(reinterpret_cast<const uint4 *>(p));
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) e[j] = __ldg(p + j);
-    }
-}
-template <typename T, int W> __device__ __forceinline__ void ps_store(T *p, const T (&e)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
-        *reinterpret_cast<uint4 *>(p) = *reinterpret_cast<const uint4 *>(e);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) p[j] = e[j];
-    }
 }
 
 template <typename T, int W, bool MEAN>
@@ -92,14 +74,14 @@ ps_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
 #pragma unroll
         for (int u = 0; u < INFLIGHT; ++u) p[u] = __ldg(order + q + u);
 #pragma unroll
-        for (int u = 0; u < INFLIGHT; ++u) ps_load<T, W>(base + (int64_t)p[u] * channels, e[u]);
+        for (int u = 0; u < INFLIGHT; ++u) row_load_raw<T, W>(base + (int64_t)p[u] * channels, e[u]);
 #pragma unroll
         for (int u = 0; u < INFLIGHT; ++u) fold(e[u], p[u]);
     }
     for (; q < end; ++q) {
         const int32_t p = __ldg(order + q);
         T e[W];
-        ps_load<T, W>(base + (int64_t)p * channels, e);
+        row_load_raw<T, W>(base + (int64_t)p * channels, e);
         fold(e, p);
     }
     const int64_t o = r * channels + ch * W;
@@ -115,7 +97,7 @@ ps_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
             argmax[o + j] = arg[j];
         }
     }
-    ps_store<T, W>(out + o, res);
+    row_store_raw<T, W>(out + o, res);
 }
 
 template <typename T, int W, bool MEAN>
@@ -134,7 +116,7 @@ ps_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ row32, int64
         const int64_t o = (int64_t)r * channels + ch * W;
         if constexpr (MEAN) {
             T g[W];
-            ps_load<T, W>(dy + o, g);
+            row_load_raw<T, W>(dy + o, g);
             const float c = (float)__ldg(count + r);      // >= 1: point p itself counts
 #pragma unroll
             for (int j = 0; j < W; ++j) e[j] = from_float<T>(__fdiv_rn(to_float(g[j]), c));
@@ -144,7 +126,7 @@ ps_bwd_kernel(const T *__restrict__ dy, const int32_t *__restrict__ row32, int64
                 if (__ldg(argmax + o + j) == (int32_t)p) e[j] = dy[o + j];
         }
     }
-    ps_store<T, W>(dx + p * channels + ch * W, e);
+    row_store_raw<T, W>(dx + p * channels + ch * W, e);
 }
 
 // ---------------------------------------------------------------- host side
@@ -176,7 +158,8 @@ template <typename T>
 static int ps_fwd_dispatch(bool mean, const void *x, const int32_t *order, const int32_t *offsets, int64_t rows,
                            int channels, void *out, int32_t *argmax, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && aligned16(x) && aligned16(out);
+    const RowWidth w = row_width(channels * sizeof(T), x, out);
+    const bool vec = w.wide && w.aligned;
     if (mean) return vec ? ps_fwd_launch<T, W, true>(x, order, offsets, rows, channels, out, argmax, stream)
                          : ps_fwd_launch<T, 1, true>(x, order, offsets, rows, channels, out, argmax, stream);
     return vec ? ps_fwd_launch<T, W, false>(x, order, offsets, rows, channels, out, argmax, stream)
@@ -197,7 +180,8 @@ template <typename T>
 static int ps_bwd_dispatch(bool mean, const void *dy, const int32_t *row32, int64_t n, int channels,
                            const int32_t *argmax, const int32_t *count, void *dx, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    const bool vec = (channels * (int)sizeof(T)) % 16 == 0 && aligned16(dy) && aligned16(dx);
+    const RowWidth w = row_width(channels * sizeof(T), dy, dx);
+    const bool vec = w.wide && w.aligned;
     if (mean) return vec ? ps_bwd_launch<T, W, true>(dy, row32, n, channels, argmax, count, dx, stream)
                          : ps_bwd_launch<T, 1, true>(dy, row32, n, channels, argmax, count, dx, stream);
     return vec ? ps_bwd_launch<T, W, false>(dy, row32, n, channels, argmax, count, dx, stream)
@@ -248,12 +232,10 @@ extern "C" int spx_point_scatter_fwd(int mode, const void *x, int64_t num_points
     if (rows == 0) return 0;
     cudaStream_t stream = (cudaStream_t)stream_;
     if (mode == 2) return sum_segments(x, num_points, order, offsets, rows, channels, dtype, out, stream);
-    switch (dtype) {
-        case SPX_F32: return ps_fwd_dispatch<float>(mode == 1, x, order, offsets, rows, channels, out, argmax, stream);
-        case SPX_F16: return ps_fwd_dispatch<__half>(mode == 1, x, order, offsets, rows, channels, out, argmax, stream);
-        default:
-            return ps_fwd_dispatch<__nv_bfloat16>(mode == 1, x, order, offsets, rows, channels, out, argmax, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) {
+        return ps_fwd_dispatch<typename decltype(t)::type>(mode == 1, x, order, offsets, rows, channels, out, argmax,
+                                                           stream);
+    });
 }
 
 extern "C" int spx_point_scatter_bwd(int mode, const void *dy, const int32_t *row32, int64_t num_points, int64_t rows,
@@ -275,10 +257,8 @@ extern "C" int spx_point_scatter_bwd(int mode, const void *dy, const int32_t *ro
         op.grads[0] = dx;
         return spx_sparse_add_gather(row32, dy, rows, &op, channels, dtype, stream_);
     }
-    switch (dtype) {
-        case SPX_F32: return ps_bwd_dispatch<float>(mode == 1, dy, row32, num_points, channels, argmax, count, dx, stream);
-        case SPX_F16: return ps_bwd_dispatch<__half>(mode == 1, dy, row32, num_points, channels, argmax, count, dx, stream);
-        default:
-            return ps_bwd_dispatch<__nv_bfloat16>(mode == 1, dy, row32, num_points, channels, argmax, count, dx, stream);
-    }
+    return dispatch_dtype(dtype, [&](auto t) {
+        return ps_bwd_dispatch<typename decltype(t)::type>(mode == 1, dy, row32, num_points, channels, argmax, count, dx,
+                                                           stream);
+    });
 }

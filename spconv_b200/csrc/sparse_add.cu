@@ -13,7 +13,7 @@
 //   gather : rows[g] = index[g] >= 0 ? src[index[g]] : 0 into per-operand row blocks -- the backward pass
 //            (index = pair_bwd[0]) and the head-row gather of RemoveDuplicate.
 // Feature rows are moved as 16-byte vectors when every row and base pointer allows it, else per element.
-#include "common.cuh"
+#include "rows.cuh"
 
 namespace spx {
 size_t radix_argsort_workspace_bytes(int64_t n);
@@ -65,31 +65,6 @@ __global__ void sa_offsets_kernel(const uint32_t *__restrict__ keys, int64_t n, 
     offsets[o] = (int32_t)lo;
 }
 
-// W elements of T per thread: W * sizeof(T) == 16 (vector path) or W == 1
-template <typename T, int W> __device__ __forceinline__ void load_row(const T *p, float (&f)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
-        const T *e = reinterpret_cast<const T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(e[j]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) f[j] = to_float(p[j]);
-    }
-}
-template <typename T, int W> __device__ __forceinline__ void store_row(T *p, const float (&f)[W]) {
-    if constexpr (W * sizeof(T) == 16) {
-        uint4 v;
-        T *e = reinterpret_cast<T *>(&v);
-#pragma unroll
-        for (int j = 0; j < W; ++j) e[j] = from_float<T>(f[j]);
-        *reinterpret_cast<uint4 *>(p) = v;
-    } else {
-#pragma unroll
-        for (int j = 0; j < W; ++j) p[j] = from_float<T>(f[j]);
-    }
-}
-
 // one thread = W channels of one output row; the rows of the segment are added in visit order
 template <typename T, int W>
 __global__ void __launch_bounds__(SA_THREADS)
@@ -107,11 +82,11 @@ sa_sum_kernel(const __grid_constant__ SaOperands ops, const int32_t *__restrict_
         const int64_t g = __ldg(order + p);
         const int t = operand_of(ops, g);
         float f[W];
-        load_row<T, W>(static_cast<const T *>(ops.features[t]) + (g - ops.start[t]) * channels + ch * W, f);
+        row_load<T, W>(static_cast<const T *>(ops.features[t]) + (g - ops.start[t]) * channels + ch * W, f);
 #pragma unroll
         for (int j = 0; j < W; ++j) acc[j] += f[j];
     }
-    store_row<T, W>(out + o * channels + ch * W, acc);
+    row_store<T, W>(out + o * channels + ch * W, acc);
 }
 
 // rows are copied bit for bit: U is a 16-byte vector or an integer of the element's size
@@ -174,9 +149,9 @@ template <typename T>
 static int dispatch_sum(const SaOperands &ops, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
                         void *out, cudaStream_t stream) {
     constexpr int W = 16 / sizeof(T);
-    bool vec = (channels * (int)sizeof(T)) % 16 == 0 && aligned16(out);
-    for (int t = 0; t < ops.count; ++t) vec = vec && aligned16(ops.features[t]);
-    if (vec) return launch_sum<T, W>(ops, order, offsets, M, channels, out, stream);
+    RowWidth w = row_width(channels * sizeof(T), out);
+    for (int t = 0; t < ops.count; ++t) w.aligned = w.aligned && aligned16(ops.features[t]);
+    if (w.wide && w.aligned) return launch_sum<T, W>(ops, order, offsets, M, channels, out, stream);
     return launch_sum<T, 1>(ops, order, offsets, M, channels, out, stream);
 }
 
@@ -311,12 +286,9 @@ int group_rows(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int3
 
 static int sum_dtype(const SaOperands &ops, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
                      int dtype, void *out, cudaStream_t stream) {
-    switch (dtype) {
-        case SPX_F32: return dispatch_sum<float>(ops, order, offsets, M, channels, out, stream);
-        case SPX_F16: return dispatch_sum<__half>(ops, order, offsets, M, channels, out, stream);
-        case SPX_BF16: return dispatch_sum<__nv_bfloat16>(ops, order, offsets, M, channels, out, stream);
-    }
-    return 2;
+    return dispatch_dtype(dtype, [&](auto t) {
+        return dispatch_sum<typename decltype(t)::type>(ops, order, offsets, M, channels, out, stream);
+    });
 }
 
 // The sum of spx_point_scatter_fwd: one operand x [rows, channels] and M segments, M may exceed rows.  The caller
@@ -368,9 +340,9 @@ extern "C" int spx_sparse_add_gather(const int32_t *index, const void *src, int6
     SPX_REQUIRE(src != nullptr || src_rows == 0, "sparse_add_gather: src is NULL");
     cudaStream_t stream = (cudaStream_t)stream_;
     const int64_t row_bytes = (int64_t)channels * dtype_bytes(dtype);
-    bool vec = row_bytes % 16 == 0 && aligned16(src);
-    for (int t = 0; t < ops.count; ++t) vec = vec && aligned16(ops.grads[t]);
-    if (vec) return launch_gather<uint4>(ops, index, total, row_bytes, src, stream);
+    RowWidth w = row_width(row_bytes, src);
+    for (int t = 0; t < ops.count; ++t) w.aligned = w.aligned && aligned16(ops.grads[t]);
+    if (w.wide && w.aligned) return launch_gather<uint4>(ops, index, total, row_bytes, src, stream);
     if (dtype_bytes(dtype) == 4) return launch_gather<uint32_t>(ops, index, total, row_bytes, src, stream);
     return launch_gather<uint16_t>(ops, index, total, row_bytes, src, stream);
 }
