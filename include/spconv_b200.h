@@ -738,6 +738,41 @@ int spx_masked_group_norm_fwd(const spx_masked_group_norm *d, void *workspace, s
 int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
                               spx_stream_t stream);
 
+/*
+ * MaskedGroupNorm with per-sample modulation and an activation (AdaGN, as guided-diffusion's use_scale_shift_norm):
+ * `norm` is the call above, unchanged, and for a kept row of sample b, channel c
+ *   h = (x - mean) * (weight * invstd) + bias          (the apply above)
+ *   z = h * (1 + scale[b][c]) + shift[b][c]            (one fmaf; z = h when scale and shift are both NULL)
+ *   y = act(z)                                         (rounded once to dtype)
+ * with relu(z) = z <= 0 ? 0 : z and silu(z) = z / (1 + exp(-z)).  Dropped rows stay 0 in y and dx and never touch
+ * scale, shift, dscale or dshift.
+ * bwd: dz = dy * act'(z), z recomputed from x as the forward computes it (relu' = z > 0,
+ *      silu' = sigmoid(z) (1 + z (1 - sigmoid(z)))); the sums of `norm` are taken over dz, weight_c becomes
+ *      weight_c (1 + scale[b][c]) in S1, S2 and dx, and
+ *        dbias_c = sum_b (1 + scale[b][c]) sum(dz),  dweight_c = sum_b (1 + scale[b][c]) sum(dz * xhat),
+ *        dshift[b][c] = sum(dz),  dscale[b][c] = weight_c sum(dz * xhat) + bias_c sum(dz)
+ *      over the kept rows of sample b (0 for an empty sample), in the fixed orders of `norm`.  Same 4 launches.
+ *      Unlike spx_masked_group_norm_bwd (which never reads it), this bwd reads norm.bias ([channels] param_dtype,
+ *      or NULL = 0) when act != SPX_GN_ACT_NONE (to recompute z) or dscale is given; otherwise it may be anything.
+ * scale, shift, dscale, dshift: fp32 [batch_size, channels], row-major, 4-byte aligned, read and written element by
+ * element; any of them may be NULL (scale / shift 0, the gradient not written).  act is checked before any launch.
+ * With scale = shift = NULL and SPX_GN_ACT_NONE the results are those of spx_masked_group_norm_fwd / _bwd bit for
+ * bit.  workspace: spx_masked_group_norm_workspace_size, as above.
+ */
+enum spx_gn_act { SPX_GN_ACT_NONE = 0, SPX_GN_ACT_RELU = 1, SPX_GN_ACT_SILU = 2 };
+
+typedef struct spx_masked_group_norm_mod {
+    spx_masked_group_norm norm;
+    const float *scale, *shift;             /* [batch_size, channels] fp32, or NULL (0) */
+    int act;                                /* spx_gn_act */
+    float *dscale, *dshift;                 /* bwd: [batch_size, channels] fp32, or NULL */
+} spx_masked_group_norm_mod;
+
+int spx_masked_group_norm_mod_fwd(const spx_masked_group_norm_mod *m, void *workspace, size_t workspace_bytes,
+                                  spx_stream_t stream);
+int spx_masked_group_norm_mod_bwd(const spx_masked_group_norm_mod *m, void *workspace, size_t workspace_bytes,
+                                  spx_stream_t stream);
+
 /* ------------------------------------------------------------------ hash table */
 
 /*

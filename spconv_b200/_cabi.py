@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(_PKG, "lib", "libspconv_b200.so")
 SPX_MAX_NDIM = 4
 SPX_F32, SPX_F16, SPX_BF16, SPX_I8 = 0, 1, 2, 3
 SPX_ACT_NONE, SPX_ACT_RELU, SPX_ACT_SIGMOID, SPX_ACT_LEAKY_RELU = 0, 1, 2, 3
+SPX_GN_ACT_NONE, SPX_GN_ACT_RELU, SPX_GN_ACT_SILU = 0, 1, 2
 SPX_F32_EXACT, SPX_F32_TF32 = 0, 1
 
 
@@ -87,6 +88,14 @@ class MaskedGroupNorm(Structure):
         ("coords", c_void_p), ("num_valid", c_void_p), ("x", c_void_p), ("y", c_void_p), ("dy", c_void_p),
         ("dx", c_void_p), ("weight", c_void_p), ("bias", c_void_p), ("dweight", c_void_p), ("dbias", c_void_p),
         ("mean", c_void_p), ("invstd", c_void_p), ("order", c_void_p), ("offsets", c_void_p), ("cstart", c_void_p),
+    ]
+
+
+class MaskedGroupNormMod(Structure):
+    """``spx_masked_group_norm_mod``: a MaskedGroupNorm call with per-sample scale / shift and an activation."""
+    _fields_ = [
+        ("norm", MaskedGroupNorm), ("scale", c_void_p), ("shift", c_void_p), ("act", c_int), ("dscale", c_void_p),
+        ("dshift", c_void_p),
     ]
 
 
@@ -217,6 +226,8 @@ SIGNATURES = {
        for p in ("fwd_local", "fwd_merge", "bwd_local", "bwd_merge")},
     "spx_masked_group_norm_workspace_size": (c_size_t, [c_int64, c_int, c_int]),
     **{f"spx_masked_group_norm_{p}": (c_int, [POINTER(MaskedGroupNorm), c_void_p, c_size_t, c_void_p])
+       for p in ("fwd", "bwd")},
+    **{f"spx_masked_group_norm_mod_{p}": (c_int, [POINTER(MaskedGroupNormMod), c_void_p, c_size_t, c_void_p])
        for p in ("fwd", "bwd")},
     "spx_hash_workspace_size": (c_size_t, [c_int64, c_int64]),
     "spx_hash_clear": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),

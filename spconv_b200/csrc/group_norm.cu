@@ -21,6 +21,9 @@
 //   coef     : per c over ascending b: dbeta = sum(dy), dgamma = sum(dy * xhat); per (b, g) over ascending c:
 //              S1 = sum(gamma_c sum(dy)), S2 = sum(gamma_c sum(dy * xhat)) -> coef [B][G] = (S1 / n, S2 / n);
 //   apply    : dx = invstd_bg * (gamma_c dy - S1 / n - xhat * S2 / n); every element of dx is written once.
+// Modulated (spx_masked_group_norm_mod): the applies write act(fmaf(h, 1 + scale_bc, shift_bc)); the backward
+// recomputes that z from x, folds dz = dy act'(z) in place of dy, and weighs gamma_c, dbeta and dgamma by
+// (1 + scale_bc); coef also writes dshift = sum(dz), dscale = gamma sum(dz xhat) + beta sum(dz).  Same launches.
 // The order of every sum depends only on the sample's kept rows, never on `rows`, the padding or the grid, and no
 // float atomics are used, so every result is bit-reproducible and independent of padding and dropped rows.
 #include "rows.cuh"
@@ -162,12 +165,45 @@ template <typename P> __device__ __forceinline__ float gn_param(const P *p, int 
     return p ? to_float(__ldg(p + c)) : dflt;
 }
 
+// Modulation of sample b: z = fmaf(h, 1 + scale[b][c], shift[b][c]), a missing operand 0; 1 + scale[b][c] is also
+// the factor of gamma_c in the backward.  gn_mod_row gives the sample's row of scale or shift (NULL stays NULL).
+__device__ __forceinline__ const float *gn_mod_row(const float *p, int b, int channels) {
+    return p ? p + (int64_t)b * channels : nullptr;
+}
+__device__ __forceinline__ float gn_scale1(const float *scale_row, int c) {
+    return scale_row ? 1.f + __ldg(scale_row + c) : 1.f;
+}
+__device__ __forceinline__ float gn_shift(const float *shift_row, int c) {
+    return shift_row ? __ldg(shift_row + c) : 0.f;
+}
+
+// y = act(z); relu keeps NaN, as torch's does
+__device__ __forceinline__ float gn_act(int act, float z) {
+    if (act == SPX_GN_ACT_RELU) return z <= 0.f ? 0.f : z;
+    if (act == SPX_GN_ACT_SILU) return z / (1.f + expf(-z));
+    return z;
+}
+
+// dz = dy act'(z): relu' = (z > 0), as threshold_backward; silu' = sigma(z) (1 + z (1 - sigma(z)))
+__device__ __forceinline__ float gn_act_grad(int act, float z, float dy) {
+    if (act == SPX_GN_ACT_RELU) return z > 0.f ? dy : 0.f;
+    if (act == SPX_GN_ACT_SILU) {
+        const float s = 1.f / (1.f + expf(-z));
+        return dy * (s * fmaf(z, 1.f - s, 1.f));
+    }
+    return dy;
+}
+
+// y = act(z) with h = (x - mean) * (gamma * invstd) + beta and z = h without scale and shift (so the unmodulated
+// call keeps h's bits, -0 included), else fmaf(h, 1 + scale, shift).  The backward recomputes z with the same
+// expressions.
 template <typename T, typename P, int W, bool A>
 __global__ void __launch_bounds__(GN_THREADS)
 gn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, const int32_t *__restrict__ coords, int64_t rows,
                     int row_ints, int batch_size, int channels, int vecs, int tpr, int groups,
                     const int32_t *__restrict__ num_valid, const P *__restrict__ weight, const P *__restrict__ bias,
-                    const float *__restrict__ mean, const float *__restrict__ invstd) {
+                    const float *__restrict__ mean, const float *__restrict__ invstd,
+                    const float *__restrict__ scale, const float *__restrict__ shift, int act) {
     const int lanes = GN_THREADS / tpr;
     const int64_t r = blockIdx.x * (int64_t)lanes + threadIdx.x / tpr;
     const int v = blockIdx.y * tpr + (threadIdx.x % tpr);
@@ -177,12 +213,16 @@ gn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, const int32_t *_
     float f[W];
     if (b >= 0) {
         row_load<T, W, A>(x + r * channels + (int64_t)v * W, f);
+        const bool mod = scale || shift;
+        const float *srow = gn_mod_row(scale, b, channels), *trow = gn_mod_row(shift, b, channels);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
             const int64_t bg = (int64_t)b * groups + c / cg;
             const float a = gn_param(weight, c, 1.f) * __ldg(invstd + bg);
             f[j] = fmaf(f[j] - __ldg(mean + bg), a, gn_param(bias, c, 0.f));
+            if (mod) f[j] = fmaf(f[j], gn_scale1(srow, c), gn_shift(trow, c));
+            f[j] = gn_act(act, f[j]);
         }
     } else {
 #pragma unroll
@@ -192,12 +232,16 @@ gn_fwd_apply_kernel(const T *__restrict__ x, T *__restrict__ y, const int32_t *_
 }
 
 // ---------------------------------------------------------------- backward
-template <typename T, int W, bool A>
+// The sums are over dz = dy act'(z); z is recomputed from x as the forward computes it.  ACT = (act != NONE): the
+// recomputation doubles the registers of the vector instances, so the plain backward does not carry it.
+template <typename T, typename P, int W, bool A, bool ACT>
 __global__ void __launch_bounds__(GN_THREADS)
 gn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, const int32_t *__restrict__ order,
                      const int32_t *__restrict__ offsets, const int32_t *__restrict__ cstart, int batch_size,
                      int channels, int vecs, int tpr, int groups, const float *__restrict__ mean_bg,
-                     const float *__restrict__ invstd_bg, float2 *__restrict__ partials) {
+                     const float *__restrict__ invstd_bg, const P *__restrict__ weight, const P *__restrict__ bias,
+                     const float *__restrict__ scale, const float *__restrict__ shift, int act,
+                     float2 *__restrict__ partials) {
     __shared__ float s_a[GN_THREADS * W], s_b[GN_THREADS * W];
     int b;
     int32_t p0, end;
@@ -216,12 +260,31 @@ gn_bwd_reduce_kernel(const T *__restrict__ x, const T *__restrict__ dy, const in
             mean[j] = __ldg(mean_bg + bg);
             invstd[j] = __ldg(invstd_bg + bg);
         }
+        // z = fmaf(fmaf(x - mean, a, beta), s1, sh) as in the forward; a chunk is one sample's, so these are constants
+        const bool mod = scale || shift;
+        const float *srow = gn_mod_row(scale, b, channels), *trow = gn_mod_row(shift, b, channels);
+        float a[W], beta[W], s1[W], sh[W];
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+            const int c = t.v * W + j;
+            a[j] = ACT ? gn_param(weight, c, 1.f) * invstd[j] : 0.f;
+            beta[j] = ACT ? gn_param(bias, c, 0.f) : 0.f;
+            s1[j] = ACT ? gn_scale1(srow, c) : 1.f;
+            sh[j] = ACT ? gn_shift(trow, c) : 0.f;
+        }
         const int64_t off = (int64_t)t.v * W;
         auto fold = [&](const float (&fx)[W], const float (&fd)[W]) {
 #pragma unroll
             for (int j = 0; j < W; ++j) {
-                sdy[j] += fd[j];
-                sdyx[j] = fmaf(fd[j], (fx[j] - mean[j]) * invstd[j], sdyx[j]);
+                const float xc = fx[j] - mean[j];
+                float d = fd[j];
+                if (ACT) {
+                    float z = fmaf(xc, a[j], beta[j]);
+                    if (mod) z = fmaf(z, s1[j], sh[j]);
+                    d = gn_act_grad(act, z, d);
+                }
+                sdy[j] += d;
+                sdyx[j] = fmaf(d, xc * invstd[j], sdyx[j]);
             }
         };
         int32_t p = p0 + t.lane;
@@ -281,20 +344,27 @@ gn_bwd_finalize_kernel(const float2 *__restrict__ partials, const int32_t *__res
     if (pl == 0 && active) bc[(int64_t)b * channels + c] = make_float2(a, s2);
 }
 
-// threads [0, C): dbias[c] / dweight[c] over ascending b; threads [C, C + B G): coef[b][g] = (S1 / n, S2 / n) with
-// S1, S2 over ascending c of the group
+// threads [0, C): dbias[c] / dweight[c] over ascending b, and dshift[b][c] / dscale[b][c]; threads [C, C + B G):
+// coef[b][g] = (S1 / n, S2 / n) with S1, S2 over ascending c of the group.  With a scale, (1 + scale[b][c]) weighs
+// the sums of sample b: without one the factor is 1 and fmaf(1, p, a) == a + p.
 template <typename P>
 __global__ void __launch_bounds__(GN_THREADS)
 gn_bwd_coef_kernel(const float2 *__restrict__ bc, const int32_t *__restrict__ offsets, int batch_size, int channels,
-                   int groups, const P *__restrict__ weight, P *__restrict__ dweight, P *__restrict__ dbias,
-                   float2 *__restrict__ coef) {
+                   int groups, const P *__restrict__ weight, const P *__restrict__ bias,
+                   const float *__restrict__ scale, P *__restrict__ dweight, P *__restrict__ dbias,
+                   float *__restrict__ dscale, float *__restrict__ dshift, float2 *__restrict__ coef) {
     const int64_t i = blockIdx.x * (int64_t)GN_THREADS + threadIdx.x;
     if (i < channels) {
         float a = 0.f, s2 = 0.f;
+        const float gamma = gn_param(weight, (int)i, 1.f), beta = gn_param(bias, (int)i, 0.f);
         for (int b = 0; b < batch_size; ++b) {
-            const float2 p = bc[(int64_t)b * channels + i];
-            a += p.x;
-            s2 += p.y;
+            const int64_t k = (int64_t)b * channels + i;
+            const float2 p = bc[k];
+            const float s = gn_scale1(gn_mod_row(scale, b, channels), (int)i);
+            a = fmaf(s, p.x, a);
+            s2 = fmaf(s, p.y, s2);
+            if (dshift) dshift[k] = p.x;
+            if (dscale) dscale[k] = fmaf(gamma, p.y, beta * p.x);
         }
         if (dbias) dbias[i] = from_float<P>(a);
         if (dweight) dweight[i] = from_float<P>(s2);
@@ -306,9 +376,10 @@ gn_bwd_coef_kernel(const float2 *__restrict__ bc, const int32_t *__restrict__ of
     const int cg = channels / groups;
     const int c0 = g * cg;
     const float2 *p = bc + (int64_t)b * channels + c0;
+    const float *srow = gn_mod_row(scale, b, channels);
     float s1 = 0.f, s2 = 0.f;
     for (int c = 0; c < cg; ++c) {
-        const float gamma = gn_param(weight, c0 + c, 1.f);
+        const float gamma = gn_param(weight, c0 + c, 1.f) * gn_scale1(srow, c0 + c);
         s1 = fmaf(gamma, p[c].x, s1);
         s2 = fmaf(gamma, p[c].y, s2);
     }
@@ -316,12 +387,13 @@ gn_bwd_coef_kernel(const float2 *__restrict__ bc, const int32_t *__restrict__ of
     coef[j] = n > 0 ? make_float2(__fdiv_rn(s1, (float)n), __fdiv_rn(s2, (float)n)) : make_float2(0.f, 0.f);
 }
 
-template <typename T, typename P, int W, bool A>
+template <typename T, typename P, int W, bool A, bool ACT>
 __global__ void __launch_bounds__(GN_THREADS)
 gn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__restrict__ dx,
                     const int32_t *__restrict__ coords, int64_t rows, int row_ints, int batch_size, int channels,
                     int vecs, int tpr, int groups, const int32_t *__restrict__ num_valid, const P *__restrict__ weight,
-                    const float *__restrict__ mean, const float *__restrict__ invstd,
+                    const P *__restrict__ bias, const float *__restrict__ mean, const float *__restrict__ invstd,
+                    const float *__restrict__ scale, const float *__restrict__ shift, int act,
                     const float2 *__restrict__ coef) {
     const int lanes = GN_THREADS / tpr;
     const int64_t r = blockIdx.x * (int64_t)lanes + threadIdx.x / tpr;
@@ -335,15 +407,24 @@ gn_bwd_apply_kernel(const T *__restrict__ x, const T *__restrict__ dy, T *__rest
         const int64_t o = r * channels + (int64_t)v * W;
         row_load<T, W, A>(x + o, fx);
         row_load<T, W, A>(dy + o, f);
+        const bool mod = scale || shift;
+        const float *srow = gn_mod_row(scale, b, channels), *trow = gn_mod_row(shift, b, channels);
 #pragma unroll
         for (int j = 0; j < W; ++j) {
             const int c = v * W + j;
             const int64_t bg = (int64_t)b * groups + c / cg;
             const float is = __ldg(invstd + bg);
-            const float xhat = (fx[j] - __ldg(mean + bg)) * is;
+            const float xc = fx[j] - __ldg(mean + bg);
+            const float xhat = xc * is;
+            const float gamma = gn_param(weight, c, 1.f);
+            if (ACT) {                                         // dz from the forward's z
+                float z = fmaf(xc, gamma * is, gn_param(bias, c, 0.f));
+                if (mod) z = fmaf(z, gn_scale1(srow, c), gn_shift(trow, c));
+                f[j] = gn_act_grad(act, z, f[j]);
+            }
             const float2 k = __ldg(coef + bg);
             // the product is rounded on its own, as in S1: one row with Cg = 1 gives gamma dy - S1 / n = 0 exactly
-            f[j] = is * (__fmul_rn(gn_param(weight, c, 1.f), f[j]) - k.x - xhat * k.y);
+            f[j] = is * (__fmul_rn(gamma * gn_scale1(srow, c), f[j]) - k.x - xhat * k.y);
         }
     } else {
 #pragma unroll
@@ -403,6 +484,9 @@ struct GnArgs {
     float eps;
     const float *mean, *invstd;
     const int32_t *order, *offsets, *cstart;
+    const float *scale, *shift;
+    int act;
+    float *dscale, *dshift;
     GnWorkspace ws;
 };
 
@@ -419,9 +503,20 @@ template <typename T, typename P, int W, bool A> static int gn_rows(const GnArgs
                 a.ws.partials);
             SPX_CHECK_LAUNCH("gn_stats_kernel");
         } else {
-            gn_bwd_reduce_kernel<T, W, A><<<grid, GN_THREADS, 0, stream>>>(
-                static_cast<const T *>(a.x), static_cast<const T *>(a.dy), a.order, a.offsets, a.cstart, a.batch_size,
-                a.channels, vecs, tpr, a.groups, a.mean, a.invstd, a.ws.partials);
+            auto reduce = [&](auto kernel, const auto *weight, const auto *bias) {
+                kernel<<<grid, GN_THREADS, 0, stream>>>(
+                    static_cast<const T *>(a.x), static_cast<const T *>(a.dy), a.order, a.offsets, a.cstart,
+                    a.batch_size, a.channels, vecs, tpr, a.groups, a.mean, a.invstd, weight, bias, a.scale, a.shift,
+                    a.act, a.ws.partials);
+            };
+            // without an activation the reduce reads no parameter: one instance per feature type serves both
+            // parameter dtypes
+            if (a.act)
+                reduce(gn_bwd_reduce_kernel<T, P, W, A, true>, static_cast<const P *>(a.weight),
+                       static_cast<const P *>(a.bias));
+            else
+                reduce(gn_bwd_reduce_kernel<T, T, W, A, false>, static_cast<const T *>(nullptr),
+                       static_cast<const T *>(nullptr));
             SPX_CHECK_LAUNCH("gn_bwd_reduce_kernel");
         }
         return 0;
@@ -432,14 +527,14 @@ template <typename T, typename P, int W, bool A> static int gn_rows(const GnArgs
         gn_fwd_apply_kernel<T, P, W, A><<<blocks, GN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<T *>(a.y), a.coords, a.rows, a.row_ints, a.batch_size,
             a.channels, vecs, tpr, a.groups, a.num_valid, static_cast<const P *>(a.weight),
-            static_cast<const P *>(a.bias),
-            a.mean, a.invstd);
+            static_cast<const P *>(a.bias), a.mean, a.invstd, a.scale, a.shift, a.act);
         SPX_CHECK_LAUNCH("gn_fwd_apply_kernel");
     } else {
-        gn_bwd_apply_kernel<T, P, W, A><<<blocks, GN_THREADS, 0, stream>>>(
+        auto kernel = a.act ? gn_bwd_apply_kernel<T, P, W, A, true> : gn_bwd_apply_kernel<T, P, W, A, false>;
+        kernel<<<blocks, GN_THREADS, 0, stream>>>(
             static_cast<const T *>(a.x), static_cast<const T *>(a.dy), static_cast<T *>(a.dx), a.coords, a.rows,
             a.row_ints, a.batch_size, a.channels, vecs, tpr, a.groups, a.num_valid, static_cast<const P *>(a.weight),
-            a.mean, a.invstd, a.ws.coef);
+            static_cast<const P *>(a.bias), a.mean, a.invstd, a.scale, a.shift, a.act, a.ws.coef);
         SPX_CHECK_LAUNCH("gn_bwd_apply_kernel");
     }
     return 0;
@@ -466,7 +561,8 @@ template <typename P> static int gn_bwd_coef(const GnArgs &a, cudaStream_t strea
     const int64_t threads = a.channels + (int64_t)a.batch_size * a.groups;
     gn_bwd_coef_kernel<P><<<(unsigned)div_up64(threads, GN_THREADS), GN_THREADS, 0, stream>>>(
         a.ws.bc, a.offsets, a.batch_size, a.channels, a.groups, static_cast<const P *>(a.weight),
-        static_cast<P *>(a.dweight), static_cast<P *>(a.dbias), a.ws.coef);
+        static_cast<const P *>(a.bias), a.scale, static_cast<P *>(a.dweight), static_cast<P *>(a.dbias), a.dscale,
+        a.dshift, a.ws.coef);
     SPX_CHECK_LAUNCH("gn_bwd_coef_kernel");
     return 0;
 }
@@ -496,7 +592,9 @@ static int gn_check_desc(const char *who, const spx_masked_group_norm *d, const 
     return 0;
 }
 
-static GnArgs gn_args(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes) {
+// m: the modulation, or NULL for none
+static GnArgs gn_args(const spx_masked_group_norm *d, const spx_masked_group_norm_mod *m, void *workspace,
+                      size_t workspace_bytes) {
     GnArgs a{};
     a.x = d->x;
     a.dy = d->dy;
@@ -519,21 +617,31 @@ static GnArgs gn_args(const spx_masked_group_norm *d, void *workspace, size_t wo
     a.order = d->order;
     a.offsets = d->offsets;
     a.cstart = d->cstart;
+    if (m) {
+        a.scale = m->scale;
+        a.shift = m->shift;
+        a.act = m->act;
+        a.dscale = m->dscale;
+        a.dshift = m->dshift;
+    }
     a.ws = gn_carve(workspace, workspace_bytes, d->rows, d->batch_size, d->channels);
     return a;
 }
 
-}  // namespace spx
+static int gn_check_mod(const char *who, const spx_masked_group_norm_mod *m) {
+    SPX_REQUIRE(m != nullptr, "%s: descriptor is NULL", who);
+    SPX_REQUIRE(m->act == SPX_GN_ACT_NONE || m->act == SPX_GN_ACT_RELU || m->act == SPX_GN_ACT_SILU,
+                "%s: unknown activation %d (SPX_GN_ACT_NONE, _RELU or _SILU)", who, m->act);
+    return 0;
+}
 
-extern "C" int spx_masked_group_norm_fwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
-                                         spx_stream_t stream_) {
-    const char *who = "masked_group_norm_fwd";
+static int gn_fwd(const char *who, const spx_masked_group_norm *d, const spx_masked_group_norm_mod *m,
+                  void *workspace, size_t workspace_bytes, cudaStream_t stream) {
     if (int rc = gn_check_desc(who, d, workspace, workspace_bytes)) return rc;
     SPX_REQUIRE(d->rows == 0 || (d->x && d->y && d->coords && d->order),
                 "%s: NULL pointer argument (x, y, coords, order)", who);
     SPX_REQUIRE(d->eps > 0.f, "%s: eps must be positive", who);
-    const GnArgs a = gn_args(d, workspace, workspace_bytes);
-    cudaStream_t stream = (cudaStream_t)stream_;
+    const GnArgs a = gn_args(d, m, workspace, workspace_bytes);
     if (int rc = group_samples(a.coords, a.rows, a.row_ints, a.batch_size, a.num_valid, a.ws.keys, d->order,
                                a.ws.sort_ws, d->offsets, d->cstart, nullptr, stream))
         return rc;
@@ -550,14 +658,15 @@ extern "C" int spx_masked_group_norm_fwd(const spx_masked_group_norm *d, void *w
     return gn_rows_typed(d->dtype, d->param_dtype, a, true, false, stream);
 }
 
-extern "C" int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
-                                         spx_stream_t stream_) {
-    const char *who = "masked_group_norm_bwd";
+static int gn_bwd(const char *who, const spx_masked_group_norm *d, const spx_masked_group_norm_mod *m,
+                  void *workspace, size_t workspace_bytes, cudaStream_t stream) {
     if (int rc = gn_check_desc(who, d, workspace, workspace_bytes)) return rc;
     SPX_REQUIRE(d->rows == 0 || (d->x && d->dy && d->dx && d->coords && d->order),
                 "%s: NULL pointer argument (x, dy, dx, coords, order)", who);
-    const GnArgs a = gn_args(d, workspace, workspace_bytes);
-    cudaStream_t stream = (cudaStream_t)stream_;
+    GnArgs a = gn_args(d, m, workspace, workspace_bytes);
+    // bias is an operand of the backward only through z (an activation) and dscale; the plain backward never
+    // reads it, whatever the field holds
+    if (!m || (m->act == SPX_GN_ACT_NONE && !m->dscale)) a.bias = nullptr;
     if (a.rows > 0)
         if (int rc = gn_rows_typed(d->dtype, d->param_dtype, a, false, true, stream)) return rc;
     gn_bwd_finalize_kernel<<<dim3((unsigned)a.batch_size, (unsigned)div_up64(a.channels, GN_FIN_CH)),
@@ -567,4 +676,30 @@ extern "C" int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *w
         dispatch_dtype(d->param_dtype, [&](auto p) { return gn_bwd_coef<typename decltype(p)::type>(a, stream); });
     if (rc || a.rows == 0) return rc;
     return gn_rows_typed(d->dtype, d->param_dtype, a, false, false, stream);
+}
+
+}  // namespace spx
+
+extern "C" int spx_masked_group_norm_fwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
+                                         spx_stream_t stream) {
+    return gn_fwd("masked_group_norm_fwd", d, nullptr, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int spx_masked_group_norm_bwd(const spx_masked_group_norm *d, void *workspace, size_t workspace_bytes,
+                                         spx_stream_t stream) {
+    return gn_bwd("masked_group_norm_bwd", d, nullptr, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int spx_masked_group_norm_mod_fwd(const spx_masked_group_norm_mod *m, void *workspace,
+                                             size_t workspace_bytes, spx_stream_t stream) {
+    const char *who = "masked_group_norm_mod_fwd";
+    if (int rc = gn_check_mod(who, m)) return rc;
+    return gn_fwd(who, &m->norm, m, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int spx_masked_group_norm_mod_bwd(const spx_masked_group_norm_mod *m, void *workspace,
+                                             size_t workspace_bytes, spx_stream_t stream) {
+    const char *who = "masked_group_norm_mod_bwd";
+    if (int rc = gn_check_mod(who, m)) return rc;
+    return gn_bwd(who, &m->norm, m, workspace, workspace_bytes, (cudaStream_t)stream);
 }

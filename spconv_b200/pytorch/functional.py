@@ -536,29 +536,45 @@ def masked_sync_batch_norm(x, weight, bias, running_mean, running_var, num_batch
 
 # ---------------------------------------------------------------------------- per-sample GroupNorm
 class MaskedGroupNormFunction(Function):
-    """``x, weight, bias, indices, batch_size, num_valid, num_groups, eps`` -> per-sample GroupNorm over the rows
-    ``[0, num_valid)`` whose batch index is in range (:func:`ops.masked_group_norm_forward`).  The backward reuses
-    the forward's grouping and gives dx (0 on padding and dropped rows), dweight and dbias."""
+    """``x, weight, bias, indices, batch_size, num_valid, num_groups, eps, scale, shift, act`` -> per-sample GroupNorm
+    over the rows ``[0, num_valid)`` whose batch index is in range, modulated by fp32 ``scale`` / ``shift`` and
+    followed by ``act`` (:func:`ops.masked_group_norm_forward`).  The backward reuses the forward's grouping and
+    gives dx (0 on padding and dropped rows), dweight, dbias, dscale and dshift."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, indices, batch_size, num_valid, num_groups, eps):
+    def forward(ctx, x, weight, bias, indices, batch_size, num_valid, num_groups, eps, scale=None, shift=None,
+                act=None):
         y, mean, invstd, order, offsets, cstart = ops.masked_group_norm_forward(
-            x, indices, batch_size, num_valid, num_groups, weight, bias, eps)
-        ctx.save_for_backward(x, weight, indices, num_valid, mean, invstd, order, offsets, cstart)
-        ctx.batch_size, ctx.num_groups = batch_size, num_groups
+            x, indices, batch_size, num_valid, num_groups, weight, bias, eps, scale, shift, act)
+        ctx.save_for_backward(x, weight, bias, indices, num_valid, mean, invstd, order, offsets, cstart, scale, shift)
+        ctx.batch_size, ctx.num_groups, ctx.act = batch_size, num_groups, act
         return y
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_output):
-        x, weight, indices, num_valid, mean, invstd, order, offsets, cstart = ctx.saved_tensors
-        dx, dw, db = ops.masked_group_norm_backward(x, grad_output, indices, ctx.batch_size, num_valid,
-                                                    ctx.num_groups, weight, mean, invstd, order, offsets, cstart,
-                                                    ctx.needs_input_grad[1], ctx.needs_input_grad[2])
-        return dx, dw, db, None, None, None, None, None
+        x, weight, bias, indices, num_valid, mean, invstd, order, offsets, cstart, scale, shift = ctx.saved_tensors
+        given = len(ctx.needs_input_grad)                   # 8 when called without scale, shift and act
+        need = tuple(ctx.needs_input_grad) + (False,) * (11 - given)
+        dx, dw, db, ds, dt = ops.masked_group_norm_backward(
+            x, grad_output, indices, ctx.batch_size, num_valid, ctx.num_groups, weight, mean, invstd, order, offsets,
+            cstart, need[1], need[2], bias, scale, shift, ctx.act, need[8], need[9])
+        return (dx, dw, db, None, None, None, None, None, ds, dt, None)[:given]
 
 
-masked_group_norm = MaskedGroupNormFunction.apply
+def _fp32(t):
+    # the kernels read scale / shift in fp32: another float dtype runs on an fp32 copy, whose gradient autograd
+    # casts back; anything else reaches the checks of ops unchanged
+    return t.float() if t is not None and t.is_floating_point() and t.dtype != torch.float32 else t
+
+
+def masked_group_norm(x, weight, bias, indices, batch_size, num_valid, num_groups, eps, scale=None, shift=None,
+                      act=None):
+    """Per-sample GroupNorm of ``x`` (:class:`MaskedGroupNormFunction`); with ``scale`` / ``shift``
+    (``[batch_size, C]``) the normalised value of sample b becomes ``h * (1 + scale[b]) + shift[b]``, then ``act``
+    (None, ``"relu"`` or ``"silu"``) is applied, all in one kernel."""
+    return MaskedGroupNormFunction.apply(x, weight, bias, indices, batch_size, num_valid, num_groups, eps,
+                                         _fp32(scale), _fp32(shift), act)
 
 
 # ---------------------------------------------------------------------------- padding-aware global pooling

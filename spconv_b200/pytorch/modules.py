@@ -335,25 +335,44 @@ class MaskedGroupNorm(SparseModule, nn.GroupNorm):
 
     A plain ``nn.GroupNorm`` inside :class:`SparseSequential` sees ``x.features`` ``[N, C]`` and so treats every row
     as its own batch element, normalising it over its own C/G channels; that behaviour of dense layers is left as it
-    is.  Use this module for per-sample statistics."""
+    is.  Use this module for per-sample statistics.
 
-    def __init__(self, num_groups, num_channels, eps=1e-5, affine=True, device=None, dtype=None):
+    Modulation and activation (AdaGN, the ResBlock norm of diffusion U-Nets): ``forward(x, scale, shift)`` with
+    ``scale`` / ``shift`` of shape ``[x.batch_size, C]`` (either may be None; any float dtype, computed in fp32)
+    gives, for a kept row of sample ``b``, ``act(h * (1 + scale[b]) + shift[b])`` where ``h`` is the GroupNorm output
+    above.  The ``1 + scale`` convention is guided-diffusion's ``use_scale_shift_norm``: a zero scale is the
+    identity.  ``act`` is None, ``"relu"`` or ``"silu"``, fixed at construction.  The modulation and the activation
+    run in the same kernels, so the output is written once and the backward recomputes them from x, still four
+    launches; dropped rows never read ``scale`` / ``shift`` and add nothing to their gradients, which are summed in a
+    fixed order like the others.  Inside :class:`SparseSequential` the module is called with ``x`` alone."""
+
+    def __init__(self, num_groups, num_channels, eps=1e-5, affine=True, device=None, dtype=None, *, act=None):
+        if act not in (None, "relu", "silu"):
+            raise ValueError(f"MaskedGroupNorm: act must be None, 'relu' or 'silu', got {act!r}")
         nn.GroupNorm.__init__(self, num_groups, num_channels, eps, affine, device, dtype)
+        self.act = act
         self.name = None
         self._sparse_unique_name = ""
 
-    def forward(self, x: SparseConvTensor):
+    def forward(self, x: SparseConvTensor, scale: Optional[torch.Tensor] = None,
+                shift: Optional[torch.Tensor] = None):
         feats = x.features
         if feats.dim() != 2 or feats.shape[1] != self.num_channels:
             raise ValueError(f"MaskedGroupNorm({self.num_groups}, {self.num_channels}): features of shape "
                              f"{tuple(feats.shape)}")
         return x.replace_feature(functional.masked_group_norm(
-            feats, self.weight, self.bias, x.indices, x.batch_size, x.num_valid, self.num_groups, self.eps))
+            feats, self.weight, self.bias, x.indices, x.batch_size, x.num_valid, self.num_groups, self.eps, scale,
+            shift, self.act))
+
+    def extra_repr(self) -> str:
+        r = super().extra_repr()
+        return r if self.act is None else f"{r}, act={self.act!r}"
 
     @classmethod
-    def from_groupnorm(cls, gn: nn.GroupNorm) -> "MaskedGroupNorm":
-        """A ``MaskedGroupNorm`` with ``gn``'s configuration that shares its parameters (the same objects)."""
-        out = cls(gn.num_groups, gn.num_channels, gn.eps, gn.affine, device="meta")
+    def from_groupnorm(cls, gn: nn.GroupNorm, act: Optional[str] = None) -> "MaskedGroupNorm":
+        """A ``MaskedGroupNorm`` with ``gn``'s configuration and activation ``act`` that shares ``gn``'s parameters
+        (the same objects)."""
+        out = cls(gn.num_groups, gn.num_channels, gn.eps, gn.affine, device="meta", act=act)
         if gn.affine:
             out.weight = gn.weight
             out.bias = gn.bias

@@ -1522,19 +1522,59 @@ def _gn_desc(x, indices, batch_size, num_groups, num_valid, code) -> "_cabi.Mask
     return d
 
 
+GROUP_NORM_ACTS = {None: _cabi.SPX_GN_ACT_NONE, "relu": _cabi.SPX_GN_ACT_RELU, "silu": _cabi.SPX_GN_ACT_SILU}
+
+
+def _gn_act_code(act: Optional[str]) -> int:
+    if not isinstance(act, (str, type(None))) or act not in GROUP_NORM_ACTS:
+        raise RuntimeError(f"masked_group_norm: act must be None, 'relu' or 'silu', got {act!r}")
+    return GROUP_NORM_ACTS[act]
+
+
+def _gn_mod_operand(t: Optional[torch.Tensor], x: torch.Tensor, batch_size: int, what: str) -> Optional[torch.Tensor]:
+    """``scale`` / ``shift`` as the contiguous fp32 ``[batch_size, C]`` matrix the kernels read (a copy when it is
+    not one already)."""
+    if t is None:
+        return None
+    _require_cuda(t, f"GroupNorm {what}")
+    if t.device != x.device:
+        raise RuntimeError(f"masked_group_norm: {what} must be on the features' device {x.device}, got {t.device}")
+    if not t.is_floating_point():
+        raise RuntimeError(f"masked_group_norm: {what} must be a floating-point tensor, got {t.dtype}")
+    if tuple(t.shape) != (int(batch_size), x.shape[1]):
+        raise RuntimeError(f"masked_group_norm: {what} must be [batch_size, C] = [{int(batch_size)}, {x.shape[1]}], "
+                           f"got {tuple(t.shape)}")
+    return t.to(torch.float32).contiguous()
+
+
+def _gn_mod_desc(d: "_cabi.MaskedGroupNorm", scale, shift, act_code: int) -> "_cabi.MaskedGroupNormMod":
+    m = _cabi.MaskedGroupNormMod()
+    m.norm = d
+    m.scale, m.shift, m.act = _ptr(scale), _ptr(shift), act_code
+    return m
+
+
 def masked_group_norm_forward(x: torch.Tensor, indices: torch.Tensor, batch_size: int, num_valid: Optional[torch.Tensor],
                               num_groups: int, weight: Optional[torch.Tensor], bias: Optional[torch.Tensor],
-                              eps: float):
+                              eps: float, scale: Optional[torch.Tensor] = None, shift: Optional[torch.Tensor] = None,
+                              act: Optional[str] = None):
     """Per-sample GroupNorm of the rows ``r < num_valid`` (all rows when ``num_valid`` is None) whose batch index
     ``indices[r, 0]`` is in ``[0, batch_size)``; every other row of ``y`` is 0.  Returns ``(y, mean, invstd, order,
     offsets, cstart)``: the fp32 statistics ``[batch_size, num_groups]`` and the grouping of the rows by sample,
     which :func:`masked_group_norm_backward` reuses.  No host synchronisation; bit-reproducible whatever the
-    padding."""
+    padding.
+
+    ``scale`` / ``shift`` (``[batch_size, C]``, float; computed in fp32) modulate the normalised value h of a row of
+    sample b as ``h * (1 + scale[b]) + shift[b]``, and ``act`` (None, ``"relu"`` or ``"silu"``) is applied to the
+    result, in the same kernel."""
     _gn_check(x, indices, batch_size, num_groups, num_valid)
     x, indices = x.contiguous(), indices.contiguous()
     code = _bn_param_code(x, [weight, bias], "masked_group_norm")
     if not eps > 0:
         raise RuntimeError(f"masked_group_norm: eps must be positive, got {eps}")
+    act_code = _gn_act_code(act)
+    scale = _gn_mod_operand(scale, x, batch_size, "scale")
+    shift = _gn_mod_operand(shift, x, batch_size, "shift")
     rows, c = x.shape
     b, g = int(batch_size), int(num_groups)
     y = torch.empty_like(x)
@@ -1547,9 +1587,10 @@ def masked_group_norm_forward(x: torch.Tensor, indices: torch.Tensor, batch_size
     d.eps, d.y, d.weight, d.bias = float(eps), _ptr(y), _ptr(weight), _ptr(bias)
     d.mean, d.invstd, d.order, d.offsets, d.cstart = (mean.data_ptr(), invstd.data_ptr(), _ptr(order),
                                                       offsets.data_ptr(), cstart.data_ptr())
+    m = _gn_mod_desc(d, scale, shift, act_code)
     lib = _lib()
     ws = _bytes(lib.spx_masked_group_norm_workspace_size(rows, b, c), x.device)
-    _cabi.check(lib.spx_masked_group_norm_fwd(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+    _cabi.check(lib.spx_masked_group_norm_mod_fwd(ctypes.byref(m), ws.data_ptr(), ws.numel(), _stream()),
                 "masked_group_norm_fwd")
     return y, mean, invstd, order, offsets, cstart
 
@@ -1557,16 +1598,27 @@ def masked_group_norm_forward(x: torch.Tensor, indices: torch.Tensor, batch_size
 def masked_group_norm_backward(x: torch.Tensor, dy: torch.Tensor, indices: torch.Tensor, batch_size: int,
                                num_valid: Optional[torch.Tensor], num_groups: int, weight: Optional[torch.Tensor],
                                mean: torch.Tensor, invstd: torch.Tensor, order: torch.Tensor, offsets: torch.Tensor,
-                               cstart: torch.Tensor, need_weight_grad: bool = True, need_bias_grad: bool = True):
-    """``(dx, dweight, dbias)`` of :func:`masked_group_norm_forward`, from its statistics and grouping (nothing is
-    sorted again).  dx is 0 on padding and dropped rows; the parameter gradients (None when not needed) have the
-    parameters' dtype (float32 without ``weight``)."""
+                               cstart: torch.Tensor, need_weight_grad: bool = True, need_bias_grad: bool = True,
+                               bias: Optional[torch.Tensor] = None, scale: Optional[torch.Tensor] = None,
+                               shift: Optional[torch.Tensor] = None, act: Optional[str] = None,
+                               need_scale_grad: Optional[bool] = None, need_shift_grad: Optional[bool] = None):
+    """``(dx, dweight, dbias, dscale, dshift)`` of :func:`masked_group_norm_forward`, from its statistics and
+    grouping (nothing is sorted again).  dx is 0 on padding and dropped rows; the parameter gradients (None when not
+    needed) have the parameters' dtype (float32 without ``weight``).  ``bias``, ``scale``, ``shift`` and ``act`` are
+    those of the forward (``bias`` is read when there is an activation or a scale gradient); ``dscale`` / ``dshift``
+    are fp32 ``[batch_size, C]``, computed when ``need_scale_grad`` / ``need_shift_grad`` (default: when ``scale`` /
+    ``shift`` is given), else None."""
     _gn_check(x, indices, batch_size, num_groups, num_valid)
     x, indices, dy = x.contiguous(), indices.contiguous(), dy.contiguous()
     if dy.shape != x.shape or dy.dtype != x.dtype:
         raise RuntimeError("masked_group_norm: the output gradient must match the features' shape and dtype")
-    code = _bn_param_code(x, [weight], "masked_group_norm")
-    pdt = weight.dtype if weight is not None else torch.float32
+    code = _bn_param_code(x, [weight, bias], "masked_group_norm")
+    act_code = _gn_act_code(act)
+    need_scale_grad = scale is not None if need_scale_grad is None else need_scale_grad
+    need_shift_grad = shift is not None if need_shift_grad is None else need_shift_grad
+    scale = _gn_mod_operand(scale, x, batch_size, "scale")
+    shift = _gn_mod_operand(shift, x, batch_size, "shift")
+    pdt = torch.float32 if code == _cabi.SPX_F32 else x.dtype
     rows, c = x.shape
     b, g = int(batch_size), int(num_groups)
     for t, shape in ((mean, (b, g)), (invstd, (b, g)), (order, (rows,)), (offsets, (b + 1,)), (cstart, (b + 1,))):
@@ -1575,15 +1627,19 @@ def masked_group_norm_backward(x: torch.Tensor, dy: torch.Tensor, indices: torch
     dx = torch.empty_like(x)
     dw = torch.empty((c,), dtype=pdt, device=x.device) if need_weight_grad else None
     db = torch.empty((c,), dtype=pdt, device=x.device) if need_bias_grad else None
+    ds = torch.empty((b, c), dtype=torch.float32, device=x.device) if need_scale_grad else None
+    dt = torch.empty((b, c), dtype=torch.float32, device=x.device) if need_shift_grad else None
     d = _gn_desc(x, indices, b, g, num_valid, code)
-    d.dy, d.dx, d.weight, d.dweight, d.dbias = _ptr(dy), _ptr(dx), _ptr(weight), _ptr(dw), _ptr(db)
+    d.dy, d.dx, d.weight, d.bias, d.dweight, d.dbias = _ptr(dy), _ptr(dx), _ptr(weight), _ptr(bias), _ptr(dw), _ptr(db)
     d.mean, d.invstd, d.order, d.offsets, d.cstart = (mean.data_ptr(), invstd.data_ptr(), _ptr(order),
                                                       offsets.data_ptr(), cstart.data_ptr())
+    m = _gn_mod_desc(d, scale, shift, act_code)
+    m.dscale, m.dshift = _ptr(ds), _ptr(dt)
     lib = _lib()
     ws = _bytes(lib.spx_masked_group_norm_workspace_size(rows, b, c), x.device)
-    _cabi.check(lib.spx_masked_group_norm_bwd(ctypes.byref(d), ws.data_ptr(), ws.numel(), _stream()),
+    _cabi.check(lib.spx_masked_group_norm_mod_bwd(ctypes.byref(m), ws.data_ptr(), ws.numel(), _stream()),
                 "masked_group_norm_bwd")
-    return dx, dw, db
+    return dx, dw, db, ds, dt
 
 
 # ---------------------------------------------------------------------------- cross-rank BatchNorm
