@@ -5,10 +5,10 @@
 //
 // Forward:
 //   keys     : key[r] = sample of row r, B for padding and dropped rows;
-//   group    : stable radix argsort of the keys (sort.cu), so the rows of sample b are
-//              order[offsets[b] .. offsets[b+1]) in ascending row order whatever the padding;
-//   segments : one block finds offsets [B+1] by binary search in the sorted keys, cuts every segment into
-//              chunks of GP_CHUNK rows and numbers the chunks (cstart [B+1], an exclusive scan);
+//   group    : sort_by_key (segments.cuh), so the rows of sample b are order[offsets[b] .. offsets[b+1]) in
+//              ascending row order whatever the padding;
+//   segments : one block finds offsets [B+1] by binary search in the sorted keys (first_at_least), cuts every
+//              segment into chunks of GP_CHUNK rows and numbers the chunks (cstart [B+1], an exclusive scan);
 //   reduce   : one block per (chunk, channel slice), grid sized for the worst case ceil(rows / GP_CHUNK) + B;
 //              blocks past the last chunk exit.  Row lane l folds rows p0 + l, p0 + l + lanes, ... in ascending
 //              order, then the lanes merge in a fixed binary tree; the partial goes to workspace [chunk][C];
@@ -23,11 +23,9 @@
 // The summation order depends only on the sample's valid rows, never on `rows`, M beyond them or the grid,
 // and no float atomics are used, so every result is bit-reproducible and independent of padding.
 #include "rows.cuh"
+#include "segments.cuh"
 
 namespace spx {
-size_t radix_argsort_workspace_bytes(int64_t n);
-int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
-                       int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
 
 constexpr int GP_THREADS = 256;
 constexpr int GP_SEG_THREADS = 1024; // the one block of the segments kernel
@@ -48,17 +46,6 @@ __global__ void gp_keys_kernel(const int32_t *__restrict__ coords, int64_t rows,
     keys[r] = key;
 }
 
-// first position of the sorted keys whose key is >= b
-__device__ __forceinline__ int32_t gp_lower_bound(const uint32_t *keys, int32_t n, uint32_t b) {
-    int32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int32_t mid = (lo + hi) >> 1;
-        if (keys[mid] < b) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
-}
-
 // One block: thread t owns the samples [t * per, (t + 1) * per).  offsets [B+1], cstart [B+1] (first chunk of
 // every sample, cstart[B] = number of chunks) and, when count != NULL, count [B].
 __global__ void __launch_bounds__(GP_SEG_THREADS)
@@ -69,10 +56,10 @@ gp_segments_kernel(const uint32_t *__restrict__ keys, int32_t n, int batch_size,
     const int per = (batch_size + GP_SEG_THREADS - 1) / GP_SEG_THREADS;
     const int lo = min(t * per, batch_size), hi = min(lo + per, batch_size);
     int32_t chunks = 0;
-    int32_t next = gp_lower_bound(keys, n, (uint32_t)lo);
+    int32_t next = first_at_least(keys, n, (uint32_t)lo);
     for (int b = lo; b < hi; ++b) {
         const int32_t cur = next;
-        next = gp_lower_bound(keys, n, (uint32_t)b + 1);
+        next = first_at_least(keys, n, (uint32_t)b + 1);
         chunks += (next - cur + GP_CHUNK - 1) / GP_CHUNK;
     }
     s_scan[t] = chunks;
@@ -84,17 +71,17 @@ gp_segments_kernel(const uint32_t *__restrict__ keys, int32_t n, int batch_size,
     }
     __syncthreads();
     int32_t c = s_scan[t] - chunks;
-    next = gp_lower_bound(keys, n, (uint32_t)lo);
+    next = first_at_least(keys, n, (uint32_t)lo);
     for (int b = lo; b < hi; ++b) {
         const int32_t cur = next;
-        next = gp_lower_bound(keys, n, (uint32_t)b + 1);
+        next = first_at_least(keys, n, (uint32_t)b + 1);
         offsets[b] = cur;
         cstart[b] = c;
         if (count) count[b] = next - cur;
         c += (next - cur + GP_CHUNK - 1) / GP_CHUNK;
     }
     if (t == GP_SEG_THREADS - 1) {
-        offsets[batch_size] = gp_lower_bound(keys, n, (uint32_t)batch_size);
+        offsets[batch_size] = first_at_least(keys, n, (uint32_t)batch_size);
         cstart[batch_size] = s_scan[t];
     }
 }
@@ -109,7 +96,7 @@ gp_reduce_kernel(const T *__restrict__ x, const int32_t *__restrict__ order, con
     // sample_chunk (rows.cuh) written out: called, it gives these kernels a different register allocation
     const int32_t k = (int32_t)blockIdx.x;
     if (k >= __ldg(cstart + batch_size)) return;
-    const int b = gp_sample_of_chunk(cstart, batch_size, k);
+    const int b = last_at_most(cstart, batch_size, k);
     const int32_t p0 = __ldg(offsets + b) + (k - __ldg(cstart + b)) * GP_CHUNK;
     const int32_t seg_end = __ldg(offsets + b + 1);
     const int32_t end = seg_end < p0 + GP_CHUNK ? seg_end : p0 + GP_CHUNK;
@@ -265,7 +252,7 @@ static int64_t gp_max_chunks(int64_t rows, int batch_size) {
     return (rows + GP_CHUNK - 1) / GP_CHUNK + batch_size;
 }
 
-// keys -> stable argsort -> segments: order [rows], offsets [B+1], cstart [B+1] and, when count != NULL, count [B]
+// keys -> sort_by_key -> segments: order [rows], offsets [B+1], cstart [B+1] and, when count != NULL, count [B]
 // (see the top of this file).  keys [rows] and sort_ws (radix_argsort_workspace_bytes(rows)) are scratch.  Shared
 // with group_norm.cu.
 int group_samples(const int32_t *coords, int64_t rows, int row_ints, int batch_size, const int32_t *num_valid,
@@ -275,10 +262,7 @@ int group_samples(const int32_t *coords, int64_t rows, int row_ints, int batch_s
         gp_keys_kernel<<<(unsigned)div_up64(rows, GP_THREADS), GP_THREADS, 0, stream>>>(
             coords, rows, row_ints, batch_size, num_valid, keys);
         SPX_CHECK_LAUNCH("gp_keys_kernel");
-        int key_bits = 1;                                  // enough bits for the keys 0..B
-        while (key_bits < 32 && (batch_size >> key_bits) != 0) ++key_bits;
-        if (int rc = radix_argsort_pair(keys, order, rows, nullptr, nullptr, 0, key_bits, sort_ws,
-                                        radix_argsort_workspace_bytes(rows), nullptr, 0, stream))
+        if (int rc = sort_by_key(keys, rows, batch_size, order, sort_ws, radix_argsort_workspace_bytes(rows), stream))
             return rc;
     }
     gp_segments_kernel<<<1, GP_SEG_THREADS, 0, stream>>>(keys, (int32_t)rows, batch_size, offsets, cstart, count);

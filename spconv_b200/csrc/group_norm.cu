@@ -4,7 +4,7 @@
 // beyond M), and 0 in y and dx.  Group g of C / G = Cg channels; sample b and group g have n = count_b * Cg values.
 //
 // Forward:
-//   group    : group_samples (global_pool.cu): keys -> stable argsort -> offsets [B+1] and chunks of GP_CHUNK rows
+//   group    : group_samples (global_pool.cu): keys -> sort_by_key -> offsets [B+1] and chunks of GP_CHUNK rows
 //              numbered by cstart [B+1].  The rows of sample b are order[offsets[b] .. offsets[b+1]) in ascending
 //              row order, whatever the padding;
 //   stats    : one block per (chunk, channel slice), grid ceil(rows / GP_CHUNK) + B, blocks past the last chunk exit.
@@ -27,12 +27,9 @@
 // The order of every sum depends only on the sample's kept rows, never on `rows`, the padding or the grid, and no
 // float atomics are used, so every result is bit-reproducible and independent of padding and dropped rows.
 #include "rows.cuh"
+#include "segments.cuh"
 
 namespace spx {
-size_t radix_argsort_workspace_bytes(int64_t n);
-int group_samples(const int32_t *coords, int64_t rows, int row_ints, int batch_size, const int32_t *num_valid,
-                  uint32_t *keys, int32_t *order, void *sort_ws, int32_t *offsets, int32_t *cstart, int32_t *count,
-                  cudaStream_t stream);
 
 constexpr int GN_THREADS = 256;
 constexpr int GN_FIN_CH = 8;         // finalize: channels per block

@@ -2,9 +2,9 @@
 // reduction of a dynamic VFE, with no host read-back.  ids [P] give every point's output row (pc_voxel_id of
 // MaskedPointToVoxel); a point whose id is outside [0, rows) is dropped.
 //
-//   group   : row32[p] = id or -1 (ps_rows_kernel), then the grouping of sparse_add.cu (group_rows): a stable
-//             radix argsort of the rows (dropped points keyed `rows`, i.e. last) and one binary search per row,
-//             so the points of row r are order[offsets[r] .. offsets[r+1]) in ascending point index;
+//   group   : row32[p] = id or -1 (ps_rows_kernel), then group_rows (segments.cuh) keyed by the rows (dropped
+//             points keyed `rows`, i.e. last), so the points of row r are order[offsets[r] .. offsets[r+1]) in
+//             ascending point index;
 //   reduce  : one thread per 16-byte chunk of an output row (per element when C * e or the pointers do not allow
 //             vectors) walks the row's points in that order.  max keeps the winner of max_beats (a NaN beats
 //             every number, then the greater value, then the lower point) and copies it bit for bit, with its
@@ -15,12 +15,9 @@
 // The order of every reduction depends only on the row's points, and no float atomics are used, so results are
 // bit-reproducible and independent of dropped points, wherever they sit.
 #include "rows.cuh"
+#include "segments.cuh"
 
 namespace spx {
-int group_rows(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int32_t *offsets, void *workspace,
-               size_t workspace_bytes, cudaStream_t stream, const char *who);
-int sum_segments(const void *x, int64_t rows, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
-                 int dtype, void *out, cudaStream_t stream);
 
 constexpr int PS_THREADS = 256;
 constexpr int PS_INFLIGHT = 4;                   // reduce (max): points loaded per step of a row's walk

@@ -13,16 +13,15 @@
 // Same hash-and-scan building blocks as rulebook.cu (hash.cuh).  Two stages because the voxel count
 // sizes the outputs (the reference returns sliced tensors of that length, pointops.py:434-490).
 // spx_point2voxel_bounded (MaskedPointToVoxel) does a batch of clouds in one pass with the count kept on the
-// device and outputs of a host-known bound; it shares p2v_coord, the insert and the scatter with the stages.
+// device and outputs of a host-known bound; it shares p2v_coord, the insert and the scatter with the stages, and
+// groups the points by row with sort_by_key and segment_offsets (segments.cuh).
 #include "common.cuh"
 #include "hash.cuh"
 #include "rank.cuh"
+#include "segments.cuh"
 #include <cub/cub.cuh>
 
 namespace spx {
-size_t radix_argsort_workspace_bytes(int64_t n);
-int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
-                       int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
 
 struct P2VGeom {
     int ndim, zyx;
@@ -53,13 +52,7 @@ __device__ __forceinline__ bool p2v_coord(const P2VGeom &g, const float *__restr
 // lies before off[0] or at / beyond off[nsamples] (padding)
 __device__ __forceinline__ int p2v_sample_of(const int32_t *__restrict__ off, int nsamples, int64_t i) {
     if (i < (int64_t)__ldg(off) || i >= (int64_t)__ldg(off + nsamples)) return -1;
-    int lo = 0, hi = nsamples - 1;                  // the last b with off[b] <= i
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if ((int64_t)__ldg(off + mid) <= i) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
+    return last_at_most(off, nsamples, i);
 }
 
 // key = b * grid volume + cell (row-major over the internal axes), -1 = no voxel.  sample_off == NULL: one
@@ -313,22 +306,6 @@ __global__ void p2v_rows_kernel(P2VGeom g, const int64_t *__restrict__ keys, con
     sort_key[i] = row >= 0 ? (uint32_t)row : (uint32_t)bound;
 }
 
-// rows sorted ascending (points without a row keyed `bound`, last): start[o] = first position with key >= o,
-// o = 0..bound, one binary search per row (filling the gap after each key from one thread would leave one
-// thread writing all of the empty rows [M, bound))
-__global__ void p2v_row_starts_kernel(const uint32_t *__restrict__ sorted_row, int64_t n, int64_t bound,
-                                      int32_t *__restrict__ start) {
-    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (o > bound) return;
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if ((int64_t)__ldg(sorted_row + mid) < o) lo = mid + 1;
-        else hi = mid;
-    }
-    start[o] = (int32_t)lo;
-}
-
 // one thread per element of voxels [bound, max_points, nf]: a slot at or beyond the row's point count gets the
 // mean of the kept points (empty_mean: the same fp32 sum and division as p2v_finish_kernel) or 0; element
 // (v, 0, 0) also writes num_per_voxel[v] and, for a row without points (padding), indices row v = -1
@@ -366,20 +343,6 @@ struct P2VWs {
     int32_t *start; int *counter;
 };
 
-static size_t p2v_sort_tmp(int64_t n) {
-    // The size query goes through the CUDA runtime: a stale error left by an earlier failed call (e.g. a
-    // refused stream capture) would make it return early with bytes = 0, and the workspace computed here
-    // would then be smaller than what the same query yields a moment later.  Clear the state first and
-    // never return less than a bound that covers CUB's double buffers + histograms.
-    cudaGetLastError();
-    size_t bytes = 0;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
-                                                    (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n);
-    const size_t floor_bytes = (size_t)(n > 0 ? n : 1) * 16 + (1u << 20);
-    if (e != cudaSuccess) { cudaGetLastError(); return floor_bytes; }
-    return bytes > floor_bytes ? bytes : floor_bytes;
-}
-
 static bool p2v_i64(const int *grid, int ndim) {
     double v = 1;
     for (int j = 0; j < ndim; ++j) v *= (double)grid[j];
@@ -395,7 +358,7 @@ static int p2v_carve(int64_t n, const int *grid, int ndim, void *workspace, size
     w.keys = ws.take<int64_t>(n);
     w.a0 = ws.take<uint32_t>(n); w.a1 = ws.take<uint32_t>(n);
     w.b0 = ws.take<uint32_t>(n); w.b1 = ws.take<uint32_t>(n);
-    w.sort_tmp_bytes = p2v_sort_tmp(n);
+    w.sort_tmp_bytes = cub_sort_pairs_temp_bytes(n);
     w.sort_tmp = ws.take<char>(w.sort_tmp_bytes);
     w.start = ws.take<int32_t>(n + 2);
     w.counter = ws.take<int>(64);
@@ -530,14 +493,10 @@ extern "C" int spx_point2voxel_bounded(const float *points, int64_t N, int num_f
     p2v_rows_kernel<<<nblk, 256, 0, stream>>>(g, w.keys, w.first, N, vol, w.bitmap, w.tile_cnt, w.rbase, w.kept,
                                               w.base, bound, pc_voxel_id, w.sort_key, indices);
     SPX_CHECK_LAUNCH("p2v_rows_kernel");
-    // stable sort of the points by row: position inside a row's segment = rank in input order
-    int key_bits = 1;                                  // enough bits for the keys 0..bound
-    while (key_bits < 32 && (bound >> key_bits) != 0) ++key_bits;
-    if (int rc = radix_argsort_pair(w.sort_key, w.order, N, nullptr, nullptr, 0, key_bits, w.sort_ws, w.sort_ws_bytes,
-                                    nullptr, 0, stream))
-        return rc;
-    p2v_row_starts_kernel<<<(unsigned)div_up64(bound + 1, 256), 256, 0, stream>>>(w.sort_key, N, bound, w.start);
-    SPX_CHECK_LAUNCH("p2v_row_starts_kernel");
+    // stable sort of the points by row (points without a row keyed `bound`, last): position inside a row's
+    // segment = rank in input order
+    if (int rc = sort_by_key(w.sort_key, N, bound, w.order, w.sort_ws, w.sort_ws_bytes, stream)) return rc;
+    if (int rc = segment_offsets(w.sort_key, N, bound, w.start, stream)) return rc;
     p2v_scatter_kernel<<<(unsigned)div_up64(N * num_features, 256), 256, 0, stream>>>(
         points, num_features, w.sort_key, (const uint32_t *)w.order, N, (uint32_t)bound, w.start, max_points_per_voxel,
         voxels);
@@ -553,7 +512,7 @@ extern "C" size_t spx_point2voxel_workspace_size(int64_t num_points, int ndim) {
     const size_t n = (size_t)num_points;
     size_t total = 0;
     total += align_up((size_t)table_capacity(num_points, 2) * 8, 256) + align_up((size_t)table_capacity(num_points, 2) * 4, 256);
-    total += align_up(n * 8, 256) + 4 * align_up(n * 4, 256) + align_up(p2v_sort_tmp(num_points), 256);
+    total += align_up(n * 8, 256) + 4 * align_up(n * 4, 256) + align_up(cub_sort_pairs_temp_bytes(num_points), 256);
     total += align_up((n + 2) * 4, 256) + 256;
     (void)ndim;
     return total + 2048;
@@ -592,11 +551,10 @@ extern "C" int spx_point2voxel_stage1(const float *points, int64_t N, int num_fe
     *total_voxels_host = total;
     *num_voxels_host = total < max_voxels ? total : max_voxels;
     if (total == 0) return 0;
-    // rank the voxels by their first point: (first point, slot) sorted by first point -> b0 / b1
-    int end_bit = 1;
-    while (end_bit < 32 && ((int64_t)1 << end_bit) < N) ++end_bit;
+    // rank the voxels by their first point (0..N - 1): (first point, slot) sorted by first point -> b0 / b1
     size_t tmp = w.sort_tmp_bytes;
-    SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp, w.a0, w.b0, w.a1, w.b1, total, 0, end_bit, stream));
+    SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp, w.a0, w.b0, w.a1, w.b1, total, 0,
+                                                   sort_key_bits(N - 1), stream));
     count_launch(3);
     return 0;
 }
@@ -630,10 +588,9 @@ extern "C" int spx_point2voxel_stage2(const float *points, int64_t N, int num_fe
         })) return rc;
     if (num_voxels == 0) return 0;
     // stable sort of the points by voxel id: position inside a segment = rank in input order
-    int end_bit = 1;
-    while (end_bit < 32 && ((int64_t)1 << end_bit) <= (int64_t)M) ++end_bit;
     size_t tmp = w.sort_tmp_bytes;
-    SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp, w.a0, w.b0, w.a1, w.b1, (int)N, 0, end_bit, stream));
+    SPX_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp, w.a0, w.b0, w.a1, w.b1, (int)N, 0, sort_key_bits(M),
+                                                   stream));
     count_launch(3);
     p2v_segments_kernel<<<(unsigned)div_up64(N + 1, 256), 256, 0, stream>>>(w.b0, N, M, w.start);
     SPX_CHECK_LAUNCH("p2v_segments_kernel");

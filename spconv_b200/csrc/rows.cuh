@@ -12,6 +12,7 @@
 // blockIdx.y selects a slice of tpr vectors.
 #pragma once
 #include "common.cuh"
+#include "segments.cuh"
 
 namespace spx {
 
@@ -114,23 +115,12 @@ __device__ __forceinline__ int64_t valid_rows(const int32_t *num_valid, int64_t 
 // [offsets[b], offsets[b+1]), cut into chunks of GP_CHUNK numbered from cstart[b]; cstart[B] chunks in all
 constexpr int GP_CHUNK = 512;        // rows per partial
 
-// the sample whose chunks hold chunk k: the last b with cstart[b] <= k (empty samples own no chunk)
-__device__ __forceinline__ int gp_sample_of_chunk(const int32_t *cstart, int batch_size, int32_t k) {
-    int lo = 0, hi = batch_size - 1;
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(cstart + mid) <= k) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
-
 // The chunk of block blockIdx.x: its sample and sorted positions [p0, end).  False past the last chunk.
 __device__ __forceinline__ bool sample_chunk(const int32_t *offsets, const int32_t *cstart, int batch_size, int &b,
                                              int32_t &p0, int32_t &end) {
     const int32_t k = (int32_t)blockIdx.x;
     if (k >= __ldg(cstart + batch_size)) return false;
-    b = gp_sample_of_chunk(cstart, batch_size, k);
+    b = last_at_most(cstart, batch_size, k);          // empty samples own no chunk
     p0 = __ldg(offsets + b) + (k - __ldg(cstart + b)) * GP_CHUNK;
     const int32_t seg_end = __ldg(offsets + b + 1);
     end = seg_end < p0 + GP_CHUNK ? seg_end : p0 + GP_CHUNK;

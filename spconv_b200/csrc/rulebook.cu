@@ -14,12 +14,10 @@
 #include "gemm.cuh"
 #include "hash.cuh"
 #include "rank.cuh"
+#include "segments.cuh"
 #include <cub/cub.cuh>
 
 namespace spx {
-size_t radix_argsort_workspace_bytes(int64_t n);
-int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
-                       int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
 int validate_sparse_add_union(const spx_conv_geometry *g, int64_t N, int64_t bound);
 }
 
@@ -1040,20 +1038,6 @@ extern "C" int64_t spx_conv_max_out(const spx_conv_geometry *g, int64_t num_in) 
     return res;
 }
 
-static size_t sort_pairs_temp_bytes(int64_t n) {
-    // The size query goes through the CUDA runtime: a stale error left by an earlier failed call (e.g. a
-    // refused stream capture) would make it return early with bytes = 0, and the workspace computed here
-    // would then be smaller than what the same query yields a moment later.  Clear the state first and
-    // never return less than a bound that covers CUB's double buffers + histograms.
-    cudaGetLastError();
-    size_t bytes = 0;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
-                                                    (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n);
-    const size_t floor_bytes = (size_t)(n > 0 ? n : 1) * 16 + (1u << 20);
-    if (e != cudaSuccess) { cudaGetLastError(); return floor_bytes; }
-    return bytes > floor_bytes ? bytes : floor_bytes;
-}
-
 static bool subm_k3_path(const Geom &gg) {
     return !needs_i64(gg, gg.in_dims) && gg.ndim == 3 && gg.ksize[0] == 3 && gg.ksize[1] == 3 && gg.ksize[2] == 3;
 }
@@ -1348,7 +1332,7 @@ extern "C" size_t spx_mask_argsort_workspace_size(int64_t N, int words) {
     if (N <= 0) return 256;
     if (words == 1) return radix_argsort_workspace_bytes(N);
     size_t n = (size_t)N;
-    return 4 * align_up(n * 4, 256) + align_up(n * 4 * (size_t)words, 256) + align_up(sort_pairs_temp_bytes(N), 256) + 1024;
+    return 4 * align_up(n * 4, 256) + align_up(n * 4 * (size_t)words, 256) + align_up(cub_sort_pairs_temp_bytes(N), 256) + 1024;
 }
 
 extern "C" int spx_mask_argsort(uint32_t *mask, int32_t *argsort, int64_t N, int words, int kv, int do_sort,
@@ -1373,7 +1357,7 @@ extern "C" int spx_mask_argsort(uint32_t *mask, int32_t *argsort, int64_t N, int
     int32_t *perm_a = ws.take<int32_t>(N);
     int32_t *perm_b = ws.take<int32_t>(N);
     uint32_t *rows_tmp = ws.take<uint32_t>((size_t)N * words);
-    size_t tmp_bytes = sort_pairs_temp_bytes(N);
+    size_t tmp_bytes = cub_sort_pairs_temp_bytes(N);
     void *tmp = ws.take<char>(tmp_bytes);
     SPX_REQUIRE(ws.ok(), "argsort workspace too small: need %zu, have %zu", ws.off, workspace_bytes);
     iota_kernel<<<nblk, 256, 0, stream>>>(perm_a, N);

@@ -14,8 +14,9 @@
 //             known here, so no later pass re-reads keys to count): merged per block in shared
 //             memory, then one global atomic per distinct (digit, block) cell.
 // The first pass reads the masks with an implicit iota payload, the last pass writes the sorted
-// masks back in place (thrust semantics) and the argsort.
-#include "common.cuh"
+// masks back in place (thrust semantics) and the argsort.  Also the host helpers of segments.cuh.
+#include "segments.cuh"
+#include <cub/cub.cuh>
 
 namespace spx {
 
@@ -291,6 +292,39 @@ int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t 
         }
     }
     return 0;
+}
+
+int sort_by_key(uint32_t *keys, int64_t n, int64_t max_key, int32_t *order, void *sort_ws, size_t sort_ws_bytes,
+                cudaStream_t stream) {
+    return radix_argsort_pair(keys, order, n, nullptr, nullptr, 0, sort_key_bits(max_key), sort_ws, sort_ws_bytes,
+                              nullptr, 0, stream);
+}
+
+__global__ void segment_offsets_kernel(const uint32_t *__restrict__ keys, int64_t n, int64_t m,
+                                       int32_t *__restrict__ offsets) {
+    const int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (k > m) return;
+    offsets[k] = (int32_t)first_at_least(keys, n, k);
+}
+
+int segment_offsets(const uint32_t *sorted_keys, int64_t n, int64_t m, int32_t *offsets, cudaStream_t stream) {
+    segment_offsets_kernel<<<(unsigned)div_up64(m + 1, 256), 256, 0, stream>>>(sorted_keys, n, m, offsets);
+    SPX_CHECK_LAUNCH("segment_offsets_kernel");
+    return 0;
+}
+
+size_t cub_sort_pairs_temp_bytes(int64_t n) {
+    // The size query goes through the CUDA runtime: a stale error left by an earlier failed call (e.g. a
+    // refused stream capture) would make it return early with bytes = 0, and the workspace computed here
+    // would then be smaller than what the same query yields a moment later.  Clear the state first and
+    // never return less than a bound that covers CUB's double buffers + histograms.
+    cudaGetLastError();
+    size_t bytes = 0;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
+                                                    (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n);
+    const size_t floor_bytes = (size_t)(n > 0 ? n : 1) * 16 + (1u << 20);
+    if (e != cudaSuccess) { cudaGetLastError(); return floor_bytes; }
+    return bytes > floor_bytes ? bytes : floor_bytes;
 }
 
 }  // namespace spx

@@ -5,8 +5,8 @@
 // stride-1, padding-0 convolution over the operands' coordinates concatenated in visit order
 // (spx_conv_rulebook_stage1/2): out_inds are the distinct in-range coordinates in first-touch order and
 // pair_bwd[0] maps every visited row to its output row (-1 = out of range).  This file adds:
-//   group  : a stable radix argsort of those output rows (dropped rows keyed M, i.e. last) and the segment
-//            offsets, so the rows of output o are order[offsets[o] .. offsets[o+1]), ascending in visit order;
+//   group  : group_rows, the grouping of segments.cuh keyed by those output rows (dropped rows keyed M, i.e.
+//            last), so the rows of output o are order[offsets[o] .. offsets[o+1]), ascending in visit order;
 //            the first of them is the row that created o;
 //   fwd    : output-stationary sum of every segment in fp32, in visit order, rounded once; each output
 //            element is written by exactly one thread (no atomics, bit-reproducible);
@@ -14,11 +14,9 @@
 //            (index = pair_bwd[0]) and the head-row gather of RemoveDuplicate.
 // Feature rows are moved as 16-byte vectors when every row and base pointer allows it, else per element.
 #include "rows.cuh"
+#include "segments.cuh"
 
 namespace spx {
-size_t radix_argsort_workspace_bytes(int64_t n);
-int radix_argsort_pair(uint32_t *mask0, int32_t *argsort0, int64_t n0, uint32_t *mask1, int32_t *argsort1, int64_t n1,
-                       int key_bits, void *ws0, size_t ws0_bytes, void *ws1, size_t ws1_bytes, cudaStream_t stream);
 int validate_sparse_add_union(const spx_conv_geometry *g, int64_t N, int64_t bound);
 
 constexpr int SA_THREADS = 256;
@@ -32,7 +30,8 @@ struct SaOperands {
     int64_t start[SA_MAX + 1];
 };
 
-// operand that holds visited row g: the last t with start[t] <= g (empty operands are skipped that way)
+// operand that holds visited row g: the last t with start[t] <= g (empty operands are skipped that way).  Not
+// last_at_most: ops lives in the kernel parameters, which __ldg cannot read.
 __device__ __forceinline__ int operand_of(const SaOperands &ops, int64_t g) {
     int lo = 0, hi = ops.count - 1;
     while (lo < hi) {
@@ -48,21 +47,6 @@ __global__ void sa_keys_kernel(const int32_t *__restrict__ dst, int64_t n, uint3
     if (i >= n) return;
     const int32_t o = __ldg(dst + i);
     keys[i] = o < 0 ? m : (uint32_t)o;
-}
-
-// keys sorted ascending: offsets[o] = first position whose key is >= o, for o = 0..m, one binary search per o.
-// (Not one thread per key filling the gap up to the next key: with a bound, outputs [M, bound) are all empty
-// and one thread would write that whole gap.)
-__global__ void sa_offsets_kernel(const uint32_t *__restrict__ keys, int64_t n, uint32_t m, int32_t *__restrict__ offsets) {
-    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    if (o > (int64_t)m) return;
-    int64_t lo = 0, hi = n;
-    while (lo < hi) {
-        const int64_t mid = (lo + hi) >> 1;
-        if ((int64_t)__ldg(keys + mid) < o) lo = mid + 1;
-        else hi = mid;
-    }
-    offsets[o] = (int32_t)lo;
 }
 
 // one thread = W channels of one output row; the rows of the segment are added in visit order
@@ -210,7 +194,7 @@ sa_pack_kernel(const __grid_constant__ SaPlan plan, const int32_t *__restrict__ 
     __syncthreads();
     const int64_t g = blockIdx.x * (int64_t)blockDim.x + t;
     if (g >= plan.start[plan.count]) return;
-    int lo = 0, hi = plan.count - 1;                           // the last operand with start <= g
+    int lo = 0, hi = plan.count - 1;                           // the last operand with start <= g (operand_of)
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
         if (plan.start[mid] <= g) lo = mid;
@@ -274,14 +258,8 @@ int group_rows(const int32_t *dst, int64_t rows, int64_t M, int32_t *order, int3
     const unsigned blk = (unsigned)div_up64(rows, SA_THREADS);
     sa_keys_kernel<<<blk, SA_THREADS, 0, stream>>>(dst, rows, (uint32_t)M, keys);
     SPX_CHECK_LAUNCH("sa_keys_kernel");
-    int key_bits = 1;                                  // enough bits for the keys 0..M
-    while (key_bits < 32 && (M >> key_bits) != 0) ++key_bits;
-    if (int rc = radix_argsort_pair(keys, order, rows, nullptr, nullptr, 0, key_bits, sort_ws,
-                                    radix_argsort_workspace_bytes(rows), nullptr, 0, stream))
-        return rc;
-    sa_offsets_kernel<<<(unsigned)div_up64(M + 1, SA_THREADS), SA_THREADS, 0, stream>>>(keys, rows, (uint32_t)M, offsets);
-    SPX_CHECK_LAUNCH("sa_offsets_kernel");
-    return 0;
+    if (int rc = sort_by_key(keys, rows, M, order, sort_ws, radix_argsort_workspace_bytes(rows), stream)) return rc;
+    return segment_offsets(keys, rows, M, offsets, stream);
 }
 
 static int sum_dtype(const SaOperands &ops, const int32_t *order, const int32_t *offsets, int64_t M, int channels,
