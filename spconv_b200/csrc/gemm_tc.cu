@@ -15,7 +15,9 @@
 //     N = out channels, K = 32 bytes per instruction) accumulating the whole offset sum in
 //     registers (one group stays in flight: a stage is released once the next stage's group is
 //     issued), and store their rows (bias / activation / int8 requantisation) once the tile's
-//     last offset is in; the producers meanwhile fill the stages of the next tile.
+//     last offset is in; the producers meanwhile fill the stages of the next tile.  The
+//     destination rows come from the argsort row of the tile's index block, read at the tile's
+//     start; bias and scales from shared memory, loaded once per CTA.
 // 384 threads leave 168 registers per thread: room for the accumulator fragment (128 fp32 per
 // consumer thread at N = 256) and for the hoisted per-lane gather addressing of the producers.
 //
@@ -68,7 +70,8 @@ struct TcParams {
     const int32_t *tile_table;   // [tiles][kv+1][128]
     const int32_t *sched_rec;    // [tiles][TT_REC_INTS] schedule records, heaviest tile first (gemm.cuh)
     int *sched_state;            // [0] ticket counter, [1] finished CTAs; zero between launches
-    const int32_t *argsort;      // destination rows of the epilogue (NULL = identity)
+    const int32_t *argsort;      // order the tile table was built with (NULL = identity); the epilogue reads its
+                                 // destination rows from row kv of each index block, which holds this order
     int kv, words, reverse;
     // epilogue
     void *y;
@@ -121,11 +124,21 @@ __device__ __forceinline__ float load_bias(const void *bias, int j) {
 
 // Store one warpgroup's accumulator fragment: register i of thread t holds row
 // (t / 4) % 8 + 16 * warp + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (t % 4) + i % 2.
-template <int OUT, bool INT8_MODE, int N, typename Acc>
-__device__ __forceinline__ void epilogue_frag(const TcParams &p, const Acc (&acc)[N / 2], int64_t dst_lo, int64_t dst_hi,
-                                              int lane) {
+// ec: the CTA's epilogue constants in shared memory, ec[j] = bias (float mode) or scale (int8 mode),
+// ec[N + j] = the int8 bias.  A float-mode call without bias and activation (the input gradient, and
+// every conv layer followed by a norm) runs the PLAIN instance: convert and store, no per-element
+// branches between the stores.
+template <int OUT, bool INT8_MODE, int N, typename Acc, bool PLAIN = false>
+__device__ __forceinline__ void epilogue_frag(const TcParams &p, const float *ec, const Acc (&acc)[N / 2], int64_t dst_lo,
+                                              int64_t dst_hi, int lane) {
+    if constexpr (!INT8_MODE && !PLAIN) {
+        if (p.bias == nullptr && p.act == SPX_ACT_NONE) {
+            epilogue_frag<OUT, false, N, Acc, true>(p, ec, acc, dst_lo, dst_hi, lane);
+            return;
+        }
+    }
     constexpr int EB = OutElem<OUT>::bytes;
-    const bool has_bias = INT8_MODE ? (p.bias_f32 != nullptr) : (p.bias != nullptr);
+    const bool has_bias = !PLAIN && (INT8_MODE ? (p.bias_f32 != nullptr) : (p.bias != nullptr));
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int64_t dst = h ? dst_hi : dst_lo;
@@ -140,14 +153,14 @@ __device__ __forceinline__ void epilogue_frag(const TcParams &p, const Acc (&acc
                 const Acc v = acc[nb * 4 + 2 * h + j];
                 if constexpr (!INT8_MODE) {
                     f[j] = (float)v;
-                    if (has_bias) f[j] += load_bias<OUT == SPX_I8 ? SPX_F32 : OUT>(p.bias, col + j);
+                    if (has_bias) f[j] += ec[col + j];
                 } else {
                     // int8 inference: y = acc * scale[k] + bias[k] (+ add * add_scale)   test/test_all_algo.py:272-287
-                    f[j] = (float)(int32_t)v * __ldg(p.scale + col + j);
-                    if (has_bias) f[j] += __ldg(p.bias_f32 + col + j);
+                    f[j] = (float)(int32_t)v * ec[col + j];
+                    if (has_bias) f[j] += ec[N + col + j];
                     if (p.output_add) f[j] += (float)p.output_add[dst * (int64_t)N + col + j] * p.output_add_scale;
                 }
-                if (p.act != SPX_ACT_NONE) f[j] = apply_act(f[j], p.act, p.alpha);
+                if (!PLAIN && p.act != SPX_ACT_NONE) f[j] = apply_act(f[j], p.act, p.alpha);
             }
             store2<OUT>(row_ptr + col * EB, f[0], f[1]);
         }
@@ -204,6 +217,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
     uint64_t *info_full = bars + 2 * TC_MAX_STAGES + 4;                    // [TC_INFO_DEPTH] scheduler -> roles
     uint64_t *info_empty = bars + 2 * TC_MAX_STAGES + 4 + TC_INFO_DEPTH;   // [TC_INFO_DEPTH] roles -> scheduler
     int32_t *info = reinterpret_cast<int32_t *>(bars + 2 * TC_MAX_STAGES + 4 + 2 * TC_INFO_DEPTH);   // [TC_INFO_DEPTH][8]: {tile, mask[4]}
+    float *ec = reinterpret_cast<float *>(smem + idx_off + 2u * p.idx_bytes + 1024u);   // [2][N] epilogue constants
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -231,7 +245,7 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
         }
         for (int a = 0; a < 2; ++a) {
             mbar_init(&idx_full[a], 1);      // expect_tx arrival of the bulk copy
-            mbar_init(&idx_empty[a], TC_PROD_WARPS);     // one release per producer warp
+            mbar_init(&idx_empty[a], TC_PROD_WARPS + TC_CONS_WARPS);   // one release per producer / consumer warp
         }
         for (int e = 0; e < TC_INFO_DEPTH; ++e) {
             mbar_init(&info_full[e], 1);
@@ -239,6 +253,16 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
         }
         mbar_fence_init();
         tma_prefetch_desc(&tmap_w);
+    }
+    // epilogue constants, read once per CTA instead of once per element and tile
+    for (int j = threadIdx.x; j < N; j += TC_THREADS) {
+        if constexpr (KIND == KIND_I8) {
+            ec[j] = __ldg(p.scale + j);
+            if (p.bias_f32) ec[N + j] = __ldg(p.bias_f32 + j);
+        } else if (p.bias) {
+            if constexpr (KIND == KIND_TF32) ec[j] = load_bias<SPX_F32>(p.bias, j);
+            else ec[j] = p.out_dtype == SPX_F16 ? load_bias<SPX_F16>(p.bias, j) : load_bias<SPX_BF16>(p.bias, j);
+        }
     }
     __syncthreads();
 
@@ -390,6 +414,19 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
             uint32_t tm[4];
             const int tile = read_info(local, tm);
             if (tile < 0) break;
+            // destination rows of this thread's two fragment rows: row kv of the tile's index block is
+            // the argsort row (-1 past the end); the block is released right after
+            int32_t d_lo, d_hi;
+            {
+                const int buf = local & 1;
+                mbar_wait_silent(&idx_full[buf], (uint32_t)((local >> 1) & 1));
+                const int32_t *dst = reinterpret_cast<const int32_t *>(smem + idx_off + (size_t)buf * p.idx_bytes) +
+                                     p.kv * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+                d_lo = dst[0];
+                d_hi = dst[8];
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&idx_empty[buf]);
+            }
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) acc[i] = (Acc)0;
             BitIter it(tm);
@@ -444,20 +481,15 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[held]);
             }
-            const int64_t r_lo = (int64_t)tile * TC_TILE_M + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-            const int64_t r_hi = r_lo + 8;
-            int64_t d_lo = -1, d_hi = -1;
-            if (r_lo < p.rows) d_lo = p.argsort ? (int64_t)__ldg(p.argsort + r_lo) : r_lo;
-            if (r_hi < p.rows) d_hi = p.argsort ? (int64_t)__ldg(p.argsort + r_hi) : r_hi;
             if constexpr (KIND == KIND_F16) {
-                if (p.out_dtype == SPX_F16) epilogue_frag<SPX_F16, false, N>(p, acc, d_lo, d_hi, lane);
-                else epilogue_frag<SPX_BF16, false, N>(p, acc, d_lo, d_hi, lane);
+                if (p.out_dtype == SPX_F16) epilogue_frag<SPX_F16, false, N>(p, ec, acc, d_lo, d_hi, lane);
+                else epilogue_frag<SPX_BF16, false, N>(p, ec, acc, d_lo, d_hi, lane);
             } else if constexpr (KIND == KIND_TF32) {
-                epilogue_frag<SPX_F32, false, N>(p, acc, d_lo, d_hi, lane);
+                epilogue_frag<SPX_F32, false, N>(p, ec, acc, d_lo, d_hi, lane);
             } else {
-                if (p.out_dtype == SPX_I8) epilogue_frag<SPX_I8, true, N>(p, acc, d_lo, d_hi, lane);
-                else if (p.out_dtype == SPX_F32) epilogue_frag<SPX_F32, true, N>(p, acc, d_lo, d_hi, lane);
-                else epilogue_frag<SPX_F16, true, N>(p, acc, d_lo, d_hi, lane);
+                if (p.out_dtype == SPX_I8) epilogue_frag<SPX_I8, true, N>(p, ec, acc, d_lo, d_hi, lane);
+                else if (p.out_dtype == SPX_F32) epilogue_frag<SPX_F32, true, N>(p, ec, acc, d_lo, d_hi, lane);
+                else epilogue_frag<SPX_F16, true, N>(p, ec, acc, d_lo, d_hi, lane);
             }
         }
     }
@@ -602,11 +634,12 @@ static int fill_params(const GatherGemmArgs &a, TcParams &p) {
 
 template <int KIND, int CPR, int N>
 static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
-    const size_t smem = (size_t)p.stages * p.stage_bytes + 2 * (size_t)p.idx_bytes + 1024 /*align slack*/ + 1024 /*barriers, tile-info ring*/;
+    const size_t smem = (size_t)p.stages * p.stage_bytes + 2 * (size_t)p.idx_bytes + 1024 /*align slack*/ + 1024 /*barriers, tile-info ring*/ +
+                        2 * N * sizeof(float) /*epilogue constants*/;
     // the opt-in is a per-DEVICE attribute: one process may drive several GPUs
     if (!func_configured((const void *)tc_gather_gemm_kernel<KIND, CPR, N>, current_device())) {
         SPX_CHECK_CUDA(cudaFuncSetAttribute(tc_gather_gemm_kernel<KIND, CPR, N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)(TC_SMEM_BUDGET + 2048)));
+                                            (int)(TC_SMEM_BUDGET + 2048 + 2 * N * sizeof(float))));
         SPX_CHECK_CUDA(cudaFuncSetAttribute(tc_gather_gemm_kernel<KIND, CPR, N>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     }
     const int64_t tiles = div_up64(p.rows, TC_TILE_M);
