@@ -39,6 +39,8 @@
  *        <- no counterpart: functional.masked_sparse_add / masked_remove_duplicate (padded operands, no read-back)
  *   spx_point_scatter_group / _fwd / _bwd (+ spx_sparse_add_gather for the sum's backward)
  *        <- no counterpart: PointVoxelScatter (per-voxel max / mean / sum of point features, no read-back)
+ *   spx_point_interp_plan / _fwd / _bwd
+ *        <- no counterpart: VoxelPointInterpolator (trilinear / nearest voxel -> point, torchsparse's voxel_to_point)
  *   spx_hash_clear / _insert / _query / _insert_exist / _rank
  *        <- HashTable (spconv/pytorch/hash.py)        spconv/csrc/hash/core.py
  *   spx_depthwise_fwd / _dgrad / _wgrad (+ _wgrad_workspace_size)
@@ -573,6 +575,64 @@ int spx_point_scatter_fwd(int mode, const void *x, int64_t num_points, int chann
 int spx_point_scatter_bwd(int mode, const void *dy, const int32_t *row32, int64_t num_points, int64_t rows,
                           int channels, int dtype, const int32_t *argmax, const int32_t *count, void *dx,
                           spx_stream_t stream);
+
+/* ------------------------------------------------------------------ voxel -> point interpolation */
+
+/*
+ * Trilinear or nearest interpolation of the features of a sparse tensor at query points (VoxelPointInterpolator:
+ * the voxel -> point step of point-voxel networks), with no host read-back.  The tensor is indices [rows, 1 + ndim]
+ * (batch, then the coordinates), spatial_shape [ndim], batch_size and num_valid (a device int32, or NULL = every
+ * row).  The arguments travel in one block, spx_point_interp (read on the host during the call), as those of
+ * spx_masked_group_norm do; each entry reads the fields it names below, plus ndim and mode (which give K).  pos [num_points, ndim] fp32 are positions in the tensor's index space, in the axis
+ * order of indices[:, 1:] (voxel v's feature sits at position v); batch_ids [num_points] int32.
+ *   A row is usable when r < M (M = *num_valid clamped to [0, rows]) and 0 <= b < batch_size and every coordinate
+ *   is in [0, shape_a).  Of rows with equal coordinates the lowest is used.  A point is dropped when its batch id
+ *   is outside [0, batch_size) or a component of pos is not finite or lies outside [-1, shape_a) (checked on the
+ *   float).
+ *   mode 0 trilinear, corners K = 2^ndim: base_a = floor(pos_a), f_a = pos_a - base_a; corner j takes base_a + 1 on
+ *          axis a when bit a of j is set, else base_a; its weight is the fp32 product, in ascending a, of f_a (bit
+ *          set) or 1 - f_a, one rounding per operation (no FMA).
+ *   mode 1 nearest, K = 1: the corner base_a + (f_a >= 0.5), weight 1.
+ *   A corner is found when a usable row has its coordinates; a missing corner gets index -1 and weight 0.
+ *   normalize != 0 divides the found weights by (S + 1e-8f), S their fp32 sum in ascending j (torchsparse's rule).
+ *   plan: index [num_points, K] int32 and weight [num_points, K] fp32, then order [num_points * K] and offsets
+ *         [rows + 1] as spx_sparse_add_group keyed by index: the entries e = p * K + j of row r are
+ *         order[offsets[r] .. offsets[r+1]) in ascending e.  workspace:
+ *         spx_point_interp_plan_workspace_size(args) bytes (ndim, spatial_shape, batch_size, rows, num_points,
+ *         mode; 0 = invalid arguments).  Launches: one insert kernel
+ *         (rows > 0) and one probe kernel (num_points > 0), then the grouping: 3 + 2 * ceil(bits / 9) kernels, bits
+ *         the key width of rows (none when num_points = 0).
+ *   fwd:  y [num_points, C]: y[p] = sum over the found corners in ascending j of weight[p, j] * x[index[p, j]], in
+ *         fp32 from +0 (one rounding per multiply and per add), rounded once to dtype; 0 for a point without a found
+ *         corner.  One launch.
+ *   bwd:  dx [rows, C]: dx[r] = sum over the entries e of row r in ascending e of weight[e] * dy[e / K], in fp32,
+ *         rounded once; every element written once, 0 for a row without entries.  One launch.
+ * No float atomics: every result is bit-reproducible and independent of padding rows and dropped points.
+ * dtype: f32 / f16 / bf16, any C >= 1 (16-byte vectors when the row size and pointers allow them, the same bits
+ * either way).  rows, num_points and num_points * K below 2^31 - 1.  Keys are 64-bit once batch_size * volume
+ * reaches 2^31 - 1.
+ */
+typedef struct spx_point_interp {
+    int ndim, batch_size, mode, normalize, channels, dtype;   /* mode 0 trilinear, 1 nearest; K from ndim and mode */
+    int spatial_shape[SPX_MAX_NDIM];
+    int64_t rows, num_points;
+    const int32_t *indices;     /* plan: [rows, 1 + ndim] */
+    const int32_t *num_valid;   /* plan: 1 int32, or NULL */
+    const float *pos;           /* plan: [num_points, ndim] */
+    const int32_t *batch_ids;   /* plan: [num_points] */
+    int32_t *index;             /* plan output, fwd input: [num_points, K] */
+    float *weight;              /* plan output, fwd / bwd input: [num_points, K] */
+    int32_t *order;             /* plan output, bwd input: [num_points * K] */
+    int32_t *offsets;           /* plan output, bwd input: [rows + 1] */
+    const void *x;              /* fwd: [rows, channels] */
+    void *y;                    /* fwd: [num_points, channels] */
+    const void *dy;             /* bwd: [num_points, channels] */
+    void *dx;                   /* bwd: [rows, channels] */
+} spx_point_interp;
+size_t spx_point_interp_plan_workspace_size(const spx_point_interp *args);
+int spx_point_interp_plan(const spx_point_interp *args, void *workspace, size_t workspace_bytes, spx_stream_t stream);
+int spx_point_interp_fwd(const spx_point_interp *args, spx_stream_t stream);
+int spx_point_interp_bwd(const spx_point_interp *args, spx_stream_t stream);
 
 /* ------------------------------------------------------------------ depthwise convolution */
 

@@ -99,6 +99,17 @@ class MaskedGroupNormMod(Structure):
     ]
 
 
+class PointInterp(Structure):
+    """``spx_point_interp``: the operands of a voxel -> point interpolation (plan, forward and backward)."""
+    _fields_ = [
+        ("ndim", c_int), ("batch_size", c_int), ("mode", c_int), ("normalize", c_int), ("channels", c_int),
+        ("dtype", c_int), ("spatial_shape", c_int * SPX_MAX_NDIM), ("rows", c_int64), ("num_points", c_int64),
+        ("indices", c_void_p), ("num_valid", c_void_p), ("pos", c_void_p), ("batch_ids", c_void_p),
+        ("index", c_void_p), ("weight", c_void_p), ("order", c_void_p), ("offsets", c_void_p),
+        ("x", c_void_p), ("y", c_void_p), ("dy", c_void_p), ("dx", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); also the list the CPU test checks against the header
 SIGNATURES = {
     "spx_last_error": (c_char_p, []),
@@ -207,6 +218,9 @@ SIGNATURES = {
                                       c_void_p, c_void_p]),
     "spx_point_scatter_bwd": (c_int, [c_int, c_void_p, c_void_p, c_int64, c_int64, c_int, c_int, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
+    "spx_point_interp_plan_workspace_size": (c_size_t, [POINTER(PointInterp)]),
+    "spx_point_interp_plan": (c_int, [POINTER(PointInterp), c_void_p, c_size_t, c_void_p]),
+    **{f"spx_point_interp_{p}": (c_int, [POINTER(PointInterp), c_void_p]) for p in ("fwd", "bwd")},
     "spx_depthwise_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int,
                                   c_int, c_int, c_float, c_void_p]),
     "spx_depthwise_dgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int64, c_int, c_int,

@@ -8,6 +8,16 @@
 
 namespace spx {
 
+// ------------------------------------------------------------------ keys
+// key of the coordinate c = (batch, c_1 .. c_ndim) in a grid of `dims`: row-major, batch outermost.  The SubM
+// rulebook (rulebook.cu) and the voxel -> point interpolation (point_interp.cu) insert and find with it.
+__device__ __forceinline__ int64_t linear_key(const int (&c)[SPX_MAX_NDIM + 1], const int *dims, int ndim) {
+    int64_t k = c[0];
+#pragma unroll
+    for (int a = 0; a < SPX_MAX_NDIM; ++a) if (a < ndim) k = k * dims[a] + c[a + 1];
+    return k;
+}
+
 // ------------------------------------------------------------------ hash tables
 __device__ __forceinline__ uint32_t mix32(uint32_t x) {
     x ^= x >> 16; x *= 0x85ebca6bu; x ^= x >> 13; x *= 0xc2b2ae35u; x ^= x >> 16;
@@ -69,6 +79,16 @@ struct Table32 {
             h = (h + 1) & cap_mask;
         }
     }
+    // find_slot one probe at a time (find_many): the first slot, then one step from slot h; true once the
+    // search ends (val = the value, or -1 when the key is absent), else h moves to the next slot
+    __device__ __forceinline__ uint32_t home(int64_t key64) const { return mix32((uint32_t)key64) & cap_mask; }
+    __device__ __forceinline__ bool find_step(int64_t key64, uint32_t &h, int32_t &val) const {
+        const unsigned long long cur = __ldg(&slots[h]);
+        if (cur == EMPTY) { val = -1; return true; }
+        if ((uint32_t)(cur >> 32) == (uint32_t)key64) { val = (int32_t)(uint32_t)cur; return true; }
+        h = (h + 1) & cap_mask;
+        return false;
+    }
     __device__ __forceinline__ bool occupied(uint32_t s, int64_t &key, int32_t &val) const {
         unsigned long long cur = slots[s];
         if (cur == EMPTY) return false;
@@ -117,6 +137,14 @@ struct Table64 {
             h = (h + 1) & cap_mask;
         }
     }
+    __device__ __forceinline__ uint32_t home(int64_t key) const { return mix64((uint64_t)key) & cap_mask; }
+    __device__ __forceinline__ bool find_step(int64_t key, uint32_t &h, int32_t &val) const {
+        const long long cur = keys[h];
+        if (cur == -1ll) { val = -1; return true; }
+        if (cur == key) { val = vals[h]; return true; }
+        h = (h + 1) & cap_mask;
+        return false;
+    }
     __device__ __forceinline__ bool occupied(uint32_t s, int64_t &key, int32_t &val) const {
         long long cur = keys[s];
         if (cur == -1ll) return false;
@@ -126,6 +154,32 @@ struct Table64 {
     __device__ __forceinline__ void set_value(uint32_t s, int32_t val) const { vals[s] = val; }
     __device__ __forceinline__ void clear_slot(uint32_t s) const { keys[s] = -1ll; }
 };
+
+// K independent finds kept in flight together: each round, every unfinished key loads its next slot, so the loads
+// of a round do not wait on each other (K find_slot calls in a row would walk the chains one after another).
+// val[j] = the value of key[j], -1 when it is absent or live[j] is false.
+template <int K, typename Table>
+__device__ __forceinline__ void find_many(const Table &t, const int64_t (&key)[K], const bool (&live)[K],
+                                          int32_t (&val)[K]) {
+    uint32_t h[K];
+    bool busy[K];
+    bool any = false;
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+        val[j] = -1;
+        busy[j] = live[j];
+        h[j] = live[j] ? t.home(key[j]) : 0u;
+        any = any || busy[j];
+    }
+    while (any) {
+        any = false;
+#pragma unroll
+        for (int j = 0; j < K; ++j) {
+            if (busy[j]) busy[j] = !t.find_step(key[j], h[j], val[j]);
+            any = any || busy[j];
+        }
+    }
+}
 
 // Host side: call f with the table over `slots` (and, for 64-bit keys, `vals`), so that one launch sequence
 // serves both key widths.  f returns 0 or an error code, which is passed on.

@@ -76,13 +76,6 @@ __device__ __forceinline__ void load_coord(const int32_t *indices, int64_t i, in
     }
 }
 
-__device__ __forceinline__ int64_t linear_key(const int (&c)[SPX_MAX_NDIM + 1], const int *dims, int ndim) {
-    int64_t k = c[0];
-#pragma unroll
-    for (int a = 0; a < SPX_MAX_NDIM; ++a) if (a < ndim) k = k * dims[a] + c[a + 1];
-    return k;
-}
-
 __device__ __forceinline__ void offset_taps(int k, const int *ksize, int ndim, int (&r)[SPX_MAX_NDIM]) {
 #pragma unroll
     for (int a = SPX_MAX_NDIM - 1; a >= 0; --a) if (a < ndim) { r[a] = k % ksize[a]; k /= ksize[a]; }

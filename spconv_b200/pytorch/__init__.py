@@ -21,7 +21,7 @@ from .spatial import MaskedRemoveDuplicate  # noqa: F401
 from .utils_fuse import (fuse_act, fuse_bn, fuse_bn_act_sequential, fuse_bn_weights)  # noqa: F401
 from . import quantized  # noqa: F401
 from .graph import GraphedStep, graph_capture  # noqa: F401
-from .utils import (MaskedPointToVoxel, PointToVoxel, PointVoxelScatter,  # noqa: F401
-                    gather_features_by_pc_voxel_id)
+from .utils import (MaskedPointToVoxel, PointToVoxel, PointVoxelScatter, VoxelPointInterpolator,  # noqa: F401
+                    gather_features_by_pc_voxel_id, grid_positions)
 from .prefetch import RulebookPrefetcher  # noqa: F401
 from .bounds import check_bounds, set_output_bounds  # noqa: F401

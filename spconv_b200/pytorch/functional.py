@@ -623,3 +623,25 @@ class PointScatterFunction(Function):
 
 
 point_scatter = PointScatterFunction.apply
+
+
+# ---------------------------------------------------------------------------- voxel -> point interpolation
+class PointInterpFunction(Function):
+    """``features, index, weight, order, offsets`` -> ``[P, C]``: the interpolation of the rows ``features [rows, C]``
+    at the points of a plan (:func:`ops.point_interp_plan`, :func:`ops.point_interp_fwd`).  The backward gives the
+    features' gradient (:func:`ops.point_interp_bwd`): a weighted segment sum per row, no atomics.  The plan is
+    constant: there is no gradient to the positions or the weights."""
+
+    @staticmethod
+    def forward(ctx, features, index, weight, order, offsets):
+        ctx.save_for_backward(weight, order, offsets)
+        return ops.point_interp_fwd(features, index, weight)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        weight, order, offsets = ctx.saved_tensors
+        return ops.point_interp_bwd(grad_output, weight, order, offsets), None, None, None, None
+
+
+point_interp = PointInterpFunction.apply

@@ -1377,6 +1377,117 @@ def point_scatter_bwd(dy: torch.Tensor, row32: torch.Tensor, aux: Optional[torch
     return dx
 
 
+# ---------------------------------------------------------------------------- voxel -> point interpolation
+POINT_INTERP_MODES = {"trilinear": 0, "nearest": 1}
+
+
+def point_interp_plan(indices: torch.Tensor, spatial_shape, batch_size: int, num_valid: Optional[torch.Tensor],
+                      pos: torch.Tensor, batch_ids: torch.Tensor, mode: str = "trilinear", normalize: bool = True):
+    """``(index [P, K], weight [P, K], order [P * K], offsets [rows + 1])`` of the points ``pos [P, ndim]`` (index
+    space, the axis order of ``indices[:, 1:]``) in batch ``batch_ids [P]`` against the tensor ``indices
+    [rows, 1 + ndim]`` (``spx_point_interp_plan``): ``K = 2^ndim`` corners (trilinear) or 1 (nearest), ``index`` -1
+    and ``weight`` 0 for a missing corner; the entries ``e = p * K + j`` of row ``r`` are
+    ``order[offsets[r]:offsets[r + 1]]`` in ascending ``e``.  Other float positions are cast to float32, int64
+    batch ids to int32 (outside ``[0, batch_size)`` they stay dropped).  No host synchronisation."""
+    for t, what in ((indices, "indices"), (pos, "pos"), (batch_ids, "batch_ids")):
+        _require_cuda(t, what)
+    if mode not in POINT_INTERP_MODES:
+        raise ValueError(f"point interpolation: mode must be 'trilinear' or 'nearest', got {mode!r}")
+    ndim = len(spatial_shape)
+    if indices.dim() != 2 or indices.dtype != torch.int32 or indices.shape[1] != ndim + 1:
+        raise RuntimeError(f"point interpolation: indices must be int32 [rows, {ndim + 1}], got {indices.dtype} "
+                           f"{tuple(indices.shape)}")
+    if pos.dim() != 2 or pos.shape[1] != ndim or not pos.is_floating_point():
+        raise RuntimeError(f"point interpolation: pos must be a float tensor [P, {ndim}], got {pos.dtype} "
+                           f"{tuple(pos.shape)}")
+    if batch_ids.shape != (pos.shape[0],) or batch_ids.dtype not in (torch.int32, torch.int64):
+        raise RuntimeError(f"point interpolation: batch_ids must be int32 or int64 [{pos.shape[0]}], got "
+                           f"{batch_ids.dtype} {tuple(batch_ids.shape)}")
+    if num_valid is not None:
+        _require_cuda(num_valid, "num_valid")
+        if num_valid.dtype != torch.int32 or num_valid.numel() != 1:
+            raise RuntimeError(f"point interpolation: num_valid must be one int32, got {num_valid.dtype} "
+                               f"{tuple(num_valid.shape)}")
+    if batch_ids.dtype == torch.int64:
+        batch_ids = torch.where((batch_ids >= 0) & (batch_ids < int(batch_size)), batch_ids, -1).int()
+    indices, pos, batch_ids = indices.contiguous(), pos.float().contiguous(), batch_ids.contiguous()
+    n, rows, dev = pos.shape[0], indices.shape[0], pos.device
+    k = 1 if mode == "nearest" else 1 << ndim
+    index = torch.empty((n, k), dtype=torch.int32, device=dev)
+    weight = torch.empty((n, k), dtype=torch.float32, device=dev)
+    order = torch.empty((n * k,), dtype=torch.int32, device=dev)
+    offsets = torch.empty((rows + 1,), dtype=torch.int32, device=dev)
+    a = _point_interp_args(ndim, mode, rows, n)
+    a.batch_size, a.normalize = int(batch_size), int(bool(normalize))
+    for i, v in enumerate(spatial_shape):
+        a.spatial_shape[i] = int(v)
+    a.indices, a.num_valid, a.pos, a.batch_ids = _ptr(indices), _ptr(num_valid), _ptr(pos), _ptr(batch_ids)
+    a.index, a.weight, a.order, a.offsets = _ptr(index), _ptr(weight), _ptr(order), offsets.data_ptr()
+    lib = _lib()
+    nbytes = lib.spx_point_interp_plan_workspace_size(ctypes.byref(a))
+    ws = _bytes(nbytes, dev)
+    _cabi.check(lib.spx_point_interp_plan(ctypes.byref(a), ws.data_ptr(), nbytes, _stream()), "point_interp_plan")
+    return index, weight, order, offsets
+
+
+def _point_interp_args(ndim: int, mode, rows: int, n: int) -> "_cabi.PointInterp":
+    a = _cabi.PointInterp()
+    a.ndim, a.rows, a.num_points = int(ndim), int(rows), int(n)
+    a.mode = POINT_INTERP_MODES[mode] if isinstance(mode, str) else int(mode)
+    return a
+
+
+def _point_interp_corners(k: int, rows: int, n: int) -> "_cabi.PointInterp":
+    """the argument block of a forward / backward over a table of k corners per point (1: nearest, 2^ndim)"""
+    if k not in (1, 2, 4, 8, 16):
+        raise RuntimeError(f"point interpolation: {k} corners per point, expected 1, 2, 4, 8 or 16")
+    return _point_interp_args(max(k.bit_length() - 1, 1), 1 if k == 1 else 0, rows, n)
+
+
+def _point_interp_dtype(x: torch.Tensor) -> int:
+    if x.dtype not in _GLOBAL_POOL_DTYPES:
+        raise RuntimeError(f"VoxelPointInterpolator supports float32, float16 and bfloat16 features, got {x.dtype}")
+    return _DTYPE_CODE[x.dtype]
+
+
+def point_interp_fwd(x: torch.Tensor, index: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """``y [P, C]`` of the rows ``x [rows, C]`` at the points of :func:`point_interp_plan`: the sum over the found
+    corners in ascending ``j`` of ``weight[p, j] * x[index[p, j]]`` in fp32 (no FMA), rounded once; 0 for a point
+    without a found corner.  One launch."""
+    code = _point_interp_dtype(x)
+    _require_cuda(x, "features")
+    if x.dim() != 2:
+        raise RuntimeError(f"point interpolation: features must be [rows, C], got {tuple(x.shape)}")
+    x = x.contiguous()
+    n, k = index.shape
+    rows, c = x.shape
+    y = torch.empty((n, c), dtype=x.dtype, device=x.device)
+    a = _point_interp_corners(k, rows, n)
+    a.channels, a.dtype = c, code
+    a.x, a.index, a.weight, a.y = _ptr(x), _ptr(index), _ptr(weight), _ptr(y)
+    _cabi.check(_lib().spx_point_interp_fwd(ctypes.byref(a), _stream()), "point_interp_fwd")
+    return y
+
+
+def point_interp_bwd(dy: torch.Tensor, weight: torch.Tensor, order: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+    """``dx [rows, C]`` of :func:`point_interp_fwd`: per row the sum over its entries ``e`` in ascending order of
+    ``weight[e] * dy[e / K]`` in fp32, rounded once; 0 for a row without entries.  Every element is written once, no
+    atomics.  One launch."""
+    code = _point_interp_dtype(dy)
+    _require_cuda(dy, "grad_output")
+    if dy.dim() != 2 or dy.shape[0] != weight.shape[0]:
+        raise RuntimeError(f"point interpolation: grad_output must be [{weight.shape[0]}, C], got {tuple(dy.shape)}")
+    dy = dy.contiguous()
+    n, k = weight.shape
+    rows, c = offsets.shape[0] - 1, dy.shape[1]
+    dx = torch.empty((rows, c), dtype=dy.dtype, device=dy.device)
+    a = _point_interp_corners(k, rows, n)
+    a.channels, a.dtype = c, code
+    a.dy, a.weight, a.order, a.offsets, a.dx = _ptr(dy), _ptr(weight), _ptr(order), offsets.data_ptr(), _ptr(dx)
+    _cabi.check(_lib().spx_point_interp_bwd(ctypes.byref(a), _stream()), "point_interp_bwd")
+    return dx
+
+
 # ---------------------------------------------------------------------------- misc
 def bias_add_act_inplace(x: torch.Tensor, bias: Optional[torch.Tensor], act_type=Activation.None_,
                          act_alpha: float = 0.0, act_beta: float = 0.0) -> torch.Tensor:

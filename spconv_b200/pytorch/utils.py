@@ -1,6 +1,7 @@
 """Point cloud -> voxel front end (``spconv/pytorch/utils.py:23-176``): ``PointToVoxel`` and
-``gather_features_by_pc_voxel_id``, plus ``MaskedPointToVoxel`` and ``PointVoxelScatter``.  CUDA only; the
-kernels live in ``csrc/pointops.cu`` and ``csrc/point_scatter.cu``.
+``gather_features_by_pc_voxel_id``, plus ``MaskedPointToVoxel``, ``PointVoxelScatter`` and the way back,
+``VoxelPointInterpolator`` with ``grid_positions``.  CUDA only; the kernels live in ``csrc/pointops.cu``,
+``csrc/point_scatter.cu`` and ``csrc/point_interp.cu``.
 
 Unlike the reference's GPU generator (atomic appends: voxel order and the points kept per voxel
 depend on scheduling) the result is deterministic and equal to the reference's CPU generator
@@ -266,6 +267,112 @@ class PointVoxelScatter(object):
 
     def sum(self, x: torch.Tensor) -> torch.Tensor:
         return self._reduce(x, "sum")
+
+
+class VoxelPointInterpolator(object):
+    """Features of a sparse tensor at query points, trilinear or nearest, in CUDA (``csrc/point_interp.cu``) with no
+    host read-back: the voxel -> point step of point-voxel networks (SPVCNN / SPVNAS, PVCNN-style point branches;
+    torchsparse's ``voxel_to_point``), from a tensor at any stride.
+
+    ``interp = VoxelPointInterpolator(x, pos, batch_ids, mode="trilinear", normalize=True)`` builds the plan once:
+
+    * ``x``: a :class:`SparseConvTensor` (its ``indices``, ``spatial_shape``, ``batch_size`` and ``num_valid``; its
+      features are not read).  A row is used when ``r < num_valid`` (every row without it) and its batch index and
+      coordinates are in range; of rows with equal coordinates the lowest is used.
+    * ``pos [P, ndim]``: positions in ``x``'s index space, in the axis order of ``indices[:, 1:]`` (zyx in 3-D); row
+      ``v``'s feature sits at the integer position ``v``.  :func:`grid_positions` computes them from point
+      coordinates.  Cast to float32.  ``batch_ids [P]`` int32 or int64.
+    * A point is dropped (output 0, no gradient) when its batch id is outside ``[0, batch_size)`` or a component of
+      ``pos`` is not finite or lies outside ``[-1, shape_a)``.
+    * ``"trilinear"``: the ``K = 2^ndim`` corners ``floor(pos) + {0, 1}`` per axis with the products of ``f`` /
+      ``1 - f`` (``f = pos - floor(pos)``) as weights; a corner without a row gets weight 0, and ``normalize=True``
+      divides the found weights by their sum ``+ 1e-8`` (torchsparse's ``calc_ti_weights``, so ported SPVCNN
+      checkpoints see the same features near empty voxels).  ``"nearest"``: the one corner ``floor(pos) + (f >= 0.5)`` with
+      weight 1 when it exists.
+
+    Then ``interp(features)`` gives ``[P, C]`` from ``features [rows, C]`` (``x.features`` or any other tensor on the
+    same coordinates: the plan is reused), differentiable in ``features``.  The forward adds the corners in ascending
+    order in fp32 and rounds once; the backward is a weighted sum per row over its points in ascending order.  No
+    float atomics: results are bit-reproducible and independent of padding rows and dropped points.  Nothing is read
+    back to the host, so a step from raw points to a per-point loss captures as one CUDA graph.
+    ``interp.index`` (int32, -1 = no corner) and ``interp.weight`` (fp32) are the ``[P, K]`` table.  float32, float16
+    and bfloat16 features; rows, P and P * K below 2^31 - 1.  CUDA only.
+
+    An SPVCNN-style step (point features -> voxels -> convs -> back to the points at stride 2)::
+
+        gen = spconv.MaskedPointToVoxel(vsize, coors_range, 4, max_voxels, 1, batch_size)
+        voxels, indices, _, pc_voxel_id, num_valid = gen(points, point_offsets)
+        scatter = spconv.PointVoxelScatter(pc_voxel_id, gen.max_num_voxels_total)
+        x = spconv.SparseConvTensor(scatter.mean(point_feats), indices, gen.grid_size, batch_size)
+        x.num_valid = num_valid
+        y = net(x)                                             # e.g. SubMConv3d, then SparseConv3d(k3, s2, p1)
+        # batch ids from the offsets, on the device (no sync): point p belongs to sample b when off[b] <= p < off[b+1]
+        p = torch.arange(points.shape[0], device=points.device, dtype=torch.int32)
+        batch_ids = torch.searchsorted(point_offsets, p, right=True).int() - 1   # -1 / batch_size for padding
+        pos = spconv.grid_positions(points[:, :3], vsize, coors_range, stride=2)          # k3 s2 p1: center 0
+        interp = spconv.VoxelPointInterpolator(y, pos, batch_ids)
+        point_feats = point_mlp(point_feats) + interp(y.features)
+    """
+
+    def __init__(self, x, pos: torch.Tensor, batch_ids: torch.Tensor, mode: str = "trilinear", normalize: bool = True):
+        if mode not in ops.POINT_INTERP_MODES:
+            raise ValueError(f"VoxelPointInterpolator: mode must be 'trilinear' or 'nearest', got {mode!r}")
+        self.mode = mode
+        self.normalize = bool(normalize)
+        self.num_rows = int(x.indices.shape[0])
+        nv = getattr(x, "num_valid", None)
+        if nv is not None:
+            nv = nv.to(device=x.indices.device, dtype=torch.int32).reshape(1)
+        self.index, self.weight, self.order, self.offsets = ops.point_interp_plan(
+            x.indices, list(x.spatial_shape), int(x.batch_size), nv, pos, batch_ids, mode, normalize)
+
+    def __call__(self, features: torch.Tensor) -> torch.Tensor:
+        ops._point_interp_dtype(features)
+        ops._require_cuda(features, "features")
+        if features.dim() != 2 or features.shape[0] != self.num_rows:
+            raise ValueError(f"VoxelPointInterpolator: features must be [{self.num_rows}, C], got "
+                             f"{tuple(features.shape)}")
+        return Fsp.point_interp(features, self.index, self.weight, self.order, self.offsets)
+
+
+def _per_axis(v, nd: int, what: str) -> List[float]:
+    vals = [float(e) for e in v] if isinstance(v, (list, tuple)) else [float(v)] * nd
+    if len(vals) != nd:
+        raise ValueError(f"grid_positions: {what} needs {nd} values (xyz order), got {len(vals)}")
+    return vals
+
+
+def grid_positions(points_xyz: torch.Tensor, vsize_xyz: List[float], coors_range_xyz: List[float],
+                   stride: Union[int, List[int]] = 1, center: Union[float, List[float]] = 0.0) -> torch.Tensor:
+    """Positions ``[P, ndim]`` (fp32, zyx) of points in the index space of a tensor at ``stride`` over the grid of
+    :class:`MaskedPointToVoxel` (``vsize_xyz``, ``coors_range_xyz``), for :class:`VoxelPointInterpolator`:
+    ``pos_a = ((p_a - lo_a) / vsize_a - 0.5 - center_a) / stride_a``, then the axes reversed (xyz -> zyx).
+    ``points_xyz [P, >= ndim]`` (the first ndim columns are used); ``stride`` and ``center`` are one value or one per
+    axis (xyz).  A voxel's centre lands on its index at stride 1.  ``center`` is where output ``o`` of the strided
+    tensor sits, in input voxels past ``o * stride``:
+
+    ====================================================  ================
+    tensor                                                 ``center``
+    ====================================================  ================
+    the voxelisation grid, or chains of k3 s2 p1 convs     ``0``
+    chains of k = s, p = 0 convs (and pools)               ``(s - 1) / 2``
+    torchsparse's convention (voxel at its lower corner)   ``-0.5``
+    ====================================================  ================
+    """
+    nd = len(vsize_xyz)
+    if len(coors_range_xyz) != 2 * nd:
+        raise ValueError(f"grid_positions: coors_range_xyz needs {2 * nd} values, got {len(coors_range_xyz)}")
+    if points_xyz.dim() != 2 or points_xyz.shape[1] < nd:
+        raise ValueError(f"grid_positions: points must be [P, >= {nd}], got {tuple(points_xyz.shape)}")
+    # the per-axis constants are filled on the device (no host -> device copy, so a captured step may call this),
+    # and divided by as tensors: a division by a host scalar would become a multiplication by its reciprocal
+    k = torch.empty((4, nd), dtype=torch.float32, device=points_xyz.device)
+    for i, vals in enumerate(([float(v) for v in coors_range_xyz[:nd]], [float(v) for v in vsize_xyz],
+                              _per_axis(center, nd, "center"), _per_axis(stride, nd, "stride"))):
+        for a, v in enumerate(vals):
+            k[i, a].fill_(v)
+    pos = ((points_xyz[:, :nd].float() - k[0]) / k[1] - 0.5 - k[2]) / k[3]
+    return pos.flip(1).contiguous()
 
 
 def gather_features_by_pc_voxel_id(seg_res_features: torch.Tensor, pc_voxel_id: torch.Tensor,
