@@ -69,7 +69,7 @@ extern "C" {
 #define SPX_MAX_NDIM 4
 
 /* element types of features / filters */
-enum spx_dtype { SPX_F32 = 0, SPX_F16 = 1, SPX_BF16 = 2, SPX_I8 = 3 };
+enum spx_dtype { SPX_F32 = 0, SPX_F16 = 1, SPX_BF16 = 2, SPX_I8 = 3, SPX_E4M3 = 4 };   /* E4M3: OCP fp8 e4m3fn */
 /* tv::gemm::Activation as used by the reference epilogues */
 enum spx_act { SPX_ACT_NONE = 0, SPX_ACT_RELU = 1, SPX_ACT_SIGMOID = 2, SPX_ACT_LEAKY_RELU = 3 };
 /* how fp32 features are multiplied: exact fp32 FMA, or TF32 tensor cores
@@ -885,6 +885,65 @@ int spx_implicit_gemm_fwd_int8(const spx_gemm_desc *d, const int8_t *features,
                                const float *scale, const float *bias, const int8_t *output_add,
                                float output_add_scale, int act, float act_alpha,
                                spx_stream_t stream);
+
+/*
+ * FP8 (e4m3) inference forward; the operands come in one argument block, spx_fp8_gemm.  d->dtype is SPX_E4M3;
+ * features [n_in, C] and filters [K, kv, C] are e4m3 bytes (OCP e4m3fn: finite range +-448, one NaN pattern per
+ * sign, no infinities).  Every scale is a device pointer, so no call reads anything back to the host:
+ *   in_scale  fp32 [1]  the features' per-tensor scale            (x_real = x_e4m3 * in_scale)
+ *   w_scale   fp32 [K]  the filter's per-output-channel scale     (W_real[k] = W_e4m3[k] * w_scale[k])
+ *   bias      fp32 [K]  or NULL
+ *   output_add          NULL, or the residual [n_out, K] in out_dtype
+ *   add_scale fp32 [1]  the residual's scale: required for an SPX_E4M3 residual; NULL = 1 otherwise
+ *   out_scale fp32 [1]  required for SPX_E4M3 output, ignored otherwise
+ * The epilogue, the same in the tensor-core and the FMA kernels, is fp32 in registers, one IEEE operation per
+ * step and no fused multiply-add, in this order:
+ *   acc = sum over k, c of x[pair[k][o], c] * W[j, k, c]    fp32 (every product of two e4m3 values is exact)
+ *   s_j = in_scale * w_scale[j]
+ *   y   = acc * s_j;  y = y + bias[j];  y = y + add[o, j] * add_scale;  y = act(y)
+ * out_dtype SPX_F32 stores y, SPX_F16 / SPX_BF16 y rounded once to nearest-even, SPX_E4M3
+ * satfinite_rne(y / out_scale): ties to even, beyond +-448 (and +-Inf) saturates to +-448, NaN stays NaN.
+ * C and K multiples of 32 up to 256 with 16-byte aligned operands run on the tensor cores (wgmma e4m3); every
+ * other shape on the FMA kernel, which gives the same result for the same summation order (the tensor cores
+ * sum a k-step's products in an order of their own).  SPX_FORCE_SIMT / SPX_FORCE_TC apply.
+ */
+typedef struct spx_fp8_gemm {
+    const void *features;       /* e4m3 [n_in, C] */
+    const void *filters;        /* e4m3 [K, kv, C] */
+    const float *in_scale, *w_scale, *bias;
+    const void *output_add;     /* NULL or [n_out, K] in out_dtype */
+    const float *add_scale;
+    void *out;                  /* [n_out, K] in out_dtype */
+    int out_dtype;
+    const float *out_scale;
+    int act;                    /* spx_act */
+    float act_alpha;
+} spx_fp8_gemm;
+int spx_implicit_gemm_fwd_fp8(const spx_gemm_desc *d, const spx_fp8_gemm *a, spx_stream_t stream);
+
+/*
+ * Quantise fp32 / fp16 / bf16 rows x [rows, channels] (spx_dtype dtype) to e4m3 rows out [rows, channels]:
+ *   out = satfinite_rne(x / scale)        rows [0, M), M = *num_valid clamped to [0, rows] (NULL: M = rows)
+ *   out = 0                               rows [M, rows), which are never read
+ * scale_in != NULL: the given device scale (fp32 [1]) is used; scale_out, when not NULL, receives a copy.
+ * scale_in == NULL: dynamic, scale = amax / 448 over rows [0, M) and all channels, NaN and +-Inf left out of
+ *   the amax, 1 when that amax is 0; written to scale_out (required).
+ * NaN stays NaN, +-Inf and values beyond +-448 * scale saturate.  No float atomics and no host read-back:
+ * the output is bit-reproducible.  One launch with a given scale, two when dynamic.
+ * workspace: spx_fp8_quantize_workspace_size(rows, channels) bytes (dynamic mode only; may be NULL otherwise).
+ */
+typedef struct spx_fp8_quant {
+    const void *x;
+    int dtype;
+    int64_t rows;
+    int channels;
+    const int32_t *num_valid;   /* device [1] or NULL */
+    const float *scale_in;      /* device [1], or NULL: dynamic */
+    void *out;                  /* e4m3 [rows, channels] */
+    float *scale_out;           /* device [1] */
+} spx_fp8_quant;
+size_t spx_fp8_quantize_workspace_size(int64_t rows, int channels);
+int spx_fp8_quantize(const spx_fp8_quant *q, void *workspace, size_t workspace_bytes, spx_stream_t stream);
 
 /* which kernel family served the last call of each kind on this thread: 0 none, 1 SIMT,
  * 2 wgmma tensor-core kernels.  Used by tests/bench to prove the tensor-core path ran. */

@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "lib", "libspconv_b200.so")
 
 SPX_MAX_NDIM = 4
-SPX_F32, SPX_F16, SPX_BF16, SPX_I8 = 0, 1, 2, 3
+SPX_F32, SPX_F16, SPX_BF16, SPX_I8, SPX_E4M3 = 0, 1, 2, 3, 4
 SPX_ACT_NONE, SPX_ACT_RELU, SPX_ACT_SIGMOID, SPX_ACT_LEAKY_RELU = 0, 1, 2, 3
 SPX_GN_ACT_NONE, SPX_GN_ACT_RELU, SPX_GN_ACT_SILU = 0, 1, 2
 SPX_F32_EXACT, SPX_F32_TF32 = 0, 1
@@ -110,6 +110,23 @@ class PointInterp(Structure):
     ]
 
 
+class Fp8Gemm(Structure):
+    """``spx_fp8_gemm``: the operands of one fp8 (e4m3) forward."""
+    _fields_ = [
+        ("features", c_void_p), ("filters", c_void_p), ("in_scale", c_void_p), ("w_scale", c_void_p),
+        ("bias", c_void_p), ("output_add", c_void_p), ("add_scale", c_void_p), ("out", c_void_p),
+        ("out_dtype", c_int), ("out_scale", c_void_p), ("act", c_int), ("act_alpha", c_float),
+    ]
+
+
+class Fp8Quant(Structure):
+    """``spx_fp8_quant``: the operands of one e4m3 quantisation."""
+    _fields_ = [
+        ("x", c_void_p), ("dtype", c_int), ("rows", c_int64), ("channels", c_int), ("num_valid", c_void_p),
+        ("scale_in", c_void_p), ("out", c_void_p), ("scale_out", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); also the list the CPU test checks against the header
 SIGNATURES = {
     "spx_last_error": (c_char_p, []),
@@ -174,6 +191,9 @@ SIGNATURES = {
     "spx_implicit_gemm_fwd_int8": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p,
                                            c_int, c_void_p, c_void_p, c_void_p, c_float, c_int,
                                            c_float, c_void_p]),
+    "spx_implicit_gemm_fwd_fp8": (c_int, [POINTER(GemmDesc), POINTER(Fp8Gemm), c_void_p]),
+    "spx_fp8_quantize_workspace_size": (c_size_t, [c_int64, c_int]),
+    "spx_fp8_quantize": (c_int, [POINTER(Fp8Quant), c_void_p, c_size_t, c_void_p]),
     "spx_point2voxel_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_point2voxel_stage1": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, POINTER(c_float), POINTER(c_int),
                                        POINTER(c_float), c_int64, POINTER(c_int64), POINTER(c_int64), c_void_p,

@@ -17,7 +17,7 @@ LIB_DIR = os.path.join(_PKG, "lib")
 OBJ_DIR = os.path.join(_PKG, "lib", "obj")
 LIB_PATH = os.path.join(LIB_DIR, "libspconv_b200.so")
 
-SOURCES = ["core.cu", "rulebook.cu", "sort.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_tc_wgrad.cu", "api_gemm.cu", "pool.cu", "pointops.cu", "peer.cu", "sparse_add.cu", "hash_table.cu", "batchnorm.cu", "global_pool.cu", "point_scatter.cu", "depthwise.cu", "group_norm.cu", "point_interp.cu"]
+SOURCES = ["core.cu", "rulebook.cu", "sort.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_tc_wgrad.cu", "api_gemm.cu", "pool.cu", "pointops.cu", "peer.cu", "sparse_add.cu", "hash_table.cu", "batchnorm.cu", "global_pool.cu", "point_scatter.cu", "depthwise.cu", "group_norm.cu", "point_interp.cu", "fp8.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

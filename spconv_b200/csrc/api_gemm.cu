@@ -190,3 +190,37 @@ extern "C" int spx_implicit_gemm_fwd_int8(const spx_gemm_desc *d, const int8_t *
     set_family(1);
     return simt_gather_gemm_int8(q, (cudaStream_t)stream);
 }
+
+extern "C" int spx_implicit_gemm_fwd_fp8(const spx_gemm_desc *d, const spx_fp8_gemm *a, spx_stream_t stream) {
+    SPX_REQUIRE(a != nullptr, "implicit_gemm_fwd_fp8: argument block is NULL");
+    const void *features = a->features, *filters = a->filters, *output_add = a->output_add;
+    const float *in_scale = a->in_scale, *w_scale = a->w_scale, *bias = a->bias, *add_scale = a->add_scale;
+    const float *out_scale = a->out_scale;
+    void *out = a->out;
+    const int out_dtype = a->out_dtype, act = a->act;
+    const float act_alpha = a->act_alpha;
+    if (check_desc(d, "implicit_gemm_fwd_fp8")) return 2;
+    SPX_REQUIRE(d->dtype == SPX_E4M3, "implicit_gemm_fwd_fp8: descriptor dtype must be SPX_E4M3");
+    SPX_REQUIRE(out_dtype == SPX_E4M3 || out_dtype == SPX_F32 || out_dtype == SPX_F16 || out_dtype == SPX_BF16,
+                "implicit_gemm_fwd_fp8: out dtype %d not supported", out_dtype);
+    SPX_REQUIRE(act >= SPX_ACT_NONE && act <= SPX_ACT_LEAKY_RELU, "implicit_gemm_fwd_fp8: unknown activation %d", act);
+    if (d->n_out == 0) return 0;
+    SPX_REQUIRE(features && filters && out && in_scale && w_scale, "implicit_gemm_fwd_fp8: NULL tensor");
+    SPX_REQUIRE(out_dtype != SPX_E4M3 || out_scale, "implicit_gemm_fwd_fp8: e4m3 output needs out_scale");
+    SPX_REQUIRE(out_dtype != SPX_E4M3 || !output_add || add_scale,
+                "implicit_gemm_fwd_fp8: an e4m3 residual needs add_scale");
+    Fp8Args q;
+    memset(&q, 0, sizeof(q));
+    q.g = make_args(d, false);
+    q.g.x = features; q.g.w = filters; q.g.y = out; q.g.act = act; q.g.alpha = act_alpha;
+    q.out_dtype = out_dtype; q.in_scale = in_scale; q.w_scale = w_scale; q.bias_f32 = bias;
+    q.output_add = output_add; q.add_scale = add_scale; q.out_scale = out_scale;
+    bool tc_ok = !force_simt() && tc_gather_gemm_fp8_supported(q);
+    if (force_tc() && !tc_ok) {
+        set_error("SPX_FORCE_TC=1 but the tensor-core fp8 path does not support C %d, K %d", d->c_in, d->c_out);
+        return 3;
+    }
+    if (tc_ok) { set_family(2); return tc_gather_gemm_fp8(q, (cudaStream_t)stream); }
+    set_family(1);
+    return simt_gather_gemm_fp8(q, (cudaStream_t)stream);
+}

@@ -98,6 +98,7 @@ __host__ __device__ static inline int dtype_bytes(int dt) {
         case SPX_F16: return 2;
         case SPX_BF16: return 2;
         case SPX_I8: return 1;
+        case SPX_E4M3: return 1;
     }
     return 0;
 }
@@ -213,7 +214,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const void *tmap) {
 }
 
 // ---- wgmma (Hopper warpgroup MMA; the instruction wrappers are in wgmma.cuh)
-enum MmaKind { KIND_F16 = 0, KIND_TF32 = 1, KIND_I8 = 2 };
+enum MmaKind { KIND_F16 = 0, KIND_TF32 = 1, KIND_I8 = 2, KIND_E4M3 = 3 };
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

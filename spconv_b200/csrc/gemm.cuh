@@ -2,6 +2,7 @@
 // (gemm_simt.cu: generic fp32-FMA kernels; gemm_tc.cu: tcgen05 / TMEM / TMA kernels).
 #pragma once
 #include "common.cuh"
+#include <cuda_fp8.h>
 
 namespace spx {
 
@@ -75,5 +76,47 @@ struct Int8Args {
 int simt_gather_gemm_int8(const Int8Args &a, cudaStream_t stream);
 bool tc_gather_gemm_int8_supported(const Int8Args &a);
 int tc_gather_gemm_int8(const Int8Args &a, cudaStream_t stream);
+
+// FP8 (e4m3) inference forward: the epilogue of include/spconv_b200.h (spx_implicit_gemm_fwd_fp8)
+struct Fp8Args {
+    GatherGemmArgs g;          // dtype = SPX_E4M3; bias field unused
+    int out_dtype;             // SPX_F32 / SPX_F16 / SPX_BF16 / SPX_E4M3
+    const float *in_scale, *w_scale, *bias_f32, *add_scale, *out_scale;
+    const void *output_add;    // [rows, c_out] in out_dtype, or NULL
+};
+int simt_gather_gemm_fp8(const Fp8Args &a, cudaStream_t stream);
+bool tc_gather_gemm_fp8_supported(const Fp8Args &a);
+int tc_gather_gemm_fp8(const Fp8Args &a, cudaStream_t stream);
+
+#ifdef __CUDACC__
+// ---- the fp8 epilogue, shared by the tensor-core and FMA kernels.  One IEEE fp32 operation per step (the
+// explicit _rn intrinsics keep the compiler from fusing them), in this order:
+//   y = acc * s;  y = y + bias;  y = y + add * add_scale;  y = act(y)        s = in_scale * w_scale[j]
+__device__ __forceinline__ float fp8_epilogue(float acc, float s, const float *bias, int j, bool has_add, float add,
+                                              float add_scale, int act, float alpha) {
+    float y = __fmul_rn(acc, s);
+    if (bias) y = __fadd_rn(y, bias[j]);
+    if (has_add) y = __fadd_rn(y, __fmul_rn(add, add_scale));
+    return apply_act(y, act, alpha);
+}
+// e4m3 byte -> float (exact)
+__device__ __forceinline__ float e4m3_to_float(uint8_t v) {
+    return __half2float(__half(__nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)v, __NV_E4M3)));
+}
+// two floats -> two e4m3 bytes (a in the low byte): cvt.rn.satfinite.e4m3x2.f32
+__device__ __forceinline__ uint16_t float2_to_e4m3x2(float a, float b) {
+    return (uint16_t)__nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+}
+__device__ __forceinline__ uint8_t float_to_e4m3(float a) {
+    return (uint8_t)__nv_cvt_float_to_fp8(a, __NV_SATFINITE, __NV_E4M3);
+}
+// one element of a row of out_dtype (OUT, an spx_dtype code) as float
+template <int OUT> __device__ __forceinline__ float load_out_elem(const void *p, int64_t i) {
+    if constexpr (OUT == SPX_F32) return ((const float *)p)[i];
+    else if constexpr (OUT == SPX_F16) return __half2float(((const __half *)p)[i]);
+    else if constexpr (OUT == SPX_BF16) return __bfloat162float(((const __nv_bfloat16 *)p)[i]);
+    else return e4m3_to_float(((const uint8_t *)p)[i]);
+}
+#endif
 
 }  // namespace spx

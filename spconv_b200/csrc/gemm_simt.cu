@@ -1,5 +1,5 @@
 // Generic fp32-FMA kernels for the gather-GEMM-scatter path: any channel counts, any of
-// fp32 / fp16 / bf16 / int8, fp32 (int32 for int8) accumulation.
+// fp32 / fp16 / bf16 / int8 / e4m3, fp32 (int32 for int8) accumulation.
 //
 // These serve (a) exact fp32 arithmetic, the reference default for fp32 tensors
 // (SPCONV_ALLOW_TF32=False, spconv/constants.py:117), and (b) layer shapes the tcgen05
@@ -22,9 +22,12 @@ template <> struct AccT<int8_t> { typedef int type; };
 
 template <typename T> __device__ __forceinline__ typename AccT<T>::type load_acc(const T *p) { return to_float(*p); }
 template <> __device__ __forceinline__ int load_acc<int8_t>(const int8_t *p) { return (int)*p; }
+template <> __device__ __forceinline__ float load_acc<__nv_fp8_e4m3>(const __nv_fp8_e4m3 *p) {
+    return e4m3_to_float(p->__x);
+}
 
 struct SimtEpilogue {   // float path: bias+act ; int8 path: scale/bias/add/act/round
-    int mode;           // 0 float, 1 int8
+    int mode;           // 0 float, 1 int8, 2 fp8
     const void *bias;
     int act;
     float alpha;
@@ -32,7 +35,30 @@ struct SimtEpilogue {   // float path: bias+act ; int8 path: scale/bias/add/act/
     const int8_t *output_add;
     float output_add_scale;
     int out_dtype;
+    // fp8 (T = __nv_fp8_e4m3): scale = w_scale, bias_f32 = bias; the residual in out_dtype
+    const float *in_scale, *add_scale, *out_scale;
+    const void *add;
 };
+
+// the fp8 epilogue (gemm.cuh fp8_epilogue) of one thread's 8 columns y0.. of output row dst, stored as out_dtype
+template <int OUT>
+__device__ __forceinline__ void simt_fp8_cols(const SimtEpilogue &ep, void *y, const float (&acc)[8], int64_t dst, int y0,
+                                           int cy) {
+    const float add_s = ep.add_scale ? *ep.add_scale : 1.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int col = y0 + j;
+        if (col >= cy) continue;
+        const int64_t o = dst * cy + col;
+        const float s = __fmul_rn(*ep.in_scale, ep.scale[col]);      // s_j = in_scale * w_scale[j]
+        const float a = ep.add ? load_out_elem<OUT>(ep.add, o) : 0.f;
+        const float v = fp8_epilogue(acc[j], s, ep.bias_f32, col, ep.add != nullptr, a, add_s, ep.act, ep.alpha);
+        if constexpr (OUT == SPX_E4M3) ((uint8_t *)y)[o] = float_to_e4m3(__fdiv_rn(v, *ep.out_scale));
+        else if constexpr (OUT == SPX_F32) ((float *)y)[o] = v;
+        else if constexpr (OUT == SPX_F16) ((__half *)y)[o] = __float2half_rn(v);
+        else ((__nv_bfloat16 *)y)[o] = __float2bfloat16_rn(v);
+    }
+}
 
 template <typename T>
 __global__ void __launch_bounds__(S_THREADS)
@@ -116,7 +142,16 @@ simt_gather_gemm_kernel(GatherGemmArgs a, SimtEpilogue ep) {
             }
         }
         int32_t dst = row_src[trow];
-        if (dst >= 0) {
+        if constexpr (std::is_same<T, __nv_fp8_e4m3>::value) {
+            if (dst >= 0) {
+                switch (ep.out_dtype) {
+                    case SPX_E4M3: simt_fp8_cols<SPX_E4M3>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
+                    case SPX_F32: simt_fp8_cols<SPX_F32>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
+                    case SPX_F16: simt_fp8_cols<SPX_F16>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
+                    default: simt_fp8_cols<SPX_BF16>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
+                }
+            }
+        } else if (dst >= 0) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 int y = n0 + tcg * 8 + j;
@@ -175,6 +210,15 @@ int simt_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
     ep.scale = q.scale; ep.bias_f32 = q.bias_f32; ep.output_add = q.output_add;
     ep.output_add_scale = q.output_add_scale; ep.out_dtype = q.out_dtype;
     return launch_simt<int8_t>(q.g, ep, stream);
+}
+
+int simt_gather_gemm_fp8(const Fp8Args &q, cudaStream_t stream) {
+    SimtEpilogue ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.mode = 2; ep.act = q.g.act; ep.alpha = q.g.alpha; ep.out_dtype = q.out_dtype;
+    ep.scale = q.w_scale; ep.bias_f32 = q.bias_f32; ep.in_scale = q.in_scale;
+    ep.add = q.output_add; ep.add_scale = q.add_scale; ep.out_scale = q.out_scale;
+    return launch_simt<__nv_fp8_e4m3>(q.g, ep, stream);
 }
 
 // ------------------------------------------------------------------ weight gradient

@@ -1,4 +1,4 @@
-// wgmma / TMA masked implicit GEMM: forward and input-gradient (and int8 forward).
+// wgmma / TMA masked implicit GEMM: forward and input-gradient (and the int8 and fp8 inference forwards).
 //
 // Persistent CTAs (one per SM) work on 128-row output tiles (rows in mask_argsort order).  Tiles
 // are handed out DYNAMICALLY: a scheduler warp draws tickets from an atomic counter and takes
@@ -76,12 +76,14 @@ struct TcParams {
     // epilogue
     void *y;
     int out_dtype;          // spx_dtype of y
-    int epi_mode;           // 0: float bias+act, 1: int8 quantised inference
+    int epi_mode;           // 0: float bias+act, 1: int8 quantised inference, 2: fp8 inference
     const void *bias;       // dtype of y (mode 0)
     int act; float alpha;
     const float *scale, *bias_f32;
     const int8_t *output_add;
     float output_add_scale;
+    // fp8 epilogue (KIND_E4M3): scale = w_scale, bias_f32 = bias, output_add = the residual in out_dtype
+    const float *in_scale, *add_scale, *out_scale;
 };
 
 // iterate set bits of a <=128-bit tile mask in ascending order (register-only: no indexed array)
@@ -167,6 +169,37 @@ __device__ __forceinline__ void epilogue_frag(const TcParams &p, const float *ec
     }
 }
 
+// The fp8 epilogue (gemm.cuh fp8_epilogue) of one warpgroup fragment, same layout as epilogue_frag.  ec[j] = s_j,
+// ec[N + j] = bias.  add_s / out_s: the residual and output scales, read once per tile.
+template <int OUT, int N>
+__device__ __forceinline__ void epilogue_fp8(const TcParams &p, const float *ec, const float (&acc)[N / 2],
+                                             int64_t dst_lo, int64_t dst_hi, int lane, float add_s, float out_s) {
+    constexpr int EB = OUT == SPX_F32 ? 4 : (OUT == SPX_E4M3 ? 1 : 2);
+    const float *bias = p.bias_f32 ? ec + N : nullptr;
+    const void *add = (const void *)p.output_add;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int64_t dst = h ? dst_hi : dst_lo;
+        if (dst < 0) continue;
+        uint8_t *row_ptr = (uint8_t *)p.y + dst * (int64_t)N * EB;
+#pragma unroll
+        for (int nb = 0; nb < N / 8; ++nb) {
+            const int col = nb * 8 + 2 * (lane & 3);
+            float f[2];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const float a = add ? load_out_elem<OUT>(add, dst * (int64_t)N + col + j) : 0.f;
+                f[j] = fp8_epilogue(acc[nb * 4 + 2 * h + j], ec[col + j], bias, col + j, add != nullptr, a, add_s,
+                                    p.act, p.alpha);
+            }
+            if constexpr (OUT == SPX_E4M3)
+                *reinterpret_cast<uint16_t *>(row_ptr + col) = float2_to_e4m3x2(__fdiv_rn(f[0], out_s), __fdiv_rn(f[1], out_s));
+            else
+                store2<OUT>(row_ptr + col * EB, f[0], f[1]);
+        }
+    }
+}
+
 // one K step of 32 bytes: D[64 x N] += A[64 x 32 B] * B[N x 32 B]^T
 template <int KIND, int N, typename Acc>
 __device__ __forceinline__ void mma_step(Acc (&acc)[N / 2], uint64_t a, uint64_t b, int b_mn, int bf16) {
@@ -180,14 +213,16 @@ __device__ __forceinline__ void mma_step(Acc (&acc)[N / 2], uint64_t a, uint64_t
         }
     } else if constexpr (KIND == KIND_TF32) {
         Wgmma<N>::tf32(acc, a, b, 1u);
-    } else {
+    } else if constexpr (KIND == KIND_I8) {
         Wgmma<N>::s8(acc, a, b, 1u);
+    } else {
+        Wgmma<N>::e4m3(acc, a, b, 1u);
     }
 }
 
+// The kernel body; tc_gather_gemm_kernel (16-bit, tf32, int8) and tc_gather_gemm_fp8_kernel (e4m3) launch it.
 template <int KIND, int CPR, int N>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams p) {
+__device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, const TcParams &p) {
     using Acc = typename std::conditional<KIND == KIND_I8, int32_t, float>::type;
     constexpr int LG_CPR = CPR == 2 ? 1 : CPR == 4 ? 2 : CPR == 8 ? 3 : CPR == 16 ? 4 : 5;
     constexpr int RPI = 32 / CPR;            // rows covered by one warp-wide cp.async instruction
@@ -258,6 +293,9 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
     for (int j = threadIdx.x; j < N; j += TC_THREADS) {
         if constexpr (KIND == KIND_I8) {
             ec[j] = __ldg(p.scale + j);
+            if (p.bias_f32) ec[N + j] = __ldg(p.bias_f32 + j);
+        } else if constexpr (KIND == KIND_E4M3) {
+            ec[j] = __fmul_rn(__ldg(p.in_scale), __ldg(p.scale + j));     // s_j = in_scale * w_scale[j]
             if (p.bias_f32) ec[N + j] = __ldg(p.bias_f32 + j);
         } else if (p.bias) {
             if constexpr (KIND == KIND_TF32) ec[j] = load_bias<SPX_F32>(p.bias, j);
@@ -486,15 +524,34 @@ tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams
                 else epilogue_frag<SPX_BF16, false, N>(p, ec, acc, d_lo, d_hi, lane);
             } else if constexpr (KIND == KIND_TF32) {
                 epilogue_frag<SPX_F32, false, N>(p, ec, acc, d_lo, d_hi, lane);
-            } else {
+            } else if constexpr (KIND == KIND_I8) {
                 if (p.out_dtype == SPX_I8) epilogue_frag<SPX_I8, true, N>(p, ec, acc, d_lo, d_hi, lane);
                 else if (p.out_dtype == SPX_F32) epilogue_frag<SPX_F32, true, N>(p, ec, acc, d_lo, d_hi, lane);
                 else epilogue_frag<SPX_F16, true, N>(p, ec, acc, d_lo, d_hi, lane);
+            } else {
+                const float add_s = p.add_scale ? __ldg(p.add_scale) : 1.f;
+                const float out_s = p.out_dtype == SPX_E4M3 ? __ldg(p.out_scale) : 1.f;
+                if (p.out_dtype == SPX_E4M3) epilogue_fp8<SPX_E4M3, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
+                else if (p.out_dtype == SPX_F32) epilogue_fp8<SPX_F32, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
+                else if (p.out_dtype == SPX_F16) epilogue_fp8<SPX_F16, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
+                else epilogue_fp8<SPX_BF16, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
             }
         }
     }
 
     __syncthreads();
+}
+
+template <int KIND, int CPR, int N>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_gather_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams p) {
+    tc_gather_gemm_body<KIND, CPR, N>(tmap_w, p);
+}
+
+template <int CPR, int N>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_gather_gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams p) {
+    tc_gather_gemm_body<KIND_E4M3, CPR, N>(tmap_w, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -550,7 +607,7 @@ static bool tc_shape_ok(int dtype, int kv, int c_in, int c_out, int transpose_w)
     const int cy = transpose_w ? c_in : c_out;
     if (cy % 16 || cy > 256) return false;
     const int xb = (transpose_w ? c_out : c_in) * e;
-    if (dtype == SPX_I8 && (c_in % 32 || c_out % 32)) return false;   // docs/INT8_GUIDE.md:10
+    if ((dtype == SPX_I8 || dtype == SPX_E4M3) && (c_in % 32 || c_out % 32)) return false;   // docs/INT8_GUIDE.md:10; wgmma e4m3: K = 32
     size_t stage = align_up((size_t)TC_TILE_M * xb, 1024) + align_up((size_t)c_in * c_out * e, 1024);
     const size_t idx = align_up((size_t)(kv + 1) * 512, 1024);
     if (2 * idx + 2 * stage > (size_t)TC_SMEM_BUDGET) return false;
@@ -578,6 +635,13 @@ bool tc_gather_gemm_int8_supported(const Int8Args &q) {
     if (!tc_operands_aligned(q.g)) return false;
     if (((size_t)q.g.kv * q.g.c_in) % 16) return false;
     return tc_shape_ok(SPX_I8, q.g.kv, q.g.c_in, q.g.c_out, 0);
+}
+
+bool tc_gather_gemm_fp8_supported(const Fp8Args &q) {
+    if (!q.g.tile_table || !q.g.tile_mask) return false;
+    if (!tc_operands_aligned(q.g)) return false;
+    if (((size_t)q.g.kv * q.g.c_in) % 16) return false;
+    return tc_shape_ok(SPX_E4M3, q.g.kv, q.g.c_in, q.g.c_out, 0);
 }
 
 static int fill_params(const GatherGemmArgs &a, TcParams &p) {
@@ -634,29 +698,32 @@ static int fill_params(const GatherGemmArgs &a, TcParams &p) {
 
 template <int KIND, int CPR, int N>
 static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
+    void (*kernel)(const CUtensorMap, const TcParams);
+    if constexpr (KIND == KIND_E4M3) kernel = tc_gather_gemm_fp8_kernel<CPR, N>;
+    else kernel = tc_gather_gemm_kernel<KIND, CPR, N>;
     const size_t smem = (size_t)p.stages * p.stage_bytes + 2 * (size_t)p.idx_bytes + 1024 /*align slack*/ + 1024 /*barriers, tile-info ring*/ +
                         2 * N * sizeof(float) /*epilogue constants*/;
     // the opt-in is a per-DEVICE attribute: one process may drive several GPUs
-    if (!func_configured((const void *)tc_gather_gemm_kernel<KIND, CPR, N>, current_device())) {
-        SPX_CHECK_CUDA(cudaFuncSetAttribute(tc_gather_gemm_kernel<KIND, CPR, N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    if (!func_configured((const void *)kernel, current_device())) {
+        SPX_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)(TC_SMEM_BUDGET + 2048 + 2 * N * sizeof(float))));
-        SPX_CHECK_CUDA(cudaFuncSetAttribute(tc_gather_gemm_kernel<KIND, CPR, N>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+        SPX_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
     }
     const int64_t tiles = div_up64(p.rows, TC_TILE_M);
     const int64_t max_ctas = (int64_t)sm_count();
     const int grid = (int)(tiles < max_ctas ? tiles : max_ctas);
-    tc_gather_gemm_kernel<KIND, CPR, N><<<grid, TC_THREADS, smem, stream>>>(tm, p);
-    SPX_CHECK_LAUNCH("tc_gather_gemm_kernel");
+    kernel<<<grid, TC_THREADS, smem, stream>>>(tm, p);
+    SPX_CHECK_LAUNCH(KIND == KIND_E4M3 ? "tc_gather_gemm_fp8_kernel" : "tc_gather_gemm_kernel");
     return 0;
 }
 
 // instantiated (channels x element bytes) combinations: rows of 32..512 bytes, N = 16..256 output
-// channels (tf32: 16..128, int8: 32..256).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
+// channels (tf32: 16..128, int8 and e4m3: 32..256).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
 // gathered tile plus a weight slice of 128 or more rows puts two stages over TC_SMEM_BUDGET.
 template <int KIND, int CPR>
 static int launch_tc_cpr(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
     switch (p.n) {
-        case 16: if constexpr (KIND != KIND_I8) return launch_tc_n<KIND, CPR, 16>(tm, p, stream); break;
+        case 16: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_n<KIND, CPR, 16>(tm, p, stream); break;
         case 32: return launch_tc_n<KIND, CPR, 32>(tm, p, stream);
         case 64: return launch_tc_n<KIND, CPR, 64>(tm, p, stream);
         case 128: if constexpr (CPR != 32) return launch_tc_n<KIND, CPR, 128>(tm, p, stream); break;
@@ -673,7 +740,7 @@ static int launch_tc(const CUtensorMap &tm, const TcParams &p, cudaStream_t stre
         case 4: return launch_tc_cpr<KIND, 4>(tm, p, stream);
         case 8: return launch_tc_cpr<KIND, 8>(tm, p, stream);
         case 16: return launch_tc_cpr<KIND, 16>(tm, p, stream);
-        case 32: if constexpr (KIND != KIND_I8) return launch_tc_cpr<KIND, 32>(tm, p, stream); break;
+        case 32: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_cpr<KIND, 32>(tm, p, stream); break;
     }
     set_error("tc_gather_gemm: unsupported row bytes %d", p.xb);
     return 2;
@@ -698,6 +765,19 @@ int tc_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
     CUtensorMap tm;
     if (make_weight_tmap(&tm, q.g.w, SPX_I8, q.g.kv, q.g.c_in, q.g.c_out, p.span_b)) return 2;
     return launch_tc<KIND_I8>(tm, p, stream);
+}
+
+// e4m3 operands take the int8 operand path (1-byte K-major rows, UINT8 tensor map) with fp32 accumulators
+int tc_gather_gemm_fp8(const Fp8Args &q, cudaStream_t stream) {
+    TcParams p;
+    if (fill_params(q.g, p)) return 2;
+    p.out_dtype = q.out_dtype;
+    p.epi_mode = 2;
+    p.scale = q.w_scale; p.bias_f32 = q.bias_f32; p.output_add = (const int8_t *)q.output_add;
+    p.in_scale = q.in_scale; p.add_scale = q.add_scale; p.out_scale = q.out_scale;
+    CUtensorMap tm;
+    if (make_weight_tmap(&tm, q.g.w, SPX_E4M3, q.g.kv, q.g.c_in, q.g.c_out, p.span_b)) return 2;
+    return launch_tc<KIND_E4M3>(tm, p, stream);
 }
 
 }  // namespace spx

@@ -20,6 +20,8 @@ from .tables import (AddTable, ConcatTable, JoinTable, MaskedAddTable, MaskedAdd
 from .spatial import MaskedRemoveDuplicate  # noqa: F401
 from .utils_fuse import (fuse_act, fuse_bn, fuse_bn_act_sequential, fuse_bn_weights)  # noqa: F401
 from . import quantized  # noqa: F401
+from .fp8 import (Fp8SparseConv, calibrate_fp8_output_scale, convert_to_fp8, dequantize_fp8,  # noqa: F401
+                  quantize_fp8, quantize_fp8_weight)
 from .graph import GraphedStep, graph_capture  # noqa: F401
 from .utils import (MaskedPointToVoxel, PointToVoxel, PointVoxelScatter, VoxelPointInterpolator,  # noqa: F401
                     gather_features_by_pc_voxel_id, grid_positions)

@@ -253,51 +253,25 @@ class SparseConvolution(SparseModule):
               f"dilation={self.dilation},subm={self.subm},transpose={self.transposed}",
               file=sys.stderr)
 
-    def _conv_forward(self, training: bool, input: SparseConvTensor, weight: torch.Tensor,
-                      bias: Optional[torch.Tensor], add_input: Optional[SparseConvTensor] = None,
-                      channel_scale: Optional[torch.Tensor] = None,
-                      output_scale: Optional[float] = None, name: Optional[str] = None,
-                      sparse_unique_name: str = "", act_type: Activation = Activation.None_,
-                      act_alpha: float = 0, act_beta: float = 0):
-        assert isinstance(input, SparseConvTensor)
-        assert input.features.shape[1] == self.in_channels, "channel size mismatch"
-        if training:
-            assert self.act_type == Activation.None_, \
-                "act don't support backward, only used in inference"
-        features = input.features
+    def _rulebook(self, input: SparseConvTensor, training: bool, algo: ConvAlgo, out_tensor: SparseConvTensor):
+        """This layer's rulebook on ``input``: taken from ``input.indice_dict`` under ``indice_key`` (SubM reuse,
+        a prefetched strided rulebook, or the paired conv's rulebook walked backwards by an inverse conv) or built
+        and registered there.  Returns ``(rb, indice_dict, out_spatial_shape, num_valid)`` with ``rb`` =
+        ``(outids, indice_pairs, indice_pair_num)`` for ConvAlgo.Native and ``(outids, pair_fwd, pair_bwd,
+        mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks)`` for the implicit-GEMM algos.  A bounded rulebook's
+        status word joins ``out_tensor.bound_status``.  The float and the fp8 convs share it."""
         indices = input.indices
         spatial_shape = input.spatial_shape
         batch_size = input.batch_size
-        # training: bias is added outside the op (it needs its own gradient);
-        # inference: bias and activation ride in the kernel epilogue
-        bias_train = bias if training else None
-        bias_infer = None if training else bias
+        timer = input._timer
         out_spatial_shape = self._out_spatial_shape(spatial_shape)
-        out_tensor = input.shadow_copy()
         # SubM inherits the padding of its input; strided and inverse layers set it below
         num_valid = input.num_valid
-
-        if self.conv1x1:
-            if self.depthwise:
-                feats = features * weight.view(self.out_channels)
-            else:
-                w2d = weight.view(self.out_channels, self.in_channels)
-                feats = torch.mm(features, w2d.t())
-            if bias is not None:
-                feats = feats + bias
-            out_tensor = out_tensor.replace_feature(feats)
-            out_tensor.spatial_shape = out_spatial_shape
-            return out_tensor
-
         indice_dict = input.indice_dict.copy()
-        if not features.is_contiguous():
-            features = features.contiguous()
-        algo = self.algo if input.force_algo is None else input.force_algo
         datas = input.find_indice_pair(self.indice_key)
         if datas is not None:
             assert algo == datas.algo, ("due to limitation of pytorch, you must provide same algo "
                                         "to layers share same indice key.")
-        timer = input._timer
 
         if algo == ConvAlgo.Native:
             if datas is not None:
@@ -331,8 +305,104 @@ class SparseConvolution(SparseModule):
                         outids, indices, indice_pairs, indice_pair_num, spatial_shape,
                         out_spatial_shape, is_subm=self.subm, algo=algo, ksize=self.kernel_size,
                         stride=self.stride, padding=self.padding, dilation=self.dilation)
-            if indice_pairs.device != features.device:
-                indice_pairs = indice_pairs.to(features.device)
+            if indice_pairs.device != input.features.device:
+                indice_pairs = indice_pairs.to(input.features.device)
+            return (outids, indice_pairs, indice_pair_num), indice_dict, out_spatial_shape, num_valid
+        if datas is not None:
+            assert isinstance(datas, ImplicitGemmIndiceData)
+        if self.inverse:
+            assert datas is not None and self.indice_key is not None
+            assert datas.is_subm is False, \
+                "inverse conv can only be used with standard conv and pool ops."
+            # the inverse conv walks the paired conv's rulebook backwards
+            outids = datas.indices
+            num_valid = datas.in_voxel_num
+            pair_fwd, pair_bwd = datas.pair_bwd, datas.pair_fwd
+            mask_fwd, mask_bwd = datas.pair_mask_bwd_splits, datas.pair_mask_fwd_splits
+            sort_fwd, sort_bwd = datas.mask_argsort_bwd_splits, datas.mask_argsort_fwd_splits
+            masks = datas.masks
+            out_spatial_shape = datas.spatial_shape
+            self._check_inverse_reuse_valid(input, spatial_shape, datas)
+        elif self.indice_key is not None and datas is not None:
+            outids = datas.out_indices
+            pair_fwd, pair_bwd = datas.pair_fwd, datas.pair_bwd
+            mask_fwd, mask_bwd = datas.pair_mask_fwd_splits, datas.pair_mask_bwd_splits
+            sort_fwd, sort_bwd = datas.mask_argsort_fwd_splits, datas.mask_argsort_bwd_splits
+            masks = datas.masks
+            if self.subm:
+                self._check_subm_reuse_valid(input, spatial_shape, datas)
+            else:
+                self._check_prefetched_valid(input, datas)
+                num_valid = datas.out_voxel_num
+        else:
+            with timer.namespace("gen_pairs"):
+                try:
+                    # regular convs always build the backward table: an inverse conv may
+                    # consume it later
+                    res = ops.get_indice_pairs_implicit_gemm(
+                        indices, batch_size, spatial_shape, algo, ksize=self.kernel_size,
+                        stride=self.stride, padding=self.padding, dilation=self.dilation,
+                        out_padding=self.output_padding, subm=self.subm,
+                        transpose=self.transposed, is_train=(not self.subm) or training,
+                        alloc=input.thrust_allocator, timer=timer,
+                        num_out_act_bound=self.num_out_act_bound if self._bounded(algo) else -1,
+                        bound_status=self._status_word(indices.device) if self._bounded(algo) else None)
+                except Exception:
+                    self._rulebook_error("implicit_gemm_pair", indices, batch_size,
+                                         spatial_shape, algo)
+                    raise
+            (outids, _num_per_loc, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd,
+             masks) = res
+            num_valid = rulebook_num_valid(outids, input, out_tensor, self.subm, self)
+            if self.indice_key is not None:
+                assert self.indice_key not in indice_dict, \
+                    f"your indice key {self.indice_key} already exists in this sparse tensor."
+                indice_dict[self.indice_key] = ImplicitGemmIndiceData.from_rulebook(
+                    res, indices, input.num_valid, self.subm, spatial_shape=spatial_shape,
+                    out_spatial_shape=out_spatial_shape, algo=algo, ksize=self.kernel_size,
+                    stride=self.stride, dilation=self.dilation, padding=self.padding)
+        return ((outids, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks), indice_dict,
+                out_spatial_shape, num_valid)
+
+    def _conv_forward(self, training: bool, input: SparseConvTensor, weight: torch.Tensor,
+                      bias: Optional[torch.Tensor], add_input: Optional[SparseConvTensor] = None,
+                      channel_scale: Optional[torch.Tensor] = None,
+                      output_scale: Optional[float] = None, name: Optional[str] = None,
+                      sparse_unique_name: str = "", act_type: Activation = Activation.None_,
+                      act_alpha: float = 0, act_beta: float = 0):
+        assert isinstance(input, SparseConvTensor)
+        assert input.features.shape[1] == self.in_channels, "channel size mismatch"
+        if training:
+            assert self.act_type == Activation.None_, \
+                "act don't support backward, only used in inference"
+        features = input.features
+        # training: bias is added outside the op (it needs its own gradient);
+        # inference: bias and activation ride in the kernel epilogue
+        bias_train = bias if training else None
+        bias_infer = None if training else bias
+        out_spatial_shape = self._out_spatial_shape(input.spatial_shape)
+        out_tensor = input.shadow_copy()
+
+        if self.conv1x1:
+            if self.depthwise:
+                feats = features * weight.view(self.out_channels)
+            else:
+                w2d = weight.view(self.out_channels, self.in_channels)
+                feats = torch.mm(features, w2d.t())
+            if bias is not None:
+                feats = feats + bias
+            out_tensor = out_tensor.replace_feature(feats)
+            out_tensor.spatial_shape = out_spatial_shape
+            return out_tensor
+
+        if not features.is_contiguous():
+            features = features.contiguous()
+        algo = self.algo if input.force_algo is None else input.force_algo
+        timer = input._timer
+        rb, indice_dict, out_spatial_shape, num_valid = self._rulebook(input, training, algo, out_tensor)
+
+        if algo == ConvAlgo.Native:
+            outids, indice_pairs, indice_pair_num = rb
             if self.depthwise:
                 out_features = self._depthwise_native(features, weight, indice_pairs, indice_pair_num,
                                                       outids.shape[0], timer, bias_infer, act_alpha, act_type)
@@ -343,59 +413,7 @@ class SparseConvolution(SparseModule):
                                        outids.shape[0], algo, timer, bias_infer, act_alpha, act_beta,
                                        act_type)
         else:
-            if datas is not None:
-                assert isinstance(datas, ImplicitGemmIndiceData)
-            if self.inverse:
-                assert datas is not None and self.indice_key is not None
-                assert datas.is_subm is False, \
-                    "inverse conv can only be used with standard conv and pool ops."
-                # the inverse conv walks the paired conv's rulebook backwards
-                outids = datas.indices
-                num_valid = datas.in_voxel_num
-                pair_fwd, pair_bwd = datas.pair_bwd, datas.pair_fwd
-                mask_fwd, mask_bwd = datas.pair_mask_bwd_splits, datas.pair_mask_fwd_splits
-                sort_fwd, sort_bwd = datas.mask_argsort_bwd_splits, datas.mask_argsort_fwd_splits
-                masks = datas.masks
-                out_spatial_shape = datas.spatial_shape
-                self._check_inverse_reuse_valid(input, spatial_shape, datas)
-            elif self.indice_key is not None and datas is not None:
-                outids = datas.out_indices
-                pair_fwd, pair_bwd = datas.pair_fwd, datas.pair_bwd
-                mask_fwd, mask_bwd = datas.pair_mask_fwd_splits, datas.pair_mask_bwd_splits
-                sort_fwd, sort_bwd = datas.mask_argsort_fwd_splits, datas.mask_argsort_bwd_splits
-                masks = datas.masks
-                if self.subm:
-                    self._check_subm_reuse_valid(input, spatial_shape, datas)
-                else:
-                    self._check_prefetched_valid(input, datas)
-                    num_valid = datas.out_voxel_num
-            else:
-                with timer.namespace("gen_pairs"):
-                    try:
-                        # regular convs always build the backward table: an inverse conv may
-                        # consume it later
-                        res = ops.get_indice_pairs_implicit_gemm(
-                            indices, batch_size, spatial_shape, algo, ksize=self.kernel_size,
-                            stride=self.stride, padding=self.padding, dilation=self.dilation,
-                            out_padding=self.output_padding, subm=self.subm,
-                            transpose=self.transposed, is_train=(not self.subm) or training,
-                            alloc=input.thrust_allocator, timer=timer,
-                            num_out_act_bound=self.num_out_act_bound if self._bounded(algo) else -1,
-                            bound_status=self._status_word(indices.device) if self._bounded(algo) else None)
-                    except Exception:
-                        self._rulebook_error("implicit_gemm_pair", indices, batch_size,
-                                             spatial_shape, algo)
-                        raise
-                (outids, _num_per_loc, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd,
-                 masks) = res
-                num_valid = rulebook_num_valid(outids, input, out_tensor, self.subm, self)
-                if self.indice_key is not None:
-                    assert self.indice_key not in indice_dict, \
-                        f"your indice key {self.indice_key} already exists in this sparse tensor."
-                    indice_dict[self.indice_key] = ImplicitGemmIndiceData.from_rulebook(
-                        res, indices, input.num_valid, self.subm, spatial_shape=spatial_shape,
-                        out_spatial_shape=out_spatial_shape, algo=algo, ksize=self.kernel_size,
-                        stride=self.stride, dilation=self.dilation, padding=self.padding)
+            outids, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = rb
             num_activate_out = outids.shape[0]
             if self.depthwise:
                 # the whole dense table is walked: no tile table, mask sort or split is needed.  SubM (whose

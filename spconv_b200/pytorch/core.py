@@ -195,7 +195,7 @@ class SparseConvTensor:
 
     # attributes copied verbatim whenever a tensor is re-wrapped
     _CARRIED = ("benchmark", "benchmark_record", "thrust_allocator", "_timer", "force_algo",
-                "int8_scale")
+                "int8_scale", "fp8_scale")
 
     def __init__(self, features: torch.Tensor, indices: torch.Tensor,
                  spatial_shape: Union[List[int], np.ndarray], batch_size: int,
@@ -223,6 +223,8 @@ class SparseConvTensor:
         self._timer = CUDAKernelTimer(enable_timer)
         self.force_algo = force_algo
         self.int8_scale: Optional[np.ndarray] = None
+        # float8_e4m3fn features: the per-tensor device scale (fp32 [1]), real value = e4m3 * fp8_scale
+        self.fp8_scale: Optional[torch.Tensor] = None
         # padded tensors (bounded rulebooks, pad_to): device int32 [1] = number of valid rows, rows beyond it
         # are padding (indices -1); None = every row is valid.  bound_status: {layer name: status word} of the
         # bounded layers the tensor went through (spconv.check_bounds)

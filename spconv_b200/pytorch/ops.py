@@ -35,6 +35,7 @@ _DTYPE_CODE = {
     torch.float16: _cabi.SPX_F16,
     torch.bfloat16: _cabi.SPX_BF16,
     torch.int8: _cabi.SPX_I8,
+    torch.float8_e4m3fn: _cabi.SPX_E4M3,
 }
 
 
@@ -507,10 +508,17 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
                   act_alpha: float = 0.0, act_beta: float = 0.0,
                   act_type=Activation.None_, output_scale: float = 1.0,
                   scale: Optional[torch.Tensor] = None, output_add: Optional[torch.Tensor] = None,
-                  output_add_scale: float = 0.0, output_dtype: Optional[torch.dtype] = None):
+                  output_add_scale: float = 0.0, output_dtype: Optional[torch.dtype] = None,
+                  in_scale: Optional[torch.Tensor] = None, out_scale: Optional[torch.Tensor] = None,
+                  add_scale: Optional[torch.Tensor] = None):
     """Forward masked implicit GEMM -> ``(out [M, K], mask_output_fwd, mask_width)``
     (``ops.py:1450-1469`` / ``convops.py:2075-2243``).  Accumulation is always fp32 in registers
-    (``fp32_accum`` is accepted and ignored)."""
+    (``fp32_accum`` is accepted and ignored).
+
+    ``torch.float8_e4m3fn`` features and filters run ``spx_implicit_gemm_fwd_fp8``: ``scale`` is the filter's
+    per-output-channel scale, ``in_scale`` / ``out_scale`` / ``add_scale`` are device fp32 ``[1]`` scales of the
+    features, an e4m3 output and an e4m3 ``output_add``; ``output_dtype`` is float32 / float16 / bfloat16 or
+    float8_e4m3fn (default: float8_e4m3fn, as the features)."""
     _require_cuda(features, "features")
     lib = _lib()
     features = _dense(features)
@@ -534,6 +542,10 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     # mask_output_fwd (per-128-row OR of the sorted masks) is the tile table's mask block
     mask_output = tiles[1].view(1, -1, words) if (is_train and tiles is not None) else torch.Tensor()
     d = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, pair_fwd, mask, argsort, tiles=tiles)
+    if features.dtype == torch.float8_e4m3fn:
+        out = _implicit_gemm_fp8(d, features, filters, n_out, c_out, scale, bias, output_add, output_dtype, in_scale,
+                                 out_scale, add_scale, act_type, act_alpha, timer)
+        return out, mask_output, MASK_WIDTH
     if is_int8:
         assert scale is not None, "int8 implicit gemm needs the per-channel scale"
         out = torch.empty((n_out, c_out), dtype=output_dtype, device=features.device)
@@ -569,6 +581,76 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     return out, mask_output, MASK_WIDTH
 
 
+_FP8_OUT = (torch.float32, torch.float16, torch.bfloat16, torch.float8_e4m3fn)
+
+
+def _scale_operand(t: Optional[torch.Tensor], n: int, what: str) -> Optional[torch.Tensor]:
+    if t is None:
+        return None
+    _require_cuda(t, what)
+    if t.numel() != n:
+        raise RuntimeError(f"fp8 implicit gemm: {what} must have {n} element(s), got {t.numel()}")
+    return t.reshape(-1).float().contiguous()
+
+
+def _implicit_gemm_fp8(d, features, filters, n_out, c_out, w_scale, bias, output_add, output_dtype, in_scale,
+                       out_scale, add_scale, act_type, act_alpha, timer):
+    """The fp8 route of :func:`implicit_gemm`: every scale stays on the device."""
+    if output_dtype not in _FP8_OUT:
+        raise RuntimeError(f"fp8 implicit gemm: output dtype {output_dtype} not supported")
+    if in_scale is None or w_scale is None:
+        raise RuntimeError("fp8 implicit gemm needs the features' scale (in_scale) and the filter's scale")
+    if output_dtype == torch.float8_e4m3fn and out_scale is None:
+        raise RuntimeError("fp8 implicit gemm: an e4m3 output needs out_scale")
+    in_scale = _scale_operand(in_scale, 1, "in_scale")
+    w_scale = _scale_operand(w_scale, c_out, "the filter scale")
+    out_scale = _scale_operand(out_scale, 1, "out_scale")
+    add_scale = _scale_operand(add_scale, 1, "add_scale")
+    bias = _scale_operand(bias, c_out, "bias")
+    if output_add is not None:
+        _require_cuda(output_add, "output_add")
+        if output_add.dtype != output_dtype or tuple(output_add.shape) != (n_out, c_out):
+            raise RuntimeError(f"fp8 implicit gemm: output_add must be {output_dtype} of shape {(n_out, c_out)}, got "
+                               f"{output_add.dtype} {tuple(output_add.shape)}")
+        if output_dtype == torch.float8_e4m3fn and add_scale is None:
+            raise RuntimeError("fp8 implicit gemm: an e4m3 output_add needs add_scale")
+        output_add = _dense(output_add)
+    out = torch.empty((n_out, c_out), dtype=output_dtype, device=features.device)
+    with timer.record("implicit_gemm_fp8", _stream()):
+        a = _cabi.Fp8Gemm(_ptr(features), _ptr(filters), _ptr(in_scale), _ptr(w_scale), _ptr(bias), _ptr(output_add),
+                          _ptr(add_scale), _ptr(out), _DTYPE_CODE[output_dtype], _ptr(out_scale), _act_code(act_type),
+                          float(act_alpha))
+        _cabi.check(_lib().spx_implicit_gemm_fwd_fp8(ctypes.byref(d), ctypes.byref(a), _stream()), "implicit_gemm_fwd_fp8")
+    return out
+
+
+def fp8_quantize(x: torch.Tensor, num_valid: Optional[torch.Tensor] = None,
+                 scale: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp32 / fp16 / bf16 rows ``x [N, C]`` -> ``(e4m3 rows, device scale fp32 [1])`` (``spx_fp8_quantize``):
+    with ``scale`` the given scale, else amax / 448 of the rows below ``num_valid``.  Rows from ``num_valid`` on
+    are 0."""
+    _require_cuda(x, "features")
+    if x.dtype not in (torch.float32, torch.float16, torch.bfloat16) or x.dim() != 2:
+        raise RuntimeError(f"fp8_quantize: x must be 2-D float32 / float16 / bfloat16, got {x.dtype} {tuple(x.shape)}")
+    x = _dense(x)
+    rows, ch = int(x.shape[0]), int(x.shape[1])
+    out = torch.empty((rows, ch), dtype=torch.float8_e4m3fn, device=x.device)
+    if scale is not None:
+        scale = _scale_operand(scale, 1, "scale")
+        scale_out, ws = scale, None
+    else:
+        scale_out = torch.empty((1,), dtype=torch.float32, device=x.device)
+        ws = _bytes(_lib().spx_fp8_quantize_workspace_size(rows, ch), x.device)
+    if num_valid is not None:
+        _require_cuda(num_valid, "num_valid")
+        num_valid = num_valid.to(torch.int32)
+    q = _cabi.Fp8Quant(_ptr(x), _DTYPE_CODE[x.dtype], rows if ch else 0, max(ch, 1), _ptr(num_valid), _ptr(scale),
+                       _ptr(out), None if scale is not None else _ptr(scale_out))
+    _cabi.check(_lib().spx_fp8_quantize(ctypes.byref(q), _ptr(ws), 0 if ws is None else ws.numel(), _stream()),
+                "fp8_quantize")
+    return out, scale_out
+
+
 def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_splits, n_out, is_train, timer,
                           bias, act_alpha, act_type, output_add, output_dtype):
     """ConvAlgo.MaskSplitImplicitGemm forward: one kernel pass per mask split (each visits only its
@@ -577,6 +659,8 @@ def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_spli
     lib = _lib()
     if features.dtype == torch.int8:
         raise NotImplementedError("int8 + MaskSplitImplicitGemm: use ConvAlgo.MaskImplicitGemm")
+    if features.dtype == torch.float8_e4m3fn:
+        raise NotImplementedError("fp8 + MaskSplitImplicitGemm: use ConvAlgo.MaskImplicitGemm")
     kv, c_in, c_out = _check_filter(features, filters)
     n_in = features.shape[0]
     words = (kv + 31) // 32
