@@ -335,10 +335,6 @@ int spx_peer_error(const spx_peer_group *pg, int *error);
 int spx_implicit_gemm_wgrad_push(const spx_gemm_desc *d, const void *features, const void *out_bp,
                                  void *dfilters, void *workspace, size_t workspace_bytes,
                                  const spx_peer_group *pg, spx_stream_t stream);
-/* push + finish back to back: dfilters = scale * sum over ranks */
-int spx_implicit_gemm_wgrad_allreduce(const spx_gemm_desc *d, const void *features, const void *out_bp,
-                                      void *dfilters, void *workspace, size_t workspace_bytes,
-                                      const spx_peer_group *pg, float scale, spx_stream_t stream);
 /* the same exchange for an existing small tensor (bias gradients ...): push sends `data` (dtype SPX_F32 /
  * SPX_F16 / SPX_BF16), finish writes out = scale * sum over ranks (out may be data); allreduce = both */
 int spx_peer_push(const spx_peer_group *pg, const void *data, int64_t count, int dtype, spx_stream_t stream);

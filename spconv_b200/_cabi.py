@@ -178,8 +178,6 @@ SIGNATURES = {
     "spx_peer_buffer_close": (c_int, [c_void_p]),
     "spx_peer_buffer_destroy": (c_int, [c_void_p]),
     "spx_peer_error": (c_int, [POINTER(PeerGroup), POINTER(c_int)]),
-    "spx_implicit_gemm_wgrad_allreduce": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
-                                                  POINTER(PeerGroup), c_float, c_void_p]),
     "spx_implicit_gemm_wgrad_push": (c_int, [POINTER(GemmDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                              POINTER(PeerGroup), c_void_p]),
     "spx_peer_push": (c_int, [POINTER(PeerGroup), c_void_p, c_int64, c_int, c_void_p]),

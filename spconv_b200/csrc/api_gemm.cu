@@ -91,33 +91,26 @@ extern "C" size_t spx_implicit_gemm_wgrad_workspace_size(const spx_gemm_desc *d)
     return 256;
 }
 
-// pg == NULL: plain weight gradient.  pg != NULL: push this rank's fp32 gradient to the group; `finish` also
-// runs the receive side right away (otherwise the caller does, after the work it wants to overlap).
+// pg == NULL: plain weight gradient.  pg != NULL: push this rank's fp32 gradient to the group; the caller runs the
+// receive side (spx_peer_finish) after the work it wants to overlap.
 static int wgrad_entry(const spx_gemm_desc *d, const void *features, const void *out_bp, void *dfilters, void *workspace,
-                       size_t workspace_bytes, const spx_peer_group *pg, bool finish, float scale, spx_stream_t stream);
+                       size_t workspace_bytes, const spx_peer_group *pg, spx_stream_t stream);
 
 extern "C" int spx_implicit_gemm_wgrad(const spx_gemm_desc *d, const void *features, const void *out_bp,
                                        void *dfilters, void *workspace, size_t workspace_bytes,
                                        spx_stream_t stream) {
-    return wgrad_entry(d, features, out_bp, dfilters, workspace, workspace_bytes, nullptr, false, 1.f, stream);
+    return wgrad_entry(d, features, out_bp, dfilters, workspace, workspace_bytes, nullptr, stream);
 }
 
 extern "C" int spx_implicit_gemm_wgrad_push(const spx_gemm_desc *d, const void *features, const void *out_bp,
                                             void *dfilters, void *workspace, size_t workspace_bytes,
                                             const spx_peer_group *pg, spx_stream_t stream) {
     SPX_REQUIRE(pg != nullptr, "implicit_gemm_wgrad_push: peer group is NULL");
-    return wgrad_entry(d, features, out_bp, dfilters, workspace, workspace_bytes, pg, false, 1.f, stream);
-}
-
-extern "C" int spx_implicit_gemm_wgrad_allreduce(const spx_gemm_desc *d, const void *features, const void *out_bp,
-                                                 void *dfilters, void *workspace, size_t workspace_bytes,
-                                                 const spx_peer_group *pg, float scale, spx_stream_t stream) {
-    SPX_REQUIRE(pg != nullptr, "implicit_gemm_wgrad_allreduce: peer group is NULL");
-    return wgrad_entry(d, features, out_bp, dfilters, workspace, workspace_bytes, pg, true, scale, stream);
+    return wgrad_entry(d, features, out_bp, dfilters, workspace, workspace_bytes, pg, stream);
 }
 
 static int wgrad_entry(const spx_gemm_desc *d, const void *features, const void *out_bp, void *dfilters, void *workspace,
-                       size_t workspace_bytes, const spx_peer_group *pg, bool finish, float scale, spx_stream_t stream) {
+                       size_t workspace_bytes, const spx_peer_group *pg, spx_stream_t stream) {
     if (check_desc(d, "implicit_gemm_wgrad")) return 2;
     SPX_REQUIRE(d->dtype == SPX_F32 || d->dtype == SPX_F16 || d->dtype == SPX_BF16,
                 "implicit_gemm_wgrad: dtype %d not supported", d->dtype);
@@ -125,12 +118,7 @@ static int wgrad_entry(const spx_gemm_desc *d, const void *features, const void 
     const int64_t dw_count = (int64_t)d->kv * d->c_in * d->c_out;
     if (d->n_out == 0 || d->n_in == 0) {       // an empty shard still takes part in the exchange
         SPX_CHECK_CUDA(cudaMemsetAsync(dfilters, 0, (size_t)dw_count * dtype_bytes(d->dtype), (cudaStream_t)stream));
-        if (pg) {
-            if (int rc = peer_push(nullptr, 0, 0, dfilters, dw_count, d->dtype, pg, (cudaStream_t)stream)) return rc;
-            if (finish) {
-                return peer_finish(dfilters, dw_count, d->dtype, pg, scale, (cudaStream_t)stream);
-            }
-        }
+        if (pg) return peer_push(nullptr, 0, 0, dfilters, dw_count, d->dtype, pg, (cudaStream_t)stream);
         return 0;
     }
     SPX_REQUIRE(features && out_bp, "implicit_gemm_wgrad: NULL tensor");
@@ -148,20 +136,11 @@ static int wgrad_entry(const spx_gemm_desc *d, const void *features, const void 
         SPX_REQUIRE(workspace && workspace_bytes >= tc_wgrad_workspace_size(w),
                     "implicit_gemm_wgrad: workspace too small (%zu < %zu)", workspace_bytes, tc_wgrad_workspace_size(w));
         set_family(2);
-        if (int rc = tc_wgrad(w, (cudaStream_t)stream)) return rc;     // with peers: partial sums pushed, dW not written yet
-        if (pg && finish) {
-            return peer_finish(dfilters, dw_count, d->dtype, pg, scale, (cudaStream_t)stream);
-        }
-        return 0;
+        return tc_wgrad(w, (cudaStream_t)stream);     // with peers: partial sums pushed, dW not written yet
     }
     set_family(1);
     if (int rc = simt_wgrad(w, (cudaStream_t)stream)) return rc;
-    if (pg) {
-        if (int rc = peer_push(nullptr, 0, 0, dfilters, dw_count, d->dtype, pg, (cudaStream_t)stream)) return rc;
-        if (finish) {
-            return peer_finish(dfilters, dw_count, d->dtype, pg, scale, (cudaStream_t)stream);
-        }
-    }
+    if (pg) return peer_push(nullptr, 0, 0, dfilters, dw_count, d->dtype, pg, (cudaStream_t)stream);
     return 0;
 }
 

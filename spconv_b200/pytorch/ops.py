@@ -765,86 +765,83 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
             _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
                                                     _ptr(din), _stream()), "implicit_gemm_dgrad")
 
-    def run_wgrad():
+    def run_wgrad(group):
         with timer.record("implicit_gemm_wgrad", _stream()):
-            if _PEERS is not None and not (_PEER_TRIAGE & 2):
+            if group is not None:
                 # data-parallel: the kernel that reduces the split-K partials pushes this rank's fp32 dW into every
-                # rank's exchange buffer (csrc/peer.cu); finish_exchange() below writes dfilters
+                # rank's exchange buffer (csrc/peer.cu); the schedule's finish writes dfilters
                 _cabi.check(lib.spx_implicit_gemm_wgrad_push(
                     ctypes.byref(d_wg), _ptr(features), _ptr(out_bp), _ptr(dfilters), ws.data_ptr(), ws.numel(),
-                    ctypes.byref(_PEERS.group), _stream()), "implicit_gemm_wgrad_push")
+                    group, _stream()), "implicit_gemm_wgrad_push")
             else:
                 _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d_wg), _ptr(features), _ptr(out_bp),
                                                         _ptr(dfilters), ws.data_ptr(), ws.numel(),
                                                         _stream()), "implicit_gemm_wgrad")
 
-    def finish_exchange():
-        if _PEER_TRIAGE & 1:
-            return
-        with timer.record("implicit_gemm_wgrad_exchange", _stream()):
-            _cabi.check(lib.spx_peer_finish(ctypes.byref(_PEERS.group), _ptr(dfilters), dfilters.numel(),
-                                            _DTYPE_CODE[dfilters.dtype], _PEERS.scale, _stream()), "peer_finish")
-
-    if _PEERS is not None:
-        if timer.enable or not (n_in and n_out) or not torch._C._cuda_isCurrentStreamCapturing():
-            # eager: one stream (a fork / join per layer costs more host time than it hides); the input gradient
-            # between publish and finish hides the NVLink latency
-            run_wgrad()
-            run_dgrad()
-            finish_exchange()
-            return din, dfilters
-        # captured: the two gradients stay parallel branches as in the single-GPU graph (measured: running them one
-        # after the other costs 17 us per config-2 step, more than the whole exchange).  Weight gradient + publish
-        # on the caller's stream, input gradient on the forked one, the receive side (wait, TMA pull, rank-order
-        # sum: a few small CTAs) behind it: every dependent kernel on the caller's stream costs ~8 us of launch and
-        # queueing when the next cloud's rulebook kernels share the GPU.
-        main = torch.cuda.current_stream()
-        side = _side_stream(features.device)
-        side.wait_stream(main)
-        run_wgrad()
-        with torch.cuda.stream(side):
-            run_dgrad()
-            side.wait_stream(main)          # the publish
-            finish_exchange()
-        main.wait_stream(side)
-        return din, dfilters
-    if _WGRAD_HOOK is not None:
-        # also for a layer without rows (dW = 0): a rank whose shard is empty enters the same collectives
-        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
-        return din, dfilters
-    if timer.enable or not (n_in and n_out) or not torch._C._cuda_isCurrentStreamCapturing():
-        # eager launches are host-bound (and an eager fork/join per call measured slower, not
-        # faster); profiling regions stay one kernel each
-        run_dgrad()
-        run_wgrad()
-        return din, dfilters
-    # Under CUDA-graph capture the two independent gradients become parallel branches.  The weight-gradient kernel (one CTA per SM, statically
-    # assigned tiles) has a long tail -- its CTAs finish over a ~15 us window -- so it goes first on
-    # the caller's stream and the dynamically scheduled input-gradient kernel is queued on a forked
-    # stream: its CTAs fill the SMs the weight gradient has already left.  Joined before returning.
-    main = torch.cuda.current_stream()
-    side = _side_stream(features.device)
-    side.wait_stream(main)
-    run_wgrad()
-    with torch.cuda.stream(side):
-        run_dgrad()
-    main.wait_stream(side)
+    _backward_schedule("implicit_gemm", run_dgrad, run_wgrad, dfilters, features.device, timer, n_in and n_out)
     return din, dfilters
 
 
 _WGRAD_HOOK = None
 
 
-def _hooked_backward(run_wgrad, run_dgrad, dfilters, device) -> None:
-    """Data-parallel overlap: weight gradient FIRST, then the hook (typically the all-reduce of dW) on a
-    forked stream while the input gradient -- which the hook does not need -- runs on this one."""
+def _backward_schedule(name, run_dgrad, run_wgrad, dfilters, device, timer, rows) -> None:
+    """The order of the two gradients of a conv backward and the data-parallel handling of its dW, for every route
+    (implicit GEMM, Native, depthwise).  ``run_wgrad(group)`` writes dW to ``dfilters``, or, given a peer group
+    (``ctypes.byref``), pushes it to the group instead; ``rows``: both sides of the layer have rows.
+
+    * Peer group installed: weight gradient + push, input gradient, finish (which writes dfilters).  The input
+      gradient between push and finish hides the NVLink latency.
+    * Otherwise, a wgrad hook installed: weight gradient, then the hook on a forked stream while the input gradient
+      runs on this one -- also for a layer without rows (dW = 0), so a rank with an empty shard enters the same
+      collectives.
+    * Otherwise: input gradient, then weight gradient.
+
+    Eager launches stay on one stream: they are host-bound and a fork / join per call measured slower; profiling
+    regions stay one kernel each.  Under CUDA-graph capture the gradients become parallel branches.  The
+    weight-gradient kernel (one CTA per SM, statically assigned tiles) has a long tail -- its CTAs finish over a
+    ~15 us window -- so it goes first on the caller's stream and the input gradient on a forked stream fills the SMs
+    it has left.  The finish goes behind the input gradient on the forked stream: every dependent kernel on the
+    caller's stream costs ~8 us of launch and queueing when the next cloud's rulebook kernels share the GPU.  (With a
+    group, running the gradients one after the other measured 17 us more per config-2 step, more than the whole
+    exchange.)  Joined before returning."""
+    if _PEERS is None and _WGRAD_HOOK is not None:
+        main = torch.cuda.current_stream()
+        side = _side_stream(device)
+        run_wgrad(None)
+        side.wait_stream(main)
+        with torch.cuda.stream(side):
+            _WGRAD_HOOK(dfilters)
+        run_dgrad()
+        main.wait_stream(side)
+        return
+    group = None if _PEERS is None or _PEER_TRIAGE & 2 else ctypes.byref(_PEERS.group)
+
+    def finish():
+        if _PEER_TRIAGE & 1:
+            return
+        with timer.record(f"{name}_wgrad_exchange", _stream()):
+            _cabi.check(_lib().spx_peer_finish(ctypes.byref(_PEERS.group), _ptr(dfilters), dfilters.numel(),
+                                               _DTYPE_CODE[dfilters.dtype], _PEERS.scale, _stream()), "peer_finish")
+
+    if timer.enable or not rows or not torch._C._cuda_isCurrentStreamCapturing():
+        if _PEERS is None:
+            run_dgrad()
+            run_wgrad(None)
+        else:
+            run_wgrad(group)
+            run_dgrad()
+            finish()
+        return
     main = torch.cuda.current_stream()
     side = _side_stream(device)
-    run_wgrad()
     side.wait_stream(main)
+    run_wgrad(group)
     with torch.cuda.stream(side):
-        _WGRAD_HOOK(dfilters)
-    run_dgrad()
+        run_dgrad()
+        if _PEERS is not None:
+            side.wait_stream(main)          # the push
+            finish()
     main.wait_stream(side)
 
 
@@ -852,12 +849,13 @@ def set_wgrad_hook(fn) -> None:
     """``fn(dfilters)`` is called on a forked stream right after the weight gradient of every layer, while
     the input gradient of the same layer runs on the caller's stream (joined before the op returns).  This
     is the place for a data-parallel all-reduce of the layer's dW: it overlaps the rest of the backward pass
-    instead of trailing it (DDP-style hook).  It covers every route, :func:`implicit_gemm_backward`,
-    :func:`indice_conv_backward` (``ConvAlgo.Native``) and :func:`depthwise_conv_backward`, and every layer, also one
-    without rows (its dW is zero), so every rank enters the same collectives.  ``ConvAlgo.MaskSplitImplicitGemm`` calls it once per
-    mask split, with that split's dW, and sums what the hook left of each split over that split's kernel
-    offsets.  The hook may change ``dfilters`` in place; the op returns what it leaves there.  Ignored while
-    a peer group is installed (:func:`set_peer_group`).  ``None`` removes the hook."""
+    instead of trailing it (DDP-style hook).  Every route, :func:`implicit_gemm_backward`,
+    :func:`indice_conv_backward` (``ConvAlgo.Native``) and :func:`depthwise_conv_backward`, runs this one schedule,
+    for every layer, also one without rows (its dW is zero), so every rank enters the same collectives.
+    ``ConvAlgo.MaskSplitImplicitGemm`` calls it once per mask split, with that split's dW, and sums what the hook
+    left of each split over that split's kernel offsets.  The hook may change ``dfilters`` in place; the op returns
+    what it leaves there.  Ignored while a peer group is installed (:func:`set_peer_group`).  ``None`` removes the
+    hook."""
     global _WGRAD_HOOK
     _WGRAD_HOOK = fn
 
@@ -868,11 +866,13 @@ _PEER_TRIAGE = 0          # bench.py --peer-triage (timing experiments only; res
 
 def set_peer_group(peers) -> None:
     """Data-parallel mode: with a :class:`spconv_b200.pytorch.dist.PeerGroup` installed, every weight
-    gradient computed by :func:`implicit_gemm_backward` / :func:`indice_conv_backward` is returned
-    already summed (x ``peers.scale``) over the ranks -- the exchange is the tail of the
-    weight-gradient kernel (NVLink peer stores, ``csrc/peer.cu``), there is no separate all-reduce.  A depthwise
-    layer's dW (:func:`depthwise_conv_backward`) is summed by :func:`peer_allreduce_` right after its kernels.
-    Every rank must run the same sequence of layers.  Only these conv weight gradients are exchanged:
+    gradient computed by :func:`implicit_gemm_backward`, :func:`indice_conv_backward` and
+    :func:`depthwise_conv_backward` is returned already summed (x ``peers.scale``) over the ranks, with one
+    schedule on every route: the weight gradient pushes this rank's dW to every rank (on the implicit-GEMM
+    routes the push is the tail of the weight-gradient kernel: NVLink peer stores, ``csrc/peer.cu``; the
+    depthwise kernels are followed by ``spx_peer_push``), the input gradient runs, then the finish sums the
+    ranks' pushes in rank order into dW.  Under CUDA-graph capture the input gradient and the finish run on a
+    forked stream.  Every rank must run the same sequence of layers.  Only these conv weight gradients are exchanged:
     biases (added outside the op in training) and every other parameter keep rank-local gradients until
     :func:`peer_allreduce_` sums them (one call per tensor, or one per flat ``dist.GradBucket``), on every
     rank in the same order.  ``None`` switches it off."""
@@ -978,22 +978,18 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
             _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
                                                     _ptr(din), _stream()), "implicit_gemm_dgrad(native)")
 
-    def run_wgrad():
+    def run_wgrad(group):
         with timer.record("indice_conv_wgrad", _stream()):
-            if _PEERS is not None:
-                _cabi.check(lib.spx_implicit_gemm_wgrad_allreduce(
+            if group is not None:
+                _cabi.check(lib.spx_implicit_gemm_wgrad_push(
                     ctypes.byref(d_wg), _ptr(features), _ptr(out_bp), _ptr(dfilters), ws.data_ptr(), ws.numel(),
-                    ctypes.byref(_PEERS.group), _PEERS.scale, _stream()), "implicit_gemm_wgrad_allreduce(native)")
+                    group, _stream()), "implicit_gemm_wgrad_push(native)")
             else:
                 _cabi.check(lib.spx_implicit_gemm_wgrad(ctypes.byref(d_wg), _ptr(features), _ptr(out_bp),
                                                         _ptr(dfilters), ws.data_ptr(), ws.numel(),
                                                         _stream()), "implicit_gemm_wgrad(native)")
 
-    if _PEERS is None and _WGRAD_HOOK is not None:
-        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
-        return din, dfilters
-    run_dgrad()
-    run_wgrad()
+    _backward_schedule("indice_conv", run_dgrad, run_wgrad, dfilters, features.device, timer, n_in and n_out)
     return din, dfilters
 
 
@@ -1041,9 +1037,10 @@ def depthwise_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_b
                             timer: CUDAKernelTimer = CUDAKernelTimer(False)):
     """Backward of :func:`depthwise_conv` -> ``(din, dfilters)``.  ``table_bwd`` ``[kv, >= N]`` maps inputs to
     outputs; ``None`` (SubM) walks ``table_fwd`` with the mirrored offset instead.  The weight gradient is summed
-    in a fixed order of the row indices (bit-reproducible, unchanged by trailing padding rows).  Data-parallel as
-    the other convs: the wgrad hook receives dW (:func:`set_wgrad_hook`); with a peer group installed dW is summed
-    over the ranks by :func:`peer_allreduce_`."""
+    in a fixed order of the row indices (bit-reproducible, unchanged by trailing padding rows).  Data-parallel with the
+    schedule of the other convs: the wgrad hook receives dW (:func:`set_wgrad_hook`); with a peer group installed
+    dW is pushed right after its kernels and summed over the ranks behind the input gradient
+    (:func:`set_peer_group`)."""
     features = features.contiguous()
     filters = filters.contiguous()
     out_bp = out_bp.contiguous()
@@ -1067,19 +1064,16 @@ def depthwise_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_b
                                                 int(table_dg.stride(0)), kv, n_in, c, dtype, int(reverse), _stream()),
                         "depthwise_dgrad")
 
-    def run_wgrad():
+    def run_wgrad(group):
         with timer.record("depthwise_conv_wgrad", _stream()):
             _cabi.check(lib.spx_depthwise_wgrad(_ptr(features), _ptr(out_bp), _ptr(dfilters), _ptr(table_fwd),
                                                 int(table_fwd.stride(0)), kv, n_out, c, dtype, ws.data_ptr(),
                                                 ws.numel(), _stream()), "depthwise_wgrad")
-            if _PEERS is not None:
-                peer_allreduce_(dfilters)
+            if group is not None:
+                _cabi.check(lib.spx_peer_push(group, dfilters.data_ptr(), dfilters.numel(), dtype, _stream()),
+                            "peer_push")
 
-    if _PEERS is None and _WGRAD_HOOK is not None:
-        _hooked_backward(run_wgrad, run_dgrad, dfilters, features.device)
-        return din, dfilters
-    run_dgrad()
-    run_wgrad()
+    _backward_schedule("depthwise_conv", run_dgrad, run_wgrad, dfilters, features.device, timer, n_in and n_out)
     return din, dfilters
 
 

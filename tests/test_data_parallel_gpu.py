@@ -241,9 +241,9 @@ def test_routes_reach_every_weight_gradient_instance():
 @pytest.mark.parametrize("mode", ["subm", "conv"])
 @pytest.mark.parametrize("case", ROUTES, ids=lambda c: "-".join(map(str, c)))
 def test_world_of_one_equals_the_plain_weight_gradient(case, mode, oracle, cuda_dev, monkeypatch):
-    """A group of one rank returns the plain weight gradient bit for bit, on the same kernel family, through
-    implicit_gemm_backward (push + finish), indice_conv_backward (spx_implicit_gemm_wgrad_allreduce) and the
-    two exchanges of a mask-split layer; and through the C ABI's push, whose kernel family is read back."""
+    """A group of one rank returns the plain weight gradient bit for bit, on the same kernel family, through the
+    push + finish of implicit_gemm_backward, of indice_conv_backward and of the two exchanges of a mask-split
+    layer; and through the C ABI's push, whose kernel family is read back."""
     from spconv_b200 import _cabi
     from spconv_b200.pytorch import ops
     algo, dt, geom, C, K = case
@@ -450,6 +450,67 @@ def test_graph_replay_of_a_training_step(world, oracle, cuda_dev):
     with _ring(world, average=True) as ring:
         refill()
         check(_round(ring, streams, step), "eager warm-up")          # all ranks together: none waits alone
+        graphs, static = [], []
+        for r in range(world):
+            ops.set_peer_group(ring[r])
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=streams[r]):
+                static.append(step(r))
+            graphs.append(g)
+        ops.set_peer_group(None)
+        for it in range(replays):
+            refill()
+            torch.cuda.synchronize()
+            for r in range(world):
+                with torch.cuda.stream(streams[r]):
+                    graphs[r].replay()
+            torch.cuda.synchronize()
+            check(static, f"replay {it}")
+        del graphs, static
+
+
+# (subm, dtype, C, K): Native SubM and strided layers, one per weight-gradient kernel family
+NATIVE_GRAPH = [(True, "f16", 32, 64), (False, "bf16", 16, 16), (False, "f32", 16, 16)]
+
+
+@gpu
+def test_graph_replay_of_native_weight_gradients(oracle, cuda_dev):
+    """ConvAlgo.Native captured with a group: each of 2 ranks captures the op-level backward of a SubM and two
+    strided layers (rulebooks built before capture; input gradient and finish on the forked stream).  The graphs replay
+    together 5 times on fresh grid inputs, and every replay must give the exact mean weight gradients,
+    bit-identical on both ranks."""
+    from spconv_b200.pytorch import ops
+    world, replays = 2, 5
+    gen = torch.Generator(device=cuda_dev).manual_seed(77)
+    layers = []
+    for it, (subm, dt, C, K) in enumerate(NATIVE_GRAPH):
+        w = _grid(gen, (K, 3, 3, 3, C), cuda_dev).to(TORCH_DT[dt])
+        layers.append((_shards(oracle, cuda_dev, world, it, "native", subm, dt, C, K, w, gen, empty=-1), w))
+
+    def step(r):
+        return [shards[r].backward(w) for shards, w in layers]
+
+    def refill():
+        for shards, w in layers:
+            for s in shards:
+                x, dout = _grid(gen, tuple(s.x.shape), cuda_dev), _grid(gen, tuple(s.dout.shape), cuda_dev)
+                s.x.copy_(x)
+                s.dout.copy_(dout)
+                ref = _reference(x, w.float(), dout, s.conv.ref_pair, cuda_dev)
+                s.dw, s.dw_abs = ref["dw"], ref["dw_abs"]
+
+    def check(results, what):
+        for i, ((shards, _), (subm, dt, C, K)) in enumerate(zip(layers, NATIVE_GRAPH)):
+            name = f"{what}, layer {i} ({'subm' if subm else 'strided'}, {dt})"
+            got = [res[i] for res in results]
+            _same_on_every_rank(name, got)
+            _assert_fused(name, got[0].reshape(K, 27, C), [s.dw for s in shards], [s.dw_abs for s in shards], dt,
+                          scale, _family(dt, 27, C, K) == 1)
+
+    streams = [torch.cuda.Stream() for _ in range(world)]
+    with _ring(world, average=True) as ring:
+        scale = ring[0].scale
+        check(_round(ring, streams, step), "eager warm-up")
         graphs, static = [], []
         for r in range(world):
             ops.set_peer_group(ring[r])

@@ -520,7 +520,9 @@ def test_wgrad_hook_eager_and_replayed(cuda_dev):
 
 
 def test_two_ranks_sum_depthwise_weight_gradients(cuda_dev):
-    """two simulated ranks on streams of one GPU: every depthwise dW comes back as the rank-order sum"""
+    """two simulated ranks on streams of one GPU: every depthwise dW comes back as the rank-order sum, eagerly and
+    from CUDA graphs of each rank's SubM layers (input gradient and finish on the forked stream) that replay
+    together on fresh inputs"""
     from spconv_b200.pytorch.dist import PeerGroup
     C, world = 16, 2
     base = _dp_net(cuda_dev, C)
@@ -532,6 +534,25 @@ def test_two_ranks_sum_depthwise_weight_gradients(cuda_dev):
         y.features.backward(torch.ones_like(y.features))
         plain.append(_grads(nets[r]))
         nets[r].zero_grad(set_to_none=True)
+    # captured: each rank's forward + backward of SubM 3x3x3 layers sharing one rulebook (no host read-back)
+    subms = [spconv.SparseSequential(copy.deepcopy(base[0]), copy.deepcopy(base[0])) for _ in range(world)]
+    feats = [x.features.clone() for x in xs]
+
+    def step(r):
+        for p in subms[r].parameters():
+            p.grad = None
+        y = subms[r](xs[r].replace_feature(feats[r]))
+        y.features.backward(torch.ones_like(y.features))
+        return [p.grad for p in subms[r].parameters()]
+
+    def rank_order_sum(what, got, parts):
+        for i in range(len(parts[0])):
+            want = (parts[0][i].double() + parts[1][i].double()).half()
+            assert torch.equal(got[0][i], got[1][i]), f"{what} layer {i}: ranks differ"
+            assert torch.equal(got[0][i], want), f"{what} layer {i}: not the rank-order sum"
+
+    for r in range(world):                          # warm-up
+        step(r)
     streams = [torch.cuda.Stream() for _ in range(world)]
     ring = PeerGroup.local_ring(world, capacity_bytes=1 << 20, average=False)
     try:
@@ -547,16 +568,32 @@ def test_two_ranks_sum_depthwise_weight_gradients(cuda_dev):
                 outs[r].features.backward(torch.ones_like(outs[r].features))
         ops.set_peer_group(None)
         torch.cuda.synchronize()
+        rank_order_sum("eager", [_grads(n) for n in nets], plain)
+        graphs, static = [], []
+        for r in range(world):
+            ops.set_peer_group(ring[r])
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=streams[r]):
+                static.append(step(r))
+            graphs.append(g)
+        ops.set_peer_group(None)
+        gen = torch.Generator(device=cuda_dev).manual_seed(21)
+        for it in range(3):
+            for f in feats:
+                f.copy_(_data(gen, tuple(f.shape), cuda_dev, True).half())
+            torch.cuda.synchronize()
+            for r in range(world):
+                with torch.cuda.stream(streams[r]):
+                    graphs[r].replay()
+            torch.cuda.synchronize()
+            got = [[t.clone() for t in static[r]] for r in range(world)]
+            rank_order_sum(f"replay {it}", got, [[t.clone() for t in step(r)] for r in range(world)])
+        del graphs, static
         assert [pg.error() for pg in ring] == [0] * world
     finally:
         ops.set_peer_group(None)
         for pg in ring:
             pg.close()
-    got = [_grads(n) for n in nets]
-    for i in range(len(plain[0])):
-        want = (plain[0][i].double() + plain[1][i].double()).half()
-        assert torch.equal(got[0][i], got[1][i]), f"layer {i}: ranks differ"
-        assert torch.equal(got[0][i], want), f"layer {i}: not the rank-order sum"
 
 
 # ------------------------------------------------------------------ 9. AMP

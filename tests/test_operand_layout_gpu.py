@@ -696,9 +696,6 @@ EXPLAINED = {
     ("spx_implicit_gemm_wgrad_push", "features"): "the data-parallel twin of spx_implicit_gemm_wgrad: same predicate",
     ("spx_implicit_gemm_wgrad_push", "out_bp"): "the data-parallel twin of spx_implicit_gemm_wgrad: same predicate",
     ("spx_implicit_gemm_wgrad_push", "dfilters"): "written element by element (peer_finish_kernel)",
-    ("spx_implicit_gemm_wgrad_allreduce", "features"): "the data-parallel twin of spx_implicit_gemm_wgrad",
-    ("spx_implicit_gemm_wgrad_allreduce", "out_bp"): "the data-parallel twin of spx_implicit_gemm_wgrad",
-    ("spx_implicit_gemm_wgrad_allreduce", "dfilters"): "written element by element (peer_finish_kernel)",
     ("spx_indice_pool_fwd", "out"): LIBRARY_OUTPUT,
     ("spx_indice_pool_bwd", "din"): LIBRARY_OUTPUT,
     ("spx_indice_pool_bwd", "out_features"): "the forward's output, allocated by the library",
