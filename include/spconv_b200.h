@@ -189,6 +189,32 @@ int spx_conv_rulebook_bounded_all(const spx_conv_geometry *g, const int32_t *ind
                                   int32_t *num_out, int32_t *status, void *workspace,
                                   size_t workspace_bytes, spx_stream_t stream);
 
+/*
+ * Rulebook onto GIVEN output coordinates: a convolution from the source rows `src_indices` [N, ndim+1] (grid in_dims)
+ * onto the target rows `out_indices` [M, ndim+1] (grid out_dims), both in batch_size samples.  The geometry is
+ * taken as given: a SubM layer passes stride 1 and padding (ksize/2) * dilation with out_dims = in_dims.
+ *   - usable source row i: i < *num_valid (every row when num_valid is NULL), batch in [0, batch_size), every
+ *     coordinate inside in_dims; among usable rows with equal coordinates the lowest row wins;
+ *   - active target row o: the same against *out_num_valid and out_dims, and no lower active row has its
+ *     coordinate (a later duplicate is inactive: pair_fwd -1, mask 0);
+ *   - per axis, for target o and tap r: regular c = o * stride - pad + r * dil; transposed
+ *     c = (o + pad - r * dil) / stride when the division is exact; valid iff 0 <= c < in_dims;
+ *   - pair_fwd [kv, M]: pair_fwd[k][o] = the usable row at c, else -1; mask_fwd [M, words] its bits;
+ *     pair_bwd [kv, N]: pair_bwd[k][i] = o for every such pair, else -1; mask_bwd [N, words] its bits.
+ * Then both mask argsorts and both tile tables, as spx_conv_rulebook_stage2_all (argsort_bwd, table_bwd and
+ * tmask_bwd all NULL for inference; pair_bwd and mask_bwd are always written).  M is the caller's, so there is no
+ * host read-back: the launch sequence is fixed and CUDA-graph capturable.  Every output is bit-reproducible.
+ * Kernel volume <= 128, 1-D to 4-D, padding >= 0, 64-bit keys once batch * prod(dims) of either grid reaches
+ * 2^31 - 1.  Both index pointers must be 16-byte aligned.  Either side may be empty.
+ */
+size_t spx_cross_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t M);
+int spx_cross_rulebook_all(const spx_conv_geometry *g, const int32_t *src_indices, int64_t N,
+                           const int32_t *num_valid, const int32_t *out_indices, int64_t M,
+                           const int32_t *out_num_valid, int32_t *pair_fwd, int32_t *pair_bwd,
+                           uint32_t *mask_fwd, uint32_t *mask_bwd, int32_t *argsort_fwd, int32_t *argsort_bwd,
+                           int do_sort, int32_t *table_fwd, uint32_t *tmask_fwd, int32_t *table_bwd,
+                           uint32_t *tmask_bwd, void *workspace, size_t workspace_bytes, spx_stream_t stream);
+
 /* Zero rows [*count, rows) of a row-major matrix with `row_bytes` (even) bytes per row; `count` is a
  * device int32 (the num_out of a bounded rulebook).  Used on gradients that arrive for padded tensors. */
 int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_bytes, const int32_t *count,

@@ -153,6 +153,10 @@ SIGNATURES = {
                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                               c_void_p]),
+    "spx_cross_rulebook_all_workspace_size": (c_size_t, [POINTER(ConvGeometry), c_int64, c_int64]),
+    "spx_cross_rulebook_all": (c_int, [POINTER(ConvGeometry), c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "spx_zero_rows_from_count": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p]),
     "spx_native_pairs": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                  c_size_t, c_void_p]),

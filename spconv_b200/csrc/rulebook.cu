@@ -14,6 +14,7 @@
 #include "gemm.cuh"
 #include "hash.cuh"
 #include "rank.cuh"
+#include "rows.cuh"
 #include "segments.cuh"
 #include <cub/cub.cuh>
 
@@ -268,6 +269,22 @@ __device__ __forceinline__ bool axis_out(int c, int pad, int r, int dil, int str
     else if (stride == 2) { if (h & 1) return false; o = h >> 1; }
     else { o = h / stride; if (o * stride != h) return false; }
     return o < odim;
+}
+// The inverse relations, for a rulebook onto given output coordinates (spx_cross_rulebook_all): the input
+// coordinate c that output o reads through tap r, valid iff it lies in [0, idim).  Regular conv (the c with
+// axis_out(c, r) = o): c = o * stride - pad + r * dil.  Transposed: c = (o + pad - r * dil) / stride, exact.
+// validate_cross keeps every intermediate inside int.
+__device__ __forceinline__ bool axis_in(int o, int pad, int r, int dil, int stride, int idim, int &c) {
+    c = o * stride - pad + r * dil;
+    return c >= 0 && c < idim;
+}
+__device__ __forceinline__ bool axis_in_transposed(int o, int pad, int r, int dil, int stride, int idim, int &c) {
+    const int h = o + pad - r * dil;
+    if (h < 0) return false;
+    if (stride == 1) c = h;
+    else if (stride == 2) { if (h & 1) return false; c = h >> 1; }
+    else { c = h / stride; if (c * stride != h) return false; }
+    return c < idim;
 }
 __device__ __forceinline__ bool conv3_out_key(const Geom &g, const int4 c, const Taps3 &t, int64_t &key) {
     int o0, o1, o2;
@@ -773,6 +790,111 @@ __global__ void pairs_to_table_kernel(const int32_t *__restrict__ pairs, const i
     if (table_bwd) table_bwd[(int64_t)k * n_in + i] = o;
     if (mask_fwd) atomicOr(&mask_fwd[o * words + (k >> 5)], 1u << (k & 31));
     if (mask_bwd) atomicOr(&mask_bwd[i * words + (k >> 5)], 1u << (k & 31));
+}
+
+// ------------------------------------------------------------------ rulebook onto given output coordinates
+// spx_cross_rulebook_all: the source rows x and the target rows t are both given.  A source row is usable when it is
+// below its num_valid, its batch is in [0, batch) and every coordinate is inside in_dims; a target row is active under
+// the same conditions against out_dims and when no lower active row has its coordinate.  Each set has its own hash
+// table, filled by insert_min, so the lowest row wins a duplicated coordinate on either side.
+constexpr int CROSS_THREADS = 128;
+constexpr int CROSS_CHUNK = 8;                  // taps whose probe chains advance together (find_many)
+
+template <int NDIM>
+__device__ __forceinline__ bool load_usable(const int32_t *__restrict__ indices, int64_t row, const int *dims, int batch,
+                                            int (&c)[SPX_MAX_NDIM + 1]) {
+    load_coord(indices, row, NDIM, c);
+    bool ok = c[0] >= 0 && c[0] < batch;
+#pragma unroll
+    for (int a = 0; a < NDIM; ++a) ok = ok && c[a + 1] >= 0 && c[a + 1] < dims[a];
+    return ok;
+}
+
+// threads [0, n) insert the usable source rows into src_table (keys over in_dims), threads [n, n + m) the usable
+// target rows into dst_table (keys over out_dims)
+template <typename Table, int NDIM>
+__global__ void __launch_bounds__(CROSS_THREADS)
+cross_insert_kernel(Table src_table, Table dst_table, Geom g, const int32_t *__restrict__ src, int64_t n,
+                    const int32_t *__restrict__ src_valid, const int32_t *__restrict__ dst, int64_t m,
+                    const int32_t *__restrict__ dst_valid) {
+    const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    const bool is_src = j < n;
+    const int64_t row = is_src ? j : j - n;
+    if (row >= (is_src ? n : m) || row >= valid_rows(is_src ? src_valid : dst_valid, is_src ? n : m)) return;
+    int dims[SPX_MAX_NDIM] = {0, 0, 0, 0};
+#pragma unroll
+    for (int a = 0; a < NDIM; ++a) dims[a] = is_src ? g.in_dims[a] : g.out_dims[a];
+    int c[SPX_MAX_NDIM + 1] = {0, 0, 0, 0, 0};
+    if (!load_usable<NDIM>(is_src ? src : dst, row, dims, g.batch, c)) return;
+    if (is_src) src_table.insert_min(linear_key(c, dims, NDIM), (int32_t)row);
+    else dst_table.insert_min(linear_key(c, dims, NDIM), (int32_t)row);
+}
+
+// one thread per target row o: pair_fwd[k][o] and mask_fwd[o] written in full (-1 / 0 for an inactive row), and
+// for every hit i the scatter pair_bwd[k][i] = o plus bit k of mask_bwd[i] (pair_bwd / mask_bwd cleared before).
+// A (source row, tap) pair maps to at most one coordinate and the active targets are distinct, so every pair_bwd
+// element has at most one writer.  The taps are probed CROSS_CHUNK at a time with their chains in flight together.
+template <typename Table, int NDIM, bool TRANSPOSED>
+__global__ void __launch_bounds__(CROSS_THREADS)
+cross_probe_kernel(Table src_table, Table dst_table, Geom g, const int32_t *__restrict__ dst, int64_t m,
+                   const int32_t *__restrict__ dst_valid, int64_t n, int32_t *__restrict__ pair_fwd,
+                   int32_t *__restrict__ pair_bwd, uint32_t *__restrict__ mask_fwd, uint32_t *__restrict__ mask_bwd,
+                   int words) {
+    const int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (o >= m) return;
+    int c[SPX_MAX_NDIM + 1] = {0, 0, 0, 0, 0};
+    bool active = o < valid_rows(dst_valid, m) && load_usable<NDIM>(dst, o, g.out_dims, g.batch, c);
+    if (active) {
+        int32_t v = -1;
+        active = dst_table.find_slot(linear_key(c, g.out_dims, NDIM), v) >= 0 && v == (int32_t)o;
+    }
+    const int kv = g.kv;
+    int r[NDIM];
+#pragma unroll
+    for (int a = 0; a < NDIM; ++a) r[a] = 0;
+    uint32_t mword = 0;
+    for (int k0 = 0; k0 < kv; k0 += CROSS_CHUNK) {
+        int64_t key[CROSS_CHUNK];
+        bool live[CROSS_CHUNK];
+        int32_t v[CROSS_CHUNK];
+#pragma unroll
+        for (int j = 0; j < CROSS_CHUNK; ++j) {
+            int q[SPX_MAX_NDIM + 1] = {c[0], 0, 0, 0, 0};
+            bool ok = active && k0 + j < kv;
+#pragma unroll
+            for (int a = 0; a < NDIM; ++a) {
+                int ca = 0;
+                const bool in = TRANSPOSED
+                    ? axis_in_transposed(c[a + 1], g.padding[a], r[a], g.dilation[a], g.stride[a], g.in_dims[a], ca)
+                    : axis_in(c[a + 1], g.padding[a], r[a], g.dilation[a], g.stride[a], g.in_dims[a], ca);
+                ok = ok && in;
+                q[a + 1] = ca;
+            }
+            live[j] = ok;
+            key[j] = ok ? linear_key(q, g.in_dims, NDIM) : 0;
+#pragma unroll
+            for (int a = NDIM - 1; a >= 0; --a) {          // next tap, last axis fastest
+                if (++r[a] < g.ksize[a]) break;
+                r[a] = 0;
+            }
+        }
+        find_many<CROSS_CHUNK>(src_table, key, live, v);
+#pragma unroll
+        for (int j = 0; j < CROSS_CHUNK; ++j) {
+            const int k = k0 + j;
+            if (k >= kv) break;
+            pair_fwd[(int64_t)k * m + o] = v[j];
+            if (v[j] >= 0) {
+                mword |= 1u << (k & 31);
+                pair_bwd[(int64_t)k * n + v[j]] = (int32_t)o;
+                atomicOr(&mask_bwd[(int64_t)v[j] * words + (k >> 5)], 1u << (k & 31));
+            }
+            if ((k & 31) == 31 || k == kv - 1) {
+                mask_fwd[o * words + (k >> 5)] = mword;
+                mword = 0;
+            }
+        }
+    }
 }
 
 // ------------------------------------------------------------------ argsort helpers
@@ -1691,5 +1813,154 @@ extern "C" int spx_zero_rows_from_count(void *ptr, int64_t rows, int64_t row_byt
     else
         zero_rows_from_count_kernel<<<blocks, 256, 0, stream>>>((uint16_t *)ptr, rows, row_bytes / 2, count);
     SPX_CHECK_LAUNCH("zero_rows_from_count_kernel");
+    return 0;
+}
+
+// ====================================================================== rulebook onto given output coordinates
+namespace {
+// Both tables use 64-bit keys when either grid needs them.  The capacities are powers of two >= 1024, so the two key
+// arrays are contiguous, and so are the two value arrays.  The mask sorts run after the probe, so their scratch shares
+// the workspace with the hash tables.
+struct CrossWs {
+    void *src_tbl, *dst_tbl;
+    int32_t *src_vals, *dst_vals;
+    uint32_t src_cap, dst_cap;
+    bool i64;
+    size_t table_bytes, sort_bytes;
+};
+
+void carve_cross_ws(const Geom &gg, int64_t N, int64_t M, void *workspace, size_t bytes, CrossWs &w) {
+    w.i64 = needs_i64(gg, gg.in_dims) || needs_i64(gg, gg.out_dims);
+    w.src_cap = table_capacity(N);
+    w.dst_cap = table_capacity(M);
+    WorkspaceCarver ws(workspace, bytes);
+    w.src_tbl = ws.take<unsigned long long>(w.src_cap);
+    w.dst_tbl = ws.take<unsigned long long>(w.dst_cap);
+    w.src_vals = w.i64 ? ws.take<int32_t>(w.src_cap) : nullptr;
+    w.dst_vals = w.i64 ? ws.take<int32_t>(w.dst_cap) : nullptr;
+    w.table_bytes = ws.off;
+    w.sort_bytes = 2 * align_up(spx_mask_argsort_workspace_size(N > M ? N : M, (gg.kv + 31) / 32), 256);
+}
+
+int validate_cross(const spx_conv_geometry *g, int64_t N, int64_t M) {
+    if (validate_geom(g) || validate_strides(g)) return 2;
+    const int64_t kv = kernel_volume(g);
+    SPX_REQUIRE(kv <= 128, "cross_rulebook_all: kernel volume %lld not in [1,128]", (long long)kv);
+    for (int a = 0; a < g->ndim; ++a) {
+        const int64_t dims = g->in_dims[a] > g->out_dims[a] ? g->in_dims[a] : g->out_dims[a];
+        SPX_REQUIRE(g->padding[a] >= 0 && dims * g->stride[a] + g->padding[a] +
+                                              (int64_t)(g->ksize[a] - 1) * g->dilation[a] < 2147483647ll,
+                    "cross_rulebook_all: padding must be >= 0 and the coordinates of axis %d must stay below 2^31 "
+                    "- 1", a);
+    }
+    SPX_REQUIRE(N >= 0 && N < 2147483647ll && M >= 0 && M < 2147483647ll,
+                "cross_rulebook_all: bad row counts (%lld source, %lld target)", (long long)N, (long long)M);
+    return 0;
+}
+
+template <typename Table, int NDIM>
+int cross_launch(const Table &src_table, const Table &dst_table, const Geom &gg, const int32_t *indices, int64_t N,
+                 const int32_t *num_valid, const int32_t *out_indices, int64_t M, const int32_t *out_num_valid,
+                 int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd, uint32_t *mask_bwd, cudaStream_t stream) {
+    cross_insert_kernel<Table, NDIM><<<(unsigned)div_up64(N + M, CROSS_THREADS), CROSS_THREADS, 0, stream>>>(
+        src_table, dst_table, gg, indices, N, num_valid, out_indices, M, out_num_valid);
+    SPX_CHECK_LAUNCH("cross_insert_kernel");
+    const unsigned blk = (unsigned)div_up64(M, CROSS_THREADS);
+    const int words = (gg.kv + 31) / 32;
+    if (gg.transposed)
+        cross_probe_kernel<Table, NDIM, true><<<blk, CROSS_THREADS, 0, stream>>>(
+            src_table, dst_table, gg, out_indices, M, out_num_valid, N, pair_fwd, pair_bwd, mask_fwd, mask_bwd, words);
+    else
+        cross_probe_kernel<Table, NDIM, false><<<blk, CROSS_THREADS, 0, stream>>>(
+            src_table, dst_table, gg, out_indices, M, out_num_valid, N, pair_fwd, pair_bwd, mask_fwd, mask_bwd, words);
+    SPX_CHECK_LAUNCH("cross_probe_kernel");
+    return 0;
+}
+
+template <typename Table>
+int cross_tables(const Table &src_table, const Table &dst_table, const Geom &gg, const int32_t *indices, int64_t N,
+                 const int32_t *num_valid, const int32_t *out_indices, int64_t M, const int32_t *out_num_valid,
+                 int32_t *pair_fwd, int32_t *pair_bwd, uint32_t *mask_fwd, uint32_t *mask_bwd, cudaStream_t stream) {
+    switch (gg.ndim) {
+        case 1: return cross_launch<Table, 1>(src_table, dst_table, gg, indices, N, num_valid, out_indices, M,
+                                              out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+        case 2: return cross_launch<Table, 2>(src_table, dst_table, gg, indices, N, num_valid, out_indices, M,
+                                              out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+        case 3: return cross_launch<Table, 3>(src_table, dst_table, gg, indices, N, num_valid, out_indices, M,
+                                              out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+        default: return cross_launch<Table, 4>(src_table, dst_table, gg, indices, N, num_valid, out_indices, M,
+                                               out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+    }
+}
+}  // namespace
+
+extern "C" size_t spx_cross_rulebook_all_workspace_size(const spx_conv_geometry *g, int64_t N, int64_t M) {
+    if (!g || g->ndim < 1 || g->ndim > SPX_MAX_NDIM || N < 0 || M < 0) return 0;
+    CrossWs w;
+    carve_cross_ws(make_geom(g, false), N, M, nullptr, SIZE_MAX, w);
+    return align_up(w.table_bytes > w.sort_bytes ? w.table_bytes : w.sort_bytes, 256) + 256;
+}
+
+extern "C" int spx_cross_rulebook_all(const spx_conv_geometry *g, const int32_t *src_indices, int64_t N,
+                                      const int32_t *num_valid, const int32_t *out_indices, int64_t M,
+                                      const int32_t *out_num_valid, int32_t *pair_fwd, int32_t *pair_bwd,
+                                      uint32_t *mask_fwd, uint32_t *mask_bwd, int32_t *argsort_fwd,
+                                      int32_t *argsort_bwd, int do_sort, int32_t *table_fwd, uint32_t *tmask_fwd,
+                                      int32_t *table_bwd, uint32_t *tmask_bwd, void *workspace,
+                                      size_t workspace_bytes, spx_stream_t stream_) {
+    if (validate_cross(g, N, M)) return 2;
+    SPX_REQUIRE(workspace, "cross_rulebook_all: NULL pointer argument (workspace)");
+    SPX_REQUIRE(M == 0 || (out_indices && pair_fwd && mask_fwd && argsort_fwd && table_fwd && tmask_fwd),
+                "cross_rulebook_all: NULL pointer argument (out_indices, pair_fwd, mask_fwd, argsort_fwd, table_fwd, "
+                "tmask_fwd)");
+    SPX_REQUIRE(N == 0 || (src_indices && pair_bwd && mask_bwd),
+                "cross_rulebook_all: NULL pointer argument (src_indices, pair_bwd, mask_bwd)");
+    const bool train = argsort_bwd != nullptr;
+    SPX_REQUIRE(N == 0 || ((table_bwd != nullptr) == train && (tmask_bwd != nullptr) == train),
+                "cross_rulebook_all: argsort_bwd, table_bwd and tmask_bwd must all be given (training) or all be "
+                "NULL (inference)");
+    if (N > 0) SPX_REQUIRE_ALIGNED16(src_indices, "cross_rulebook_all");
+    if (M > 0) SPX_REQUIRE_ALIGNED16(out_indices, "cross_rulebook_all");
+    const size_t need = spx_cross_rulebook_all_workspace_size(g, N, M);
+    SPX_REQUIRE(workspace_bytes >= need, "cross_rulebook_all: workspace too small: need %zu, have %zu", need,
+                workspace_bytes);
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const Geom gg = make_geom(g, false);
+    const int kv = gg.kv, words = (kv + 31) / 32;
+    CrossWs w;
+    carve_cross_ws(gg, N, M, workspace, workspace_bytes, w);
+    if (N > 0) {                                  // the probe scatters into the backward direction
+        SPX_CHECK_CUDA(cudaMemsetAsync(pair_bwd, 0xFF, (size_t)kv * N * 4, stream));
+        SPX_CHECK_CUDA(cudaMemsetAsync(mask_bwd, 0, (size_t)N * words * 4, stream));
+    }
+    if (M > 0) {
+        const size_t slots = (size_t)w.src_cap + w.dst_cap;      // each pair of arrays is contiguous
+        SPX_CHECK_CUDA(cudaMemsetAsync(w.src_tbl, 0xFF, slots * 8, stream));
+        if (w.i64) SPX_CHECK_CUDA(cudaMemsetAsync(w.src_vals, 0x7F, slots * 4, stream));
+        int rc;
+        if (w.i64)
+            rc = cross_tables(Table64{(long long *)w.src_tbl, w.src_vals, w.src_cap - 1},
+                              Table64{(long long *)w.dst_tbl, w.dst_vals, w.dst_cap - 1}, gg, src_indices, N, num_valid,
+                              out_indices, M, out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+        else
+            rc = cross_tables(Table32{(unsigned long long *)w.src_tbl, w.src_cap - 1},
+                              Table32{(unsigned long long *)w.dst_tbl, w.dst_cap - 1}, gg, src_indices, N, num_valid,
+                              out_indices, M, out_num_valid, pair_fwd, pair_bwd, mask_fwd, mask_bwd, stream);
+        if (rc) return rc;
+    }
+    if (M > 0 && N > 0)
+        return conv_sort_and_tiles(kv, N, M, pair_fwd, pair_bwd, mask_fwd, mask_bwd, argsort_fwd, argsort_bwd, do_sort,
+                                   table_fwd, tmask_fwd, table_bwd, tmask_bwd, workspace, w.sort_bytes, stream_);
+    // one side empty: the other side's sort and tile table alone
+    if (M > 0) {
+        if (int rc = spx_mask_argsort(mask_fwd, argsort_fwd, M, words, kv, do_sort, workspace, w.sort_bytes, stream_))
+            return rc;
+        return spx_build_tile_table(pair_fwd, M, kv, argsort_fwd, mask_fwd, M, table_fwd, tmask_fwd, stream_);
+    }
+    if (N > 0 && train) {
+        if (int rc = spx_mask_argsort(mask_bwd, argsort_bwd, N, words, kv, do_sort, workspace, w.sort_bytes, stream_))
+            return rc;
+        return spx_build_tile_table(pair_bwd, N, kv, argsort_bwd, mask_bwd, N, table_bwd, tmask_bwd, stream_);
+    }
     return 0;
 }

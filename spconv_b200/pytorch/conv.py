@@ -232,11 +232,18 @@ class SparseConvolution(SparseModule):
             t_bwd = torch.empty((kv, 0), dtype=torch.int32, device=features.device)     # no backward will run
         return Fsp.depthwise_conv(features, weight, t_fwd, t_bwd, n_out, timer, bias, act_alpha, act_type)
 
-    def forward(self, input: SparseConvTensor, add_input: Optional[SparseConvTensor] = None):
+    def forward(self, input: SparseConvTensor, add_input: Optional[SparseConvTensor] = None, *,
+                target: Optional[SparseConvTensor] = None):
+        """``target``: convolve onto the coordinates of this tensor instead of the layer's own output set (SubM,
+        strided and transposed layers, depthwise included).  It must have the input's ``batch_size`` and the layer's
+        output spatial shape; the output takes its ``indices``, ``spatial_shape``, ``num_valid`` and a copy of its
+        ``indice_dict``.  Only the input features, the weight and the bias get gradients.  The rulebook is
+        registered under ``indice_key``: a later layer of the same geometry on the same input and target index tensors,
+        given a target that carries the key, reuses it, and an inverse conv with the key walks it back to the input's coordinates."""
         return self._conv_forward(self.training, input, self.weight, self.bias, add_input,
                                   name=self.name, sparse_unique_name=self._sparse_unique_name,
                                   act_type=self.act_type, act_alpha=self.act_alpha,
-                                  act_beta=self.act_beta)
+                                  act_beta=self.act_beta, target=target)
 
     def _out_spatial_shape(self, spatial_shape):
         if self.subm:
@@ -246,6 +253,79 @@ class SparseConvolution(SparseModule):
                                               self.padding, self.dilation, self.output_padding)
         return ops.get_conv_output_size(spatial_shape, self.kernel_size, self.stride,
                                         self.padding, self.dilation)
+
+    # ------------------------------------------------------------------ convolution onto given coordinates
+    def _check_target(self, input: SparseConvTensor, target: SparseConvTensor, algo: ConvAlgo) -> None:
+        """Every refusal of a ``target`` happens here, on the host, before any launch."""
+        if not isinstance(target, SparseConvTensor):
+            raise TypeError(f"target must be a SparseConvTensor, got {type(target).__name__}")
+        if self.inverse:
+            raise ValueError("an inverse conv restores the coordinates of the conv sharing its indice_key: it takes "
+                             "no target")
+        if algo == ConvAlgo.MaskSplitImplicitGemm:
+            raise NotImplementedError("a conv onto given coordinates does not support ConvAlgo.MaskSplitImplicitGemm: "
+                                      "use ConvAlgo.MaskImplicitGemm or ConvAlgo.Native")
+        if int(np.prod(self.kernel_size)) > 128:
+            raise NotImplementedError(f"a conv onto given coordinates supports kernel volume <= 128, this layer has "
+                                      f"{self.kernel_size}")
+        if target.batch_size != input.batch_size:
+            raise ValueError(f"target batch_size {target.batch_size} differs from the input's {input.batch_size}")
+        want = self._out_spatial_shape(input.spatial_shape)
+        if target.indices.shape[1] != input.indices.shape[1] or list(target.spatial_shape) != list(want):
+            raise ValueError(f"target spatial shape {target.spatial_shape} (indices {tuple(target.indices.shape)}) "
+                             f"must be this layer's output shape {want} for the input's {input.spatial_shape}")
+
+    def _cross_geometry(self) -> Tuple[List[int], List[int], bool]:
+        """(stride, padding, transposed) of the relation a target is read through; SubM is stride 1, pad (k//2)*d."""
+        if self.subm:
+            return [1] * self.ndim, [(k // 2) * d for k, d in zip(self.kernel_size, self.dilation)], False
+        return list(self.stride), list(self.padding), bool(self.transposed)
+
+    def _cross_rulebook(self, input: SparseConvTensor, target: Optional[SparseConvTensor], algo: ConvAlgo):
+        """The rulebook onto ``target``'s coordinates (``ops.get_indice_pairs_to``), reused from ``target``'s
+        ``indice_dict`` under ``indice_key`` when present (built on the same input and target index tensors); with ``target`` None, the one under ``indice_key`` in the
+        input's dict walked back by an inverse conv.  Returns ``_rulebook``'s 4-tuple in the implicit-GEMM form."""
+        if target is None:
+            datas = input.find_indice_pair(self.indice_key)
+            self._check_inverse_reuse_valid(input, input.spatial_shape, datas)
+            rb = (datas.indices, datas.pair_bwd, datas.pair_fwd, datas.pair_mask_bwd_splits,
+                  datas.pair_mask_fwd_splits, datas.mask_argsort_bwd_splits, datas.mask_argsort_fwd_splits, datas.masks)
+            return rb, input.indice_dict.copy(), datas.spatial_shape, datas.in_voxel_num
+        stride, padding, transposed = self._cross_geometry()
+        indice_dict = target.indice_dict.copy()
+        datas = target.find_indice_pair(self.indice_key)
+        if datas is not None:
+            same = (getattr(datas, "cross", False) and self.kernel_size == datas.ksize and stride == datas.stride
+                    and padding == datas.padding and self.dilation == datas.dilation
+                    and transposed == datas.transposed and input.spatial_shape == datas.spatial_shape
+                    and target.spatial_shape == datas.out_spatial_shape
+                    and input.indices.shape[0] == datas.indices.shape[0]
+                    and target.indices.shape[0] == datas.out_indices.shape[0]
+                    # the same coordinate tensors, not only the same row counts (padded tensors all share theirs)
+                    and input.indices.data_ptr() == datas.indices.data_ptr()
+                    and target.indices.data_ptr() == datas.out_indices.data_ptr())
+            if not same:
+                raise ValueError(f"the rulebook under indice_key {self.indice_key} in the target does not match this "
+                                 f"layer and input: expect a conv onto given coordinates with ksize {datas.ksize} "
+                                 f"stride {datas.stride} padding {datas.padding} dilation {datas.dilation} from the "
+                                 f"{datas.indices.shape[0]} voxels in {datas.spatial_shape} it was built on onto its "
+                                 f"{datas.out_indices.shape[0]} target voxels in {datas.out_spatial_shape}")
+        else:
+            with input._timer.namespace("gen_pairs"):
+                res = ops.get_indice_pairs_to(input.indices, target.indices, input.batch_size, input.spatial_shape,
+                                              target.spatial_shape, self.kernel_size, stride, padding, self.dilation,
+                                              transposed, True, input.num_valid, target.num_valid)
+            # the record keeps the target's own index tensor (res[0] may be an aligned copy of it)
+            datas = ImplicitGemmIndiceData.from_rulebook(
+                (target.indices, *res[1:]), input.indices, input.num_valid, False, spatial_shape=input.spatial_shape,
+                out_spatial_shape=target.spatial_shape, algo=algo, ksize=self.kernel_size, stride=stride,
+                dilation=self.dilation, padding=padding, cross=True, transposed=transposed)
+            datas.out_voxel_num = target.num_valid
+            if self.indice_key is not None:
+                indice_dict[self.indice_key] = datas
+        rb = (target.indices, datas.pair_fwd, datas.pair_bwd, datas.pair_mask_fwd_splits, datas.pair_mask_bwd_splits,
+              datas.mask_argsort_fwd_splits, datas.mask_argsort_bwd_splits, datas.masks)
+        return rb, indice_dict, target.spatial_shape, target.num_valid
 
     def _rulebook_error(self, tag, indices, batch_size, spatial_shape, algo):
         print(f"[Exception|{tag}]indices={indices.shape},bs={batch_size},ss={spatial_shape},"
@@ -269,6 +349,9 @@ class SparseConvolution(SparseModule):
         num_valid = input.num_valid
         indice_dict = input.indice_dict.copy()
         datas = input.find_indice_pair(self.indice_key)
+        if getattr(datas, "cross", False):
+            raise ValueError(f"indice_key {self.indice_key} holds the rulebook of a conv onto given coordinates: only a "
+                             "layer given a target carrying it or a float inverse conv can use it")
         if datas is not None:
             assert algo == datas.algo, ("due to limitation of pytorch, you must provide same algo "
                                         "to layers share same indice key.")
@@ -369,7 +452,8 @@ class SparseConvolution(SparseModule):
                       channel_scale: Optional[torch.Tensor] = None,
                       output_scale: Optional[float] = None, name: Optional[str] = None,
                       sparse_unique_name: str = "", act_type: Activation = Activation.None_,
-                      act_alpha: float = 0, act_beta: float = 0):
+                      act_alpha: float = 0, act_beta: float = 0,
+                      target: Optional[SparseConvTensor] = None):
         assert isinstance(input, SparseConvTensor)
         assert input.features.shape[1] == self.in_channels, "channel size mismatch"
         if training:
@@ -382,8 +466,14 @@ class SparseConvolution(SparseModule):
         bias_infer = None if training else bias
         out_spatial_shape = self._out_spatial_shape(input.spatial_shape)
         out_tensor = input.shadow_copy()
+        algo = self.algo if input.force_algo is None else input.force_algo
+        if target is not None:
+            self._check_target(input, target, algo)
+        # a conv onto given coordinates, or an inverse conv walking one back: dense tables whatever the algo
+        cross = target is not None or (self.inverse and getattr(input.find_indice_pair(self.indice_key), "cross",
+                                                                False))
 
-        if self.conv1x1:
+        if self.conv1x1 and not cross:
             if self.depthwise:
                 feats = features * weight.view(self.out_channels)
             else:
@@ -397,11 +487,14 @@ class SparseConvolution(SparseModule):
 
         if not features.is_contiguous():
             features = features.contiguous()
-        algo = self.algo if input.force_algo is None else input.force_algo
         timer = input._timer
-        rb, indice_dict, out_spatial_shape, num_valid = self._rulebook(input, training, algo, out_tensor)
+        if cross:
+            rb, indice_dict, out_spatial_shape, num_valid = self._cross_rulebook(input, target, algo)
+        else:
+            rb, indice_dict, out_spatial_shape, num_valid = self._rulebook(input, training, algo, out_tensor)
+        is_subm = self.subm and not cross          # cross tables are not symmetric
 
-        if algo == ConvAlgo.Native:
+        if algo == ConvAlgo.Native and not cross:
             outids, indice_pairs, indice_pair_num = rb
             if self.depthwise:
                 out_features = self._depthwise_native(features, weight, indice_pairs, indice_pair_num,
@@ -418,18 +511,18 @@ class SparseConvolution(SparseModule):
             if self.depthwise:
                 # the whole dense table is walked: no tile table, mask sort or split is needed.  SubM (whose
                 # inference rulebook has no pair_bwd) walks pair_fwd with mirrored offsets in the backward
-                out_features = Fsp.depthwise_conv(features, weight, pair_fwd, None if self.subm else pair_bwd,
+                out_features = Fsp.depthwise_conv(features, weight, pair_fwd, None if is_subm else pair_bwd,
                                                   num_activate_out, timer, bias_infer, act_alpha, act_type)
             elif training:
                 out_features = Fsp.implicit_gemm(features, weight, pair_fwd, pair_bwd, mask_fwd,
                                                  mask_bwd, sort_fwd, sort_bwd, num_activate_out,
-                                                 masks, training, self.subm, timer,
+                                                 masks, training, is_subm, timer,
                                                  self.fp32_accum, bias_infer, act_alpha, act_beta,
                                                  act_type)
             else:
                 out_features, _, _ = ops.implicit_gemm(
                     features, weight, pair_fwd, mask_fwd, sort_fwd, num_activate_out, masks,
-                    training, self.subm, timer, self.fp32_accum, bias_infer, act_alpha, act_beta,
+                    training, is_subm, timer, self.fp32_accum, bias_infer, act_alpha, act_beta,
                     act_type, 1.0 if output_scale is None else output_scale, channel_scale,
                     output_add=None, output_add_scale=0.0,
                     output_dtype=weight.dtype if output_scale is None else None)
@@ -447,6 +540,8 @@ class SparseConvolution(SparseModule):
         out_tensor.indices = outids
         out_tensor.indice_dict = indice_dict
         out_tensor.spatial_shape = out_spatial_shape
+        if target is not None and (input.bound_status or target.bound_status):
+            out_tensor.bound_status = {**(input.bound_status or {}), **(target.bound_status or {})}
         if add_input is not None:
             out_tensor = out_tensor.replace_feature(
                 _activate(out_tensor.features + add_input.features, self.act_type, self.act_alpha,

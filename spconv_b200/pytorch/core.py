@@ -150,6 +150,10 @@ class ImplicitGemmIndiceData:
     # built ahead of the forward pass by RulebookPrefetcher: the only case in which a strided conv may
     # pick its rulebook up from the indice_dict (the reference lets SubM layers alone reuse a key)
     prefetched: bool = False
+    # the rulebook of a conv onto given coordinates (SparseConvolution's ``target``): stride / padding are those of
+    # the relation (SubM: 1 and (k // 2) * d), ``transposed`` its kind
+    cross: bool = False
+    transposed: bool = False
 
     @classmethod
     def from_rulebook(cls, res, indices: torch.Tensor, in_voxel_num, is_subm: bool, **geometry):

@@ -427,6 +427,77 @@ def get_indice_pairs_implicit_gemm(indices: torch.Tensor, batch_size: int,
                                   bound, bound_status)
 
 
+def _row_count(num_valid: Optional[torch.Tensor], what: str) -> Optional[torch.Tensor]:
+    if num_valid is None:
+        return None
+    _require_cuda(num_valid, what)
+    if num_valid.dtype != torch.int32 or num_valid.numel() != 1:
+        raise ValueError(f"{what} must be a device int32 tensor of one element, got {num_valid.dtype} "
+                         f"{tuple(num_valid.shape)}")
+    return num_valid
+
+
+def get_indice_pairs_to(indices: torch.Tensor, out_indices: torch.Tensor, batch_size: int,
+                        spatial_shape: List[int], out_spatial_shape: List[int], ksize: List[int], stride: List[int],
+                        padding: List[int], dilation: List[int], transpose: bool, is_train: bool,
+                        num_valid: Optional[torch.Tensor] = None, out_num_valid: Optional[torch.Tensor] = None,
+                        do_sort: bool = True):
+    """Masked implicit-GEMM rulebook of a convolution from ``indices`` (grid ``spatial_shape``) onto the given
+    coordinates ``out_indices`` (grid ``out_spatial_shape``), ``spx_cross_rulebook_all``.  Returns the 9-tuple of
+    :func:`get_indice_pairs_implicit_gemm` with ``out_inds = out_indices``.
+
+    The geometry is taken as given (a SubM layer passes stride 1 and padding ``(k // 2) * d``).  Source rows from
+    ``num_valid`` on, rows whose batch or coordinates are out of range and all but the lowest row of a duplicated
+    coordinate take part in no pair; the same holds for the target rows against ``out_num_valid`` and
+    ``out_spatial_shape``.  Target row o reads source coordinate ``o * s - p + r * d`` per axis (regular) or
+    ``(o + p - r * d) / s`` when exact (``transpose``).  ``pair_bwd`` and the backward mask are always built; their
+    argsort and tile table only with ``is_train``.  The output count is the caller's, so nothing is read back and
+    the call captures in a CUDA graph."""
+    _require_cuda(indices, "indices")
+    _require_cuda(out_indices, "out_indices")
+    for t, what in ((indices, "indices"), (out_indices, "out_indices")):
+        if t.dtype != torch.int32 or t.dim() != 2:
+            raise ValueError(f"{what} must be int32 [rows, ndim + 1], got {t.dtype} {tuple(t.shape)}")
+    ndim = indices.shape[1] - 1
+    if out_indices.shape[1] != ndim + 1 or len(spatial_shape) != ndim or len(out_spatial_shape) != ndim:
+        raise ValueError(f"source {tuple(indices.shape)} / target {tuple(out_indices.shape)} indices and the shapes "
+                         f"{list(spatial_shape)} / {list(out_spatial_shape)} must have the same ndim")
+    kv = _prod(ksize)
+    if kv > 128:
+        raise NotImplementedError("a rulebook onto given coordinates supports kernel volume <= 128")
+    num_valid = _row_count(num_valid, "num_valid")
+    out_num_valid = _row_count(out_num_valid, "out_num_valid")
+    lib = _lib()
+    dev = indices.device
+    indices, out_indices = _dense(indices), _dense(out_indices)
+    n_in, m = indices.shape[0], out_indices.shape[0]
+    words = (kv + 31) // 32
+    geo = _geometry(indices, batch_size, spatial_shape, out_spatial_shape, ksize, stride, padding, dilation, transpose)
+    pair_fwd = torch.empty((kv, m), dtype=torch.int32, device=dev)
+    pair_bwd = torch.empty((kv, n_in), dtype=torch.int32, device=dev)
+    mask_fwd = torch.empty((1, m, words), dtype=torch.int32, device=dev)
+    mask_bwd = torch.empty((1, n_in, words), dtype=torch.int32, device=dev)
+    sort_fwd = torch.empty((1, m), dtype=torch.int32, device=dev)
+    sort_bwd = torch.empty((1, n_in), dtype=torch.int32, device=dev) if is_train else None
+    t_fwd, tm_fwd = _alloc_tile_tables(m, kv, dev)
+    t_bwd, tm_bwd = _alloc_tile_tables(n_in, kv, dev) if is_train else (None, None)
+    ws = _bytes(lib.spx_cross_rulebook_all_workspace_size(ctypes.byref(geo), n_in, m), dev)
+    _cabi.check(lib.spx_cross_rulebook_all(
+        ctypes.byref(geo), _ptr(indices), n_in, _ptr(num_valid), _ptr(out_indices), m, _ptr(out_num_valid),
+        _ptr(pair_fwd), _ptr(pair_bwd), _ptr(mask_fwd), _ptr(mask_bwd), _ptr(sort_fwd), _ptr(sort_bwd),
+        int(bool(do_sort)), _ptr(t_fwd), _ptr(tm_fwd), _ptr(t_bwd), _ptr(tm_bwd), ws.data_ptr(), ws.numel(),
+        _stream()), "cross_rulebook_all")
+    masks = [np.array([0xffffffff], dtype=np.uint32)]
+    sf = sort_fwd[0]
+    sf._spx_tile_cache = (_tile_key(pair_fwd, sf, m), t_fwd, tm_fwd)
+    res = (out_indices, _zero_counts(kv, dev), pair_fwd, pair_bwd, [mask_fwd[0]])
+    if not is_train:
+        return (*res, [], [sf], [], masks)
+    sb = sort_bwd[0]
+    sb._spx_tile_cache = (_tile_key(pair_bwd, sb, n_in), t_bwd, tm_bwd)
+    return (*res, [mask_bwd[0]], [sf], [sb], masks)
+
+
 # ---------------------------------------------------------------------------- GEMM descriptor
 def _f32_mode() -> int:
     return _cabi.SPX_F32_TF32 if SPCONV_ALLOW_TF32 else _cabi.SPX_F32_EXACT
