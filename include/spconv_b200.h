@@ -926,8 +926,10 @@ int spx_implicit_gemm_fwd_int8(const spx_gemm_desc *d, const int8_t *features,
  * out_dtype SPX_F32 stores y, SPX_F16 / SPX_BF16 y rounded once to nearest-even, SPX_E4M3
  * satfinite_rne(y / out_scale): ties to even, beyond +-448 (and +-Inf) saturates to +-448, NaN stays NaN.
  * C and K multiples of 32 up to 256 with 16-byte aligned operands run on the tensor cores (wgmma e4m3); every
- * other shape on the FMA kernel, which gives the same result for the same summation order (the tensor cores
- * sum a k-step's products in an order of their own).  SPX_FORCE_SIMT / SPX_FORCE_TC apply.
+ * other shape on the FMA kernel, which sums in fp32 throughout.  The tensor cores sum each kernel offset's
+ * channels in the FP8 MMA, which keeps about 14 bits per 32-channel step, and add the offsets in fp32: a row's
+ * error stays below (33 * ceil(C / 32) * 2^-13 + offsets * 2^-24) * sum |x| |W| before the epilogue.
+ * SPX_FORCE_SIMT / SPX_FORCE_TC apply.
  */
 typedef struct spx_fp8_gemm {
     const void *features;       /* e4m3 [n_in, C] */

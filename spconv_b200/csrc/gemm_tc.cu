@@ -84,6 +84,7 @@ struct TcParams {
     float output_add_scale;
     // fp8 epilogue (KIND_E4M3): scale = w_scale, bias_f32 = bias, output_add = the residual in out_dtype
     const float *in_scale, *add_scale, *out_scale;
+    int ldy;                // elements between output (and residual) rows: c_out, of which this pass writes N
 };
 
 // iterate set bits of a <=128-bit tile mask in ascending order (register-only: no indexed array)
@@ -170,7 +171,7 @@ __device__ __forceinline__ void epilogue_frag(const TcParams &p, const float *ec
 }
 
 // The fp8 epilogue (gemm.cuh fp8_epilogue) of one warpgroup fragment, same layout as epilogue_frag.  ec[j] = s_j,
-// ec[N + j] = bias.  add_s / out_s: the residual and output scales, read once per tile.
+// ec[N + j] = bias.  add_s / out_s: the residual and output scales, read once per tile.  Rows are p.ldy apart.
 template <int OUT, int N>
 __device__ __forceinline__ void epilogue_fp8(const TcParams &p, const float *ec, const float (&acc)[N / 2],
                                              int64_t dst_lo, int64_t dst_hi, int lane, float add_s, float out_s) {
@@ -181,14 +182,14 @@ __device__ __forceinline__ void epilogue_fp8(const TcParams &p, const float *ec,
     for (int h = 0; h < 2; ++h) {
         const int64_t dst = h ? dst_hi : dst_lo;
         if (dst < 0) continue;
-        uint8_t *row_ptr = (uint8_t *)p.y + dst * (int64_t)N * EB;
+        uint8_t *row_ptr = (uint8_t *)p.y + dst * (int64_t)p.ldy * EB;
 #pragma unroll
         for (int nb = 0; nb < N / 8; ++nb) {
             const int col = nb * 8 + 2 * (lane & 3);
             float f[2];
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
-                const float a = add ? load_out_elem<OUT>(add, dst * (int64_t)N + col + j) : 0.f;
+                const float a = add ? load_out_elem<OUT>(add, dst * (int64_t)p.ldy + col + j) : 0.f;
                 f[j] = fp8_epilogue(acc[nb * 4 + 2 * h + j], ec[col + j], bias, col + j, add != nullptr, a, add_s,
                                     p.act, p.alpha);
             }
@@ -448,6 +449,11 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
                                            : gmma_desc_hi(16u, 8u * p.span_b, p.span_b);
         const uint32_t b_sub16 = (uint32_t)p.b_sub_bytes >> 4;
         Acc acc[N / 2];
+        // e4m3: the FP8 MMA adds each k-step's products with about 14 bits kept, aligned to the largest
+        // addend, so a large running sum would swallow the small products of later offsets.  Each offset's
+        // k-steps (at most 8) therefore start from zero in `acc`, and the finished offset is added into `sum`
+        // in fp32 registers (DeepSeek-V3 report section 3.3.2 promotes every 128 channels the same way).
+        float sum[KIND == KIND_E4M3 ? N / 2 : 1];
         for (int local = 0;; ++local) {
             uint32_t tm[4];
             const int tile = read_info(local, tm);
@@ -467,6 +473,10 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
             }
 #pragma unroll
             for (int i = 0; i < N / 2; ++i) acc[i] = (Acc)0;
+            if constexpr (KIND == KIND_E4M3) {
+#pragma unroll
+                for (int i = 0; i < N / 2; ++i) sum[i] = 0.f;
+            }
             BitIter it(tm);
             // One wgmma group stays in flight across stages: stage s is released once the group of
             // stage s+1 is issued (wait_group 1), so the next stage's full-barrier wait and MMA issue
@@ -504,13 +514,26 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
                     }
                 }
                 wgmma_commit();
-                wgmma_wait<1>();
-                fence_regs(acc);
-                if (held >= 0) {
+                if constexpr (KIND == KIND_E4M3) {
+                    // promote: the offset's group must finish before its sum leaves the accumulator
+                    wgmma_wait<0>();
+                    fence_regs(acc);
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty[held]);      // this warp is done reading that stage
+                    if (lane == 0) mbar_arrive(&empty[stage]);
+#pragma unroll
+                    for (int i = 0; i < N / 2; ++i) {
+                        sum[i] = __fadd_rn(sum[i], acc[i]);
+                        acc[i] = 0.f;
+                    }
+                } else {
+                    wgmma_wait<1>();
+                    fence_regs(acc);
+                    if (held >= 0) {
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty[held]);      // this warp is done reading that stage
+                    }
+                    held = stage;
                 }
-                held = stage;
                 if (++stage == p.stages) { stage = 0; phase ^= 1u; }
             }
             wgmma_wait<0>();
@@ -531,10 +554,10 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
             } else {
                 const float add_s = p.add_scale ? __ldg(p.add_scale) : 1.f;
                 const float out_s = p.out_dtype == SPX_E4M3 ? __ldg(p.out_scale) : 1.f;
-                if (p.out_dtype == SPX_E4M3) epilogue_fp8<SPX_E4M3, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
-                else if (p.out_dtype == SPX_F32) epilogue_fp8<SPX_F32, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
-                else if (p.out_dtype == SPX_F16) epilogue_fp8<SPX_F16, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
-                else epilogue_fp8<SPX_BF16, N>(p, ec, acc, d_lo, d_hi, lane, add_s, out_s);
+                if (p.out_dtype == SPX_E4M3) epilogue_fp8<SPX_E4M3, N>(p, ec, sum, d_lo, d_hi, lane, add_s, out_s);
+                else if (p.out_dtype == SPX_F32) epilogue_fp8<SPX_F32, N>(p, ec, sum, d_lo, d_hi, lane, add_s, out_s);
+                else if (p.out_dtype == SPX_F16) epilogue_fp8<SPX_F16, N>(p, ec, sum, d_lo, d_hi, lane, add_s, out_s);
+                else epilogue_fp8<SPX_BF16, N>(p, ec, sum, d_lo, d_hi, lane, add_s, out_s);
             }
         }
     }
@@ -718,7 +741,7 @@ static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t st
 }
 
 // instantiated (channels x element bytes) combinations: rows of 32..512 bytes, N = 16..256 output
-// channels (tf32: 16..128, int8 and e4m3: 32..256).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
+// channels (tf32: 16..128, int8: 32..256, e4m3: 32..128).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
 // gathered tile plus a weight slice of 128 or more rows puts two stages over TC_SMEM_BUDGET.
 template <int KIND, int CPR>
 static int launch_tc_cpr(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
@@ -727,7 +750,7 @@ static int launch_tc_cpr(const CUtensorMap &tm, const TcParams &p, cudaStream_t 
         case 32: return launch_tc_n<KIND, CPR, 32>(tm, p, stream);
         case 64: return launch_tc_n<KIND, CPR, 64>(tm, p, stream);
         case 128: if constexpr (CPR != 32) return launch_tc_n<KIND, CPR, 128>(tm, p, stream); break;
-        case 256: if constexpr (KIND != KIND_TF32 && CPR != 32) return launch_tc_n<KIND, CPR, 256>(tm, p, stream); break;
+        case 256: if constexpr (KIND != KIND_TF32 && KIND != KIND_E4M3 && CPR != 32) return launch_tc_n<KIND, CPR, 256>(tm, p, stream); break;
     }
     set_error("tc_gather_gemm: unsupported output channel count %d", p.n);
     return 2;
@@ -767,17 +790,33 @@ int tc_gather_gemm_int8(const Int8Args &q, cudaStream_t stream) {
     return launch_tc<KIND_I8>(tm, p, stream);
 }
 
-// e4m3 operands take the int8 operand path (1-byte K-major rows, UINT8 tensor map) with fp32 accumulators
+// e4m3 operands take the int8 operand path (1-byte K-major rows, UINT8 tensor map) with fp32 accumulators.
+// The fp32 sum beside the wgmma accumulator takes N / 2 more registers per consumer thread, which N = 256
+// cannot spare: 256 output channels run as two passes of 128, each over its half of the filter rows, scales,
+// biases, output and residual columns.
 int tc_gather_gemm_fp8(const Fp8Args &q, cudaStream_t stream) {
-    TcParams p;
-    if (fill_params(q.g, p)) return 2;
-    p.out_dtype = q.out_dtype;
-    p.epi_mode = 2;
-    p.scale = q.w_scale; p.bias_f32 = q.bias_f32; p.output_add = (const int8_t *)q.output_add;
-    p.in_scale = q.in_scale; p.add_scale = q.add_scale; p.out_scale = q.out_scale;
-    CUtensorMap tm;
-    if (make_weight_tmap(&tm, q.g.w, SPX_E4M3, q.g.kv, q.g.c_in, q.g.c_out, p.span_b)) return 2;
-    return launch_tc<KIND_E4M3>(tm, p, stream);
+    const int half = q.g.c_out > 128 ? 2 : 1;
+    const int n = q.g.c_out / half;
+    const int ob = dtype_bytes(q.out_dtype);
+    for (int h = 0; h < half; ++h) {
+        GatherGemmArgs g = q.g;
+        g.c_out = n;
+        g.w = (const uint8_t *)q.g.w + (size_t)h * n * q.g.kv * q.g.c_in;
+        g.y = (uint8_t *)q.g.y + (size_t)h * n * ob;
+        TcParams p;
+        if (fill_params(g, p)) return 2;
+        p.out_dtype = q.out_dtype;
+        p.epi_mode = 2;
+        p.scale = q.w_scale + h * n;
+        p.bias_f32 = q.bias_f32 ? q.bias_f32 + h * n : nullptr;
+        p.output_add = q.output_add ? (const int8_t *)q.output_add + (size_t)h * n * ob : nullptr;
+        p.in_scale = q.in_scale; p.add_scale = q.add_scale; p.out_scale = q.out_scale;
+        p.ldy = q.g.c_out;
+        CUtensorMap tm;
+        if (make_weight_tmap(&tm, g.w, SPX_E4M3, g.kv, g.c_in, g.c_out, p.span_b)) return 2;
+        if (int rc = launch_tc<KIND_E4M3>(tm, p, stream)) return rc;
+    }
+    return 0;
 }
 
 }  // namespace spx

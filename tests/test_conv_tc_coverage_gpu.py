@@ -531,18 +531,22 @@ def test_int8_against_exact_reference(case, oracle, cuda_dev):
         _check("int8 -> f16 out", got, relu, torch.zeros_like(relu), torch.zeros_like(relu), "f16", extra=fp32_err)
 
 
-def _compiled_instances():
+def library_symbols():
+    """the library's demangled symbol names (nm, or cuobjdump's kernel list)"""
     from spconv_b200 import _cabi
     _cabi.load()
     if shutil.which("nm"):
-        text = subprocess.run(["nm", "-C", "--defined-only", _cabi.LIB_PATH], capture_output=True, text=True,
+        return subprocess.run(["nm", "-C", "--defined-only", _cabi.LIB_PATH], capture_output=True, text=True,
                               check=True).stdout
-    elif shutil.which("cuobjdump") and shutil.which("c++filt"):
+    if shutil.which("cuobjdump") and shutil.which("c++filt"):
         dump = subprocess.run(["cuobjdump", "-res-usage", _cabi.LIB_PATH], capture_output=True, text=True,
                               check=True).stdout
-        text = subprocess.run(["c++filt"], input=dump, capture_output=True, text=True, check=True).stdout
-    else:
-        pytest.skip("neither nm nor cuobjdump is available")
+        return subprocess.run(["c++filt"], input=dump, capture_output=True, text=True, check=True).stdout
+    pytest.skip("neither nm nor cuobjdump is available")
+
+
+def _compiled_instances():
+    text = library_symbols()
     found = {("gemm", int(a), int(b), int(c))
              for a, b, c in re.findall(r"tc_gather_gemm_kernel<(\d+), (\d+), (\d+)>", text)}
     found |= {("wgrad", int(a), int(b), c == "true")
