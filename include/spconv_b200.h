@@ -322,6 +322,44 @@ int spx_implicit_gemm_wgrad(const spx_gemm_desc *d, const void *features, const 
                             void *dfilters, void *workspace, size_t workspace_bytes,
                             spx_stream_t stream);
 
+/*
+ * Grouped convolution, 1 < groups: group j maps input channels [j Cg, (j+1) Cg) to output channels [j Kg, (j+1) Kg)
+ * (Cg = c_in / groups, Kg = c_out / groups) with filter rows [j Kg, (j+1) Kg) of the filter [c_out, kv, Cg], torch's
+ * grouped convention on the KRSC filter.  The descriptor is the dense one: c_in / c_out are the totals, the row counts,
+ * tables and tile tables those of the layer's rulebook.  Cg and Kg must be multiples of 16; groups == 1 is refused
+ * (the dense entry points are the one path for it), and so is every other bad shape, before any launch.
+ *
+ * Each call runs one pass per group, in ascending j, on `stream`: the dense kernel instance for (Cg, Kg), with the
+ * same schedule and fp32 summation order, reading gathered rows at the full row stride (C or K) from the group's
+ * column offset and writing output rows the same way.  So for every group, out[:, j Kg:(j+1) Kg], din[:, j Cg:(j+1) Cg]
+ * and dW[j Kg:(j+1) Kg] equal bit for bit what spx_implicit_gemm_fwd / _dgrad / _wgrad return on the contiguous
+ * slices of that group.  Routes: fp16 / bf16 run on the tensor cores when the dense calls would at (Cg, Kg) (tile
+ * tables given, 16-byte aligned operands); fp32, in both f32 modes, and every other shape run on the FMA kernels (an
+ * fp32 call in SPX_F32_TF32 mode therefore equals the dense call in SPX_F32_EXACT mode).  Pointers must be aligned to
+ * their element size.  SPX_FORCE_SIMT / SPX_FORCE_TC apply; spx_last_kernel_family reports the route.  A tensor-core
+ * pass holds one of the tile table's scheduler slots while it runs.
+ *
+ * The weight gradient's passes reuse one workspace (spx_grouped_gemm_wgrad_workspace_size).  _push writes dfilters
+ * locally, then pushes the whole gradient to the peer group (spx_peer_push); spx_peer_finish completes the exchange.
+ */
+typedef struct spx_grouped_gemm {
+    const void *features;       /* fwd, wgrad: [n_in, c_in] */
+    const void *filters;        /* fwd, dgrad: [c_out, kv, c_in / groups] */
+    const void *out_bp;         /* dgrad, wgrad: [n_out, c_out] */
+    const void *bias;           /* fwd: [c_out] or NULL, dtype of features */
+    void *out;                  /* fwd: [n_out, c_out] */
+    void *din;                  /* dgrad: [n_in, c_in]; `pair` is the backward table, as in spx_implicit_gemm_dgrad */
+    void *dfilters;             /* wgrad: [c_out, kv, c_in / groups]; `pair` is the forward table */
+    void *workspace;            /* wgrad */
+    size_t workspace_bytes;
+    int act;                    /* fwd: spx_act */
+    float act_alpha;
+} spx_grouped_gemm;
+int spx_grouped_gemm_fwd(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, spx_stream_t stream);
+int spx_grouped_gemm_dgrad(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, spx_stream_t stream);
+size_t spx_grouped_gemm_wgrad_workspace_size(const spx_gemm_desc *d, int groups);
+int spx_grouped_gemm_wgrad(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, spx_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Data-parallel weight-gradient exchange over NVLink peer memory (SURVEY 8e).  The reference has no
  * distributed code: users wrap it in torch DDP, i.e. an NCCL all-reduce of dW after the backward
@@ -361,6 +399,10 @@ int spx_peer_error(const spx_peer_group *pg, int *error);
 int spx_implicit_gemm_wgrad_push(const spx_gemm_desc *d, const void *features, const void *out_bp,
                                  void *dfilters, void *workspace, size_t workspace_bytes,
                                  const spx_peer_group *pg, spx_stream_t stream);
+/* Grouped weight gradient (see spx_grouped_gemm_wgrad) written to a->dfilters, then pushed whole to the group;
+ * spx_peer_finish(pg, dfilters, kv*C/groups*K, dtype, scale) completes it. */
+int spx_grouped_gemm_wgrad_push(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a,
+                                const spx_peer_group *pg, spx_stream_t stream);
 /* the same exchange for an existing small tensor (bias gradients ...): push sends `data` (dtype SPX_F32 /
  * SPX_F16 / SPX_BF16), finish writes out = scale * sum over ranks (out may be data); allreduce = both */
 int spx_peer_push(const spx_peer_group *pg, const void *data, int64_t count, int dtype, spx_stream_t stream);

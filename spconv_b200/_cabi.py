@@ -119,6 +119,15 @@ class Fp8Gemm(Structure):
     ]
 
 
+class GroupedGemm(Structure):
+    """``spx_grouped_gemm``: the operands of one grouped-conv GEMM (forward, input or weight gradient)."""
+    _fields_ = [
+        ("features", c_void_p), ("filters", c_void_p), ("out_bp", c_void_p), ("bias", c_void_p), ("out", c_void_p),
+        ("din", c_void_p), ("dfilters", c_void_p), ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+        ("act", c_int), ("act_alpha", c_float),
+    ]
+
+
 class Fp8Quant(Structure):
     """``spx_fp8_quant``: the operands of one e4m3 quantisation."""
     _fields_ = [
@@ -194,6 +203,12 @@ SIGNATURES = {
                                            c_int, c_void_p, c_void_p, c_void_p, c_float, c_int,
                                            c_float, c_void_p]),
     "spx_implicit_gemm_fwd_fp8": (c_int, [POINTER(GemmDesc), POINTER(Fp8Gemm), c_void_p]),
+    "spx_grouped_gemm_fwd": (c_int, [POINTER(GemmDesc), c_int, POINTER(GroupedGemm), c_void_p]),
+    "spx_grouped_gemm_dgrad": (c_int, [POINTER(GemmDesc), c_int, POINTER(GroupedGemm), c_void_p]),
+    "spx_grouped_gemm_wgrad_workspace_size": (c_size_t, [POINTER(GemmDesc), c_int]),
+    "spx_grouped_gemm_wgrad": (c_int, [POINTER(GemmDesc), c_int, POINTER(GroupedGemm), c_void_p]),
+    "spx_grouped_gemm_wgrad_push": (c_int, [POINTER(GemmDesc), c_int, POINTER(GroupedGemm), POINTER(PeerGroup),
+                                            c_void_p]),
     "spx_fp8_quantize_workspace_size": (c_size_t, [c_int64, c_int]),
     "spx_fp8_quantize": (c_int, [POINTER(Fp8Quant), c_void_p, c_size_t, c_void_p]),
     "spx_point2voxel_workspace_size": (c_size_t, [c_int64, c_int]),

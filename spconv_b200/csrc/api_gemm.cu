@@ -203,3 +203,168 @@ extern "C" int spx_implicit_gemm_fwd_fp8(const spx_gemm_desc *d, const spx_fp8_g
     set_family(1);
     return simt_gather_gemm_fp8(q, (cudaStream_t)stream);
 }
+
+// ------------------------------------------------------------------ grouped conv (1 < groups)
+// One pass per group j, in ascending j, on the caller's stream.  Each pass is the dense (Cg -> Kg) GEMM of that
+// group (Cg = c_in / groups, Kg = c_out / groups): the same kernel family and instance as the dense entry point would
+// run on the group's contiguous slices, with the gathered and written rows read at the full row stride.  The route is
+// chosen once, from group 0 (every group has the same shape, and its column offsets are multiples of 32 bytes, so it
+// has the same alignment); every argument is checked before the first launch.
+
+static int check_grouped(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, const char *who) {
+    if (check_desc(d, who)) return 2;
+    SPX_REQUIRE(a != nullptr, "%s: argument block is NULL", who);
+    SPX_REQUIRE(groups > 1, "%s: groups %d must be at least 2 (groups == 1 is the dense entry point)", who, groups);
+    SPX_REQUIRE(d->dtype == SPX_F32 || d->dtype == SPX_F16 || d->dtype == SPX_BF16, "%s: dtype %d not supported", who,
+                d->dtype);
+    SPX_REQUIRE(d->c_in % groups == 0 && d->c_out % groups == 0, "%s: groups %d must divide C %d and K %d", who, groups,
+                d->c_in, d->c_out);
+    SPX_REQUIRE((d->c_in / groups) % 16 == 0 && (d->c_out / groups) % 16 == 0,
+                "%s: group widths C/groups = %d and K/groups = %d must be multiples of 16", who, d->c_in / groups,
+                d->c_out / groups);
+    return 0;
+}
+
+// every tensor the FMA kernels read element by element must at least be aligned to its element
+static int check_elem_aligned(const void *p, int dtype, const char *who, const char *what) {
+    SPX_REQUIRE(((uintptr_t)p % (uintptr_t)dtype_bytes(dtype)) == 0, "%s: %s is not aligned to its element size", who,
+                what);
+    return 0;
+}
+
+static bool route_tc_16bit(int dtype, bool tc_supported) {
+    return !force_simt() && (dtype == SPX_F16 || dtype == SPX_BF16) && tc_supported;
+}
+
+// the dense GEMM of group j: operands at the group's columns, filter rows and bias
+static GatherGemmArgs group_args(const GatherGemmArgs &all, int groups, int j, size_t e) {
+    GatherGemmArgs g = all;
+    g.c_in = all.c_in / groups; g.c_out = all.c_out / groups;
+    const int cx = g.cx(), cy = g.cy();
+    g.x = (const uint8_t *)all.x + (size_t)j * cx * e;
+    g.y = (uint8_t *)all.y + (size_t)j * cy * e;
+    g.w = (const uint8_t *)all.w + (size_t)j * g.c_out * g.kv * g.c_in * e;
+    g.bias = all.bias ? (const uint8_t *)all.bias + (size_t)j * g.c_out * e : nullptr;
+    return g;
+}
+
+static int run_grouped_gemm(const GatherGemmArgs &all, int groups, const char *who, cudaStream_t stream) {
+    if (all.rows == 0) return 0;
+    const size_t e = (size_t)dtype_bytes(all.dtype);
+    const GatherGemmArgs g0 = group_args(all, groups, 0, e);
+    const bool tc_ok = route_tc_16bit(all.dtype, tc_gather_gemm_supported(g0));
+    if (force_tc() && !tc_ok) {
+        set_error("%s: SPX_FORCE_TC=1 but the tensor-core path does not support this call (dtype %d, C/g %d, K/g %d)",
+                  who, all.dtype, g0.c_in, g0.c_out);
+        return 3;
+    }
+    set_family(tc_ok ? 2 : 1);
+    const int64_t ldx = all.cx(), ldy = all.cy();
+    for (int j = 0; j < groups; ++j) {
+        const GatherGemmArgs g = group_args(all, groups, j, e);
+        if (int rc = tc_ok ? tc_gather_gemm(g, stream, ldx, ldy) : simt_gather_gemm(g, stream, ldx, ldy)) return rc;
+    }
+    return 0;
+}
+
+extern "C" int spx_grouped_gemm_fwd(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, spx_stream_t stream) {
+    const char *who = "grouped_gemm_fwd";
+    if (check_grouped(d, groups, a, who)) return 2;
+    SPX_REQUIRE(a->act >= SPX_ACT_NONE && a->act <= SPX_ACT_LEAKY_RELU, "%s: unknown activation %d", who, a->act);
+    if (d->n_out == 0) return 0;
+    SPX_REQUIRE(a->features && a->filters && a->out, "%s: NULL tensor", who);
+    if (check_elem_aligned(a->features, d->dtype, who, "features") || check_elem_aligned(a->filters, d->dtype, who, "filters") ||
+        check_elem_aligned(a->out, d->dtype, who, "out") || check_elem_aligned(a->bias, d->dtype, who, "bias"))
+        return 2;
+    GatherGemmArgs all = make_args(d, false);
+    all.x = a->features; all.w = a->filters; all.y = a->out; all.bias = a->bias; all.act = a->act; all.alpha = a->act_alpha;
+    return run_grouped_gemm(all, groups, who, (cudaStream_t)stream);
+}
+
+extern "C" int spx_grouped_gemm_dgrad(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a,
+                                      spx_stream_t stream) {
+    const char *who = "grouped_gemm_dgrad";
+    if (check_grouped(d, groups, a, who)) return 2;
+    if (d->n_in == 0) return 0;
+    SPX_REQUIRE(a->out_bp && a->filters && a->din, "%s: NULL tensor", who);
+    if (check_elem_aligned(a->out_bp, d->dtype, who, "out_bp") || check_elem_aligned(a->filters, d->dtype, who, "filters") ||
+        check_elem_aligned(a->din, d->dtype, who, "din"))
+        return 2;
+    GatherGemmArgs all = make_args(d, true);
+    all.x = a->out_bp; all.w = a->filters; all.y = a->din; all.bias = nullptr; all.act = SPX_ACT_NONE;
+    return run_grouped_gemm(all, groups, who, (cudaStream_t)stream);
+}
+
+// the dense weight gradient of group j: x and dout at the group's columns, dW at its filter rows
+static WgradArgs group_wgrad(const WgradArgs &all, int groups, int j, size_t e) {
+    WgradArgs g = all;
+    g.c_in = all.c_in / groups; g.c_out = all.c_out / groups;
+    g.x = (const uint8_t *)all.x + (size_t)j * g.c_in * e;
+    g.dout = (const uint8_t *)all.dout + (size_t)j * g.c_out * e;
+    g.dw = (uint8_t *)all.dw + (size_t)j * g.c_out * g.kv * g.c_in * e;
+    return g;
+}
+
+static bool grouped_wgrad_tc(const WgradArgs &g0) {
+    return route_tc_16bit(g0.dtype, tc_wgrad_supported(g0));
+}
+
+extern "C" size_t spx_grouped_gemm_wgrad_workspace_size(const spx_gemm_desc *d, int groups) {
+    if (!d || groups < 2 || d->c_in % groups || d->c_out % groups) return 0;
+    WgradArgs all = make_wgrad(d);
+    const WgradArgs g0 = group_wgrad(all, groups, 0, (size_t)dtype_bytes(d->dtype));
+    // the passes run one after another and reuse one workspace
+    return grouped_wgrad_tc(g0) ? tc_wgrad_workspace_size(g0) : 256;
+}
+
+static int grouped_wgrad_entry(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a, const spx_peer_group *pg,
+                               spx_stream_t stream_) {
+    const char *who = pg ? "grouped_gemm_wgrad_push" : "grouped_gemm_wgrad";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (check_grouped(d, groups, a, who)) return 2;
+    SPX_REQUIRE(a->dfilters != nullptr, "%s: dfilters is NULL", who);
+    if (check_elem_aligned(a->dfilters, d->dtype, who, "dfilters")) return 2;
+    const int64_t dw_count = (int64_t)d->kv * (d->c_in / groups) * d->c_out;
+    if (d->n_out == 0 || d->n_in == 0) {       // an empty shard still takes part in the exchange
+        SPX_CHECK_CUDA(cudaMemsetAsync(a->dfilters, 0, (size_t)dw_count * dtype_bytes(d->dtype), stream));
+        if (pg) return peer_push(nullptr, 0, 0, a->dfilters, dw_count, d->dtype, pg, stream);
+        return 0;
+    }
+    SPX_REQUIRE(a->features && a->out_bp, "%s: NULL tensor", who);
+    if (check_elem_aligned(a->features, d->dtype, who, "features") || check_elem_aligned(a->out_bp, d->dtype, who, "out_bp"))
+        return 2;
+    WgradArgs all = make_wgrad(d);
+    all.x = a->features; all.dout = a->out_bp; all.dw = a->dfilters;
+    all.workspace = a->workspace; all.workspace_bytes = a->workspace_bytes;
+    const size_t e = (size_t)dtype_bytes(d->dtype);
+    const WgradArgs g0 = group_wgrad(all, groups, 0, e);
+    const bool tc_ok = grouped_wgrad_tc(g0);
+    if (force_tc() && !tc_ok) {
+        set_error("%s: SPX_FORCE_TC=1 but the tensor-core wgrad does not support this call (dtype %d, C/g %d, K/g %d)",
+                  who, d->dtype, g0.c_in, g0.c_out);
+        return 3;
+    }
+    if (tc_ok)
+        SPX_REQUIRE(a->workspace && a->workspace_bytes >= tc_wgrad_workspace_size(g0),
+                    "%s: workspace too small (%zu < %zu)", who, a->workspace_bytes, tc_wgrad_workspace_size(g0));
+    set_family(tc_ok ? 2 : 1);
+    for (int j = 0; j < groups; ++j) {
+        const WgradArgs g = group_wgrad(all, groups, j, e);
+        if (int rc = tc_ok ? tc_wgrad(g, stream, d->c_in, d->c_out) : simt_wgrad(g, stream, d->c_in, d->c_out))
+            return rc;
+    }
+    // data-parallel: dW is complete locally; push it whole, as the FMA and depthwise routes do
+    if (pg) return peer_push(nullptr, 0, 0, a->dfilters, dw_count, d->dtype, pg, stream);
+    return 0;
+}
+
+extern "C" int spx_grouped_gemm_wgrad(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a,
+                                      spx_stream_t stream) {
+    return grouped_wgrad_entry(d, groups, a, nullptr, stream);
+}
+
+extern "C" int spx_grouped_gemm_wgrad_push(const spx_gemm_desc *d, int groups, const spx_grouped_gemm *a,
+                                           const spx_peer_group *pg, spx_stream_t stream) {
+    SPX_REQUIRE(pg != nullptr, "grouped_gemm_wgrad_push: peer group is NULL");
+    return grouped_wgrad_entry(d, groups, a, pg, stream);
+}

@@ -57,14 +57,18 @@ __host__ __device__ inline int64_t tt_total_elems(int64_t tiles, int kv) {
     return tt_blocks_elems(tiles, kv) + tiles * TT_REC_INTS + TT_STATE_INTS;
 }
 
-int simt_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream);
-int simt_wgrad(const WgradArgs &a, cudaStream_t stream);
+// ldx / ldy / ldd != 0: one group of a grouped conv (api_gemm.cu).  The args describe the group's dense
+// (C / groups -> K / groups) GEMM, with x, w, y (bias, dout, dw) already at the group's column block, filter rows
+// and bias; gathered x rows are ldx elements apart, output rows ldy and dout rows ldd.  The grouped instances
+// run the dense instance's schedule and summation order: only the row addressing differs.
+int simt_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream, int64_t ldx = 0, int64_t ldy = 0);
+int simt_wgrad(const WgradArgs &a, cudaStream_t stream, int64_t ldx = 0, int64_t ldd = 0);
 
 bool tc_gather_gemm_supported(const GatherGemmArgs &a);
-int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream);
+int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream, int64_t ldx = 0, int64_t ldy = 0);
 bool tc_wgrad_supported(const WgradArgs &a);
 size_t tc_wgrad_workspace_size(const WgradArgs &a);
-int tc_wgrad(const WgradArgs &a, cudaStream_t stream);
+int tc_wgrad(const WgradArgs &a, cudaStream_t stream, int64_t ldx = 0, int64_t ldd = 0);
 
 struct Int8Args {
     GatherGemmArgs g;          // dtype = SPX_I8; bias / act fields unused

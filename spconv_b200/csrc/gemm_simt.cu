@@ -63,142 +63,44 @@ __device__ __forceinline__ void simt_fp8_cols(const SimtEpilogue &ep, void *y, c
 template <typename T>
 __global__ void __launch_bounds__(S_THREADS)
 simt_gather_gemm_kernel(GatherGemmArgs a, SimtEpilogue ep) {
-    typedef typename AccT<T>::type acc_t;
-    __shared__ acc_t As[S_TM][S_TK + 1];
-    __shared__ acc_t Bs[S_TK][S_TN + 1];
-    __shared__ int32_t row_src[S_TM];     // source row (after argsort) of each tile row, -1 = out of range
-    __shared__ int32_t row_idx[S_TM];     // gathered X row for the current offset
-    __shared__ uint32_t tile_mask[4];
-
-    const int tid = threadIdx.x;
-    const int words = (a.kv + 31) / 32;
-    const int cx = a.cx(), cy = a.cy();
-    const T *X = (const T *)a.x;
-    const T *W = (const T *)a.w;
-    const int64_t w_sx = a.transpose_w ? (int64_t)a.kv * a.c_in : 1;   // stride of contraction channel
-    const int64_t w_sy = a.transpose_w ? 1 : (int64_t)a.kv * a.c_in;   // stride of output channel
-    const int64_t base = (int64_t)blockIdx.x * S_TM;
-
-    if (tid < 4) tile_mask[tid] = 0;
-    if (tid < S_TM) {
-        int64_t r = base + tid;
-        row_src[tid] = r < a.rows ? (a.argsort ? a.argsort[r] : (int32_t)r) : -1;
-    }
-    __syncthreads();
-    if (tid < S_TM * words && tid / words < S_TM) {
-        int r = tid / words, w = tid % words;
-        if (base + r < a.rows) {
-            uint32_t m;
-            if (a.mask) m = a.mask[(base + r) * words + w];
-            else {
-                int hi = a.kv - 32 * w;
-                m = hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u);
-            }
-            atomicOr(&tile_mask[w], m);
-        }
-    }
-    __syncthreads();
-
-    const int trow = tid / 8;          // 0..31
-    const int tcg = tid % 8;           // column group: columns tcg*8 .. tcg*8+7
-    for (int n0 = 0; n0 < cy; n0 += S_TN) {
-        acc_t acc[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = 0;
-        for (int k = 0; k < a.kv; ++k) {
-            if (!((tile_mask[k >> 5] >> (k & 31)) & 1u)) continue;
-            const int kw = a.reverse ? a.kv - 1 - k : k;
-            __syncthreads();
-            if (tid < S_TM) {
-                int32_t s = row_src[tid];
-                row_idx[tid] = s >= 0 ? a.pair[(int64_t)k * a.pair_stride + s] : -1;
-            }
-            __syncthreads();
-            for (int x0 = 0; x0 < cx; x0 += S_TK) {
-                for (int e = tid; e < S_TM * S_TK; e += S_THREADS) {
-                    int r = e / S_TK, x = e % S_TK;
-                    int32_t idx = row_idx[r];
-                    acc_t v = 0;
-                    if (idx >= 0 && x0 + x < cx) v = load_acc<T>(X + (int64_t)idx * cx + x0 + x);
-                    As[r][x] = v;
-                }
-                for (int e = tid; e < S_TK * S_TN; e += S_THREADS) {
-                    int x, y;
-                    if (a.transpose_w) { x = e / S_TN; y = e % S_TN; }   // y contiguous in memory
-                    else { y = e / S_TK; x = e % S_TK; }                 // x contiguous in memory
-                    acc_t v = 0;
-                    if (x0 + x < cx && n0 + y < cy)
-                        v = load_acc<T>(W + (int64_t)(x0 + x) * w_sx + (int64_t)(n0 + y) * w_sy + (int64_t)kw * a.c_in);
-                    Bs[x][y] = v;
-                }
-                __syncthreads();
-#pragma unroll 8
-                for (int x = 0; x < S_TK; ++x) {
-                    acc_t av = As[trow][x];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) acc[j] += av * Bs[x][tcg * 8 + j];
-                }
-                __syncthreads();
-            }
-        }
-        int32_t dst = row_src[trow];
-        if constexpr (std::is_same<T, __nv_fp8_e4m3>::value) {
-            if (dst >= 0) {
-                switch (ep.out_dtype) {
-                    case SPX_E4M3: simt_fp8_cols<SPX_E4M3>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
-                    case SPX_F32: simt_fp8_cols<SPX_F32>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
-                    case SPX_F16: simt_fp8_cols<SPX_F16>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
-                    default: simt_fp8_cols<SPX_BF16>(ep, a.y, acc, dst, n0 + tcg * 8, cy); break;
-                }
-            }
-        } else if (dst >= 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                int y = n0 + tcg * 8 + j;
-                if (y >= cy) continue;
-                int64_t o = (int64_t)dst * cy + y;
-                if (ep.mode == 0) {
-                    float v = (float)acc[j];
-                    if (ep.bias) v += to_float(((const T *)ep.bias)[y]);
-                    v = apply_act(v, ep.act, ep.alpha);
-                    if constexpr (!std::is_same<T, int8_t>::value) ((T *)a.y)[o] = from_float<T>(v);
-                } else {
-                    // int8 inference epilogue: test/test_all_algo.py:272-287
-                    float v = (float)acc[j] * ep.scale[y] + (ep.bias_f32 ? ep.bias_f32[y] : 0.f);
-                    if (ep.output_add) v += (float)ep.output_add[o] * ep.output_add_scale;
-                    v = apply_act(v, ep.act, ep.alpha);
-                    if (ep.out_dtype == SPX_I8) {
-                        float q = rintf(v);                         // round-half-even, as numpy
-                        q = fminf(fmaxf(q, -128.f), 127.f);
-                        ((int8_t *)a.y)[o] = (int8_t)q;
-                    } else if (ep.out_dtype == SPX_F32) {
-                        ((float *)a.y)[o] = v;
-                    } else {
-                        ((__half *)a.y)[o] = __float2half_rn(v);
-                    }
-                }
-            }
-        }
-    }
+    constexpr bool GROUPED = false;
+    constexpr int64_t ldx = 0, ldy = 0;
+#include "simt_gather_body.cuh"
 }
 
 template <typename T>
-static int launch_simt(const GatherGemmArgs &a, const SimtEpilogue &ep, cudaStream_t stream) {
+__global__ void __launch_bounds__(S_THREADS)
+simt_grouped_gemm_kernel(GatherGemmArgs a, SimtEpilogue ep, int ldx, int ldy) {
+    constexpr bool GROUPED = true;
+#include "simt_gather_body.cuh"
+}
+
+template <typename T>
+static int launch_simt(const GatherGemmArgs &a, const SimtEpilogue &ep, cudaStream_t stream, int64_t ldx = 0,
+                       int64_t ldy = 0) {
     if (a.rows == 0) return 0;
     unsigned nblk = (unsigned)div_up64(a.rows, S_TM);
+    if constexpr (std::is_same<T, float>::value || std::is_same<T, __half>::value ||
+                  std::is_same<T, __nv_bfloat16>::value) {
+        if (ldx) {
+            simt_grouped_gemm_kernel<T><<<nblk, S_THREADS, 0, stream>>>(a, ep, (int)ldx, (int)ldy);
+            SPX_CHECK_LAUNCH("simt_grouped_gemm_kernel");
+            return 0;
+        }
+    }
     simt_gather_gemm_kernel<T><<<nblk, S_THREADS, 0, stream>>>(a, ep);
     SPX_CHECK_LAUNCH("simt_gather_gemm_kernel");
     return 0;
 }
 
-int simt_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
+int simt_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream, int64_t ldx, int64_t ldy) {
     SimtEpilogue ep;
     memset(&ep, 0, sizeof(ep));
     ep.mode = 0; ep.bias = a.bias; ep.act = a.act; ep.alpha = a.alpha;
     switch (a.dtype) {
-        case SPX_F32: return launch_simt<float>(a, ep, stream);
-        case SPX_F16: return launch_simt<__half>(a, ep, stream);
-        case SPX_BF16: return launch_simt<__nv_bfloat16>(a, ep, stream);
+        case SPX_F32: return launch_simt<float>(a, ep, stream, ldx, ldy);
+        case SPX_F16: return launch_simt<__half>(a, ep, stream, ldx, ldy);
+        case SPX_BF16: return launch_simt<__nv_bfloat16>(a, ep, stream, ldx, ldy);
         default: set_error("simt_gather_gemm: unsupported dtype %d", a.dtype); return 2;
     }
 }
@@ -227,9 +129,9 @@ int simt_gather_gemm_fp8(const Fp8Args &q, cudaStream_t stream) {
 constexpr int WG_T = 16;
 constexpr int WG_ROWS = 64;
 
-template <typename T>
-__global__ void __launch_bounds__(WG_T *WG_T)
-simt_wgrad_kernel(WgradArgs a) {
+// GROUPED: x rows are ldx elements apart and dout rows ldd (simt_grouped_wgrad_kernel, one group of a grouped conv)
+template <typename T, bool GROUPED>
+__device__ __forceinline__ void simt_wgrad_body(WgradArgs a, int64_t ldx, int64_t ldd) {
     __shared__ float Ds[WG_ROWS][WG_T + 1];
     __shared__ float Xs[WG_ROWS][WG_T + 1];
     __shared__ int32_t idx_s[WG_ROWS];
@@ -251,8 +153,8 @@ simt_wgrad_kernel(WgradArgs a) {
             int32_t idx = idx_s[r];
             float dv = 0.f, xv = 0.f;
             if (idx >= 0) {
-                if (n0 + j < a.c_out) dv = to_float(D[(r0 + r) * a.c_out + n0 + j]);
-                if (c0 + j < a.c_in) xv = to_float(X[(int64_t)idx * a.c_in + c0 + j]);
+                if (n0 + j < a.c_out) dv = to_float(D[(r0 + r) * (GROUPED ? ldd : a.c_out) + n0 + j]);
+                if (c0 + j < a.c_in) xv = to_float(X[(int64_t)idx * (GROUPED ? ldx : a.c_in) + c0 + j]);
             }
             Ds[r][j] = dv;
             Xs[r][j] = xv;
@@ -266,16 +168,34 @@ simt_wgrad_kernel(WgradArgs a) {
         ((T *)a.dw)[((int64_t)(n0 + tn) * a.kv + k) * a.c_in + c0 + tc] = from_float<T>(acc);
 }
 
-int simt_wgrad(const WgradArgs &a, cudaStream_t stream) {
+template <typename T>
+__global__ void __launch_bounds__(WG_T *WG_T)
+simt_wgrad_kernel(WgradArgs a) {
+    simt_wgrad_body<T, false>(a, 0, 0);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(WG_T *WG_T)
+simt_grouped_wgrad_kernel(WgradArgs a, int64_t ldx, int64_t ldd) {
+    simt_wgrad_body<T, true>(a, ldx, ldd);
+}
+
+template <typename T>
+static void launch_simt_wgrad(const WgradArgs &a, dim3 grid, dim3 block, int64_t ldx, int64_t ldd, cudaStream_t stream) {
+    if (ldx) simt_grouped_wgrad_kernel<T><<<grid, block, 0, stream>>>(a, ldx, ldd);
+    else simt_wgrad_kernel<T><<<grid, block, 0, stream>>>(a);
+}
+
+int simt_wgrad(const WgradArgs &a, cudaStream_t stream, int64_t ldx, int64_t ldd) {
     dim3 grid((a.c_in + WG_T - 1) / WG_T, (a.c_out + WG_T - 1) / WG_T, a.kv);
     dim3 block(WG_T, WG_T);
     switch (a.dtype) {
-        case SPX_F32: simt_wgrad_kernel<float><<<grid, block, 0, stream>>>(a); break;
-        case SPX_F16: simt_wgrad_kernel<__half><<<grid, block, 0, stream>>>(a); break;
-        case SPX_BF16: simt_wgrad_kernel<__nv_bfloat16><<<grid, block, 0, stream>>>(a); break;
+        case SPX_F32: launch_simt_wgrad<float>(a, grid, block, ldx, ldd, stream); break;
+        case SPX_F16: launch_simt_wgrad<__half>(a, grid, block, ldx, ldd, stream); break;
+        case SPX_BF16: launch_simt_wgrad<__nv_bfloat16>(a, grid, block, ldx, ldd, stream); break;
         default: set_error("simt_wgrad: unsupported dtype %d", a.dtype); return 2;
     }
-    SPX_CHECK_LAUNCH("simt_wgrad_kernel");
+    SPX_CHECK_LAUNCH(ldx ? "simt_grouped_wgrad_kernel" : "simt_wgrad_kernel");
     return 0;
 }
 

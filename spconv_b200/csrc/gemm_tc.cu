@@ -85,6 +85,7 @@ struct TcParams {
     // fp8 epilogue (KIND_E4M3): scale = w_scale, bias_f32 = bias, output_add = the residual in out_dtype
     const float *in_scale, *add_scale, *out_scale;
     int ldy;                // elements between output (and residual) rows: c_out, of which this pass writes N
+    int ldx;                // grouped instances: bytes between gathered rows (the full row, of which a group reads xb)
 };
 
 // iterate set bits of a <=128-bit tile mask in ascending order (register-only: no indexed array)
@@ -130,13 +131,13 @@ __device__ __forceinline__ float load_bias(const void *bias, int j) {
 // ec: the CTA's epilogue constants in shared memory, ec[j] = bias (float mode) or scale (int8 mode),
 // ec[N + j] = the int8 bias.  A float-mode call without bias and activation (the input gradient, and
 // every conv layer followed by a norm) runs the PLAIN instance: convert and store, no per-element
-// branches between the stores.
-template <int OUT, bool INT8_MODE, int N, typename Acc, bool PLAIN = false>
+// branches between the stores.  STRIDED (grouped instances): output rows are p.ldy elements apart, not N.
+template <int OUT, bool INT8_MODE, int N, typename Acc, bool PLAIN = false, bool STRIDED = false>
 __device__ __forceinline__ void epilogue_frag(const TcParams &p, const float *ec, const Acc (&acc)[N / 2], int64_t dst_lo,
                                               int64_t dst_hi, int lane) {
     if constexpr (!INT8_MODE && !PLAIN) {
         if (p.bias == nullptr && p.act == SPX_ACT_NONE) {
-            epilogue_frag<OUT, false, N, Acc, true>(p, ec, acc, dst_lo, dst_hi, lane);
+            epilogue_frag<OUT, false, N, Acc, true, STRIDED>(p, ec, acc, dst_lo, dst_hi, lane);
             return;
         }
     }
@@ -146,7 +147,7 @@ __device__ __forceinline__ void epilogue_frag(const TcParams &p, const float *ec
     for (int h = 0; h < 2; ++h) {
         const int64_t dst = h ? dst_hi : dst_lo;
         if (dst < 0) continue;
-        uint8_t *row_ptr = (uint8_t *)p.y + dst * (int64_t)N * EB;
+        uint8_t *row_ptr = (uint8_t *)p.y + dst * (int64_t)(STRIDED ? p.ldy : N) * EB;
 #pragma unroll
         for (int nb = 0; nb < N / 8; ++nb) {
             const int col = nb * 8 + 2 * (lane & 3);
@@ -221,8 +222,10 @@ __device__ __forceinline__ void mma_step(Acc (&acc)[N / 2], uint64_t a, uint64_t
     }
 }
 
-// The kernel body; tc_gather_gemm_kernel (16-bit, tf32, int8) and tc_gather_gemm_fp8_kernel (e4m3) launch it.
-template <int KIND, int CPR, int N>
+// The kernel body; tc_gather_gemm_kernel (16-bit, tf32, int8), tc_gather_gemm_fp8_kernel (e4m3) and
+// tc_grouped_gemm_kernel (16-bit, one group of a grouped conv) launch it.  GROUPED: gathered rows are p.ldx bytes
+// apart and output rows p.ldy elements; everything else is the dense instance.
+template <int KIND, int CPR, int N, bool GROUPED = false>
 __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, const TcParams &p) {
     using Acc = typename std::conditional<KIND == KIND_I8, int32_t, float>::type;
     constexpr int LG_CPR = CPR == 2 ? 1 : CPR == 4 ? 2 : CPR == 8 ? 3 : CPR == 16 ? 4 : 5;
@@ -341,7 +344,7 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
                 const uint32_t a_stage = smem_base + (uint32_t)stage * p.stage_bytes;
 #pragma unroll
                 for (int itc = 0; itc < ITERS; ++itc)
-                    cp_async_16(a_stage + dst_off[itc], x_lane + (int64_t)max(ridx[itc], 0) * XB,
+                    cp_async_16(a_stage + dst_off[itc], x_lane + (int64_t)max(ridx[itc], 0) * (GROUPED ? p.ldx : XB),
                                 ridx[itc] >= 0 ? 16u : 0u);
                 cp_async_mbar_arrive_noinc(&full[stage]);
                 k = it.next();
@@ -543,8 +546,8 @@ __device__ __forceinline__ void tc_gather_gemm_body(const CUtensorMap &tmap_w, c
                 if (lane == 0) mbar_arrive(&empty[held]);
             }
             if constexpr (KIND == KIND_F16) {
-                if (p.out_dtype == SPX_F16) epilogue_frag<SPX_F16, false, N>(p, ec, acc, d_lo, d_hi, lane);
-                else epilogue_frag<SPX_BF16, false, N>(p, ec, acc, d_lo, d_hi, lane);
+                if (p.out_dtype == SPX_F16) epilogue_frag<SPX_F16, false, N, Acc, false, GROUPED>(p, ec, acc, d_lo, d_hi, lane);
+                else epilogue_frag<SPX_BF16, false, N, Acc, false, GROUPED>(p, ec, acc, d_lo, d_hi, lane);
             } else if constexpr (KIND == KIND_TF32) {
                 epilogue_frag<SPX_F32, false, N>(p, ec, acc, d_lo, d_hi, lane);
             } else if constexpr (KIND == KIND_I8) {
@@ -575,6 +578,12 @@ template <int CPR, int N>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gather_gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams p) {
     tc_gather_gemm_body<KIND_E4M3, CPR, N>(tmap_w, p);
+}
+
+template <int CPR, int N>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+tc_grouped_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const TcParams p) {
+    tc_gather_gemm_body<KIND_F16, CPR, N, true>(tmap_w, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -719,10 +728,11 @@ static int fill_params(const GatherGemmArgs &a, TcParams &p) {
     return 0;
 }
 
-template <int KIND, int CPR, int N>
+template <int KIND, int CPR, int N, bool GROUPED>
 static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
     void (*kernel)(const CUtensorMap, const TcParams);
-    if constexpr (KIND == KIND_E4M3) kernel = tc_gather_gemm_fp8_kernel<CPR, N>;
+    if constexpr (GROUPED) kernel = tc_grouped_gemm_kernel<CPR, N>;
+    else if constexpr (KIND == KIND_E4M3) kernel = tc_gather_gemm_fp8_kernel<CPR, N>;
     else kernel = tc_gather_gemm_kernel<KIND, CPR, N>;
     const size_t smem = (size_t)p.stages * p.stage_bytes + 2 * (size_t)p.idx_bytes + 1024 /*align slack*/ + 1024 /*barriers, tile-info ring*/ +
                         2 * N * sizeof(float) /*epilogue constants*/;
@@ -736,44 +746,54 @@ static int launch_tc_n(const CUtensorMap &tm, const TcParams &p, cudaStream_t st
     const int64_t max_ctas = (int64_t)sm_count();
     const int grid = (int)(tiles < max_ctas ? tiles : max_ctas);
     kernel<<<grid, TC_THREADS, smem, stream>>>(tm, p);
-    SPX_CHECK_LAUNCH(KIND == KIND_E4M3 ? "tc_gather_gemm_fp8_kernel" : "tc_gather_gemm_kernel");
+    SPX_CHECK_LAUNCH(GROUPED ? "tc_grouped_gemm_kernel" : KIND == KIND_E4M3 ? "tc_gather_gemm_fp8_kernel" : "tc_gather_gemm_kernel");
     return 0;
 }
 
 // instantiated (channels x element bytes) combinations: rows of 32..512 bytes, N = 16..256 output
 // channels (tf32: 16..128, int8: 32..256, e4m3: 32..128).  512-byte rows (CPR = 32) stop at N = 64: a 64 KB
-// gathered tile plus a weight slice of 128 or more rows puts two stages over TC_SMEM_BUDGET.
-template <int KIND, int CPR>
+// gathered tile plus a weight slice of 128 or more rows puts two stages over TC_SMEM_BUDGET.  The grouped
+// (16-bit) instances cover the same (CPR, N) set as the dense 16-bit ones.
+template <int KIND, int CPR, bool GROUPED>
 static int launch_tc_cpr(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
     switch (p.n) {
-        case 16: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_n<KIND, CPR, 16>(tm, p, stream); break;
-        case 32: return launch_tc_n<KIND, CPR, 32>(tm, p, stream);
-        case 64: return launch_tc_n<KIND, CPR, 64>(tm, p, stream);
-        case 128: if constexpr (CPR != 32) return launch_tc_n<KIND, CPR, 128>(tm, p, stream); break;
-        case 256: if constexpr (KIND != KIND_TF32 && KIND != KIND_E4M3 && CPR != 32) return launch_tc_n<KIND, CPR, 256>(tm, p, stream); break;
+        case 16: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_n<KIND, CPR, 16, GROUPED>(tm, p, stream); break;
+        case 32: return launch_tc_n<KIND, CPR, 32, GROUPED>(tm, p, stream);
+        case 64: return launch_tc_n<KIND, CPR, 64, GROUPED>(tm, p, stream);
+        case 128: if constexpr (CPR != 32) return launch_tc_n<KIND, CPR, 128, GROUPED>(tm, p, stream); break;
+        case 256: if constexpr (KIND != KIND_TF32 && KIND != KIND_E4M3 && CPR != 32) return launch_tc_n<KIND, CPR, 256, GROUPED>(tm, p, stream); break;
     }
     set_error("tc_gather_gemm: unsupported output channel count %d", p.n);
     return 2;
 }
 
-template <int KIND>
+template <int KIND, bool GROUPED = false>
 static int launch_tc(const CUtensorMap &tm, const TcParams &p, cudaStream_t stream) {
+    static_assert(!GROUPED || KIND == KIND_F16, "grouped instances are 16-bit only");
     switch (p.xb >> 4) {
-        case 2: if constexpr (KIND != KIND_TF32) return launch_tc_cpr<KIND, 2>(tm, p, stream); break;
-        case 4: return launch_tc_cpr<KIND, 4>(tm, p, stream);
-        case 8: return launch_tc_cpr<KIND, 8>(tm, p, stream);
-        case 16: return launch_tc_cpr<KIND, 16>(tm, p, stream);
-        case 32: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_cpr<KIND, 32>(tm, p, stream); break;
+        case 2: if constexpr (KIND != KIND_TF32) return launch_tc_cpr<KIND, 2, GROUPED>(tm, p, stream); break;
+        case 4: return launch_tc_cpr<KIND, 4, GROUPED>(tm, p, stream);
+        case 8: return launch_tc_cpr<KIND, 8, GROUPED>(tm, p, stream);
+        case 16: return launch_tc_cpr<KIND, 16, GROUPED>(tm, p, stream);
+        case 32: if constexpr (KIND != KIND_I8 && KIND != KIND_E4M3) return launch_tc_cpr<KIND, 32, GROUPED>(tm, p, stream); break;
     }
     set_error("tc_gather_gemm: unsupported row bytes %d", p.xb);
     return 2;
 }
 
-int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream) {
+// ldx != 0: one group of a grouped conv (16-bit only); the tensor map covers the group's [c_out, kv * c_in] filter
+// block, which is contiguous in the grouped filter
+int tc_gather_gemm(const GatherGemmArgs &a, cudaStream_t stream, int64_t ldx, int64_t ldy) {
     TcParams p;
     if (fill_params(a, p)) return 2;
     CUtensorMap tm;
     if (make_weight_tmap(&tm, a.w, a.dtype, a.kv, a.c_in, a.c_out, p.b_transposed ? 128 : p.span_b)) return 2;
+    if (ldx) {
+        SPX_REQUIRE(a.dtype == SPX_F16 || a.dtype == SPX_BF16, "tc_gather_gemm: grouped calls are 16-bit only");
+        p.ldx = (int)ldx * dtype_bytes(a.dtype);
+        p.ldy = (int)ldy;
+        return launch_tc<KIND_F16, true>(tm, p, stream);
+    }
     if (a.dtype == SPX_F32) return launch_tc<KIND_TF32>(tm, p, stream);
     return launch_tc<KIND_F16>(tm, p, stream);
 }

@@ -57,9 +57,13 @@ class SparseConvolution(SparseModule):
                  act_beta: float = 0, large_kernel_fast_algo: bool = False,
                  name=None, device=None, dtype=None):
         super().__init__(name=name)
-        # groups: 1, or depthwise (groups == in_channels == out_channels > 1); general groups are not supported
-        assert groups == 1 or (groups > 1 and groups == in_channels == out_channels), \
-            f"groups must be 1 or in_channels == out_channels (depthwise), got groups={groups} for " \
+        # groups: 1, depthwise (groups == in_channels == out_channels > 1), or grouped: both group widths
+        # in_channels / groups and out_channels / groups multiples of 16 (every group is a dense GEMM of that width)
+        grouped = (groups > 1 and in_channels % groups == 0 and out_channels % groups == 0
+                   and (in_channels // groups) % 16 == 0 and (out_channels // groups) % 16 == 0)
+        assert groups == 1 or (groups > 1 and groups == in_channels == out_channels) or grouped, \
+            f"groups must be 1, in_channels == out_channels (depthwise), or leave group widths in_channels / groups " \
+            f"and out_channels / groups that are multiples of 16; got groups={groups} for " \
             f"{in_channels} -> {out_channels} channels"
         self.ndim = ndim
         self.in_channels = in_channels
@@ -70,7 +74,7 @@ class SparseConvolution(SparseModule):
         self.padding = expand_nd(ndim, padding)
         self.output_padding = expand_nd(ndim, output_padding)
         self.groups = groups
-        self.depthwise = groups > 1
+        self.depthwise = groups > 1 and groups == in_channels == out_channels
         self.subm = subm
         self.transposed = transposed
         self.inverse = inverse
@@ -476,6 +480,12 @@ class SparseConvolution(SparseModule):
         if self.conv1x1 and not cross:
             if self.depthwise:
                 feats = features * weight.view(self.out_channels)
+            elif self.groups > 1:
+                # one batched matmul over the groups: [g, N, C/g] x [g, C/g, K/g]
+                g = self.groups
+                x3 = features.reshape(-1, g, self.in_channels // g).transpose(0, 1)
+                w3 = weight.reshape(g, self.out_channels // g, self.in_channels // g)
+                feats = torch.bmm(x3, w3.transpose(1, 2)).transpose(0, 1).reshape(-1, self.out_channels)
             else:
                 w2d = weight.view(self.out_channels, self.in_channels)
                 feats = torch.mm(features, w2d.t())
@@ -504,7 +514,7 @@ class SparseConvolution(SparseModule):
                            Fsp.indice_inverse_conv if self.inverse else Fsp.indice_conv)
                 out_features = conv_fn(features, weight, indice_pairs, indice_pair_num,
                                        outids.shape[0], algo, timer, bias_infer, act_alpha, act_beta,
-                                       act_type)
+                                       act_type, groups=self.groups)
         else:
             outids, pair_fwd, pair_bwd, mask_fwd, mask_bwd, sort_fwd, sort_bwd, masks = rb
             num_activate_out = outids.shape[0]
@@ -518,14 +528,14 @@ class SparseConvolution(SparseModule):
                                                  mask_bwd, sort_fwd, sort_bwd, num_activate_out,
                                                  masks, training, is_subm, timer,
                                                  self.fp32_accum, bias_infer, act_alpha, act_beta,
-                                                 act_type)
+                                                 act_type, self.groups)
             else:
                 out_features, _, _ = ops.implicit_gemm(
                     features, weight, pair_fwd, mask_fwd, sort_fwd, num_activate_out, masks,
                     training, is_subm, timer, self.fp32_accum, bias_infer, act_alpha, act_beta,
                     act_type, 1.0 if output_scale is None else output_scale, channel_scale,
                     output_add=None, output_add_scale=0.0,
-                    output_dtype=weight.dtype if output_scale is None else None)
+                    output_dtype=weight.dtype if output_scale is None else None, groups=self.groups)
 
         if bias_train is not None:
             out_features = out_features + bias_train.to(out_features.dtype)

@@ -78,6 +78,8 @@ def fp8_refusal(mod: nn.Module) -> Optional[str]:
         return "already an fp8 layer (its filter is e4m3 with its own scale)"
     if getattr(mod, "depthwise", False):
         return f"depthwise convolution (groups={mod.groups}) has no fp8 kernel"
+    if mod.groups != 1:
+        return f"grouped convolution (groups={mod.groups}) has no fp8 kernel"
     if mod.conv1x1:
         return "a 1x1 convolution is a dense matmul, not a sparse conv kernel"
     if mod.algo == ConvAlgo.MaskSplitImplicitGemm:

@@ -34,20 +34,20 @@ def _report(tag: str, **shapes) -> None:
 
 class _NativeConv(Function):
     """features, filters, indice_pairs, indice_pair_num, num_activate_out, algo, timer, bias,
-    act_alpha, act_beta, act_type, inverse, subm"""
+    act_alpha, act_beta, act_type, inverse, subm, groups"""
 
     @staticmethod
     @_amp_fwd
     def forward(ctx, features, filters, indice_pairs, indice_pair_num, num_activate_out, algo,
-                timer, bias, act_alpha, act_beta, act_type, inverse, subm):
+                timer, bias, act_alpha, act_beta, act_type, inverse, subm, groups=1):
         ctx.save_for_backward(indice_pairs, indice_pair_num, features, filters)
-        ctx.spx = (algo, timer, inverse, subm)
+        ctx.spx = (algo, timer, inverse, subm, groups)
         ctx.spx_scope = timer.snapshot()
         try:
             return ops.indice_conv(features, filters, indice_pairs, indice_pair_num,
                                    num_activate_out, inverse, subm, algo=algo, timer=timer,
                                    bias=bias, act_alpha=act_alpha, act_beta=act_beta,
-                                   act_type=act_type)
+                                   act_type=act_type, groups=groups)
         except Exception:
             _report("indice_conv", feat=tuple(features.shape), w=tuple(filters.shape),
                     pair=tuple(indice_pairs.shape), act=num_activate_out, algo=algo,
@@ -59,17 +59,17 @@ class _NativeConv(Function):
     @_amp_bwd
     def backward(ctx, grad_output):
         indice_pairs, indice_pair_num, features, filters = ctx.saved_tensors
-        algo, timer, inverse, subm = ctx.spx
+        algo, timer, inverse, subm, groups = ctx.spx
         try:
             with timer.scoped(ctx.spx_scope):
                 din, dw = ops.indice_conv_backward(features, filters, grad_output, indice_pairs,
                                                    indice_pair_num, inverse, subm, algo=algo,
-                                                   timer=timer)
+                                                   timer=timer, groups=groups)
         except Exception:
             _report("indice_conv_backward", feat=tuple(features.shape), w=tuple(filters.shape),
                     pair=tuple(indice_pairs.shape), do=tuple(grad_output.shape))
             raise
-        return (din, dw) + (None,) * 11
+        return (din, dw) + (None,) * 12
 
 
 class SparseImplicitGemmFunction(Function):
@@ -85,12 +85,12 @@ class SparseImplicitGemmFunction(Function):
                 masks: List[np.ndarray], is_train: bool, is_subm: bool,
                 timer: CUDAKernelTimer = CUDAKernelTimer(False),
                 fp32_accum: Optional[bool] = None, bias: Optional[torch.Tensor] = None,
-                act_alpha: float = 0.0, act_beta: float = 0.0, act_type=Activation.None_):
+                act_alpha: float = 0.0, act_beta: float = 0.0, act_type=Activation.None_, groups: int = 1):
         try:
             out, mask_out, mask_width = ops.implicit_gemm(
                 features, filters, pair_fwd, pair_mask_fwd_splits, mask_argsort_fwd_splits,
                 num_activate_out, masks, is_train, is_subm, timer, fp32_accum, bias, act_alpha,
-                act_beta, act_type)
+                act_beta, act_type, groups=groups)
         except Exception:
             _report("implicit_gemm", feat=tuple(features.shape), w=tuple(filters.shape),
                     pair=tuple(pair_fwd.shape), act=num_activate_out, issubm=is_subm,
@@ -99,7 +99,7 @@ class SparseImplicitGemmFunction(Function):
         ctx.save_for_backward(features, filters, pair_fwd, pair_bwd)
         ctx.spx = dict(mask_width=mask_width, mask_out=mask_out, timer=timer, masks=masks,
                        scope=timer.snapshot(),
-                       is_subm=is_subm, fp32_accum=fp32_accum,
+                       is_subm=is_subm, fp32_accum=fp32_accum, groups=groups,
                        mask_fwd=pair_mask_fwd_splits, mask_bwd=pair_mask_bwd_splits,
                        sort_fwd=mask_argsort_fwd_splits, sort_bwd=mask_argsort_bwd_splits)
         return out
@@ -116,12 +116,12 @@ class SparseImplicitGemmFunction(Function):
                     features, filters, grad_output, pair_fwd, pair_bwd, s["mask_fwd"], s["mask_bwd"],
                     s["sort_fwd"], s["sort_bwd"], mask_output_fwd=s["mask_out"], masks=s["masks"],
                     mask_width=s["mask_width"], is_subm=s["is_subm"], timer=s["timer"],
-                    fp32_accum=s["fp32_accum"])
+                    fp32_accum=s["fp32_accum"], groups=s["groups"])
         except Exception:
             _report("implicit_gemm_backward", feat=tuple(features.shape), w=tuple(filters.shape),
                     pair=tuple(pair_fwd.shape), issubm=s["is_subm"], do=tuple(grad_output.shape))
             raise
-        return (din, dw) + (None,) * 16
+        return (din, dw) + (None,) * 17
 
 
 class ZeroPaddingGrad(Function):
@@ -204,31 +204,34 @@ class SparseAvgPoolImplicitGemmFunction(Function):
 
 
 def _native(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo, timer, bias,
-            act_alpha, act_beta, act_type, inverse, subm):
+            act_alpha, act_beta, act_type, inverse, subm, groups=1):
     if timer is None:
         timer = CUDAKernelTimer(False)
+    if groups == 1:
+        return _NativeConv.apply(features, filters, indice_pairs, indice_pair_num, num_activate_out,
+                                 algo, timer, bias, act_alpha, act_beta, act_type, inverse, subm)
     return _NativeConv.apply(features, filters, indice_pairs, indice_pair_num, num_activate_out,
-                             algo, timer, bias, act_alpha, act_beta, act_type, inverse, subm)
+                             algo, timer, bias, act_alpha, act_beta, act_type, inverse, subm, groups)
 
 
 def indice_conv(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo,
-                timer=None, bias=None, act_alpha=0.0, act_beta=0.0, act_type=Activation.None_):
+                timer=None, bias=None, act_alpha=0.0, act_beta=0.0, act_type=Activation.None_, groups=1):
     return _native(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo, timer,
-                   bias, act_alpha, act_beta, act_type, False, False)
+                   bias, act_alpha, act_beta, act_type, False, False, groups)
 
 
 def indice_inverse_conv(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo,
                         timer=None, bias=None, act_alpha=0.0, act_beta=0.0,
-                        act_type=Activation.None_):
+                        act_type=Activation.None_, groups=1):
     return _native(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo, timer,
-                   bias, act_alpha, act_beta, act_type, True, False)
+                   bias, act_alpha, act_beta, act_type, True, False, groups)
 
 
 def indice_subm_conv(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo,
                      timer=None, bias=None, act_alpha=0.0, act_beta=0.0,
-                     act_type=Activation.None_):
+                     act_type=Activation.None_, groups=1):
     return _native(features, filters, indice_pairs, indice_pair_num, num_activate_out, algo, timer,
-                   bias, act_alpha, act_beta, act_type, False, True)
+                   bias, act_alpha, act_beta, act_type, False, True, groups)
 
 
 class DepthwiseConvFunction(Function):

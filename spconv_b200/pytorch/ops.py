@@ -554,13 +554,50 @@ def _desc(dtype, kv, c_in, c_out, n_in, n_out, pair, mask, argsort, reverse=Fals
     return d
 
 
-def _check_filter(features, filters):
+def _check_filter(features, filters, groups=1):
+    """``(kv, C, K)`` of the KRSC filter ``[K, *ksize, C / groups]``"""
     if filters.dtype != features.dtype:
         raise RuntimeError(f"features ({features.dtype}) and filters ({filters.dtype}) must have the same dtype")
     if features.dtype not in _DTYPE_CODE:
         raise RuntimeError(f"unsupported dtype {features.dtype}")
     kv = _prod(filters.shape[1:-1])
-    return kv, int(filters.shape[-1]), int(filters.shape[0])
+    if groups == 1:
+        return kv, int(filters.shape[-1]), int(filters.shape[0])
+    if groups < 1 or int(filters.shape[0]) % groups:
+        raise RuntimeError(f"groups {groups} must divide the filter's {int(filters.shape[0])} output channels")
+    if features.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+        raise NotImplementedError(f"grouped conv: {features.dtype} is not supported (float32, float16, bfloat16)")
+    return kv, int(filters.shape[-1]) * groups, int(filters.shape[0])
+
+
+# grouped conv (groups > 1): each call runs one dense GEMM pass per group (include/spconv_b200.h)
+def _grouped_fwd(d, groups, features, filters, out, bias, act_code, act_alpha, what):
+    a = _cabi.GroupedGemm(features=_ptr(features), filters=_ptr(filters), bias=_ptr(bias), out=_ptr(out),
+                          act=act_code, act_alpha=float(act_alpha))
+    _cabi.check(_lib().spx_grouped_gemm_fwd(ctypes.byref(d), int(groups), ctypes.byref(a), _stream()), what)
+
+
+def _grouped_dgrad(d, groups, out_bp, filters, din, what):
+    a = _cabi.GroupedGemm(out_bp=_ptr(out_bp), filters=_ptr(filters), din=_ptr(din))
+    _cabi.check(_lib().spx_grouped_gemm_dgrad(ctypes.byref(d), int(groups), ctypes.byref(a), _stream()), what)
+
+
+def _grouped_wgrad(d, groups, features, out_bp, dfilters, ws, group, what):
+    """``group``: None, or the peer group (``ctypes.byref``) that dW is pushed to once written"""
+    a = _cabi.GroupedGemm(features=_ptr(features), out_bp=_ptr(out_bp), dfilters=_ptr(dfilters),
+                          workspace=ws.data_ptr(), workspace_bytes=ws.numel())
+    if group is not None:
+        _cabi.check(_lib().spx_grouped_gemm_wgrad_push(ctypes.byref(d), int(groups), ctypes.byref(a), group, _stream()),
+                    what + "_push")
+    else:
+        _cabi.check(_lib().spx_grouped_gemm_wgrad(ctypes.byref(d), int(groups), ctypes.byref(a), _stream()), what)
+
+
+def _wgrad_workspace(d, groups, device):
+    lib = _lib()
+    if groups == 1:
+        return _bytes(lib.spx_implicit_gemm_wgrad_workspace_size(ctypes.byref(d)), device)
+    return _bytes(lib.spx_grouped_gemm_wgrad_workspace_size(ctypes.byref(d), int(groups)), device)
 
 
 def _first(split_list):
@@ -581,7 +618,7 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
                   scale: Optional[torch.Tensor] = None, output_add: Optional[torch.Tensor] = None,
                   output_add_scale: float = 0.0, output_dtype: Optional[torch.dtype] = None,
                   in_scale: Optional[torch.Tensor] = None, out_scale: Optional[torch.Tensor] = None,
-                  add_scale: Optional[torch.Tensor] = None):
+                  add_scale: Optional[torch.Tensor] = None, groups: int = 1):
     """Forward masked implicit GEMM -> ``(out [M, K], mask_output_fwd, mask_width)``
     (``ops.py:1450-1469`` / ``convops.py:2075-2243``).  Accumulation is always fp32 in registers
     (``fp32_accum`` is accepted and ignored).
@@ -589,19 +626,21 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     ``torch.float8_e4m3fn`` features and filters run ``spx_implicit_gemm_fwd_fp8``: ``scale`` is the filter's
     per-output-channel scale, ``in_scale`` / ``out_scale`` / ``add_scale`` are device fp32 ``[1]`` scales of the
     features, an e4m3 output and an e4m3 ``output_add``; ``output_dtype`` is float32 / float16 / bfloat16 or
-    float8_e4m3fn (default: float8_e4m3fn, as the features)."""
+    float8_e4m3fn (default: float8_e4m3fn, as the features).
+
+    ``groups > 1``: a grouped conv, filters ``[K, kv, C / groups]`` (float32 / float16 / bfloat16)."""
     _require_cuda(features, "features")
     lib = _lib()
     features = _dense(features)
     filters = _dense(filters)
-    kv, c_in, c_out = _check_filter(features, filters)
+    kv, c_in, c_out = _check_filter(features, filters, groups)
     assert features.shape[1] == c_in, "channel size mismatch"
     n_in, n_out = features.shape[0], int(num_activate_out)
     n_splits = len(pair_mask_fwd_splits) if isinstance(pair_mask_fwd_splits, (list, tuple)) else 1
     if n_splits > 1:
         return _implicit_gemm_splits(features, filters, pair_fwd, pair_mask_fwd_splits,
                                      mask_argsort_fwd_splits, n_out, is_train, timer, bias, act_alpha,
-                                     act_type, output_add, output_dtype)
+                                     act_type, output_add, output_dtype, groups=groups)
     mask = _first(pair_mask_fwd_splits)
     argsort = _first(mask_argsort_fwd_splits)
     is_int8 = features.dtype == torch.int8
@@ -642,9 +681,12 @@ def implicit_gemm(features: torch.Tensor, filters: torch.Tensor, pair_fwd: torch
     if bias is not None:
         bias = bias.to(features.dtype).contiguous()
     with timer.record("implicit_gemm", _stream()):
-        _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
-                                              _ptr(out), _ptr(bias), _act_code(act_type),
-                                              float(act_alpha), _stream()), "implicit_gemm_fwd")
+        if groups != 1:
+            _grouped_fwd(d, groups, features, filters, out, bias, _act_code(act_type), act_alpha, "grouped_gemm_fwd")
+        else:
+            _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
+                                                  _ptr(out), _ptr(bias), _act_code(act_type),
+                                                  float(act_alpha), _stream()), "implicit_gemm_fwd")
     if output_add is not None:
         out = out + output_add
     if output_dtype != out.dtype:
@@ -723,7 +765,7 @@ def fp8_quantize(x: torch.Tensor, num_valid: Optional[torch.Tensor] = None,
 
 
 def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_splits, n_out, is_train, timer,
-                          bias, act_alpha, act_type, output_add, output_dtype):
+                          bias, act_alpha, act_type, output_add, output_dtype, groups=1):
     """ConvAlgo.MaskSplitImplicitGemm forward: one kernel pass per mask split (each visits only its
     own offsets, rows in that split's sorted order), partial outputs summed, bias / activation after
     the last split (the reference fuses them into the last pass, ``convops.py:2196-2234``)."""
@@ -732,7 +774,7 @@ def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_spli
         raise NotImplementedError("int8 + MaskSplitImplicitGemm: use ConvAlgo.MaskImplicitGemm")
     if features.dtype == torch.float8_e4m3fn:
         raise NotImplementedError("fp8 + MaskSplitImplicitGemm: use ConvAlgo.MaskImplicitGemm")
-    kv, c_in, c_out = _check_filter(features, filters)
+    kv, c_in, c_out = _check_filter(features, filters, groups)
     n_in = features.shape[0]
     words = (kv + 31) // 32
     out = None
@@ -742,9 +784,12 @@ def _implicit_gemm_splits(features, filters, pair_fwd, mask_splits, argsort_spli
         d = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, pair_fwd, mask, argsort, tiles=tiles)
         part = torch.empty((n_out, c_out), dtype=features.dtype, device=features.device)
         with timer.record("implicit_gemm", _stream()):
-            _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters), _ptr(part),
-                                                  None, _cabi.SPX_ACT_NONE, 0.0, _stream()),
-                        "implicit_gemm_fwd(split)")
+            if groups != 1:
+                _grouped_fwd(d, groups, features, filters, part, None, _cabi.SPX_ACT_NONE, 0.0, "grouped_gemm_fwd(split)")
+            else:
+                _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters), _ptr(part),
+                                                      None, _cabi.SPX_ACT_NONE, 0.0, _stream()),
+                            "implicit_gemm_fwd(split)")
         out = part if out is None else out.add_(part)
         if tiles is not None:
             tile_masks.append(tiles[1].view(1, -1, words))
@@ -780,9 +825,9 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
                            mask_output_fwd: Optional[torch.Tensor], masks: List[np.ndarray],
                            mask_width: int, is_subm: bool,
                            timer: CUDAKernelTimer = CUDAKernelTimer(False),
-                           fp32_accum: Optional[bool] = None):
+                           fp32_accum: Optional[bool] = None, groups: int = 1):
     """Input gradient + weight gradient of the masked implicit GEMM -> ``(din, dfilters)``
-    (``ops.py:1667-1681`` / ``convops.py:2247-2440``)."""
+    (``ops.py:1667-1681`` / ``convops.py:2247-2440``).  ``groups > 1``: a grouped conv (see :func:`implicit_gemm`)."""
     _require_cuda(features, "features")
     lib = _lib()
     features = _dense(features)
@@ -790,7 +835,7 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
     out_bp = _dense(out_bp)
     if out_bp.dtype != features.dtype:
         out_bp = out_bp.to(features.dtype)
-    kv, c_in, c_out = _check_filter(features, filters)
+    kv, c_in, c_out = _check_filter(features, filters, groups)
     n_in, n_out = features.shape[0], out_bp.shape[0]
     n_splits = len(pair_mask_fwd_splits) if isinstance(pair_mask_fwd_splits, (list, tuple)) else 1
     if n_splits > 1:
@@ -801,12 +846,12 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
             bwd_s = [mask_argsort_bwd_splits[j]] if mask_argsort_bwd_splits else []
             di, dw = implicit_gemm_backward(features, filters, out_bp, pair_fwd, pair_bwd,
                                             [pair_mask_fwd_splits[j]], bwd_m, [mask_argsort_fwd_splits[j]],
-                                            bwd_s, None, masks, mask_width, is_subm, timer, fp32_accum)
+                                            bwd_s, None, masks, mask_width, is_subm, timer, fp32_accum, groups)
             # dW of split j is only meaningful on ITS offsets: the tensor-core kernel leaves the others zero, the
             # generic FMA kernel (odd channel counts) walks the whole pair table -- zero them either way.  The
             # offsets come from the host-side split constant, so no mask tensor is copied to the device (a
             # blocking copy per layer eagerly, refused under CUDA-graph capture)
-            dw = dw.view(c_out, kv, c_in)
+            dw = dw.view(c_out, kv, c_in // groups)
             for a, b in _zero_runs(masks[j], kv):
                 dw[:, a:b].zero_()
             din = di if din is None else din.add_(di)
@@ -828,17 +873,21 @@ def implicit_gemm_backward(features: torch.Tensor, filters: torch.Tensor, out_bp
                      tiles=tiles_bwd)
     d_wg = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, pair_fwd, mask_fwd, argsort_fwd,
                  tiles=tiles_fwd)
-    ws_bytes = lib.spx_implicit_gemm_wgrad_workspace_size(ctypes.byref(d_wg))
-    ws = _bytes(ws_bytes, features.device)
+    ws = _wgrad_workspace(d_wg, groups, features.device)
 
     def run_dgrad():
         with timer.record("implicit_gemm_dgrad", _stream()):
+            if groups != 1:
+                _grouped_dgrad(d_dg, groups, out_bp, filters, din, "grouped_gemm_dgrad")
+                return
             _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
                                                     _ptr(din), _stream()), "implicit_gemm_dgrad")
 
     def run_wgrad(group):
         with timer.record("implicit_gemm_wgrad", _stream()):
-            if group is not None:
+            if groups != 1:
+                _grouped_wgrad(d_wg, groups, features, out_bp, dfilters, ws, group, "grouped_gemm_wgrad")
+            elif group is not None:
                 # data-parallel: the kernel that reduces the split-K partials pushes this rank's fp32 dW into every
                 # rank's exchange buffer (csrc/peer.cu); the schedule's finish writes dfilters
                 _cabi.check(lib.spx_implicit_gemm_wgrad_push(
@@ -987,7 +1036,7 @@ def indice_conv(features: torch.Tensor, filters: torch.Tensor, indice_pairs: tor
                 subm: bool = False, algo: ConvAlgo = ConvAlgo.Native,
                 timer: CUDAKernelTimer = CUDAKernelTimer(False),
                 bias: Optional[torch.Tensor] = None, act_alpha: float = 0.0,
-                act_beta: float = 0.0, act_type=Activation.None_):
+                act_beta: float = 0.0, act_type=Activation.None_, groups: int = 1):
     """Gather-GEMM-scatter forward over a compact rulebook (``ops.py:811-823`` /
     ``convops.py:1504-1747``).  The compact pairs are scattered into a dense gather table on the
     device (no ``indice_pair_num.cpu()`` sync) and the output-stationary implicit-GEMM kernel
@@ -997,7 +1046,7 @@ def indice_conv(features: torch.Tensor, filters: torch.Tensor, indice_pairs: tor
     features = _dense(features)
     filters = _dense(filters)
     indice_pairs = indice_pairs.contiguous()
-    kv, c_in, c_out = _check_filter(features, filters)
+    kv, c_in, c_out = _check_filter(features, filters, groups)
     assert features.shape[1] == c_in, "channel size mismatch"
     assert indice_pairs.shape[1] == kv, "indice_pairs / filter kernel volume mismatch"
     n_in, n_out = features.shape[0], int(num_activate_out)
@@ -1010,10 +1059,14 @@ def indice_conv(features: torch.Tensor, filters: torch.Tensor, indice_pairs: tor
     tiles = _tile_tables(t_fwd, m_fwd, None, n_out, kv) if n_out else None
     d = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, t_fwd, m_fwd, None, tiles=tiles)
     with timer.record("indice_conv", _stream()):
-        _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
-                                              _ptr(out), _ptr(bias), _act_code(act_type),
-                                              float(act_alpha), _stream()),
-                    "implicit_gemm_fwd(native)")
+        if groups != 1:
+            _grouped_fwd(d, groups, features, filters, out, bias, _act_code(act_type), act_alpha,
+                         "grouped_gemm_fwd(native)")
+        else:
+            _cabi.check(lib.spx_implicit_gemm_fwd(ctypes.byref(d), _ptr(features), _ptr(filters),
+                                                  _ptr(out), _ptr(bias), _act_code(act_type),
+                                                  float(act_alpha), _stream()),
+                        "implicit_gemm_fwd(native)")
     return out
 
 
@@ -1021,7 +1074,7 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
                          indice_pairs: torch.Tensor, indice_pair_num: torch.Tensor,
                          inverse: bool = False, subm: bool = False,
                          algo: ConvAlgo = ConvAlgo.Native,
-                         timer: CUDAKernelTimer = CUDAKernelTimer(False)):
+                         timer: CUDAKernelTimer = CUDAKernelTimer(False), groups: int = 1):
     """Backward of :func:`indice_conv` -> ``(din, dfilters)`` (``ops.py:1103-1111`` /
     ``convops.py:1751-2071``)."""
     _require_cuda(features, "features")
@@ -1032,7 +1085,7 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
     if out_bp.dtype != features.dtype:
         out_bp = out_bp.to(features.dtype)
     indice_pairs = indice_pairs.contiguous()
-    kv, c_in, c_out = _check_filter(features, filters)
+    kv, c_in, c_out = _check_filter(features, filters, groups)
     n_in, n_out = features.shape[0], out_bp.shape[0]
     t_fwd, m_fwd, t_bwd, m_bwd = _native_tables(indice_pairs, indice_pair_num, n_in, n_out, kv,
                                                 subm, inverse, True, True)
@@ -1042,16 +1095,21 @@ def indice_conv_backward(features: torch.Tensor, filters: torch.Tensor, out_bp: 
     tiles_fwd = _tile_tables(t_fwd, m_fwd, None, n_out, kv) if n_out else None
     d_dg = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, t_bwd, m_bwd, None, tiles=tiles_bwd)
     d_wg = _desc(features.dtype, kv, c_in, c_out, n_in, n_out, t_fwd, m_fwd, None, tiles=tiles_fwd)
-    ws = _bytes(lib.spx_implicit_gemm_wgrad_workspace_size(ctypes.byref(d_wg)), features.device)
+    ws = _wgrad_workspace(d_wg, groups, features.device)
 
     def run_dgrad():
         with timer.record("indice_conv_dgrad", _stream()):
+            if groups != 1:
+                _grouped_dgrad(d_dg, groups, out_bp, filters, din, "grouped_gemm_dgrad(native)")
+                return
             _cabi.check(lib.spx_implicit_gemm_dgrad(ctypes.byref(d_dg), _ptr(out_bp), _ptr(filters),
                                                     _ptr(din), _stream()), "implicit_gemm_dgrad(native)")
 
     def run_wgrad(group):
         with timer.record("indice_conv_wgrad", _stream()):
-            if group is not None:
+            if groups != 1:
+                _grouped_wgrad(d_wg, groups, features, out_bp, dfilters, ws, group, "grouped_gemm_wgrad(native)")
+            elif group is not None:
                 _cabi.check(lib.spx_implicit_gemm_wgrad_push(
                     ctypes.byref(d_wg), _ptr(features), _ptr(out_bp), _ptr(dfilters), ws.data_ptr(), ws.numel(),
                     group, _stream()), "implicit_gemm_wgrad_push(native)")

@@ -69,6 +69,9 @@ class QuantizedSparseConv(SparseConvolution):
         if getattr(mod, "depthwise", False):
             raise NotImplementedError(f"int8 depthwise convolution is not supported (groups={mod.groups}); "
                                       "keep this layer in floating point")
+        if mod.groups != 1:
+            raise NotImplementedError(f"int8 grouped convolution is not supported (groups={mod.groups}); "
+                                      "keep this layer in floating point")
         q = cls(mod.ndim, mod.in_channels, mod.out_channels, mod.kernel_size, mod.stride, mod.padding,
                 mod.dilation, mod.groups, mod.bias is not None, subm=mod.subm,
                 output_padding=mod.output_padding, transposed=mod.transposed, inverse=mod.inverse,
